@@ -47,18 +47,21 @@ def parse_args():
                     help="world > 1: K7 trains in the row-sharded tables over NVLink (no block cache); not the default")
     ap.add_argument("--no-pipeline", action="store_true",
                     help="world > 1: train / pull / push strictly one after the other (-is_pipeline 0)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what they computed (loss, pair count, a fixed sample of "
+                         "rows of both embedding tables) as DIR/<name>.npy, so that two builds can be compared")
     return ap.parse_args()
 
 
 class ClockSampler:
-    """SM clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md's clocks line).
+    """SM clocks / throttle reasons sampled DURING the timed region.
 
     Started before the warm-up, stopped after the timed region; only samples taken inside the timed
     region are reported.  Source: NVML in-process (``pynvml``, the library nvidia-smi itself uses: SM
     clock, max SM clock, clocks-event reasons) every 200 ms, falling back to the recipe's looping
     ``nvidia-smi --query-gpu=... -lms 200`` when pynvml is missing.  Polling is kept sparse on purpose:
-    on 2 GPUs a 50 ms poll / the nvidia-smi loop coincided with device-timed steps of 27-38 ms against
-    22-24 ms unpolled (same binary, same box; `profiles/README.md`).  BENCH_CLOCK_SAMPLER=smi|nvml|none."""
+    a fast poll / the nvidia-smi loop can stall kernel launches inside device-timed steps.
+    BENCH_CLOCK_SAMPLER=smi|nvml|none."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
@@ -185,11 +188,11 @@ def main():
     if world != args.gpus and world > 1:
         args.gpus = world
     if not torch.cuda.is_available():
-        # the headline benchmark is a B200 measurement; say so instead of a CUDA traceback
+        # the headline benchmark is a GPU measurement; say so instead of a CUDA traceback
         # (bench/cpu_apps.py measures the CPU plumbing mode)
         if int(os.environ.get("RANK", "0")) == 0:
             print(json.dumps({"metric": "wordembedding_words_per_sec", "value": None, "n_gpus": args.gpus,
-                              "unavailable": "no CUDA device in this process; run on a B200"}), flush=True)
+                              "unavailable": "no CUDA device in this process; run on an H100"}), flush=True)
         return
     mv.init()
     rank = mv.rank()
@@ -268,6 +271,8 @@ def main():
     monitors = mv.Dashboard.snapshot()
     pairs = int(we.pairs.item())
     loss_per_pair = float(we.loss.item()) / max(pairs, 1)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, we, torch)
 
     # ------------------------------------------------------------ end-to-end arm
     # Through the public API, every step: one H2D copy of a block of inputs from pinned host memory and
@@ -366,7 +371,7 @@ def main():
             "vs_baseline": None, "dtype": "fp32", "data": "synthetic", "impl": "ours",
             "config": {"model": CONFIG_MODEL, "global_batch": B * world, "seq_len": 1000,
                        "parallelism": (f"dp{world} row-sharded PS tables" + (", pipelined pull/push (-is_pipeline 1)" if pipelined else "")) if world > 1 else "1 GPU (worker+server)",
-                       "block_words_per_gpu": B, "l2": "tables 2.4 GB >> 126 MB L2; new token block every step",
+                       "block_words_per_gpu": B, "l2": "tables 2.4 GB >> 50 MB L2; new token block every step",
                        "pairs_per_word": pairs / max(1, words_per_block * (K + W)),
                        "loss_per_pair": loss_per_pair},
             "clocks": clocks,
@@ -386,13 +391,35 @@ def main():
     mv.shutdown()
 
 
+DUMP_HOT_ROWS = 1024          # the most frequent words of the Zipf corpus: the rows every step updates
+DUMP_SAMPLED_ROWS = 16384     # plus a fixed random sample of the rest; 2 tables x ~17k rows x 300 x 4 B = 41 MB
+
+
+def dump_outputs(out_dir, we, torch):
+    """Write what the timed steps hand back to a caller of train_block: the loss and pair
+    count summed over all steps so far, and both embedding tables after the last step.  The tables hold vocab x dim floats each, so a
+    fixed, seeded set of rows is written (the hottest rows + a uniform sample), capped at 64 MB in all."""
+    import numpy as np
+    hot = np.arange(min(DUMP_HOT_ROWS, we.V))
+    rng = np.random.default_rng(2024)
+    ids = np.union1d(hot, rng.choice(we.V, size=min(DUMP_SAMPLED_ROWS, we.V), replace=False))
+    ids = ids[:max(1, (60 << 20) // (2 * 4 * we.D))]
+    rows = torch.from_numpy(ids).to(we.dev)
+    arrays = {"loss_cumulative": we.loss.double(), "pairs_cumulative": we.pairs.double(), "row_ids": rows.double(),
+              "input_embedding_rows": we.input_table.get_rows(rows)[:, :we.D].float(),
+              "output_embedding_rows": we.output_table.get_rows(rows)[:, :we.D].float()}
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a.cpu().numpy())
+
+
 def secondary_block(extra, world):
     return {"metric": "matrix_table_get_plus_add_gbs", "value": extra["get_plus_add_gbs"], "unit": "GB/s",
             "higher_is_better": True, "add_ms": extra["add_ms"], "get_ms": extra["get_ms"],
             "add_gbs": extra["add_gbs"], "get_gbs": extra["get_gbs"], "iters": 5,
             "config": {"table": "MatrixTable 1000000x512 fp32, whole-table Add (sgd updater fused) + whole-table Get",
                        "parallelism": f"{world} GPU(s), row-sharded, fused P2P kernels (no NCCL on the path)",
-                       "timing": "CUDA events, max over ranks; 2.05 GB table >> 126 MB L2",
+                       "timing": "CUDA events, max over ranks; 2.05 GB table >> 50 MB L2",
                        "staging": "Add reads the delta from the table's zero-copy symmetric staging buffer "
                                   "(table.staging()); an Add from an ordinary tensor pays one extra local copy"}}
 

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Fused Get+GEMM (tcgen05/TMEM/TMA, K2-fused) vs the unfused path (P2P Get into HBM, then
+"""Fused Get+GEMM (wgmma/TMA, K2-fused) vs the unfused path (P2P Get into HBM, then
 cuBLAS TF32 matmul), device-timed, max over ranks.  Y[M x N] = X[M x K] @ W[N x K]^T, W = a
 row-sharded MatrixTable (peer HBM when world > 1).  Writes gpurun_out/get_gemm_n<N>.json."""
 import argparse
@@ -58,7 +58,7 @@ def main():
         get_only = timed(lambda: t.get(wbuf), a.iters, world)
         flops = 2.0 * M * Nr * K
         wbytes = Nr * K * 4
-        link_floor = (wbytes * (world - 1) / world / 770e9 * 1e3) if world > 1 else (wbytes / 6571.9e9 * 1e3)
+        link_floor = (wbytes * (world - 1) / world / 450e9 * 1e3) if world > 1 else (wbytes / 3350e9 * 1e3)
         out.append({"M": M, "N": Nr, "K": K, "fused_ms": fused, "unfused_get_plus_cublas_ms": unf, "get_only_ms": get_only,
                     "fused_tflops": flops / fused / 1e9, "w_bytes": wbytes, "w_stream_floor_ms": link_floor,
                     "speedup_vs_unfused": unf / fused,

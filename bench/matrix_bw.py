@@ -88,8 +88,8 @@ def main():
             nt.get(out)
         res["nccl_add_plus_get_ms"] = timed(nccl_add_get, a.iters, world)
         del delta
-    link = 770.0   # GB/s per direction per GPU (measured peer copy, B200_PROFILING.md)
-    hbm = 6571.9
+    link = 450.0   # GB/s per direction per GPU: H100 SXM NVLink 4 (18 links), data-sheet figure
+    hbm = 3350.0   # GB/s: H100 SXM HBM3, data-sheet figure
     cross = nbytes * (world - 1) / world
     res["floor_ms"] = (cross / link / 1e6) if world > 1 else (2 * nbytes / hbm / 1e6)
     for k in ("ours_add", "ours_get", "nccl_add", "nccl_get"):

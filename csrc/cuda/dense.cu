@@ -413,7 +413,7 @@ __global__ void __launch_bounds__(256) get_dense_kernel(const __grid_constant__ 
 // in flight per GPU. Here ONE thread per CTA drives a ring of kBulkStages x kBulkChunk bytes of
 // shared memory with the bulk-copy engine: cp.async.bulk global(peer) -> smem (mbarrier
 // complete_tx), then cp.async.bulk smem -> global(local), no registers and no LSU instructions
-// on the data path; 1 CTA per SM (the ring takes the shared memory) x 148 SMs x 192 KB in flight.
+// on the data path; 1 CTA per SM (the ring takes the shared memory) x 132 SMs x 192 KB in flight.
 // ---------------------------------------------------------------------------
 constexpr int kBulkStages = 6;
 constexpr uint32_t kBulkChunk = 32 * 1024;

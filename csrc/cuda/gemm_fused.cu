@@ -5,27 +5,12 @@
 // W is a MatrixTable whose rows are range-sharded over the servers (peer-mapped HBM). The
 // reference pulls the table into a host buffer (MatrixWorkerTable::Get -> ProcessReplyGet
 // memcpy, src/table/matrix_table.cpp:58-76,316-341) and only then multiplies on the device.
-// Here the pulled row block never lands in local HBM: a work item is one tile of W rows (one
-// server's shard) times up to 512 rows of X.  The W tile is streamed from its owner over NVLink
-// with TMA (cp.async.bulk.tensor, 128B swizzle) straight into shared memory and is the *A*
-// operand of tcgen05.mma (kind::tf32, N=256, K=8): the accumulator is the transposed tile
-// Y^T[w_row, x_row] -- 128 TMEM lanes x 2 x 256 columns = all of TMEM -- so W crosses NVLink
-// ceil(M/512) times while X (the B operand, N=256 per instruction: the shape the tensor pipe runs
-// at full rate) is re-read from local L2.  Lanes = consecutive Y columns, so the epilogue's
-// tcgen05.ld registers store straight to 128-byte coalesced row segments of Y.
-//
-// NC = 2 (default): a CTA pair (cluster of 2, one TPC) runs tcgen05.mma.cta_group::2 with M=256:
-// each CTA stages its own 128 W rows and HALF of every 256-row X chunk, so the X bytes an SM pulls
-// from L2 (the limiter of the single-CTA version) halve and the smem ring holds twice as many
-// k-blocks.  Both CTAs' TMA loads signal the leader's "full" barriers; the leader's single MMA
-// thread multicasts its tcgen05.commit to both CTAs' "empty" / "accumulator full" barriers.
-//
-//   warp 0      TMA producer: W ring (one tile per k-block) + X ring (<=2 chunks per k-block)
-//   warp 1      TMEM alloc; (leader CTA) single-thread tcgen05.mma issue
-//   warps 2-5   epilogue: tcgen05.ld (32 lanes x 32 columns) -> registers -> global stores
-// Persistent CTAs; the two 256-column accumulators are handed back to the MMA issuer one by one,
-// so the next item's MMAs overlap the rest of the epilogue (items with M <= 256 alternate
-// accumulators = full double buffering).
+// Here the pulled row block never lands in local HBM: an item is a 128-row X tile times a 128-row W
+// tile of one shard, both streamed by TMA (128B swizzle; W from its owner over NVLink) into a 6-stage
+// mbarrier ring by one producer warp group, multiplied by two consumer warp groups with wgmma
+// (m64n128k8, TF32, K-major operands, fp32 accumulators in registers, stored from registers).
+// Persistent CTAs take items X tile fastest: resident CTAs share a local W tile through L2; a remote
+// tile is re-read over NVLink once per X tile.
 #include <cuda.h>
 #include <algorithm>
 #include <cstdio>
@@ -34,17 +19,15 @@
 
 namespace {
 
-constexpr int WM = 128;          // W rows per CTA (TMEM lanes); UMMA_M = WM * NC
-constexpr int XN = 256;          // UMMA_N: X rows per MMA (TMEM columns per accumulator)
-constexpr int XC_MAX = 2;        // accumulators (X chunks) per item: 2 * 256 = 512 TMEM columns
+constexpr int BM = 128;                      // X rows per item: kConsumers warp groups x wgmma M = 64
+constexpr int BN = 128;                      // W rows per item = wgmma N
 constexpr int BK = 32;           // fp32 elements per k-block = 128 bytes = one swizzle row
-constexpr int UK = 8;            // UMMA_K for tf32
-constexpr int W_STAGES = 6;      // 16 KB each
-constexpr int X_RING_BYTES = 128 * 1024;   // 4 x 32 KB (NC=1) or 8 x 16 KB (NC=2)
-constexpr int W_BYTES = WM * BK * 4;
-constexpr int kEpiWarps = 4;
-constexpr int kThreads = 64 + 32 * kEpiWarps;
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;   // shared::cluster address of the pair's even CTA
+constexpr int UK = 8;                        // wgmma K for tf32
+constexpr int STAGES = 6;                    // 6 x 32 KB of the 227 KB a block may hold
+constexpr int X_BYTES = BM * BK * 4;
+constexpr int W_BYTES = BN * BK * 4;
+constexpr int kConsumers = 2;
+constexpr int kThreads = 128 * (1 + kConsumers);
 
 struct GemmDev {
   float* y;
@@ -52,14 +35,9 @@ struct GemmDev {
   int64_t ldy;
   int S;
   int64_t row_begin[MVB_MAX_RANKS + 1];   // global row range of server s
-  int tile_begin[MVB_MAX_RANKS + 1];      // first W-tile index of server s (tile = 128 * NC rows)
+  int tile_begin[MVB_MAX_RANKS + 1];      // first W-tile index of server s (tile = BN rows)
   int tiles_n;                            // total W tiles
-  int x_groups;                           // ceil(M / (256 * xc_item))
-  int local_s;                            // server whose shard is local HBM (-1: none)
-  int cache_on;                           // stage remote W tiles in the per-worker scratch (see below)
-  unsigned long long* prof;               // optional cycle counters (MVB_GEMM_PROF=1), else null
-  int xc_item;                            // X chunks (accumulators) per item: 2 = W streamed ceil(M/512) times,
-                                          // 1 = ceil(M/256) times but consecutive items double-buffer TMEM
+  int m_tiles;                            // ceil(M / BM)
 };
 
 MVB_DEVINL uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -69,11 +47,8 @@ MVB_DEVINL void mbar_init(uint64_t* bar, int count) {
 MVB_DEVINL void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
-// arrive on the barrier at the same offset in CTA `rank` of the cluster (rank 0 = the MMA leader)
-MVB_DEVINL void mbar_arrive_cluster(uint64_t* bar, uint32_t rank) {
-  asm volatile(
-      "{\n.reg .b32 ra;\nmapa.shared::cluster.u32 ra, %0, %1;\n"
-      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n}\n" ::"r"(smem_u32(bar)), "r"(rank) : "memory");
+MVB_DEVINL void mbar_arrive(uint64_t* bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 MVB_DEVINL void mbar_wait(uint64_t* bar, uint32_t parity) {
   asm volatile(
@@ -81,362 +56,165 @@ MVB_DEVINL void mbar_wait(uint64_t* bar, uint32_t parity) {
       "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
       "@p bra LAB_DONE;\nbra LAB_WAIT;\nLAB_DONE:\n}\n" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
 }
-MVB_DEVINL void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {
-  asm volatile(
-      "{\n.reg .pred p;\nLAB_WAIT:\n"
-      "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%0], %1;\n"
-      "@p bra LAB_DONE;\nbra LAB_WAIT;\nLAB_DONE:\n}\n" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
-}
-// mbar_wait that charges its cycles to *acc when profiling (acc != nullptr)
-MVB_DEVINL void mbar_wait_prof(uint64_t* bar, uint32_t parity, unsigned long long* acc, bool cluster = false) {
-  if (acc) {
-    const long long t0 = clock64();
-    if (cluster) mbar_wait_cluster(bar, parity); else mbar_wait(bar, parity);
-    *acc += (unsigned long long)(clock64() - t0);
-  } else {
-    if (cluster) mbar_wait_cluster(bar, parity); else mbar_wait(bar, parity);
-  }
-}
-template <int NC>
 MVB_DEVINL void tma_load_2d(void* smem_dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
-  if constexpr (NC == 1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(smem_u32(smem_dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1) : "memory");
-  } else {
-    // data lands in THIS CTA's smem, the transaction bytes are counted on the LEADER's barrier
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(smem_u32(smem_dst)), "l"(map), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1) : "memory");
-  }
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
+      ::"r"(smem_u32(smem_dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1) : "memory");
 }
-MVB_DEVINL void tma_store_2d(const CUtensorMap* map, int c0, int c1, const void* smem_src) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
-               ::"l"(map), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1) : "memory");
-  asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-}
-// K-major operand, 128B swizzle: 8-row groups are 1024 B apart (SBO), LBO unused, version 1.
+// K-major operand, 128B swizzle: 8-row groups are 1024 B apart (SBO), LBO unused for swizzled K-major
 MVB_DEVINL uint64_t make_smem_desc(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);          // start address  [0,14)
-  d |= (uint64_t)0 << 16;                               // leading byte offset (ignored)
+  d |= (uint64_t)1 << 16;                               // leading byte offset [16,30)
   d |= (uint64_t)(1024 >> 4) << 32;                     // stride byte offset [32,46)
-  d |= (uint64_t)1 << 46;                               // descriptor version (sm100)
-  d |= (uint64_t)2 << 61;                               // SWIZZLE_128B
+  d |= (uint64_t)1 << 62;                               // layout: SWIZZLE_128B
   return d;
 }
-// c=F32, a=b=TF32, both K-major, N>>3 at [17,23), M>>4 at [24,29)
-template <int NC>
-struct InstrDesc {
-  static constexpr uint32_t value =
-      (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(XN >> 3) << 17) | ((uint32_t)((WM * NC) >> 4) << 24);
-};
-template <int NC>
-MVB_DEVINL void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
-  if constexpr (NC == 1) {
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n}\n"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(InstrDesc<1>::value), "r"(accumulate) : "memory");
-  } else {
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::2.kind::tf32 [%0], %1, %2, %3, p;\n}\n"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(InstrDesc<2>::value), "r"(accumulate) : "memory");
-  }
+MVB_DEVINL void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+MVB_DEVINL void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+MVB_DEVINL void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs
+MVB_DEVINL void fence_acc(float (&d)[64]) {
+#pragma unroll
+  for (int i = 0; i < 64; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-// NC = 2: the arrive is delivered to the barrier at this offset in BOTH CTAs of the pair
-template <int NC>
-MVB_DEVINL void umma_commit(uint64_t* bar) {
-  if constexpr (NC == 1) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];"
-                 ::"r"(smem_u32(bar)) : "memory");
-  } else {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(smem_u32(bar)), "h"((uint16_t)3) : "memory");
-  }
-}
-MVB_DEVINL void tmem_ld_32x32(uint32_t taddr, uint32_t (&v)[32]) {
+#define MVB_ACC8(d, i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), \
+                       "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
+#define MVB_ACC64(d) MVB_ACC8(d, 0), MVB_ACC8(d, 8), MVB_ACC8(d, 16), MVB_ACC8(d, 24), \
+                     MVB_ACC8(d, 32), MVB_ACC8(d, 40), MVB_ACC8(d, 48), MVB_ACC8(d, 56)
+// D[64 x 128] (+)= A[64 x 8] * B[128 x 8]^T; accumulate == 0 overwrites D
+MVB_DEVINL void wgmma_tf32(float (&d)[64], uint64_t adesc, uint64_t bdesc, int accumulate) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
       "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-        "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-        "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr));
-}
-template <int NC>
-MVB_DEVINL void cta_or_cluster_sync() {
-  if constexpr (NC == 1) {
-    __syncthreads();
-  } else {
-    asm volatile("barrier.cluster.arrive.release.aligned;\nbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-  }
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1;\n}\n"
+      : MVB_ACC64(d)
+      : "l"(adesc), "l"(bdesc), "r"(accumulate)
+      : "memory");
 }
 
-constexpr int X_STAGES_MAX = 8;
-struct SmemLayout {
-  uint64_t w_full[W_STAGES], w_empty[W_STAGES], x_full[X_STAGES_MAX], x_empty[X_STAGES_MAX];
-  uint64_t acc_full[XC_MAX], acc_empty[XC_MAX];
-  uint32_t tmem_base;
-};
-
-// Schedule: the (W tile, x-group) units, x-group fastest, are cut into one contiguous, balanced range
-// per worker (a CTA, or a CTA pair): a worker runs the x-groups of a tile back to back (X, a few MB,
-// stays in L2 for everybody) and meets its W tile again right away:
-//  * local shard: the second read is an L2 hit instead of a second HBM pass;
-//  * remote shard (peer lines are never cached in the local L2): during the tile's first unit every
-//    W stage that the MMAs have consumed is written to a per-CTA scratch tile in local memory with
-//    a TMA store, and the later units load from the scratch (which stays L2-resident: 128 rows x K
-//    per CTA) -- W crosses NVLink exactly once whatever M is.
 struct Tile {
   int s;
-  int64_t n_local, n_global, n_valid;        // this CTA's 128 rows of the tile
+  int64_t n_local, n_global, n_valid;        // the tile's BN rows inside shard s
 };
-template <int NC>
-MVB_DEVINL Tile decode_tile(const GemmDev& g, int ntile, int cta_rank) {
+MVB_DEVINL Tile decode_tile(const GemmDev& g, int ntile) {
   Tile t;
   int s = 0;
   while (s + 1 < g.S && ntile >= g.tile_begin[s + 1]) ++s;
   t.s = s;
-  t.n_local = (int64_t)(ntile - g.tile_begin[s]) * (WM * NC) + (int64_t)cta_rank * WM;   // row inside the shard
+  t.n_local = (int64_t)(ntile - g.tile_begin[s]) * BN;
   t.n_global = g.row_begin[s] + t.n_local;
-  t.n_valid = min((int64_t)WM, g.row_begin[s + 1] - t.n_global);                         // may be <= 0
+  t.n_valid = min((int64_t)BN, g.row_begin[s + 1] - t.n_global);
   return t;
 }
-MVB_DEVINL int chunks_of_group(const GemmDev& g, int xg) {
-  const int64_t x0 = (int64_t)xg * (XN * g.xc_item);
-  return (int)min((int64_t)g.xc_item, (g.M - x0 + XN - 1) / XN);
-}
 
-template <int NC>
 __global__ void __launch_bounds__(kThreads, 1)
 get_gemm_fused_kernel(const __grid_constant__ CUtensorMap map_x,
                       const __grid_constant__ CUtensorMap map_w0, const __grid_constant__ CUtensorMap map_w1,
                       const __grid_constant__ CUtensorMap map_w2, const __grid_constant__ CUtensorMap map_w3,
                       const __grid_constant__ CUtensorMap map_w4, const __grid_constant__ CUtensorMap map_w5,
                       const __grid_constant__ CUtensorMap map_w6, const __grid_constant__ CUtensorMap map_w7,
-                      const __grid_constant__ CUtensorMap map_c, const __grid_constant__ GemmDev g) {
-  constexpr int XH = XN / NC;                 // X rows this CTA stages per chunk
-  constexpr int X_BYTES = XH * BK * 4;
-  constexpr int X_STAGES = X_RING_BYTES / X_BYTES;
+                      const __grid_constant__ GemmDev g) {
   extern __shared__ unsigned char smem_raw[];
-  // SWIZZLE_128B tiles need 1024-byte alignment: align the dynamic segment by hand (the offset is
-  // the same in both CTAs of a pair: identical kernel, identical static layout)
+  // SWIZZLE_128B tiles need 1024-byte alignment: align the dynamic segment by hand
   unsigned char* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  unsigned char* x_tiles = smem;                              // X ring (1024-aligned)
-  unsigned char* w_tiles = smem + X_RING_BYTES;               // W_STAGES * 16 KB
-  SmemLayout* sl = reinterpret_cast<SmemLayout*>(w_tiles + W_STAGES * W_BYTES);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  uint32_t cta_rank = 0;
-  if constexpr (NC == 2) asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(cta_rank));
-  const bool leader = cta_rank == 0;
-  const int worker = blockIdx.x / NC, num_workers = gridDim.x / NC;
-
+  unsigned char* x_tiles = smem;                              // STAGES x 16 KB
+  unsigned char* w_tiles = smem + STAGES * X_BYTES;           // STAGES x 16 KB
+  uint64_t* full = reinterpret_cast<uint64_t*>(w_tiles + STAGES * W_BYTES);
+  uint64_t* empty = full + STAGES;
+  const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
   const int num_kb = (int)((g.K + BK - 1) / BK);
-  // contiguous, balanced range of (tile, x-group) units, x-group fastest
-  const int64_t units = (int64_t)g.tiles_n * g.x_groups;
-  const int64_t u_begin = units * worker / num_workers, u_end = units * (worker + 1) / num_workers;
+  const int64_t units = (int64_t)g.tiles_n * g.m_tiles;
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < W_STAGES; ++i) { mbar_init(&sl->w_full[i], 1); mbar_init(&sl->w_empty[i], 1); }
-    for (int i = 0; i < X_STAGES; ++i) { mbar_init(&sl->x_full[i], 1); mbar_init(&sl->x_empty[i], 1); }
-    for (int i = 0; i < XC_MAX; ++i) { mbar_init(&sl->acc_full[i], 1); mbar_init(&sl->acc_empty[i], kEpiWarps * NC); }
+    for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], kConsumers); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  __syncthreads();      // keeps the barrier words and tcgen05.alloc's smem result in separate epochs (racecheck)
-  if (warp == 1) {
-    if constexpr (NC == 1) {
-      asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(smem_u32(&sl->tmem_base)));
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    } else {
-      asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(smem_u32(&sl->tmem_base)));
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;");
-    }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;");
   __syncthreads();
-  cta_or_cluster_sync<NC>();                  // barriers of both CTAs are initialised before any remote signal
-  asm volatile("tcgen05.fence::after_thread_sync;");
-  const uint32_t tmem_base = sl->tmem_base;
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (wg == 0) {
+    if (tid == 0) {
       // ============================== TMA PRODUCER ======================================
-      int iw = 0, ix = 0;
-      uint32_t pw = 0, px = 0;
-      unsigned long long c_we = 0, c_xe = 0;
-      unsigned long long* a_we = g.prof ? &c_we : nullptr, * a_xe = g.prof ? &c_xe : nullptr;
-      // scratch tile of this CTA: rows [c_row, c_row + 128) of map_c.  w_store[slot] >= 0: the slot
-      // holds k-block w_store[slot] of a remote tile's first pass and must be saved before reuse.
-      const int c_row = (int)blockIdx.x * WM;
-      int w_store[W_STAGES];
-#pragma unroll
-      for (int i = 0; i < W_STAGES; ++i) w_store[i] = -1;
-      Tile t{};
-      const CUtensorMap* map_w = &map_w0;
-      bool cached = false;
-      for (int64_t u = u_begin; u < u_end; ++u) {
-        const int ntile = (int)(u / g.x_groups), xg = (int)(u - (int64_t)ntile * g.x_groups);
-        const bool first = (u == u_begin) || xg == 0;       // first unit of this tile on this worker
-        if (first) {
-          t = decode_tile<NC>(g, ntile, (int)cta_rank);
-          const int s = t.s;
-          map_w = s == 0 ? &map_w0 : s == 1 ? &map_w1 : s == 2 ? &map_w2 : s == 3 ? &map_w3
-                : s == 4 ? &map_w4 : s == 5 ? &map_w5 : s == 6 ? &map_w6 : &map_w7;
-          // worth staging only if this worker meets the tile again
-          cached = g.cache_on && s != g.local_s && (u + 1 < u_end) && (xg + 1 < g.x_groups);
-        }
-        {
-          const int XC = chunks_of_group(g, xg);
-          const int64_t x0 = (int64_t)xg * (XN * g.xc_item);
-          const bool from_scratch = cached && !first;
-          for (int kb = 0; kb < num_kb; ++kb) {
-            mbar_wait_prof(&sl->w_empty[iw], pw ^ 1u, a_we);
-            // the previous content of this slot has been consumed by the MMAs: save it if it was a
-            // first-pass stage of a remote tile (the smem read must finish before the slot is refilled)
-            int pending = -1;
-#pragma unroll
-            for (int i = 0; i < W_STAGES; ++i) if (i == iw) { pending = w_store[i]; w_store[i] = (cached && first) ? kb : -1; }
-            if (pending >= 0) {
-              tma_store_2d(&map_c, pending * BK, c_row, w_tiles + iw * W_BYTES);
-              asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-            }
-            if (leader) mbar_expect_tx(&sl->w_full[iw], W_BYTES * NC);
-            if (from_scratch) {
-              // stores of this k-block were committed >= num_kb - W_STAGES groups ago (host guarantees >= 2)
-              asm volatile("cp.async.bulk.wait_group 2;" ::: "memory");
-              tma_load_2d<NC>(w_tiles + iw * W_BYTES, &map_c, kb * BK, c_row, &sl->w_full[iw]);
-            } else {
-              tma_load_2d<NC>(w_tiles + iw * W_BYTES, map_w, kb * BK, (int)t.n_local, &sl->w_full[iw]);   // peer HBM
-            }
-            if (++iw == W_STAGES) { iw = 0; pw ^= 1u; }
-            for (int xc = 0; xc < XC; ++xc) {
-              mbar_wait_prof(&sl->x_empty[ix], px ^ 1u, a_xe);
-              if (leader) mbar_expect_tx(&sl->x_full[ix], X_BYTES * NC);
-              tma_load_2d<NC>(x_tiles + ix * X_BYTES, &map_x, kb * BK, (int)(x0 + xc * XN + (int)cta_rank * XH),
-                              &sl->x_full[ix]);
-              if (++ix == X_STAGES) { ix = 0; px ^= 1u; }
-            }
-          }
-        }
-      }
-      asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-      if (g.prof && leader) { atomicAdd(&g.prof[4], c_we); atomicAdd(&g.prof[5], c_xe); }
-    }
-  } else if (warp == 1) {
-    if (lane == 0 && leader) {
-      // ============================== MMA ISSUER =========================================
-      int iw = 0, ix = 0;
-      uint32_t pw = 0, px = 0;
-      uint32_t q = 0;                                 // running accumulator-chunk counter: slot = q & 1
-      unsigned long long c_wf = 0, c_xf = 0, c_ae = 0;
-      unsigned long long* a_wf = g.prof ? &c_wf : nullptr, * a_xf = g.prof ? &c_xf : nullptr,
-                        * a_ae = g.prof ? &c_ae : nullptr;
-      const long long t_start = clock64();
-      for (int64_t u = u_begin; u < u_end; ++u) {
-        const int XC = chunks_of_group(g, (int)(u % g.x_groups));
+      int st = 0;
+      uint32_t ph = 0;
+      for (int64_t u = blockIdx.x; u < units; u += gridDim.x) {
+        const int ntile = (int)(u / g.m_tiles), mt = (int)(u - (int64_t)ntile * g.m_tiles);
+        const Tile t = decode_tile(g, ntile);
+        const int s = t.s;
+        const CUtensorMap* map_w = s == 0 ? &map_w0 : s == 1 ? &map_w1 : s == 2 ? &map_w2 : s == 3 ? &map_w3
+                                 : s == 4 ? &map_w4 : s == 5 ? &map_w5 : s == 6 ? &map_w6 : &map_w7;
         for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait_prof(&sl->w_full[iw], pw, a_wf);
-          const uint32_t w_addr = smem_u32(w_tiles + iw * W_BYTES);
-          for (int xc = 0; xc < XC; ++xc) {
-            const uint32_t qc = q + (uint32_t)xc, slot = qc & 1u;
-            // the slot must have been drained by the epilogue(s) of its previous use
-            if (kb == 0 && qc >= 2) mbar_wait_prof(&sl->acc_empty[slot], ((qc >> 1) - 1u) & 1u, a_ae, true);
-            mbar_wait_prof(&sl->x_full[ix], px, a_xf);
-            asm volatile("tcgen05.fence::after_thread_sync;");
-            const uint32_t x_addr = smem_u32(x_tiles + ix * X_BYTES);
-#pragma unroll
-            for (int k = 0; k < BK / UK; ++k) {
-              // advance 32 bytes inside the 128-byte swizzle row per UMMA_K step
-              umma_tf32<NC>(tmem_base + slot * XN, make_smem_desc(w_addr + k * UK * 4),
-                            make_smem_desc(x_addr + k * UK * 4), (kb | k) ? 1u : 0u);
-            }
-            umma_commit<NC>(&sl->x_empty[ix]);        // X slot is free once these MMAs retire
-            if (++ix == X_STAGES) { ix = 0; px ^= 1u; }
-          }
-          umma_commit<NC>(&sl->w_empty[iw]);
-          if (++iw == W_STAGES) { iw = 0; pw ^= 1u; }
+          mbar_wait(&empty[st], ph ^ 1u);
+          // out-of-range rows / columns are zero-filled and still counted in the transaction bytes
+          mbar_expect_tx(&full[st], X_BYTES + W_BYTES);
+          tma_load_2d(x_tiles + st * X_BYTES, &map_x, kb * BK, mt * BM, &full[st]);
+          tma_load_2d(w_tiles + st * W_BYTES, map_w, kb * BK, (int)t.n_local, &full[st]);   // peer HBM
+          if (++st == STAGES) { st = 0; ph ^= 1u; }
         }
-        for (int xc = 0; xc < XC; ++xc) umma_commit<NC>(&sl->acc_full[(q + (uint32_t)xc) & 1u]);
-        q += (uint32_t)XC;
-      }
-      if (g.prof) {
-        atomicAdd(&g.prof[0], (unsigned long long)(clock64() - t_start));
-        atomicAdd(&g.prof[1], c_wf); atomicAdd(&g.prof[2], c_xf); atomicAdd(&g.prof[3], c_ae);
       }
     }
   } else {
-    // ================================ EPILOGUE ===========================================
-    // lanes = consecutive W rows = consecutive Y columns: register j of the warp is one 128-byte
-    // segment of Y row (x0 + ... + j).
-    const int quarter = warp & 3;                   // TMEM lane quarter this warp may access
-    uint32_t q = 0;
-    unsigned long long c_af = 0;
-    unsigned long long* a_af = (g.prof && warp == 2 && lane == 0 && leader) ? &c_af : nullptr;
-    const long long t_start = clock64();
-    for (int64_t u = u_begin; u < u_end; ++u) {
-     const int ntile = (int)(u / g.x_groups), xg = (int)(u - (int64_t)ntile * g.x_groups);
-     const Tile t = decode_tile<NC>(g, ntile, (int)cta_rank);
-     const bool n_ok = quarter * 32 + lane < t.n_valid;
-     float* ycol = g.y + t.n_global + quarter * 32 + lane;
-     {
-      const int XC = chunks_of_group(g, xg);
-      const int64_t x0 = (int64_t)xg * (XN * g.xc_item);
-      for (int xc = 0; xc < XC; ++xc, ++q) {
-        const uint32_t slot = q & 1u;
-        mbar_wait_prof(&sl->acc_full[slot], (q >> 1) & 1u, a_af);
-        asm volatile("tcgen05.fence::after_thread_sync;");
-        const int64_t m0 = x0 + (int64_t)xc * XN;
-        const int rows = (int)min((int64_t)XN, g.M - m0);
-#pragma unroll 1
-        for (int cc = 0; cc < XN; cc += 64) {
-          if (cc < rows) {
-            uint32_t v0[32], v1[32];
-            const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + slot * XN + (uint32_t)cc;
-            tmem_ld_32x32(taddr, v0);
-            tmem_ld_32x32(taddr + 32, v1);
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-            if (cc + 64 >= rows || cc + 64 >= XN) {
-              // last TMEM read of this accumulator: hand the columns back before storing
-              asm volatile("tcgen05.fence::before_thread_sync;");
-              __syncwarp();
-              if (lane == 0) mbar_arrive_cluster(&sl->acc_empty[slot], 0);
-            }
-            if (n_ok) {
-              float* out = ycol + (m0 + cc) * g.ldy;
-              if (cc + 64 <= rows) {
+    // ================================ CONSUMERS ==========================================
+    const int cw = wg - 1;                          // X rows [64 cw, 64 cw + 64) of each item
+    const int warp = tid >> 5, lane = tid & 31;
+    int st = 0;
+    uint32_t ph = 0;
+    float acc[64];
 #pragma unroll
-                for (int j = 0; j < 32; ++j) out[(int64_t)j * g.ldy] = __uint_as_float(v0[j]);
+    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+    for (int64_t u = blockIdx.x; u < units; u += gridDim.x) {
+      const int ntile = (int)(u / g.m_tiles), mt = (int)(u - (int64_t)ntile * g.m_tiles);
+      const Tile t = decode_tile(g, ntile);
+      int prev = -1;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(&full[st], ph);
+        const uint32_t xa = smem_u32(x_tiles + st * X_BYTES + cw * 64 * BK * 4);
+        const uint32_t wa = smem_u32(w_tiles + st * W_BYTES);
+        fence_acc(acc);
+        wgmma_fence();
 #pragma unroll
-                for (int j = 0; j < 32; ++j) out[(int64_t)(32 + j) * g.ldy] = __uint_as_float(v1[j]);
-              } else {
+        for (int k = 0; k < BK / UK; ++k)         // advance 32 bytes inside the 128-byte swizzle row
+          wgmma_tf32(acc, make_smem_desc(xa + k * UK * 4), make_smem_desc(wa + k * UK * 4), (kb | k) ? 1 : 0);
+        wgmma_commit();
+        // the previous k-block's MMAs have retired: its stage may be refilled
+        wgmma_wait<1>();
+        fence_acc(acc);
+        if (prev >= 0 && tid == 0) mbar_arrive(&empty[prev]);
+        prev = st;
+        if (++st == STAGES) { st = 0; ph ^= 1u; }
+      }
+      wgmma_wait<0>();
+      fence_acc(acc);
+      if (prev >= 0 && tid == 0) mbar_arrive(&empty[prev]);
+      // accumulator layout of wgmma m64nN f32: register 4j + 2h + c holds row 16 warp + lane/4 + 8h,
+      // column 8j + 2 (lane % 4) + c
+      const int64_t m_row = (int64_t)mt * BM + cw * 64 + warp * 16 + (lane >> 2);
+      const int n_col = 2 * (lane & 3);
+      const bool pairs = ((g.ldy | t.n_global) & 1) == 0;    // float2 stores are 8-byte aligned
+      float* yt = g.y + t.n_global;
 #pragma unroll
-                for (int j = 0; j < 32; ++j)
-                  if (cc + j < rows) out[(int64_t)j * g.ldy] = __uint_as_float(v0[j]);
+      for (int h = 0; h < 2; ++h) {
+        const int64_t m = m_row + 8 * h;
+        if (m >= g.M) continue;
+        float* yr = yt + m * g.ldy;
 #pragma unroll
-                for (int j = 0; j < 32; ++j)
-                  if (cc + 32 + j < rows) out[(int64_t)(32 + j) * g.ldy] = __uint_as_float(v1[j]);
-              }
-            }
+        for (int j = 0; j < BN / 8; ++j) {
+          const int n = 8 * j + n_col;
+          const float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+          if (pairs && n + 1 < t.n_valid) {
+            *reinterpret_cast<float2*>(yr + n) = make_float2(v0, v1);
+          } else {
+            if (n < t.n_valid) yr[n] = v0;
+            if (n + 1 < t.n_valid) yr[n + 1] = v1;
           }
         }
       }
-     }
     }
-    if (a_af) { atomicAdd(&g.prof[6], c_af); atomicAdd(&g.prof[7], (unsigned long long)(clock64() - t_start)); }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;");
-  __syncthreads();
-  cta_or_cluster_sync<NC>();                  // the peer may still be fed by / signalling this CTA
-  if (warp == 1) {
-    asm volatile("tcgen05.fence::after_thread_sync;");
-    if constexpr (NC == 1)
-      asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem_base));
-    else
-      asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, 512;" ::"r"(tmem_base));
   }
 }
 
@@ -472,13 +250,14 @@ int make_map(CUtensorMap* map, const void* base, int64_t rows, int64_t cols, int
   return r == CUDA_SUCCESS ? 0 : -31;
 }
 
-template <int NC>
-int launch_get_gemm(const MvbGetGemm* h, cudaStream_t st, int max_workers_override, int* last_grid) {
+int g_last_grid = 0;
+
+int launch_get_gemm(const MvbGetGemm* h, cudaStream_t st) {
   const MvbRowMap& wm = h->wmap;
   GemmDev g{};
   g.y = h->y; g.M = h->M; g.N = h->N; g.K = h->K; g.ldy = h->N; g.S = wm.nservers;
   CUtensorMap maps[1 + MVB_MAX_RANKS];
-  int rc = make_map(&maps[0], h->x, h->M, h->K, h->K, XN / NC);
+  int rc = make_map(&maps[0], h->x, h->M, h->K, h->K, BM);
   if (rc) return rc;
   int tiles = 0;
   for (int s = 0; s < wm.nservers; ++s) {
@@ -489,88 +268,22 @@ int launch_get_gemm(const MvbGetGemm* h, cudaStream_t st, int max_workers_overri
     g.row_begin[s] = lo;
     g.row_begin[s + 1] = hi;
     g.tile_begin[s] = tiles;
-    tiles += (int)((hi - lo + WM * NC - 1) / (WM * NC));
+    tiles += (int)((hi - lo + BN - 1) / BN);
     g.tile_begin[s + 1] = tiles;
-    rc = make_map(&maps[1 + s], wm.shard_ptrs[s], hi - lo > 0 ? hi - lo : 1, h->K, h->K, WM);
+    rc = make_map(&maps[1 + s], wm.shard_ptrs[s], hi - lo > 0 ? hi - lo : 1, h->K, h->K, BN);
     if (rc) return rc;
   }
   for (int s = wm.nservers; s < MVB_MAX_RANKS; ++s) maps[1 + s] = maps[1];
-  const int num_kb = (int)((h->K + BK - 1) / BK);
-  // remote shards: stage each W tile in a per-CTA scratch during its first x-group (W crosses NVLink
-  // once whatever M is).  Needs >= 8 k-blocks so that a stage's store retires long before its re-load.
-  static const int wcache_env = [] { const char* e = getenv("MVB_GEMM_WCACHE"); return e ? atoi(e) : 1; }();
-  g.local_s = (wm.nservers == 1) ? 0 : h->local_server;
-  bool any_remote = false;
-  for (int s = 0; s < wm.nservers; ++s) any_remote = any_remote || (s != g.local_s && g.row_begin[s + 1] > g.row_begin[s]);
-  const bool can_cache = any_remote && wcache_env != 0 && num_kb >= 8;
-  // Short K: prefer one accumulator per item so that consecutive items double-buffer TMEM and the
-  // epilogue hides under the next item's MMAs (re-reading the W tile is an L2 hit: local shard or
-  // scratch).  Measured 569 vs 533 TFLOP/s at K=512; at K=1024 the longer mainloop hides less and the
-  // extra X/W traffic costs more (522 vs 595).  Remote W without the scratch: fewest NVLink passes.
-  static const int xc_env = [] { const char* e = getenv("MVB_GEMM_XC"); return e ? atoi(e) : 0; }();
-  g.xc_item = (xc_env == 1 || xc_env == 2) ? xc_env
-            : (((!any_remote || can_cache) && h->K <= 512) ? 1 : XC_MAX);
-  g.x_groups = (int)((h->M + XN * g.xc_item - 1) / (XN * g.xc_item));
-  g.cache_on = (can_cache && g.x_groups > 1) ? 1 : 0;
-  static const bool prof_on = getenv("MVB_GEMM_PROF") != nullptr;
-  static unsigned long long* prof_buf = nullptr;
-  if (prof_on) {
-    if (!prof_buf) MVB_CUDA_CHECK(cudaMalloc(&prof_buf, 8 * sizeof(unsigned long long)));
-    MVB_CUDA_CHECK(cudaMemsetAsync(prof_buf, 0, 8 * sizeof(unsigned long long), st));
-    g.prof = prof_buf;
-  }
   g.tiles_n = tiles;
-  const size_t smem = X_RING_BYTES + W_STAGES * W_BYTES + sizeof(SmemLayout) + 1024;
-  auto kern = get_gemm_fused_kernel<NC>;
-  MVB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  cudaLaunchConfig_t cfg{};
-  cfg.blockDim = dim3(kThreads);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  int max_workers = mvb_num_sms() / NC;
-  if (NC == 2) {
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr; cfg.numAttrs = 1;
-    cfg.gridDim = dim3(2 * (unsigned)max_workers);
-    int nclusters = 0;
-    if (cudaOccupancyMaxActiveClusters(&nclusters, kern, &cfg) != cudaSuccess || nclusters < 1) {
-      cudaGetLastError();
-      return -34;                              // pairs cannot be scheduled: caller falls back to NC = 1
-    }
-    max_workers = std::min(max_workers, nclusters);
-  }
-  if (max_workers_override > 0) max_workers = std::min(max_workers, max_workers_override);
-  const unsigned workers = (unsigned)std::min<int64_t>((int64_t)tiles * g.x_groups, max_workers);
-  cfg.gridDim = dim3(workers * NC);
-  // scratch for remote W tiles: one [128 x K] tile per CTA, grown on demand, reused by every call
-  // (calls are expected on one stream; the buffer is only live inside a launch)
-  static float* scratch = nullptr;
-  static size_t scratch_bytes = 0;
-  const size_t need = g.cache_on ? (size_t)workers * NC * WM * (size_t)h->K * 4 : 4096;
-  if (need > scratch_bytes) {
-    if (scratch) { MVB_CUDA_CHECK(cudaDeviceSynchronize()); MVB_CUDA_CHECK(cudaFree(scratch)); scratch = nullptr; }
-    MVB_CUDA_CHECK(cudaMalloc(&scratch, need));
-    scratch_bytes = need;
-  }
-  CUtensorMap map_c;
-  rc = g.cache_on ? make_map(&map_c, scratch, (int64_t)workers * NC * WM, h->K, h->K, WM) : 0;
-  if (rc) return rc;
-  if (!g.cache_on) map_c = maps[0];
-  *last_grid = (int)(workers * NC);
-  MVB_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kern, maps[0], maps[1], maps[2], maps[3], maps[4], maps[5], maps[6],
-                                    maps[7], maps[8], map_c, g));
-  if (prof_on) {
-    unsigned long long hp[8];
-    MVB_CUDA_CHECK(cudaStreamSynchronize(st));
-    MVB_CUDA_CHECK(cudaMemcpy(hp, prof_buf, sizeof(hp), cudaMemcpyDeviceToHost));
-    const double n = (double)workers;
-    fprintf(stderr, "[get_gemm prof NC=%d xc=%d workers=%u] per-worker kcycles: mma_total %.0f  wait w_full %.0f  x_full %.0f  "
-            "acc_empty %.0f | producer wait w_empty %.0f  x_empty %.0f | epilogue total %.0f  wait acc_full %.0f\n",
-            NC, g.xc_item, workers, hp[0] / n / 1e3, hp[1] / n / 1e3, hp[2] / n / 1e3, hp[3] / n / 1e3, hp[4] / n / 1e3,
-            hp[5] / n / 1e3, hp[7] / n / 1e3, hp[6] / n / 1e3);
-  }
+  g.m_tiles = (int)((h->M + BM - 1) / BM);
+  const size_t smem = STAGES * (X_BYTES + W_BYTES) + 2 * STAGES * sizeof(uint64_t) + 1024;
+  MVB_CUDA_CHECK(cudaFuncSetAttribute(get_gemm_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  const int64_t units = (int64_t)tiles * g.m_tiles;
+  const unsigned grid = (unsigned)std::min<int64_t>(units, mvb_num_sms());
+  g_last_grid = (int)grid;
+  get_gemm_fused_kernel<<<grid, kThreads, smem, st>>>(maps[0], maps[1], maps[2], maps[3], maps[4], maps[5], maps[6],
+                                                      maps[7], maps[8], g);
+  MVB_CUDA_CHECK(cudaGetLastError());
   return 0;
 }
 
@@ -578,11 +291,9 @@ int launch_get_gemm(const MvbGetGemm* h, cudaStream_t st, int max_workers_overri
 
 extern "C" int mvb_get_gemm_supported(void) { return get_encode() != nullptr ? 1 : 0; }
 
-static int g_last_ctas = 0, g_last_grid = 0;
-// (CTAs per MMA group) * 1000 + persistent grid size of the most recent launch: 2148 = pairs on 148 SMs
-extern "C" int mvb_get_gemm_last_config(void) { return g_last_ctas * 1000 + g_last_grid; }
+// (CTAs per MMA group) * 1000 + persistent grid size of the most recent launch: 1132 = one CTA per SM on 132 SMs
+extern "C" int mvb_get_gemm_last_config(void) { return 1000 + g_last_grid; }
 
-// MVB_GEMM_CTAS=1 forces the single-CTA kernel; MVB_GEMM_WORKERS caps the persistent grid.
 extern "C" int mvb_get_gemm_fused(const MvbGetGemm* h, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   if (h->M <= 0 || h->N <= 0 || h->K <= 0) return 0;
@@ -590,12 +301,5 @@ extern "C" int mvb_get_gemm_fused(const MvbGetGemm* h, void* stream) {
   if (h->K % 4 != 0) return -32;
   const MvbRowMap& wm = h->wmap;
   if (wm.nservers < 1 || wm.nservers > MVB_MAX_RANKS || wm.num_col != h->K || wm.num_row != h->N) return -33;
-  static const int ctas = [] { const char* e = getenv("MVB_GEMM_CTAS"); return e ? atoi(e) : 2; }();
-  static const int cap = [] { const char* e = getenv("MVB_GEMM_WORKERS"); return e ? atoi(e) : 0; }();
-  if (ctas != 1) {
-    int rc = launch_get_gemm<2>(h, st, cap, &g_last_grid);
-    if (rc != -34) { g_last_ctas = 2; return rc; }
-  }
-  g_last_ctas = 1;
-  return launch_get_gemm<1>(h, st, cap, &g_last_grid);
+  return launch_get_gemm(h, st);
 }

@@ -212,7 +212,7 @@ __global__ void regularize_kernel(float* grad, const float* w, int64_t len, int 
   }
 }
 
-// ---- wide dense models (> 64 classes / GEMM-sized minibatches): the two products run on the tcgen05
+// ---- wide dense models (> 64 classes / GEMM-sized minibatches): the two products run on the wgmma
 // kernel of gemm_fused.cu (logits = X W^T with W streamed from its table, grad = E^T X); this is the
 // epilogue between them: per sample softmax / sigmoid / linear, loss, accuracy and the error matrix
 // E = (P - Y) * sample_weight / n, written TRANSPOSED ([out x n_pad], zero padded) so that it is the

@@ -1,4 +1,4 @@
-// multiverso-b200 :: C ABI of the sm_100a data-plane library (libmvb200.so).
+// multiverso-b200 :: C ABI of the sm_90a data-plane library (libmvb200.so).
 //
 // Every entry point takes raw device pointers + a cudaStream_t (as void*) so the
 // Python layer can drive it with torch tensors (tensor.data_ptr(), current stream)
@@ -294,6 +294,8 @@ typedef struct MvbSgns {
 int mvb_sgns_train(const MvbSgns* a, void* stream);
 int mvb_sgns_train_tma(const MvbSgns* a, void* stream);   /* TMA bulk-copy pipeline variant */
 int mvb_sgns_train_win(const MvbSgns* a, void* stream);   /* window-batched TMA pipeline      */
+int mvb_sgns_train_det(const MvbSgns* a, void* stream);   /* deterministic waves (default)    */
+int mvb_sgns_last_launches(void);   /* kernel launches of the last mvb_sgns_train call */
 int mvb_sgns_win_inflight(int dim, int negative, int window, int max_ctas);  /* centre positions in flight */
 /* ---- key-addressed shards for application-defined tables (keys.cu): the device-side extension point ---- */
 typedef struct MvbKeyMap {

@@ -1,4 +1,4 @@
-// multiverso-b200 :: device-side common definitions (sm_100a only).
+// multiverso-b200 :: device-side common definitions (sm_90a only).
 //
 // Everything the data-plane kernels share: the peer-pointer table, the
 // system-scope memory-model helpers used on signal pads, 128-bit vector
@@ -247,7 +247,7 @@ static inline int mvb_num_sms() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (sms <= 0) sms = 148;
+    if (sms <= 0) sms = 132;
   }
   return sms;
 }

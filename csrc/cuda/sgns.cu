@@ -393,9 +393,14 @@ SgnsDev to_dev(const MvbSgns* h) {
 
 extern "C" int mvb_sgns_train_tma(const MvbSgns* h, void* stream);
 extern "C" int mvb_sgns_train_win(const MvbSgns* h, void* stream);
+extern "C" int mvb_sgns_train_det(const MvbSgns* h, void* stream);
+
+int mvb_sgns_launches = 1;   // kernel launches of the last mvb_sgns_train call
+extern "C" int mvb_sgns_last_launches(void) { return mvb_sgns_launches; }
 
 extern "C" int mvb_sgns_train(const MvbSgns* h, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
+  mvb_sgns_launches = 1;
   if (h->n_tokens <= 0) return 0;
   if (h->window < 1) return -5;
   if (!h->hs && h->negative > 0 && !h->neg_pool && !(h->alias_prob && h->alias_idx)) return -6;
@@ -415,12 +420,17 @@ extern "C" int mvb_sgns_train(const MvbSgns* h, void* stream) {
     if (blocks > cap) blocks = cap;
     int variant = h->variant;
     if (const char* e = getenv("MVB_SGNS_VARIANT")) variant = atoi(e);
+    // default: deterministic; the Hogwild kernels below by variant (window-batched: also direct mode)
+    if (variant == 0 && h->nservers <= 1) {
+      int rc = mvb_sgns_train_det(h, stream);
+      if (rc != -20 && rc != -21) return rc;
+    }
     // window-batched pipeline (one centre position per warp, negatives shared by the position's contexts)
     if ((variant == 20 || variant == 0) && h->negative <= 7 && h->window <= 15) {
       int rc = mvb_sgns_train_win(h, stream);
       if (rc != -22 && rc != -20 && rc != -21) return rc;   // else: rows do not fit the smem rings
     }
-    // measured on B200 (dim 300, K 5): TMA pipeline 52.3 vs best register variant 46.4 Mwords/s
+    // pair-at-a-time TMA pipeline before the register variants
     if ((variant == 10 || variant == 0 || variant == 20) && h->negative <= 6 && h->window <= 15) {
       int rc = mvb_sgns_train_tma(h, stream);
       if (rc != -22 && rc != -20 && rc != -21) return rc;   // else: rows do not fit the smem ring
@@ -430,7 +440,6 @@ extern "C" int mvb_sgns_train(const MvbSgns* h, void* stream) {
       case 2: sgns_fast_kernel<2, 5, 3><<<(int)blocks, 128, 0, st>>>(d); break;
       case 3:
         // register/occupancy trade-off: KB rows of 12 registers each stay live per warp
-        // measured on B200 (dim 300, K 5): KB=5 31.5, KB=3 41.4, KB=2 40.4, KB=1 46.4 Mwords/s
         if (variant == 5) sgns_fast_kernel<3, 5, 3><<<(int)blocks, 128, 0, st>>>(d);
         else if (variant == 3) sgns_fast_kernel<3, 3, 4><<<(int)blocks, 128, 0, st>>>(d);
         else if (variant == 2) sgns_fast_kernel<3, 2, 5><<<(int)blocks, 128, 0, st>>>(d);

@@ -109,20 +109,12 @@ MVB_DEVINL void bulk_wait_read() {
 }
 MVB_DEVINL void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-// packed fp32x2 math (Blackwell FFMA2): halves the FMA instruction count of dots / axpys
+// fp32 pair math: sm_90 has no packed FFMA2, so each lane is one round-to-nearest FFMA / FMUL
 MVB_DEVINL float2 ffma2(float2 a, float2 b, float2 c) {
-  float2 d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;"
-      : "=l"(reinterpret_cast<uint64_t&>(d))
-      : "l"(reinterpret_cast<uint64_t&>(a)), "l"(reinterpret_cast<uint64_t&>(b)), "l"(reinterpret_cast<uint64_t&>(c)));
-  return d;
+  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
 }
 MVB_DEVINL float2 fmul2(float2 a, float2 b) {
-  float2 d;
-  asm("mul.rn.f32x2 %0, %1, %2;"
-      : "=l"(reinterpret_cast<uint64_t&>(d))
-      : "l"(reinterpret_cast<uint64_t&>(a)), "l"(reinterpret_cast<uint64_t&>(b)));
-  return d;
+  return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y));
 }
 MVB_DEVINL float sigm_fast(float x) { return __fdividef(1.0f, 1.0f + __expf(-x)); }
 MVB_DEVINL float softplus_neg(float x) { return fmaxf(-x, 0.f) + log1pf(__expf(-fabsf(x))); }

@@ -137,20 +137,9 @@ MVB_DEVINL void bulk_wait_read() {
 }
 MVB_DEVINL void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-// packed fp32x2 math (Blackwell FFMA2): halves the FMA instruction count of dots / axpys
+// fp32 pair math: sm_90 has no packed FFMA2, so each lane is one round-to-nearest FFMA
 MVB_DEVINL float2 ffma2(float2 a, float2 b, float2 c) {
-  float2 d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;"
-      : "=l"(reinterpret_cast<uint64_t&>(d))
-      : "l"(reinterpret_cast<uint64_t&>(a)), "l"(reinterpret_cast<uint64_t&>(b)), "l"(reinterpret_cast<uint64_t&>(c)));
-  return d;
-}
-MVB_DEVINL float2 fmul2(float2 a, float2 b) {
-  float2 d;
-  asm("mul.rn.f32x2 %0, %1, %2;"
-      : "=l"(reinterpret_cast<uint64_t&>(d))
-      : "l"(reinterpret_cast<uint64_t&>(a)), "l"(reinterpret_cast<uint64_t&>(b)));
-  return d;
+  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
 }
 MVB_DEVINL float sigm_fast(float x) { return __fdividef(1.0f, 1.0f + __expf(-x)); }
 MVB_DEVINL float softplus_neg(float x) { return fmaxf(-x, 0.f) + log1pf(__expf(-fabsf(x))); }
@@ -171,7 +160,7 @@ MVB_DEVINL void sts_f4(unsigned char* p, F4 v) {
 
 // A row of `dim` floats spread over the 32 lanes of a warp: NF4 chunks of one float4 per lane (the last
 // one possibly partial) and, when 16 or fewer float4 remain (dim 300: 11), a TAIL of one float2 per lane over twice
-// as many lanes instead of a half-empty float4 chunk -- 10 registers and 5 FFMA2 per 300-float row and dot
+// as many lanes instead of a half-empty float4 chunk -- 10 registers and 10 FFMA per 300-float row and dot
 // instead of 12 and 6.
 template <int NF4, bool TAIL>
 struct Row {
@@ -653,6 +642,209 @@ sgns_win_kernel(const __grid_constant__ WinDev a) {
   }
 }
 
+// ---- deterministic K7 (DESIGN.md §11): the maths above in waves of its in-flight count; reads see the tables as
+// the last wave left them, deltas / loss are summed in 64-bit fixed point, then applied.  Warp per centre.
+constexpr float kFixScale = 0x1p40f;              // 2^-40 resolution, +-2^23 range
+constexpr float kLossScale = 0x1p32f;
+
+struct DetDev {
+  const int* tokens;
+  int64_t n_tokens, p0, p1;                       // centres of this wave
+  float* w_in;
+  float* w_out;
+  int dim;
+  int64_t ld;
+  int window, ko;
+  float lr;
+  const float* alias_prob;
+  const int* alias_idx;
+  int vocab;
+  const int* neg_pool;
+  int neg_pool_size;
+  const int* neg_pool_size_ptr;
+  const int* map_in;
+  const int* map_out;
+  const float* scale_in;
+  const float* scale_out;
+  uint64_t seed;
+  bool want_loss;
+  unsigned long long* pair_count;
+  unsigned long long* acc[2];                     // [rows x dim] deltas of the input / output table
+  int* flag[2];                                   // row touched in this wave
+  int* list[2];                                   // touched rows (any order)
+  int* count;                                     // [2]
+  unsigned long long* loss_acc;
+};
+
+MVB_DEVINL void det_touch(const DetDev& a, int t, int r) {
+  if (atomicExch(a.flag[t] + r, 1) == 0) a.list[t][atomicAdd(a.count + t, 1)] = r;
+}
+template <int NJ>
+MVB_DEVINL void det_add(const DetDev& a, int t, int r, const float (&v)[NJ], int lane) {
+  unsigned long long* dst = a.acc[t] + (int64_t)r * a.dim;
+#pragma unroll
+  for (int u = 0; u < NJ; ++u) {
+    const int j = lane + 32 * u;
+    if (j < a.dim) atomicAdd(dst + j, (unsigned long long)__float2ll_rn(v[u] * kFixScale));
+  }
+  if (lane == 0) det_touch(a, t, r);
+}
+template <int NJ>
+MVB_DEVINL void det_load(float (&v)[NJ], const float* row, int dim, int lane, bool on) {
+#pragma unroll
+  for (int u = 0; u < NJ; ++u) v[u] = (on && lane + 32 * u < dim) ? row[lane + 32 * u] : 0.f;
+}
+template <int NJ>
+MVB_DEVINL float det_dot(const float (&x)[NJ], const float (&y)[NJ]) {
+  float s = 0.f;
+#pragma unroll
+  for (int u = 0; u < NJ; ++u) s = __fmaf_rn(x[u], y[u], s);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  return s;
+}
+
+template <int NJ, int KO>
+__global__ void __launch_bounds__(256)
+sgns_det_kernel(const __grid_constant__ DetDev a) {
+  const int lane = threadIdx.x & 31;
+  const int64_t warp0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+  const int W = a.window;
+  const int pool_n = a.neg_pool_size_ptr ? __ldg(a.neg_pool_size_ptr) : a.neg_pool_size;
+  float loss = 0.f;
+  unsigned long long pairs = 0ull;
+  for (int64_t p = a.p0 + warp0; p < a.p1; p += nwarps) {
+    const int tp = __ldg(a.tokens + p);
+    if (tp < 0) continue;
+    // centre + negatives (lane k < ko holds output row k), exactly as the window kernel samples them
+    const uint64_t prng = hash64(a.seed ^ (uint64_t)(p + 1) * 0x9E3779B97F4A7C15ull);
+    int rid = -1;
+    float osc = 1.f;
+    if (lane == 0) {
+      rid = a.map_out ? __ldg(a.map_out + tp) : tp;
+      if (a.scale_out) osc = __ldg(a.scale_out + tp);
+    } else if (lane < a.ko) {
+      const uint64_t r = hash64(prng ^ ((uint64_t)lane * 0xD6E8FEB86659FD93ull));
+      int t;
+      if (a.neg_pool) {
+        t = pool_n > 0 ? __ldg(a.neg_pool + (r >> 8) % (uint64_t)pool_n) : -1;
+      } else {
+        const uint32_t idx = (uint32_t)((r >> 32) % (uint64_t)a.vocab);
+        const float u = (float)(r & 0xFFFFFF) * (1.0f / 16777216.0f);
+        t = (u < __ldg(a.alias_prob + idx)) ? (int)idx : __ldg(a.alias_idx + idx);
+      }
+      if (t == tp) t = -1;                         // Parse(): target == word_idx is skipped
+      if (t >= 0) {
+        rid = a.map_out ? __ldg(a.map_out + t) : t;
+        if (a.scale_out) osc = __ldg(a.scale_out + t);
+      }
+    }
+    if (__shfl_sync(0xffffffffu, rid, 0) < 0) continue;
+    const uint32_t used = __ballot_sync(0xffffffffu, rid >= 0) & ((1u << a.ko) - 1u);
+    // window (ParseSentence): lane l <-> offset d = l - hw; contexts stop at the first break on either side
+    const int hw = W - (int)((prng >> 16) % (uint64_t)W);
+    int crid = -1;
+    float csc = 1.f;
+    if (lane <= 2 * hw && lane != hw) {
+      const int64_t q = p + (lane - hw);
+      if (q >= 0 && q < a.n_tokens) {
+        const int tq = __ldg(a.tokens + q);
+        if (tq >= 0) {
+          crid = a.map_in ? __ldg(a.map_in + tq) : tq;
+          if (a.scale_in) csc = __ldg(a.scale_in + tq);
+        }
+      }
+    }
+    const uint32_t isnull = __ballot_sync(0xffffffffu, lane <= 2 * hw && lane != hw && crid < 0);
+    const uint32_t left_null = isnull & ((1u << hw) - 1u);
+    const int lo = left_null ? (32 - __clz(left_null)) : 0;
+    const uint32_t right_null = isnull >> (hw + 1);
+    const int hi = right_null ? (hw + __ffs(right_null) - 1) : 2 * hw;
+    const uint32_t ctx = (((hi >= 31) ? 0xffffffffu : ((1u << (hi + 1)) - 1u)) & ~((1u << lo) - 1u)) & ~(1u << hw);
+    if (!ctx) continue;
+    float O[KO][NJ];
+#pragma unroll
+    for (int k = 0; k < KO; ++k) {
+      const int r = __shfl_sync(0xffffffffu, rid, k);
+      det_load(O[k], a.w_out + (int64_t)(r < 0 ? 0 : r) * a.ld, a.dim, lane, (used >> k) & 1u);
+    }
+    // phase 1: per context 1+K dots on the rows as the wave found them, input-row delta
+    float gs[KO];                                  // lane t keeps the error terms of context t
+#pragma unroll
+    for (int k = 0; k < KO; ++k) gs[k] = 0.f;
+    const bool want_loss = a.want_loss && (p & 7) == 0;
+    for (uint32_t m = ctx; m; m &= m - 1) {
+      const int t = __ffs(m) - 1;
+      const int r = __shfl_sync(0xffffffffu, crid, t);
+      const float isc = __shfl_sync(0xffffffffu, csc, t);
+      float h[NJ], e[NJ] = {};
+      det_load(h, a.w_in + (int64_t)r * a.ld, a.dim, lane, true);
+#pragma unroll
+      for (int k = 0; k < KO; ++k) {
+        if (!((used >> k) & 1u)) continue;
+        const float f = det_dot(h, O[k]);
+        const float g = ((k == 0 ? 1.f : 0.f) - sigm_fast(f)) * a.lr;
+        if (want_loss && lane == 0) loss += 8.f * softplus_neg(k == 0 ? f : -f);
+        if (lane == t) gs[k] = g;
+#pragma unroll
+        for (int u = 0; u < NJ; ++u) e[u] = __fmaf_rn(g * isc, O[k][u], e[u]);
+      }
+      det_add(a, 0, r, e, lane);
+      ++pairs;
+    }
+    // phase 2: output-row deltas sum_c g_ck * in_c
+#pragma unroll
+    for (int k = 0; k < KO; ++k)
+#pragma unroll
+      for (int u = 0; u < NJ; ++u) O[k][u] = 0.f;
+    for (uint32_t m = ctx; m; m &= m - 1) {
+      const int t = __ffs(m) - 1;
+      const int r = __shfl_sync(0xffffffffu, crid, t);
+      float h[NJ];
+      det_load(h, a.w_in + (int64_t)r * a.ld, a.dim, lane, true);
+#pragma unroll
+      for (int k = 0; k < KO; ++k) {
+        const float gk = __shfl_sync(0xffffffffu, gs[k], t) * __shfl_sync(0xffffffffu, osc, k);
+#pragma unroll
+        for (int u = 0; u < NJ; ++u) O[k][u] = __fmaf_rn(gk, h[u], O[k][u]);
+      }
+    }
+#pragma unroll
+    for (int k = 0; k < KO; ++k)
+      if ((used >> k) & 1u) det_add(a, 1, __shfl_sync(0xffffffffu, rid, k), O[k], lane);
+  }
+  if (lane == 0) {
+    if (a.want_loss && loss != 0.f) atomicAdd(a.loss_acc, (unsigned long long)__float2ll_rn(loss * kLossScale));
+    if (a.pair_count && pairs) atomicAdd(a.pair_count, pairs);
+  }
+}
+
+// adds each touched row's sum to its table, clears the wave; resets the NEXT wave's (idle) counters
+template <typename I>                              // element index: int below 2^31 elements
+__global__ void sgns_det_apply(float* w_in, float* w_out, int dim, int64_t ld, unsigned long long* acc_in,
+                               unsigned long long* acc_out, int* flag_in, int* flag_out, const int* list_in,
+                               const int* list_out, const int* count, int* next, unsigned long long* loss_acc,
+                               float* loss_sum) {
+  const I n_in = (I)count[0] * dim, n_all = n_in + (I)count[1] * dim;
+  for (I i = (I)blockIdx.x * blockDim.x + threadIdx.x; i < n_all; i += (I)gridDim.x * blockDim.x) {
+    const bool in = i < n_in;
+    const I k = in ? i : i - n_in;
+    const int r = (in ? list_in : list_out)[k / dim];
+    const int j = (int)(k - (k / dim) * dim);
+    unsigned long long* q = (in ? acc_in : acc_out) + (int64_t)r * dim + j;
+    const long long v = (long long)*q;
+    if (v) (in ? w_in : w_out)[(int64_t)r * ld + j] += (float)((double)v * (1.0 / (double)kFixScale));
+    *q = 0ull;
+    if (j == 0) (in ? flag_in : flag_out)[r] = 0;
+  }
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    next[0] = next[1] = 0;
+    if (loss_sum && *loss_acc) *loss_sum += (float)((double)(long long)*loss_acc * (1.0 / (double)kLossScale));
+    *loss_acc = 0ull;
+  }
+}
+
 }  // namespace
 
 // Centre positions the window-batched kernel keeps in flight on this device (every consumer warp owns
@@ -727,9 +919,8 @@ extern "C" int mvb_sgns_train_win(const MvbSgns* h, void* stream) {
   const int64_t by_len = (h->n_tokens + 63) / 64;
   if ((int64_t)blocks > by_len) blocks = (int)by_len;
   // One chunk per CTA by default (a static partition: every chunk boundary drains and refills the rings, and
-  // the measured imbalance between CTAs is smaller than that: 1M tokens on 148 SMs, chunks of 256 / 512 /
-  // 1024 tokens handed out by an atomic ticket ran at 103 / 106 / 107 M words/s against 110 with one chunk per
-  // CTA).  MVB_WIN_CHUNK=n deals n-token chunks round-robin instead.
+  // the imbalance between CTAs is smaller than that: on 1M-token blocks, chunks of 256 / 512 / 1024 tokens
+  // handed out by an atomic ticket ran slower than one chunk per CTA).  MVB_WIN_CHUNK=n deals n-token chunks round-robin instead.
   a.chunk = (int)((h->n_tokens + blocks - 1) / blocks);
   if (const char* e = getenv("MVB_WIN_CHUNK")) {
     const int v = atoi(e);
@@ -767,6 +958,79 @@ extern "C" int mvb_sgns_train_win(const MvbSgns* h, void* stream) {
   else MVB_DISPATCH_WIN(8);
 #undef MVB_DISPATCH_WIN
 #undef MVB_LAUNCH_WIN
+  MVB_CUDA_CHECK(cudaGetLastError());
+  return 0;
+}
+
+extern int mvb_sgns_launches;
+// Deterministic K7 on local tables or block caches; -20/-21: not covered (the caller falls back).
+extern "C" int mvb_sgns_train_det(const MvbSgns* h, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
+  if (h->n_tokens <= 0) return 0;
+  if (h->cbow || h->hs || h->use_adagrad || h->negative < 1 || h->negative > kKO - 1) return -20;
+  if (h->nservers > 1 || h->dim < 1 || h->dim > 512 || h->window < 1 || h->window > 15 || h->vocab <= 0) return -21;
+  mvb_sgns_launches = 0;
+  // rows are word ids or cache slots (< vocab).  Scratch (one stream): counters [4] | loss | acc [2 x rows x dim] |
+  // flags, lists [2 x rows]; grown on demand, cleared when its layout changes (a wave leaves it clear but for counters)
+  static unsigned char* buf = nullptr;
+  static int64_t cap = 0, last_elems = -1;
+  static int parity = 0;
+  const int64_t rows = h->vocab, elems = rows * h->dim, bytes = 16 + 8 + 2 * elems * 8 + 4 * rows * 4;
+  if (bytes > cap) {
+    MVB_CUDA_CHECK(cudaDeviceSynchronize());
+    if (buf) MVB_CUDA_CHECK(cudaFree(buf));
+    MVB_CUDA_CHECK(cudaMalloc(&buf, bytes));
+    cap = bytes;
+    last_elems = -1;
+  }
+  if (elems != last_elems) {
+    MVB_CUDA_CHECK(cudaMemsetAsync(buf, 0, bytes, st));
+    last_elems = elems;
+    parity = 0;
+  }
+  int* counters = reinterpret_cast<int*>(buf);
+  unsigned long long* loss_acc = reinterpret_cast<unsigned long long*>(buf + 16);
+  unsigned long long* acc = loss_acc + 1;
+  int* ints = reinterpret_cast<int*>(acc + 2 * elems);
+  DetDev a{};
+  a.tokens = h->tokens; a.n_tokens = h->n_tokens; a.w_in = h->w_in; a.w_out = h->w_out;
+  a.dim = h->dim; a.ld = h->ld; a.window = h->window; a.ko = 1 + h->negative; a.lr = h->lr;
+  a.alias_prob = h->alias_prob; a.alias_idx = h->alias_idx; a.vocab = h->vocab;
+  a.neg_pool = h->neg_pool; a.neg_pool_size = h->neg_pool_size; a.neg_pool_size_ptr = h->neg_pool_size_ptr;
+  a.map_in = h->map_in; a.map_out = h->map_out; a.scale_in = h->scale_in; a.scale_out = h->scale_out;
+  a.seed = h->seed; a.want_loss = h->loss_sum != nullptr; a.pair_count = h->pair_count;
+  a.acc[0] = acc; a.acc[1] = acc + elems;
+  a.flag[0] = ints; a.flag[1] = ints + rows;
+  a.list[0] = ints + 2 * rows; a.list[1] = ints + 3 * rows;
+  a.loss_acc = loss_acc;
+  int wave = mvb_sgns_win_inflight(h->dim, h->negative, h->window, h->max_ctas);
+  if (wave <= 0) wave = 2 * mvb_num_sms() * kNW;
+  const int det_blocks = (wave + 7) / 8;           // a warp per centre
+  const int apply_blocks = mvb_num_sms() * 4;
+  const int nj = (h->dim + 31) / 32;
+  for (int64_t p0 = 0; p0 < h->n_tokens; p0 += wave) {
+    a.p0 = p0;
+    a.p1 = p0 + wave < h->n_tokens ? p0 + wave : h->n_tokens;
+    a.count = counters + 2 * parity;
+#define MVB_LAUNCH_DET(NJ)                                                              \
+  case NJ:                                                                              \
+    if (a.ko <= 6) sgns_det_kernel<NJ, 6><<<det_blocks, 256, 0, st>>>(a);               \
+    else sgns_det_kernel<NJ, 8><<<det_blocks, 256, 0, st>>>(a);                         \
+    break;
+    switch (nj) {
+      MVB_LAUNCH_DET(1) MVB_LAUNCH_DET(2) MVB_LAUNCH_DET(3) MVB_LAUNCH_DET(4)
+      MVB_LAUNCH_DET(5) MVB_LAUNCH_DET(6) MVB_LAUNCH_DET(7) MVB_LAUNCH_DET(8)
+      MVB_LAUNCH_DET(9) MVB_LAUNCH_DET(10) MVB_LAUNCH_DET(11) MVB_LAUNCH_DET(12)
+      MVB_LAUNCH_DET(13) MVB_LAUNCH_DET(14) MVB_LAUNCH_DET(15) MVB_LAUNCH_DET(16)
+      default: return -21;
+    }
+#undef MVB_LAUNCH_DET
+    (elems < (1ll << 31) ? sgns_det_apply<int> : sgns_det_apply<int64_t>)<<<apply_blocks, 256, 0, st>>>(h->w_in, h->w_out, h->dim, h->ld, a.acc[0], a.acc[1], a.flag[0],
+                                                  a.flag[1], a.list[0], a.list[1], a.count,
+                                                  counters + 2 * (parity ^ 1), loss_acc, h->loss_sum);
+    parity ^= 1;
+    mvb_sgns_launches += 2;
+  }
   MVB_CUDA_CHECK(cudaGetLastError());
   return 0;
 }

@@ -1,4 +1,4 @@
-// logreg_gpu -- the LogisticRegression application on the B200 data plane, entirely native: C++
+// logreg_gpu -- the LogisticRegression application on the GPU data plane, entirely native: C++
 // driver, native sample readers (csrc/host/applib), K8 kernels (csrc/cuda/logreg.cu) through the
 // kernel library's C ABI, weights in a device ArrayTable (HBM shards; the server-side updater is
 // fused into the Add kernel). Same config file as build/bin/logreg (CPU) and

@@ -1,4 +1,4 @@
-// wordembedding_gpu -- the WordEmbedding application on the B200 data plane, entirely native:
+// wordembedding_gpu -- the WordEmbedding application on the GPU data plane, entirely native:
 // C++ driver, host data pipeline (csrc/host/applib), device tables through
 // multiverso::device (HBM shards, fused kernels over NVLink) and the K7 training kernel
 // (csrc/cuda/sgns*.cu) through the kernel library's C ABI. Same 21 flags and the same block

@@ -3,7 +3,7 @@
 //
 // It exports exactly the 17 entry points the reference's Python / Lua / C# bindings bind to, so
 // a binding that loads this library instead of libmultiverso.so gets tables that live in HBM and
-// Add / Get that are the fused sm_100a kernels; the host arrays of the caller are staged through
+// Add / Get that are the fused sm_90a kernels; the host arrays of the caller are staged through
 // the device (H2D before an Add, D2H after a Get). One process per GPU, started by any launcher
 // that sets MV_RANK / MV_SIZE / MV_PORT (tools/mvrun.py) or RANK / WORLD_SIZE / MASTER_PORT.
 //

@@ -2,7 +2,7 @@
 // Mirrors multiverso_b200/runtime.py (Zoo of the device plane: bootstrap, symmetric
 // allocations, signal pads, epochs, watchdog, FinishTrain drain) and tables/device.py (Dense /
 // Matrix / KV tables, staging double buffers, fused vs one-sided Adds) over the C ABI of the
-// sm_100a kernel library, csrc/cuda/mvb200.h.
+// sm_90a kernel library, csrc/cuda/mvb200.h.
 #include "vmm.h"
 #include "multiverso/device/device.h"
 

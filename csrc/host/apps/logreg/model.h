@@ -1,7 +1,7 @@
 // Model of the native LogisticRegression application (reference: Model / PSModel / Objective /
 // Regular / Updater, Applications/LogisticRegression/src/model/*.cpp, objective/objective.cpp,
 // regular/regular.cpp, updater/updater.cpp). CPU implementation on the host runtime; the
-// sm_100a implementation of the same maths is csrc/cuda/logreg.cu + multiverso_b200/models.
+// sm_90a implementation of the same maths is csrc/cuda/logreg.cu + multiverso_b200/models.
 //
 // Weights are W[out x dim], dim = input_size + 1 (the reader appends a constant-1 bias feature
 // with key input_size); key of (class c, feature k) = c * dim + k. Gradients are accumulated in

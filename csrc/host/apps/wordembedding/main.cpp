@@ -11,7 +11,7 @@
 //   python tools/mvrun.py -n 4 -- build/bin/wordembedding -train_file corpus.txt ... -sync=false
 //
 // The GPU implementation of the same application is multiverso_b200/apps/wordembedding.py
-// (sm_100a kernels, HBM-resident tables); this binary is the CPU plumbing mode.
+// (sm_90a kernels, HBM-resident tables); this binary is the CPU plumbing mode.
 #include <condition_variable>
 #include <cstdio>
 #include <cstring>

@@ -3,7 +3,7 @@
 // ParseSentence / Parse / TrainSample / FeedForward / BPOutputLayer,
 // Applications/WordEmbedding/src/wordembedding.cpp:17-283; Sampler, util.cpp:116-146).
 // This is the CPU implementation used by the native `wordembedding` binary on the host
-// runtime; the sm_100a kernels (csrc/cuda/sgns*.cu) are the device implementation of the
+// runtime; the sm_90a kernels (csrc/cuda/sgns*.cu) are the device implementation of the
 // same maths.
 #ifndef MVAPP_WORDEMBEDDING_TRAINER_H_
 #define MVAPP_WORDEMBEDDING_TRAINER_H_

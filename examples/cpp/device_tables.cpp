@@ -1,4 +1,4 @@
-// The same program on the GPUs: tables live in HBM, Add / Get are the fused sm_100a kernels,
+// The same program on the GPUs: tables live in HBM, Add / Get are the fused sm_90a kernels,
 // all pointers are device pointers (include/multiverso/device/device.h). One process per GPU.
 //
 //   g++ -std=c++17 -Iinclude examples/cpp/device_tables.cpp -o device_tables \

@@ -1,7 +1,7 @@
 /* C API of the native application support library (data pipelines of the two shipped
  * applications). Reference: Applications/WordEmbedding/src/{dictionary,reader,huffman_encoder,
  * util}.cpp and Applications/LogisticRegression/src/reader.cpp -- all native C++ there, native
- * C++ here; the Python app drivers (multiverso_b200/apps) feed the sm_100a kernels from it. */
+ * C++ here; the Python app drivers (multiverso_b200/apps) feed the sm_90a kernels from it. */
 #ifndef MULTIVERSO_APPS_APP_API_H_
 #define MULTIVERSO_APPS_APP_API_H_
 #include <stdint.h>

@@ -2,7 +2,7 @@
 //
 // The C++ counterpart of multiverso_b200/runtime.py + tables/device.py for programs that are
 // not Python: the same tables (Array / Matrix / KV), updaters, BSP / async modes and
-// MV_Aggregate, driven from C++ over the C ABI of the sm_100a kernel library
+// MV_Aggregate, driven from C++ over the C ABI of the sm_90a kernel library
 // (csrc/cuda/mvb200.h -> libmvb200.so). Nothing here needs torch or a CUDA header:
 //
 //   * bootstrap, roles, dense worker / server ids and the host barrier come from the C++ host

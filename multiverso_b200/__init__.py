@@ -1,4 +1,4 @@
-"""multiverso_b200 -- a Blackwell-native parameter-server engine with the capabilities of
+"""multiverso_b200 -- an H100-native (Hopper, sm_90a) parameter-server engine with the capabilities of
 Microsoft/multiverso (tables with Get/Add/GetAsync/AddAsync, server-side updaters, BSP /
 async / model-averaging modes, WordEmbedding and LogisticRegression applications)."""
 from .api import (aggregate, barrier, dashboard_display, init, is_master_worker, load_table, net_bind,

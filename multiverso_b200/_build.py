@@ -3,8 +3,8 @@
 Two artefacts, both built with explicit compiler invocations (no JIT cache, so the
 ``.so`` files travel with the repo snapshot to the GPU box):
 
-* ``multiverso_b200/_lib/libmvb200.so``      -- sm_100a data-plane kernels (nvcc,
-  ``-gencode arch=compute_100a,code=sm_100a -lineinfo``), sources ``csrc/cuda/*.cu``
+* ``multiverso_b200/_lib/libmvb200.so``      -- sm_90a data-plane kernels (nvcc,
+  ``-gencode arch=compute_90a,code=sm_90a -lineinfo``), sources ``csrc/cuda/*.cu``
 * ``multiverso_b200/_lib/libmultiverso.so``  -- C++17 host runtime + C API (g++),
   sources ``csrc/host/**/*.cpp``; plus the native tools/apps under ``build/bin``.
 
@@ -22,7 +22,7 @@ LIBDIR = Path(__file__).resolve().parent / "_lib"
 BUILD = ROOT / "build"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
 ]
 CXX_FLAGS = ["-O2", "-g", "-std=c++17", "-fPIC", "-Wall", "-pthread", "-fopenmp"]
@@ -50,7 +50,7 @@ def _find(tool, fallback):
 
 
 def build_cuda(verbose: bool = False) -> Path:
-    """Compile csrc/cuda/*.cu for sm_100a and link libmvb200.so."""
+    """Compile csrc/cuda/*.cu for sm_90a and link libmvb200.so."""
     nvcc = _find("nvcc", "/usr/local/cuda/bin/nvcc")
     out = LIBDIR / "libmvb200.so"
     srcs = sorted((ROOT / "csrc" / "cuda").glob("*.cu"))

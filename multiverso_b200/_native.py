@@ -1,6 +1,6 @@
 """ctypes bindings of the two native libraries.
 
-* :func:`cuda_lib` -> ``libmvb200.so`` (sm_100a kernels, ``csrc/cuda/mvb200.h``)
+* :func:`cuda_lib` -> ``libmvb200.so`` (sm_90a kernels, ``csrc/cuda/mvb200.h``)
 * :func:`host_lib` -> ``libmultiverso.so`` (C++ host runtime + C API, ``include/multiverso/c_api.h``)
 
 The CUDA library is mandatory whenever a GPU is present: ops raise instead of silently
@@ -159,7 +159,7 @@ def _ensure_built(name: str) -> Path:
 
 
 def cuda_lib():
-    """Load (building if needed) the sm_100a kernel library."""
+    """Load (building if needed) the sm_90a kernel library."""
     global _cuda
     if _cuda is None:
         lib = C.CDLL(str(_ensure_built("libmvb200.so")), mode=C.RTLD_GLOBAL)

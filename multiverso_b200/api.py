@@ -1,7 +1,7 @@
 """Public API: the reference's MV_* surface (include/multiverso/multiverso.h:9-65) and the
 Python binding's names (binding/python/multiverso/api.py:12-75).
 
-The same calls work on both backends: ``device`` (CUDA present: HBM tables + sm_100a
+The same calls work on both backends: ``device`` (CUDA present: HBM tables + sm_90a
 kernels) and ``host`` (no CUDA: the C++ runtime in libmultiverso.so, TCP control plane).
 """
 from __future__ import annotations

@@ -61,7 +61,7 @@ class LogRegConfig:
     objective_type: str = "default"
     regular_type: str = "default"
     show_time_per_sample: int = 10000
-    server_updater: str = "sgd"         # B200 addition: sgd | adagrad | momentum_sgd (server side)
+    server_updater: str = "sgd"         # addition: sgd | adagrad | momentum_sgd (server side)
     extra: Dict[str, str] = field(default_factory=dict)
 
     @classmethod
@@ -134,8 +134,8 @@ def dense_gemm_step(x: torch.Tensor, labels: torch.Tensor, w: torch.Tensor, grad
 
 
 def _tc_gemm_nt(x: torch.Tensor, w: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
-    """out[M, N] = x[M, K] @ w[N, K]^T on the hand-written tcgen05 kernel (gemm_fused.cu: TMA-fed
-    tcgen05.mma, CTA pairs, TF32 operands, fp32 accumulation in TMEM) -- `w` is presented as a one-server
+    """out[M, N] = x[M, K] @ w[N, K]^T on the hand-written wgmma kernel (gemm_fused.cu: TMA-fed
+    wgmma, TF32 operands, fp32 accumulation in registers) -- `w` is presented as a one-server
     row map, so the same kernel that streams table shards multiplies two local matrices.  K % 4 == 0."""
     M, K = x.shape
     Nr = w.shape[0]
@@ -242,7 +242,7 @@ class LogRegModel:
         n = labels.numel()
         wide = self.out >= GEMM_PATH_MIN_CLASSES or n * self.dim * self.out >= GEMM_PATH_MIN_WORK
         if wide and self.dim % 4 == 0 and x.is_cuda and os.environ.get("MVB_LR_TC", "1") != "0":
-            # GEMM-shaped minibatch: logits = X W^T and grad += E^T X both on the tcgen05 kernel (TF32 in,
+            # GEMM-shaped minibatch: logits = X W^T and grad += E^T X both on the wgmma kernel (TF32 in,
             # fp32 accumulate), softmax / loss / error in the hand-written epilogue between them; no
             # library GEMM anywhere (Objective::Predict + Gradient, objective.cpp:113-120, 202-218)
             lib, st = N.cuda_lib(), C.c_void_p(N.stream_ptr())

@@ -7,8 +7,8 @@ parameter-server glue is Communicator (src/communicator.cpp): two MatrixTables
 for the global word count, per data block RequestParameter -> train -> AddDeltaParameter
 with delta = (trained - server_now) / num_workers.
 
-B200 mapping
-------------
+Device mapping
+--------------
 * ``world == 1``: the shard *is* the table, so the block protocol degenerates exactly
   ((trained - cur)/1 added back == trained) and the K7 kernel trains in place on the HBM
   resident shards -- no gather, no scatter.
@@ -181,7 +181,7 @@ class WordEmbedding:
     def _build_hot_row_cap(self) -> None:
         """Per-word step scales for the window-batched K7.
 
-        The kernel keeps P centre positions in flight per device (148 CTAs x 10 warps x 2 stages),
+        The kernel keeps P centre positions in flight per device (one CTA per SM x 10 warps x 2 stages),
         i.e. ~P (W+1) (context, centre) samples whose rows were read before any of their updates
         landed.  The reference's Hogwild has <= `-threads` samples in flight; with ~18 000 the rows
         of the Zipf head collect hundreds of same-direction stale steps per staleness window and
@@ -257,7 +257,7 @@ class WordEmbedding:
             a.variant = 20
         a.scale_in, a.scale_out = N.ptr(self.scale_in), N.ptr(self.scale_out)
         N.check(N.cuda_lib().mvb_sgns_train(C.byref(a), C.c_void_p(N.stream_ptr())), "mvb_sgns_train")
-        self.kernel_launches += 1
+        self.kernel_launches += int(N.cuda_lib().mvb_sgns_last_launches())
 
     # ------------------------------------------------------------------ one data block
     def train_block(self, tokens: torch.Tensor, compute_loss: bool = True,

@@ -2,10 +2,8 @@
 
 The pulled row block is never materialised: a persistent, warp-specialised kernel streams each
 W tile from its owner (local or peer HBM over NVLink) with TMA into shared memory and multiplies
-it with tcgen05.mma (CTA pairs, cta_group::2, TF32 operands, fp32 accumulation in TMEM) against
-the local activations; remote tiles are staged once in an L2-resident scratch, so W crosses NVLink
-once whatever M is.  Knobs (env): MVB_GEMM_CTAS=1 single-CTA MMAs, MVB_GEMM_XC=1|2 accumulators per
-work item, MVB_GEMM_WCACHE=0 no scratch staging, MVB_GEMM_PROF=1 in-kernel wait-cycle counters.
+it with Hopper warp-group MMAs (wgmma, TF32 operands, fp32 accumulation in registers) against
+the local activations.
 Reference analogue: MatrixWorkerTable::Get followed by the application's first GEMM
 (e.g. LogReg Objective::Predict, Applications/LogisticRegression/src/objective/objective.cpp:113-120).
 """
@@ -19,7 +17,7 @@ from .. import _native as N
 
 
 def get_gemm_supported() -> bool:
-    """True when the fused tcgen05 kernel can run here (sm_100a device present)."""
+    """True when the fused wgmma kernel can run here (sm_90a device present)."""
     if not torch.cuda.is_available():
         return False
     return bool(N.cuda_lib().mvb_get_gemm_supported())

@@ -1,4 +1,4 @@
-"""The Zoo of the B200 runtime: one process per GPU, every rank worker + server.
+"""The Zoo of the device runtime: one process per GPU, every rank worker + server.
 
 Reference: Zoo (src/zoo.cpp:41-186) parses flags, initialises the net, decides the role
 from ``-ps_role``, starts the controller / communicator / server / worker actors and

@@ -6,7 +6,7 @@ MatrixServerTable (src/table/matrix_table.cpp), MatrixWorker/MatrixServer with s
 delta-pull (src/table/matrix.cpp), SparseMatrixTable (src/table/sparse_matrix_table.cpp),
 KVWorkerTable/KVServerTable (include/multiverso/table/kv_table.h).
 
-B200 design: every rank holds its shard (and updater state) in a symmetric, peer-mapped
+Device design: every rank holds its shard (and updater state) in a symmetric, peer-mapped
 HBM slab.  There is no worker half / server half exchanging messages:
 
 * ``add`` (whole table, BSP or stateful):  K1 ``mvb_add_dense_fused`` -- the owner pulls its

@@ -23,7 +23,7 @@ _DEFAULTS: Dict[str, Any] = {
     "logtostderr": False,
     # include/multiverso/net/zmq_net.h:20-21
     "machine_file": "", "port": 55555,
-    # --- B200 additions -------------------------------------------------------------------
+    # --- device additions -------------------------------------------------------------------
     "barrier_timeout_s": 120.0,   # watchdog on device-side spins (SURVEY 5.3)
     "request_stall_warn_s": 60.0,  # host backend: log a line whenever a table request has waited this long
     "kv_capacity": 1 << 20,       # slots per KV shard

@@ -235,7 +235,7 @@ def scenario_async():
     from multiverso_b200.parallel import aggregate as _agg
     _agg(z, algo="nvls")
     check("aggregate_nvls_or_fallback", torch.equal(z, torch.full((5_000_000,), W * (W + 1) / 2.0, device="cuda")))
-    # fused Get+GEMM with the W tiles streamed from peer shards by TMA (tcgen05 / TMEM)
+    # fused Get+GEMM with the W tiles streamed from peer shards by TMA (wgmma)
     from multiverso_b200.ops import get_gemm
     wt = mv.MatrixTable(1000, 256, "float32", min_value=-1.0, max_value=1.0, seed=3)
     mv.barrier()

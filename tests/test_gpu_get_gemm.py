@@ -1,4 +1,4 @@
-"""tcgen05 / TMEM / TMA fused Get+GEMM against a plain PyTorch fp32 reference (TF32 operands:
+"""wgmma / TMA fused Get+GEMM against a plain PyTorch fp32 reference (TF32 operands:
 10-bit mantissa, so the tolerance is relative to |x||w| sqrt(K))."""
 import pytest
 import torch

@@ -1,5 +1,5 @@
 """K8 numerics against plain PyTorch references: the sparse / dense CUDA-core kernels, FTRL, regularisers
-(csrc/cuda/logreg.cu) and the wide dense path whose two products run on the hand-written tcgen05 kernel
+(csrc/cuda/logreg.cu) and the wide dense path whose two products run on the hand-written wgmma kernel
 (no library GEMM), each compared with fp32/fp64 torch on the same inputs."""
 import ctypes as C
 
