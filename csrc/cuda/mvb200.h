@@ -446,6 +446,27 @@ int mvb_get_gemm_fused(const MvbGetGemm* g, void* stream);
 int mvb_get_gemm_supported(void);
 int mvb_get_gemm_last_config(void);  /* ctas*1000 + grid of the last launch */
 
+/* ---- fused cosine top-k over a row-sharded MatrixTable (TMA + tf32 wgmma, top-k epilogue) ---- */
+/* For each query row: the k rows of [0, n_rows) with the largest cosine over the first dim columns,
+ * sorted by score descending, ties by the smaller id; zero rows score 0; missing slots get id -1 and
+ * score -inf. tf32 selects k + 8 candidates, their cosines are recomputed in fp64 from the rows. W is
+ * read from its owners' shards like mvb_get_gemm_fused (no collective). MVB_TOPK_MAX: k + 8 sorted
+ * candidates per query next to the candidate buffer in the 227 KB of shared memory. */
+#define MVB_TOPK_MAX 64
+typedef struct MvbTopkCos {
+  const float* q;            /* [M x ldq] fp32, ldq % 4 == 0, columns >= dim unused    */
+  int64_t M, ldq;            /* M <= 65535 per call                                    */
+  int64_t dim, n_rows;       /* columns compared (<= wmap.num_col); rows searched      */
+  MvbRowMap wmap;            /* the table's shards, row pitch wmap.num_col (% 4 == 0)  */
+  int k;                     /* 1 <= k <= MVB_TOPK_MAX                                 */
+  float* scores;             /* [M x k] out                                            */
+  int64_t* ids;              /* [M x k] out                                            */
+  void* scratch;             /* device, mvb_topk_cos_scratch_bytes(M, k, n_rows) bytes */
+  int64_t scratch_bytes;
+} MvbTopkCos;
+int64_t mvb_topk_cos_scratch_bytes(int64_t M, int k, int64_t n_rows);
+int mvb_topk_cosine(const MvbTopkCos* a, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

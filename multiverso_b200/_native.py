@@ -138,6 +138,11 @@ class GetGemm(C.Structure):
                 ("wmap", RowMap), ("local_server", C.c_int)]
 
 
+class TopkCos(C.Structure):
+    _fields_ = [("q", vp), ("M", i64), ("ldq", i64), ("dim", i64), ("n_rows", i64), ("wmap", RowMap),
+                ("k", C.c_int), ("scores", vp), ("ids", vp), ("scratch", vp), ("scratch_bytes", i64)]
+
+
 class NativeError(RuntimeError):
     pass
 

@@ -530,6 +530,31 @@ class WordEmbedding:
         self.flush()
         return self.input_table.get().view(self.V, self.LD)[:, :self.D]
 
+    def _input_rows(self, ids: torch.Tensor) -> torch.Tensor:
+        return self.input_table.get_rows(ids)[:, :self.D]
+
+    def most_similar(self, word_ids, k: int = 10, rows: Optional[int] = None):
+        """Nearest input-embedding rows by cosine (word2vec's ``distance``) of each word in ``word_ids``,
+        the word itself excluded; only rows [0, ``rows``) are searched. Returns (scores [n, k], ids [n, k]).
+        Searches the live table through its shards (fused top-k kernel), nothing is pulled whole."""
+        from ..ops.topk import check_k, take_excluding, topk_cosine
+        k = check_k(k, 1, "most_similar")
+        self.flush()
+        ids = torch.as_tensor(word_ids, dtype=torch.int64).to(self.dev).view(-1)
+        s, i = topk_cosine(self.input_table, self._input_rows(ids), k + 1, rows)
+        return take_excluding(s, i, ids[:, None], k)
+
+    def analogy(self, a, b, c, k: int = 1, rows: Optional[int] = None):
+        """3CosAdd (word2vec's ``word-analogy``): the rows nearest to unit(b) - unit(a) + unit(c), with a, b
+        and c excluded, for equally long id lists a, b, c. Returns (scores [n, k], ids [n, k])."""
+        from ..ops.topk import analogy_queries, check_k, take_excluding, topk_cosine
+        k = check_k(k, 3, "analogy")
+        self.flush()
+        abc = [torch.as_tensor(x, dtype=torch.int64).to(self.dev).view(-1) for x in (a, b, c)]
+        q = analogy_queries(*(self._input_rows(x) for x in abc))
+        s, i = topk_cosine(self.input_table, q, k + 3, rows)
+        return take_excluding(s, i, torch.stack(abc, 1), k)
+
     def save_embedding(self, path: str, words=None, binary: bool = False) -> None:
         """word2vec text / binary format (distributed_wordembedding.cpp:263-325); rank 0 only."""
         self.flush()
