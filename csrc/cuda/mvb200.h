@@ -467,6 +467,45 @@ typedef struct MvbTopkCos {
 int64_t mvb_topk_cos_scratch_bytes(int64_t M, int k, int64_t n_rows);
 int mvb_topk_cosine(const MvbTopkCos* a, void* stream);
 
+/* ---- embedding bag over a row-sharded fp32 MatrixTable (emb_bag.cu) ---------------------------- */
+/* Bag b holds the lookups [offsets[b], offsets[b + 1]) (the last bag ends at L); its output row is the sum
+ * (mean: the sum over the bag length) of psw_j * W[ids_j, :dim]; an empty bag gives zeros. Rows are read
+ * from their owners' shards through wmap, as mvb_get_rows does. Results are bitwise reproducible and the
+ * same for every sharding of the table. The caller validates ids (in [0, num_row)) and offsets. */
+enum { MVB_EMB_PUSH = 0, MVB_EMB_COMPACT = 1 };
+typedef struct MvbEmbBag {
+  MvbRowMap wmap;            /* fp32 shards, row pitch wmap.num_col (% 4 == 0)                         */
+  int64_t dim;               /* columns used, 1 <= dim <= wmap.num_col; padding columns are never read  */
+  const int64_t* ids;        /* [L]; backward: sorted ascending, equal ids in ascending position        */
+  int64_t L;
+  const int64_t* offsets;    /* [B]: offsets[0] == 0, non-decreasing, <= L                              */
+  int64_t B;
+  const float* psw;          /* [L] per-sample weights by lookup position, or NULL                      */
+  int mean;                  /* 0 sum, 1 mean                                                           */
+  float* out;                /* forward: [B x ldo], ldo % 4 == 0, 16-byte aligned                       */
+  int64_t ldo;
+  const float* dout;         /* backward, psw grad: [B x ldd], ldd % 4 == 0, >= round4(dim) columns     */
+  int64_t ldd;
+  const int64_t* perm;       /* backward: lookup position of each sorted id                             */
+  int epilogue;              /* MVB_EMB_PUSH: red.add of scale * g into the owner's row (default / sgd);
+                                MVB_EMB_COMPACT: grads[u] = scale * g, uniq[u] = id, ids ascending      */
+  float scale;
+  float* grads;              /* compact: [U x ldg] (ldg % 4 == 0); NULL: only write *n_unique           */
+  int64_t ldg;
+  int64_t* uniq;             /* compact: [U]                                                            */
+  int64_t* n_unique;         /* backward: device int64, the number of unique ids U, or NULL             */
+  float* dpsw;               /* psw grad: [L]                                                           */
+  void* scratch;             /* backward: mvb_embedding_bag_scratch_bytes(L, dim) bytes of device memory */
+  int64_t scratch_bytes;
+} MvbEmbBag;
+int mvb_embedding_bag_fwd(const MvbEmbBag* a, void* stream);
+int64_t mvb_embedding_bag_scratch_bytes(int64_t L, int64_t dim);
+/* sum of psw_j * s_bag * dout[bag(j)] per run of equal ids, in ascending position (s_bag = 1, or 1 / bag
+ * length for mean), then the epilogue once per unique id */
+int mvb_embedding_bag_bwd(const MvbEmbBag* a, void* stream);
+/* dpsw[j] = s_bag * <dout[bag(j)], W[ids_j, :dim]> (ids in lookup order) */
+int mvb_embedding_bag_psw_grad(const MvbEmbBag* a, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -143,6 +143,16 @@ class TopkCos(C.Structure):
                 ("k", C.c_int), ("scores", vp), ("ids", vp), ("scratch", vp), ("scratch_bytes", i64)]
 
 
+EMB_PUSH, EMB_COMPACT = 0, 1
+
+
+class EmbBag(C.Structure):
+    _fields_ = [("wmap", RowMap), ("dim", i64), ("ids", vp), ("L", i64), ("offsets", vp), ("B", i64),
+                ("psw", vp), ("mean", C.c_int), ("out", vp), ("ldo", i64), ("dout", vp), ("ldd", i64),
+                ("perm", vp), ("epilogue", C.c_int), ("scale", C.c_float), ("grads", vp), ("ldg", i64),
+                ("uniq", vp), ("n_unique", vp), ("dpsw", vp), ("scratch", vp), ("scratch_bytes", i64)]
+
+
 class NativeError(RuntimeError):
     pass
 

@@ -92,21 +92,21 @@ def topk_cosine_reference(weights: torch.Tensor, queries: torch.Tensor, k: int,
     return best_s, best_i
 
 
-def _rowmap_of(table) -> Tuple[N.RowMap, int, int]:
-    """(row map, rows, row pitch) of a MatrixDeviceTable or of a 2-D fp32 CUDA tensor (one local shard)."""
+def _rowmap_of(table, what: str = "topk_cosine") -> Tuple[N.RowMap, int, int]:
+    """(row map, rows, row width) of a MatrixDeviceTable or of a 2-D fp32 CUDA tensor (one local shard)."""
     rm = N.RowMap()
     if isinstance(table, torch.Tensor):
         if table.dtype != torch.float32 or table.dim() != 2 or not table.is_cuda:
-            raise TypeError(f"topk_cosine: a table tensor must be 2-D float32 on CUDA, got {table.dtype} "
+            raise TypeError(f"{what}: a table tensor must be 2-D float32 on CUDA, got {table.dtype} "
                             f"{tuple(table.shape)} on {table.device}")
         if table.stride(1) != 1:
-            raise ValueError("topk_cosine: table rows must be contiguous")
+            raise ValueError(f"{what}: table rows must be contiguous")
         rm.num_row, rm.num_col = table.shape[0], table.stride(0) if table.shape[0] > 1 else table.shape[1]
         rm.nservers, rm.rows_per_server = 1, max(table.shape[0], 1)
         rm.shard_ptrs[0] = table.data_ptr()
         return rm, table.shape[0], table.shape[1]
     if getattr(table, "dtype", None) != torch.float32:
-        raise TypeError("topk_cosine: the table must be float32")
+        raise TypeError(f"{what}: the table must be float32")
     src = table._rowmap
     rm.num_row, rm.num_col, rm.nservers, rm.rows_per_server = src.num_row, src.num_col, src.nservers, src.rows_per_server
     for s in range(src.nservers):
