@@ -8,8 +8,6 @@
 kernel is measured against this on the same box and shapes (bench/matrix_bw.py)."""
 from __future__ import annotations
 
-import ctypes as C
-
 import torch
 import torch.distributed as dist
 
@@ -34,10 +32,8 @@ class NcclDenseTable:
             src = self.recv
         else:
             src = delta
-        N.check(N.cuda_lib().mvb_updater_apply(N.F32, self.updater, C.c_void_p(self.shard.data_ptr()),
-                                               C.c_void_p(src.data_ptr()), C.c_void_p(self.state.data_ptr()), None,
-                                               C.c_int64(self.shard_len), C.byref(self.opt), C.c_float(1.0),
-                                               C.c_void_p(N.stream_ptr())), "mvb_updater_apply")
+        N.cuda_lib().mvb_updater_apply(N.F32, self.updater, self.shard, src, self.state, None, self.shard_len, self.opt,
+                                       1.0, N.stream_ptr())
 
     def get(self, out: torch.Tensor) -> torch.Tensor:
         if self.world > 1:

@@ -12,6 +12,8 @@ import ctypes as C
 import os
 from pathlib import Path
 
+import torch
+
 MAX_RANKS = 8
 PAD_CHANNELS = 64
 PAD_WORDS = PAD_CHANNELS * MAX_RANKS
@@ -157,6 +159,120 @@ class NativeError(RuntimeError):
     pass
 
 
+class Ptr:
+    """ctypes parameter type of a data pointer: a torch tensor (its ``data_ptr()``), an int address, or
+    None for NULL. A ``c_void_p`` passes through unchanged, so callers that still wrap pointers by hand keep
+    working. Anything else raises TypeError instead of reaching the kernel as a wrong value."""
+
+    @classmethod
+    def from_param(cls, obj):
+        if isinstance(obj, torch.Tensor):
+            return C.c_void_p(obj.data_ptr())
+        if isinstance(obj, int) or obj is None:
+            return C.c_void_p(obj)
+        if isinstance(obj, C.c_void_p):
+            return obj
+        raise TypeError(f"expected a tensor, an int address, a c_void_p or None, got {type(obj).__name__}")
+
+
+def _raise_on_error(rc, func, args):
+    check(rc, func.__name__)
+    return rc
+
+
+def _status(*argtypes):
+    """Returns 0 or an error code; an error raises NativeError with mvb_last_error()."""
+    return C.c_int, argtypes, _raise_on_error
+
+
+def _unchecked(restype, *argtypes):
+    return restype, argtypes, None
+
+
+# The entry points of csrc/cuda/mvb200.h that Python calls (tests/test_native_abi_cpu.py checks them
+# against the header). Struct parameters take the struct itself, void* const* / void** a c_void_p array or
+# instance, and the host int64_t arrays of the dense push a c_int64 array.
+i32, u32, u64, f32, f64 = C.c_int, C.c_uint32, C.c_uint64, C.c_float, C.c_double
+vpp, i64p = C.POINTER(vp), C.POINTER(i64)
+_CUDA_FUNCS = {
+    "mvb_last_error": _unchecked(C.c_char_p),
+    "mvb_set_device": _status(i32),
+    "mvb_symm_alloc": _status(i64, vpp),
+    "mvb_ipc_get_handle": _status(Ptr, Ptr),
+    "mvb_ipc_open_handle": _status(Ptr, vpp),
+    # teardown: a failure must not stop the release of the remaining slabs
+    "mvb_symm_free": _unchecked(i32, Ptr),
+    "mvb_ipc_close_handle": _unchecked(i32, Ptr),
+    "mvb_signal": _status(vpp, i32, i32, i32, u64, Ptr),
+    "mvb_wait": _status(vpp, i32, i32, i32, u64, u32, Ptr, f64, Ptr),
+    "mvb_barrier": _status(vpp, i32, i32, i32, u64, Ptr, f64, Ptr),
+    "mvb_add_dense_fused": _status(C.POINTER(DenseAdd), Ptr),
+    "mvb_updater_apply": _status(i32, i32, Ptr, Ptr, Ptr, Ptr, i64, C.POINTER(AddOpt), f32, Ptr),
+    "mvb_get_dense": _status(C.POINTER(DenseGet), Ptr),
+    "mvb_push_dense_red": _status(i32, Ptr, i32, vpp, i64p, i64p, f32, Ptr),
+    "mvb_push_dense_stateful": _status(i32, i32, Ptr, i32, vpp, vpp, vpp, i64p, i64p, i64p, C.POINTER(AddOpt), i32,
+                                       Ptr),
+    "mvb_get_rows": _status(i32, C.POINTER(RowMap), Ptr, i64, Ptr, i64, Ptr),
+    "mvb_add_rows_red": _status(i32, C.POINTER(RowMap), Ptr, i64, Ptr, i64, f32, Ptr),
+    "mvb_add_rows_delta": _status(C.POINTER(RowMap), Ptr, i64, Ptr, Ptr, i64, f32, Ptr),
+    "mvb_add_rows_owner": _status(i32, i32, Ptr, Ptr, Ptr, i64, i64, i64, i64, Ptr, i64, Ptr, i64, C.POINTER(AddOpt),
+                                  Ptr),
+    "mvb_row_nonzero_mask": _status(i32, Ptr, i64, i64, i64, Ptr, Ptr),
+    "mvb_stale_mark": _status(Ptr, i64, i32, Ptr, i64, Ptr),
+    "mvb_stale_take": _status(Ptr, i64, Ptr, i64, Ptr, Ptr),
+    "mvb_kv_init": _status(Ptr, i64, Ptr),
+    "mvb_kv_count": _status(Ptr, i64, Ptr, Ptr),
+    "mvb_kv_rehash": _status(i32, Ptr, Ptr, i64, Ptr, Ptr, i64, Ptr, Ptr),
+    "mvb_kv_add": _status(C.POINTER(KV), Ptr, Ptr, i64, Ptr, Ptr),
+    "mvb_kv_get": _status(C.POINTER(KV), Ptr, Ptr, i64, Ptr),
+    "mvb_kv_dump": _status(i32, Ptr, Ptr, i64, Ptr, Ptr, Ptr, Ptr),
+    "mvb_allreduce_oneshot": _status(C.POINTER(Allreduce), Ptr),
+    "mvb_allreduce_twoshot": _status(C.POINTER(Allreduce), Ptr),
+    "mvb_allreduce_fused": _status(C.POINTER(Allreduce), Ptr, i64, Ptr),
+    "mvb_allreduce_nvls": _status(C.POINTER(Allreduce), Ptr, Ptr),
+    "mvb_sgns_train": _status(C.POINTER(Sgns), Ptr),
+    "mvb_sgns_train_win": _status(C.POINTER(Sgns), Ptr),
+    "mvb_sgns_train_det": _status(C.POINTER(Sgns), Ptr),
+    "mvb_sgns_last_launches": _unchecked(i32),
+    "mvb_sgns_win_inflight": _unchecked(i32, i32, i32, i32, i32),
+    "mvb_keys_add": _status(C.POINTER(KeyMap), Ptr, Ptr, i64, f32, Ptr),
+    "mvb_keys_get": _status(C.POINTER(KeyMap), Ptr, Ptr, i64, Ptr),
+    "mvb_keys_collect": _status(C.POINTER(KeyMap), Ptr, Ptr, Ptr, i64, Ptr),
+    "mvb_stale_on_add": _status(vpp, i32, Ptr, Ptr, Ptr, i32, Ptr),
+    "mvb_stale_on_get": _status(vpp, i32, Ptr, Ptr, Ptr),
+    "mvb_rowbox_slot_bytes": _unchecked(i64, i64, i64),
+    "mvb_rowbox_slots": _unchecked(i32),
+    "mvb_rowbox_push_delta": _status(C.POINTER(RowBox), Ptr, Ptr, i64, Ptr, Ptr, i64, f32, u64, C.POINTER(AddOpt), i32,
+                                     Ptr),
+    "mvb_rowbox_push_vals": _status(C.POINTER(RowBox), Ptr, Ptr, i64, Ptr, i64, f32, u64, C.POINTER(AddOpt), i32, Ptr),
+    "mvb_rowbox_poll": _status(C.POINTER(RowBox), i32, i32, Ptr),
+    "mvb_rowbox_apply": _status(C.POINTER(RowBox), i32, Ptr, Ptr, Ptr, i64, i64, i32, i32, Ptr),
+    "mvb_we_prepare": _status(C.POINTER(WePrep), Ptr),
+    "mvb_we_prepare_launches": _unchecked(i32, i32),
+    "mvb_rows_pull_bulk": _status(C.POINTER(RowMap), i32, Ptr, Ptr, i64, Ptr, Ptr, i64, i32, Ptr),
+    "mvb_rows_push_delta_bulk": _status(C.POINTER(RowMap), Ptr, Ptr, i64, Ptr, Ptr, i64, f32, i32, Ptr),
+    "mvb_build_alias_table": _status(Ptr, i32, Ptr, Ptr),
+    "mvb_lr_sparse_fwd_bwd": _status(C.POINTER(LrSparse), Ptr),
+    "mvb_lr_dense_fwd_bwd": _status(C.POINTER(LrDense), Ptr),
+    "mvb_lr_wide_epilogue": _status(Ptr, Ptr, i64, i32, i32, Ptr, i64, Ptr, Ptr, Ptr, Ptr),
+    "mvb_transpose_pad_f32": _status(Ptr, i64, i64, i64, Ptr, i64, Ptr),
+    "mvb_axpy_f32": _status(Ptr, Ptr, i64, f32, Ptr),
+    "mvb_ftrl_weights": _status(Ptr, Ptr, Ptr, i64, f32, f32, f32, f32, Ptr),
+    "mvb_ftrl_update": _status(Ptr, Ptr, Ptr, Ptr, i64, f32, Ptr),
+    "mvb_ftrl_delta": _status(Ptr, Ptr, Ptr, Ptr, Ptr, i64, f32, Ptr),
+    "mvb_regularize": _status(Ptr, Ptr, i64, i32, f32, Ptr),
+    "mvb_get_gemm_fused": _status(C.POINTER(GetGemm), Ptr),
+    "mvb_get_gemm_supported": _unchecked(i32),
+    "mvb_get_gemm_last_config": _unchecked(i32),
+    "mvb_topk_cos_scratch_bytes": _unchecked(i64, i64, i32, i64),
+    "mvb_topk_cosine": _status(C.POINTER(TopkCos), Ptr),
+    "mvb_embedding_bag_scratch_bytes": _unchecked(i64, i64, i64),
+    "mvb_embedding_bag_fwd": _status(C.POINTER(EmbBag), Ptr),
+    "mvb_embedding_bag_bwd": _status(C.POINTER(EmbBag), Ptr),
+    "mvb_embedding_bag_psw_grad": _status(C.POINTER(EmbBag), Ptr),
+}
+
+
 def _ensure_built(name: str) -> Path:
     path = _LIBDIR / name
     if os.environ.get("MVB200_NO_BUILD") == "1" and path.exists():
@@ -178,7 +294,11 @@ def cuda_lib():
     global _cuda
     if _cuda is None:
         lib = C.CDLL(str(_ensure_built("libmvb200.so")), mode=C.RTLD_GLOBAL)
-        lib.mvb_last_error.restype = C.c_char_p
+        for name, (restype, argtypes, errcheck) in _CUDA_FUNCS.items():
+            f = getattr(lib, name)
+            f.restype, f.argtypes = restype, argtypes
+            if errcheck is not None:
+                f.errcheck = errcheck
         _cuda = lib
     return _cuda
 
@@ -192,6 +312,8 @@ def host_lib():
 
 
 def check(rc: int, what: str = ""):
+    """Raise NativeError for a non-zero status. The declared status functions already raise on their own;
+    this serves code that checks a status by hand."""
     if rc != 0:
         msg = cuda_lib().mvb_last_error()
         raise NativeError(f"{what or 'mvb200 call'} failed rc={rc}: {msg.decode() if msg else ''}")
@@ -203,11 +325,9 @@ def ptr(t) -> int:
 
 
 def stream_ptr() -> int:
-    import torch
     return torch.cuda.current_stream().cuda_stream
 
 
 def dtype_code(torch_dtype) -> int:
-    import torch
     return {torch.float32: F32, torch.float64: F64, torch.int32: I32, torch.int64: I64,
             torch.int8: I8}[torch_dtype]

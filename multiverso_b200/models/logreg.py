@@ -15,7 +15,6 @@ regular/regular.cpp, updater/updater.cpp) -- with the hot loops on the GPU:
 """
 from __future__ import annotations
 
-import ctypes as C
 import os
 from dataclasses import dataclass, field
 from typing import Dict, Optional
@@ -145,7 +144,7 @@ def _tc_gemm_nt(x: torch.Tensor, w: torch.Tensor, out: torch.Tensor) -> torch.Te
     g.wmap.num_row, g.wmap.num_col, g.wmap.nservers, g.wmap.rows_per_server = Nr, K, 1, Nr
     g.wmap.shard_ptrs[0] = w.data_ptr()
     g.local_server = 0
-    N.check(N.cuda_lib().mvb_get_gemm_fused(C.byref(g), C.c_void_p(N.stream_ptr())), "mvb_get_gemm_fused")
+    N.cuda_lib().mvb_get_gemm_fused(g, N.stream_ptr())
     return out
 
 
@@ -219,10 +218,8 @@ class LogRegModel:
     def _weights(self) -> torch.Tensor:
         if self.ftrl:
             c = self.cfg
-            N.check(N.cuda_lib().mvb_ftrl_weights(C.c_void_p(self.z.data_ptr()), C.c_void_p(self.nacc.data_ptr()),
-                                                  C.c_void_p(self.w.data_ptr()), C.c_int64(self.n_w),
-                                                  C.c_float(c.alpha), C.c_float(c.beta), C.c_float(c.lambda1),
-                                                  C.c_float(c.lambda2), C.c_void_p(N.stream_ptr())), "mvb_ftrl_weights")
+            N.cuda_lib().mvb_ftrl_weights(self.z, self.nacc, self.w, self.n_w, c.alpha, c.beta, c.lambda1, c.lambda2,
+                                          N.stream_ptr())
             self.kernel_launches += 1
         return self.w
 
@@ -235,7 +232,7 @@ class LogRegModel:
         a.objective, a.w, a.dim, a.out = self.objective, self._weights().data_ptr(), self.dim, self.out
         a.grad, a.loss_sum, a.correct = self.grad.data_ptr(), self.loss.data_ptr(), self.correct.data_ptr()
         a.pred, a.err, a.compute_grad = N.ptr(pred), self._err.data_ptr(), int(train)
-        N.check(N.cuda_lib().mvb_lr_sparse_fwd_bwd(C.byref(a), C.c_void_p(N.stream_ptr())), "mvb_lr_sparse_fwd_bwd")
+        N.cuda_lib().mvb_lr_sparse_fwd_bwd(a, N.stream_ptr())
         self.kernel_launches += 1
 
     def forward_backward_dense(self, x, labels, train=True, pred=None):
@@ -245,27 +242,22 @@ class LogRegModel:
             # GEMM-shaped minibatch: logits = X W^T and grad += E^T X both on the wgmma kernel (TF32 in,
             # fp32 accumulate), softmax / loss / error in the hand-written epilogue between them; no
             # library GEMM anywhere (Objective::Predict + Gradient, objective.cpp:113-120, 202-218)
-            lib, st = N.cuda_lib(), C.c_void_p(N.stream_ptr())
+            lib, st = N.cuda_lib(), N.stream_ptr()
             dev = x.device
             x2 = x.view(n, self.dim)
             n_pad = (n + 3) // 4 * 4
             logits = torch.empty(n, self.out, device=dev)
             _tc_gemm_nt(x2, self._weights().view(self.out, self.dim), logits)
             err_t = torch.empty(self.out, n_pad, device=dev)
-            N.check(lib.mvb_lr_wide_epilogue(C.c_void_p(logits.data_ptr()), C.c_void_p(labels.data_ptr()), C.c_int64(n),
-                                             C.c_int(self.out), C.c_int(self.objective), C.c_void_p(err_t.data_ptr()),
-                                             C.c_int64(n_pad), C.c_void_p(N.ptr(pred)), C.c_void_p(self.loss.data_ptr()),
-                                             C.c_void_p(self.correct.data_ptr()), st), "mvb_lr_wide_epilogue")
+            lib.mvb_lr_wide_epilogue(logits, labels, n, self.out, self.objective, err_t, n_pad, pred, self.loss,
+                                     self.correct, st)
             self.kernel_launches += 2
             if train:
                 x_t = torch.empty(self.dim, n_pad, device=dev)
-                N.check(lib.mvb_transpose_pad_f32(C.c_void_p(x2.data_ptr()), C.c_int64(n), C.c_int64(self.dim),
-                                                  C.c_int64(self.dim), C.c_void_p(x_t.data_ptr()), C.c_int64(n_pad), st),
-                        "mvb_transpose_pad_f32")
+                lib.mvb_transpose_pad_f32(x2, n, self.dim, self.dim, x_t, n_pad, st)
                 dw = torch.empty(self.out, self.dim, device=dev)
                 _tc_gemm_nt(err_t, x_t, dw)                      # [out x n] . [dim x n]^T
-                N.check(lib.mvb_axpy_f32(C.c_void_p(self.grad.data_ptr()), C.c_void_p(dw.data_ptr()),
-                                         C.c_int64(self.out * self.dim), C.c_float(1.0), st), "mvb_axpy_f32")
+                lib.mvb_axpy_f32(self.grad, dw, self.out * self.dim, 1.0, st)
                 self.kernel_launches += 3
             return
         if wide:
@@ -283,31 +275,25 @@ class LogRegModel:
         a.objective, a.w = self.objective, self._weights().data_ptr()
         a.grad, a.loss_sum, a.correct = self.grad.data_ptr(), self.loss.data_ptr(), self.correct.data_ptr()
         a.pred, a.err, a.compute_grad = N.ptr(pred), self._err.data_ptr(), int(train)
-        N.check(N.cuda_lib().mvb_lr_dense_fwd_bwd(C.byref(a), C.c_void_p(N.stream_ptr())), "mvb_lr_dense_fwd_bwd")
+        N.cuda_lib().mvb_lr_dense_fwd_bwd(a, N.stream_ptr())
         self.kernel_launches += 2 if train else 1
 
     def apply_gradient(self, n_samples: int) -> None:
         """Regularise, scale by the learning rate and update (local) or push (PS); then the
         SGD learning-rate schedule lr = max(1e-3, lr0 - t/(coef*minibatch)) (updater.cpp:44-71)."""
-        cfg, lib, st = self.cfg, N.cuda_lib(), C.c_void_p(N.stream_ptr())
+        cfg, lib, st = self.cfg, N.cuda_lib(), N.stream_ptr()
         if self.regular and not self.ftrl:
-            N.check(lib.mvb_regularize(C.c_void_p(self.grad.data_ptr()), C.c_void_p(self.w.data_ptr()),
-                                       C.c_int64(self.n_w), self.regular, C.c_float(cfg.regular_coef), st))
+            lib.mvb_regularize(self.grad, self.w, self.n_w, self.regular, cfg.regular_coef, st)
             self.kernel_launches += 1
         if self.ftrl:
             if self.table is None:
-                N.check(lib.mvb_ftrl_update(C.c_void_p(self.z.data_ptr()), C.c_void_p(self.nacc.data_ptr()),
-                                            C.c_void_p(self.w.data_ptr()), C.c_void_p(self.grad.data_ptr()),
-                                            C.c_int64(self.n_w), C.c_float(cfg.alpha), st))
+                lib.mvb_ftrl_update(self.z, self.nacc, self.w, self.grad, self.n_w, cfg.alpha, st)
                 self.kernel_launches += 1
             else:
                 # FTRLObjective emits (dz, dn); the server subtracts, so the kernel emits the negatives
                 if getattr(self, "_dz", None) is None:
                     self._dz, self._dn = torch.empty_like(self.grad), torch.empty_like(self.grad)
-                N.check(lib.mvb_ftrl_delta(C.c_void_p(self.nacc.data_ptr()), C.c_void_p(self.w.data_ptr()),
-                                           C.c_void_p(self.grad.data_ptr()), C.c_void_p(self._dz.data_ptr()),
-                                           C.c_void_p(self._dn.data_ptr()), C.c_int64(self.n_w), C.c_float(cfg.alpha), st),
-                        "mvb_ftrl_delta")
+                lib.mvb_ftrl_delta(self.nacc, self.w, self.grad, self._dz, self._dn, self.n_w, cfg.alpha, st)
                 self.kernel_launches += 1
                 self.table.add_async(self._dz)
                 self.table_n.add_async(self._dn)

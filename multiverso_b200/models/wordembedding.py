@@ -127,11 +127,7 @@ class WordEmbedding:
             prob = np.empty(self.V, dtype=np.float32)
             alias = np.empty(self.V, dtype=np.int32)
             w = np.power(self.counts, 0.75)
-            rc = N.cuda_lib().mvb_build_alias_table(
-                w.ctypes.data_as(C.c_void_p), C.c_int(self.V), prob.ctypes.data_as(C.c_void_p),
-                alias.ctypes.data_as(C.c_void_p))
-            if rc != 0:
-                Log.fatal("alias table construction failed (%d)", rc)
+            N.cuda_lib().mvb_build_alias_table(w.ctypes.data, self.V, prob.ctypes.data, alias.ctypes.data)
             self.alias_prob = torch.from_numpy(prob).to(self.dev)
             self.alias_idx = torch.from_numpy(alias).to(self.dev)
         else:
@@ -193,8 +189,7 @@ class WordEmbedding:
         cap = float(os.environ.get("MVB_WE_HOT_CAP", "128"))
         if cap <= 0 or o.cbow or o.hs or o.use_adagrad or o.negative_num < 1:
             return
-        pos = int(N.cuda_lib().mvb_sgns_win_inflight(C.c_int(self.D), C.c_int(o.negative_num),
-                                                     C.c_int(o.window_size), C.c_int(self.max_ctas)))
+        pos = N.cuda_lib().mvb_sgns_win_inflight(self.D, o.negative_num, o.window_size, self.max_ctas)
         if pos <= 0:
             return
         f = self.counts / self.counts.sum()
@@ -256,8 +251,8 @@ class WordEmbedding:
                 a.w_in_peers[s_], a.w_out_peers[s_] = ti.shard_ptrs[s_], to.shard_ptrs[s_]
             a.variant = 20
         a.scale_in, a.scale_out = N.ptr(self.scale_in), N.ptr(self.scale_out)
-        N.check(N.cuda_lib().mvb_sgns_train(C.byref(a), C.c_void_p(N.stream_ptr())), "mvb_sgns_train")
-        self.kernel_launches += int(N.cuda_lib().mvb_sgns_last_launches())
+        N.cuda_lib().mvb_sgns_train(a, N.stream_ptr())
+        self.kernel_launches += N.cuda_lib().mvb_sgns_last_launches()
 
     # ------------------------------------------------------------------ one data block
     def train_block(self, tokens: torch.Tensor, compute_loss: bool = True,
@@ -371,7 +366,7 @@ class WordEmbedding:
         self._map_slot ^= 1
         b = self._block_buffers(slot, tokens.numel())
         o, lib = self.opt, N.cuda_lib()
-        st = C.c_void_p(N.stream_ptr())
+        st = N.stream_ptr()
         self._step += 1
         p = N.WePrep()
         p.tokens, p.n_tokens, p.vocab, p.negative = tokens.data_ptr(), tokens.numel(), self.V, o.negative_num
@@ -383,23 +378,20 @@ class WordEmbedding:
         p.neg_pool, p.pool_cap, p.counts = b["neg_pool"].data_ptr(), b["neg_pool"].numel(), b["counts"].data_ptr()
         p.cap_in, p.cap_out = b["cap_in"], b["cap_out"]
         with monitor("WE_PREPARE_DATA", cuda=True):
-            N.check(lib.mvb_we_prepare(C.byref(p), st), "mvb_we_prepare")
-        self.kernel_launches += int(lib.mvb_we_prepare_launches(C.c_int(o.negative_num)))
+            lib.mvb_we_prepare(p, st)
+        self.kernel_launches += lib.mvb_we_prepare_launches(o.negative_num)
         ctas = (self.side_ctas if self.side_mode == "bulk" else -self.side_ctas) if side else 32
         cnt = b["counts"].data_ptr()
         with monitor("WE_REQUEST_PARAMETER", cuda=True):
             for tab, ids, ci, cache, old, cap in ((self.input_table, b["ids_in"], 0, b["cache_in"], b["old_in"], b["cap_in"]),
                                                   (self.output_table, b["ids_out"], 1, b["cache_out"], b["old_out"], b["cap_out"])):
-                N.check(lib.mvb_rows_pull_bulk(C.byref(tab._rowmap), C.c_int(4), C.c_void_p(ids.data_ptr()),
-                                               C.c_void_p(cnt + 4 * ci), C.c_int64(cap), C.c_void_p(cache.data_ptr()),
-                                               C.c_void_p(old.data_ptr()), C.c_int64(self.LD), C.c_int(ctas), st),
-                        "mvb_rows_pull_bulk")
+                lib.mvb_rows_pull_bulk(tab._rowmap, 4, ids, cnt + 4 * ci, cap, cache, old, self.LD, ctas, st)
         self.kernel_launches += 2
         return b
 
     def _add_delta_dev(self, b: dict, side: bool) -> None:
         """AddDeltaParameter (communicator.cpp:206-249): rows += (trained - pulled) / W, pushed one-sided."""
-        lib, st = N.cuda_lib(), C.c_void_p(N.stream_ptr())
+        lib, st = N.cuda_lib(), N.stream_ptr()
         cnt = b["counts"].data_ptr()
         if self.side_mode == "mbox":
             cur = torch.cuda.current_stream()
@@ -418,11 +410,8 @@ class WordEmbedding:
         with monitor("WE_ADD_DELTA", cuda=True):
             for tab, ids, ci, cache, old, cap in ((self.input_table, b["ids_in"], 0, b["cache_in"], b["old_in"], b["cap_in"]),
                                                   (self.output_table, b["ids_out"], 1, b["cache_out"], b["old_out"], b["cap_out"])):
-                N.check(lib.mvb_rows_push_delta_bulk(C.byref(tab._rowmap), C.c_void_p(ids.data_ptr()),
-                                                     C.c_void_p(cnt + 4 * ci), C.c_int64(cap),
-                                                     C.c_void_p(cache.data_ptr()), C.c_void_p(old.data_ptr()),
-                                                     C.c_int64(self.LD), C.c_float(1.0 / self.W), C.c_int(ctas), st),
-                        "mvb_rows_push_delta_bulk")
+                lib.mvb_rows_push_delta_bulk(tab._rowmap, ids, cnt + 4 * ci, cap, cache, old, self.LD, 1.0 / self.W,
+                                             ctas, st)
         self.kernel_launches += 2
 
     def _prepare_block(self, tokens: torch.Tensor, wait: bool) -> dict:

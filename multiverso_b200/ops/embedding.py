@@ -26,7 +26,6 @@ backward pushes the gradient coalesced in torch with ``add_rows``: the same sema
 """
 from __future__ import annotations
 
-import ctypes as C
 from typing import Optional, Tuple
 
 import numpy as np
@@ -146,7 +145,7 @@ def _fwd_device(rm, dim, ids, offsets, psw, mode) -> torch.Tensor:
     a = _args(rm, dim, ids, offsets, psw, mode)
     a.out, a.ldo = out.data_ptr(), ldo
     with monitor("WORKER_TABLE_EMBEDDING_BAG", cuda=True, nbytes=ids.numel() * dim * 4):
-        N.check(N.cuda_lib().mvb_embedding_bag_fwd(C.byref(a), C.c_void_p(N.stream_ptr())), "mvb_embedding_bag_fwd")
+        N.cuda_lib().mvb_embedding_bag_fwd(a, N.stream_ptr())
     return out if ldo == dim else out[:, :dim]
 
 
@@ -166,8 +165,7 @@ def _psw_grad_device(rm, dim, ids, offsets, mode, dout) -> torch.Tensor:
     dpsw = torch.empty(ids.numel(), dtype=torch.float32, device=ids.device)
     a = _args(rm, dim, ids, offsets, None, mode)
     a.dout, a.ldd, a.dpsw = d.data_ptr(), ldd, dpsw.data_ptr()
-    N.check(N.cuda_lib().mvb_embedding_bag_psw_grad(C.byref(a), C.c_void_p(N.stream_ptr())),
-            "mvb_embedding_bag_psw_grad")
+    N.cuda_lib().mvb_embedding_bag_psw_grad(a, N.stream_ptr())
     return dpsw
 
 
@@ -179,30 +177,29 @@ def _push_device(table, rm, dim, ids, offsets, psw, mode, dout, push_scale: floa
     lib = N.cuda_lib()
     d, ldd = _dout_padded(dout, dim)
     sid, perm = torch.sort(ids, stable=True)               # (id, position) order
-    lib.mvb_embedding_bag_scratch_bytes.restype = C.c_int64
-    nbytes = int(lib.mvb_embedding_bag_scratch_bytes(C.c_int64(L), C.c_int64(dim)))
+    nbytes = lib.mvb_embedding_bag_scratch_bytes(L, dim)
     scratch = torch.empty(nbytes, dtype=torch.uint8, device=ids.device)
     a = _args(rm, dim, sid, offsets, psw, mode)
     a.dout, a.ldd, a.perm = d.data_ptr(), ldd, perm.data_ptr()
     a.scratch, a.scratch_bytes = scratch.data_ptr(), nbytes
-    st = C.c_void_p(N.stream_ptr())
+    st = N.stream_ptr()
     fused = table.updater in (N.UPD_DEFAULT, N.UPD_SGD) and not table.is_sparse
     with monitor("WORKER_TABLE_EMBEDDING_BAG_GRAD", cuda=True, nbytes=L * dim * 4):
         if fused:
             a.epilogue = N.EMB_PUSH
             a.scale = (-1.0 if table.updater == N.UPD_SGD else 1.0) * push_scale
-            N.check(lib.mvb_embedding_bag_bwd(C.byref(a), st), "mvb_embedding_bag_bwd")
+            lib.mvb_embedding_bag_bwd(a, st)
             return
         a.epilogue, a.scale = N.EMB_COMPACT, push_scale
         n_unique = torch.empty(1, dtype=torch.int64, device=ids.device)
         a.n_unique = n_unique.data_ptr()
-        N.check(lib.mvb_embedding_bag_bwd(C.byref(a), st), "mvb_embedding_bag_bwd")     # count only
+        lib.mvb_embedding_bag_bwd(a, st)     # count only
         U = int(n_unique.item())
         alloc = torch.empty if dim == table.num_col else torch.zeros
         grads = alloc(U, table.num_col, dtype=torch.float32, device=ids.device)
         uniq = torch.empty(U, dtype=torch.int64, device=ids.device)
         a.grads, a.ldg, a.uniq = grads.data_ptr(), table.num_col, uniq.data_ptr()
-        N.check(lib.mvb_embedding_bag_bwd(C.byref(a), st), "mvb_embedding_bag_bwd")
+        lib.mvb_embedding_bag_bwd(a, st)
     table.add_rows_async(uniq, grads, option)
 
 

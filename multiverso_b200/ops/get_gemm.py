@@ -9,8 +9,6 @@ Reference analogue: MatrixWorkerTable::Get followed by the application's first G
 """
 from __future__ import annotations
 
-import ctypes as C
-
 import torch
 
 from .. import _native as N
@@ -51,5 +49,5 @@ def get_gemm(table, x: torch.Tensor, out: torch.Tensor = None) -> torch.Tensor:
     for s in range(table.S):
         g.wmap.shard_ptrs[s] = table.shard_ptrs[s]
     g.local_server = table.sid if table.S > 1 else 0
-    N.check(N.cuda_lib().mvb_get_gemm_fused(C.byref(g), C.c_void_p(N.stream_ptr())), "mvb_get_gemm_fused")
+    N.cuda_lib().mvb_get_gemm_fused(g, N.stream_ptr())
     return out

@@ -20,7 +20,6 @@ top-k with the same tie rule, :func:`topk_cosine_reference`.
 """
 from __future__ import annotations
 
-import ctypes as C
 from typing import Optional, Tuple
 
 import torch
@@ -138,11 +137,10 @@ def _topk_device(rm: N.RowMap, width: int, queries: torch.Tensor, k: int,
     scores = torch.empty(M, k, dtype=torch.float32, device=dev)
     ids = torch.empty(M, k, dtype=torch.int64, device=dev)
     lib = N.cuda_lib()
-    lib.mvb_topk_cos_scratch_bytes.restype = C.c_int64
     # the kernel's need (queries x ranges per query tile) is not monotone in the query count: size the scratch
     # for every chunk size used, the full chunks and the last one
     chunks = {min(M, _Q_CHUNK), M % _Q_CHUNK or _Q_CHUNK} if M else {1}
-    nbytes = max(int(lib.mvb_topk_cos_scratch_bytes(C.c_int64(c), C.c_int(k), C.c_int64(n))) for c in chunks)
+    nbytes = max(lib.mvb_topk_cos_scratch_bytes(c, k, n) for c in chunks)
     scratch = torch.empty(max(nbytes, 16), dtype=torch.uint8, device=dev)
     a = N.TopkCos()
     a.ldq, a.dim, a.n_rows, a.wmap, a.k = ldq, dim, n, rm, k
@@ -151,7 +149,7 @@ def _topk_device(rm: N.RowMap, width: int, queries: torch.Tensor, k: int,
         hi = min(M, lo + _Q_CHUNK)
         a.q, a.M = q[lo].data_ptr(), hi - lo
         a.scores, a.ids = scores[lo].data_ptr(), ids[lo].data_ptr()
-        N.check(lib.mvb_topk_cosine(C.byref(a), C.c_void_p(N.stream_ptr())), "mvb_topk_cosine")
+        lib.mvb_topk_cosine(a, N.stream_ptr())
     return scores, ids
 
 

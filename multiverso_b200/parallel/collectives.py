@@ -83,10 +83,7 @@ def _aggregate_fused(rt, lib, st, data: torch.Tensor, nbytes: int) -> torch.Tens
         rt.barrier()                                     # everybody's staging is mapped before the first flag
     st.f_epoch += 1
     a.dtype, a.n, a.out, a.epoch = N.dtype_code(data.dtype), data.numel(), data.data_ptr(), st.f_epoch
-    rc = lib.mvb_allreduce_fused(C.byref(a), C.c_void_p(data.data_ptr()), C.c_int64((st.f_epoch & 1) * FUSED_BYTES),
-                                 C.c_void_p(N.stream_ptr()))
-    if rc:
-        N.check(rc, "mvb_allreduce_fused")
+    lib.mvb_allreduce_fused(a, data, (st.f_epoch & 1) * FUSED_BYTES, N.stream_ptr())
     return data
 
 
@@ -94,13 +91,12 @@ def _aggregate_in_place(rt, lib, st, data, nbytes, buf, off, algo) -> torch.Tens
     """``data`` lives in symmetric memory: two-shot (or NVLS) directly on it, no staging copy.
     Uses the staged path's channels / epochs, so the two may be mixed freely."""
     ch = 1
-    stream = C.c_void_p(N.stream_ptr())
+    stream = N.stream_ptr()
     if st.counter is None:
         st.counter = rt.done_counter_ptr()
     if st.epoch > 0:
-        N.check(lib.mvb_wait(rt.pads_array(), rt.rank, rt.size, ch + 1, C.c_uint64(st.epoch),
-                             C.c_uint32((1 << rt.size) - 1), C.c_void_p(rt.err_flag.data_ptr()),
-                             C.c_double(float(FLAGS.get("barrier_timeout_s"))), stream), "mvb_wait")
+        lib.mvb_wait(rt.pads_array(), rt.rank, rt.size, ch + 1, st.epoch, (1 << rt.size) - 1, rt.err_flag,
+                     float(FLAGS.get("barrier_timeout_s")), stream)
     st.epoch += 1
     a = N.Allreduce()
     a.dtype, a.n = N.dtype_code(data.dtype), data.numel()
@@ -119,9 +115,9 @@ def _aggregate_in_place(rt, lib, st, data, nbytes, buf, off, algo) -> torch.Tens
     use_nvls = bool(mc) and data.dtype == torch.float32 and (algo == "nvls" or (algo == "auto" and rt.size >= 4))
     with monitor("MV_AGGREGATE", cuda=True, nbytes=nbytes):
         if use_nvls:
-            N.check(lib.mvb_allreduce_nvls(C.byref(a), C.c_void_p(mc + off), stream), "mvb_allreduce_nvls")
+            lib.mvb_allreduce_nvls(a, mc + off, stream)
         else:
-            N.check(lib.mvb_allreduce_twoshot(C.byref(a), stream), "mvb_allreduce")
+            lib.mvb_allreduce_twoshot(a, stream)
     return data
 
 
@@ -147,12 +143,11 @@ def aggregate(data: torch.Tensor, algo: str = "auto") -> torch.Tensor:
         st.staging = rt.alloc_multicast(st.cap) or rt.alloc_symm(st.cap)
         st.counter = rt.done_counter_ptr()
     ch = 1  # channels 1 (ready) and 2 (done) are reserved for aggregate
-    stream = C.c_void_p(N.stream_ptr())
+    stream = N.stream_ptr()
     if st.epoch > 0:
         # nobody may still be reading our staging buffer from the previous call
-        N.check(lib.mvb_wait(rt.pads_array(), rt.rank, rt.size, ch + 1, C.c_uint64(st.epoch),
-                             C.c_uint32((1 << rt.size) - 1), C.c_void_p(rt.err_flag.data_ptr()),
-                             C.c_double(float(FLAGS.get("barrier_timeout_s"))), stream), "mvb_wait")
+        lib.mvb_wait(rt.pads_array(), rt.rank, rt.size, ch + 1, st.epoch, (1 << rt.size) - 1, rt.err_flag,
+                     float(FLAGS.get("barrier_timeout_s")), stream)
     stage = st.staging.tensor(data.dtype, data.numel())
     stage.copy_(data.view(-1))
     st.epoch += 1
@@ -172,8 +167,8 @@ def aggregate(data: torch.Tensor, algo: str = "auto") -> torch.Tensor:
     use_nvls = bool(mc) and data.dtype == torch.float32 and (algo == "nvls" or (algo == "auto" and two and rt.size >= 4))
     with monitor("MV_AGGREGATE", cuda=True, nbytes=nbytes):
         if use_nvls:
-            N.check(lib.mvb_allreduce_nvls(C.byref(a), C.c_void_p(mc), stream), "mvb_allreduce_nvls")
+            lib.mvb_allreduce_nvls(a, mc, stream)
         else:
             fn = lib.mvb_allreduce_twoshot if two else lib.mvb_allreduce_oneshot
-            N.check(fn(C.byref(a), stream), "mvb_allreduce")
+            fn(a, stream)
     return data

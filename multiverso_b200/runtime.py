@@ -56,21 +56,21 @@ class SymmBuffer:
         self.nbytes = max(int(nbytes), 16)
         lib = N.cuda_lib()
         p = C.c_void_p()
-        N.check(lib.mvb_symm_alloc(C.c_int64(self.nbytes), C.byref(p)), "mvb_symm_alloc")
+        lib.mvb_symm_alloc(self.nbytes, p)
         self.local_ptr = p.value
         self.ptrs: List[int] = [0] * rt.size
         self.ptrs[rt.rank] = self.local_ptr
         self._opened: List[int] = []
         if rt.size > 1:
             h = (C.c_char * 64)()
-            N.check(lib.mvb_ipc_get_handle(C.c_void_p(self.local_ptr), h), "mvb_ipc_get_handle")
+            lib.mvb_ipc_get_handle(self.local_ptr, C.addressof(h))
             handles = rt.all_gather_object(bytes(h.raw))
             for r, hb in enumerate(handles):
                 if r == rt.rank:
                     continue
                 q = C.c_void_p()
                 buf = C.create_string_buffer(hb, 64)
-                N.check(lib.mvb_ipc_open_handle(buf, C.byref(q)), "mvb_ipc_open_handle")
+                lib.mvb_ipc_open_handle(C.addressof(buf), q)
                 self.ptrs[r] = q.value
                 self._opened.append(q.value)
         self._view = _CudaView(self.local_ptr, self.nbytes, self)
@@ -95,7 +95,7 @@ class SymmBuffer:
         """Phase 1 of a release: unmap the peers' slabs from this process."""
         lib = N.cuda_lib()
         for q in self._opened:
-            lib.mvb_ipc_close_handle(C.c_void_p(q))
+            lib.mvb_ipc_close_handle(q)
         self._opened = []
 
     def free_local(self):
@@ -103,7 +103,7 @@ class SymmBuffer:
         has the slab mapped must never see it freed; same ordering as csrc/device_rt/device_rt.cpp)."""
         if self.local_ptr:
             self._base = None
-            N.cuda_lib().mvb_symm_free(C.c_void_p(self.local_ptr))
+            N.cuda_lib().mvb_symm_free(self.local_ptr)
             self.local_ptr = 0
 
     def free(self):
@@ -435,10 +435,8 @@ class Runtime:
             import torch
             lib = N.cuda_lib()
             ep = self.next_epoch(0)
-            N.check(lib.mvb_barrier(self.pads_array(), self.rank, self.size, 0, C.c_uint64(ep),
-                                    C.c_void_p(self.err_flag.data_ptr()),
-                                    C.c_double(float(FLAGS.get("barrier_timeout_s"))),
-                                    C.c_void_p(N.stream_ptr())), "mvb_barrier")
+            lib.mvb_barrier(self.pads_array(), self.rank, self.size, 0, ep, self.err_flag,
+                            float(FLAGS.get("barrier_timeout_s")), N.stream_ptr())
             if self.barrier_hooks:
                 # Row mailboxes: a rank waiting here still serves the pushes of the ranks that have not
                 # arrived yet (they may be spinning for its ack), then -- every rank has rung its doorbells
@@ -453,10 +451,8 @@ class Runtime:
                 for h in self.barrier_hooks:
                     h(True)
                 ep = self.next_epoch(0)
-                N.check(lib.mvb_barrier(self.pads_array(), self.rank, self.size, 0, C.c_uint64(ep),
-                                        C.c_void_p(self.err_flag.data_ptr()),
-                                        C.c_double(float(FLAGS.get("barrier_timeout_s"))),
-                                        C.c_void_p(N.stream_ptr())), "mvb_barrier")
+                lib.mvb_barrier(self.pads_array(), self.rank, self.size, 0, ep, self.err_flag,
+                                float(FLAGS.get("barrier_timeout_s")), N.stream_ptr())
             torch.cuda.current_stream().synchronize()
             self.check_watchdog()
         else:

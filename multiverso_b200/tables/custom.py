@@ -19,7 +19,6 @@ this base with the key-addressed kernels of csrc/cuda/keys.cu.
 """
 from __future__ import annotations
 
-import ctypes as C
 import struct
 from typing import List, Optional, Tuple
 
@@ -138,8 +137,7 @@ class SparseDeviceTable(CustomDeviceTable):
         k = self._keys(keys)
         v = torch.as_tensor(vals, dtype=torch.float32).to(self.rt.device).contiguous().view(-1)
         assert v.numel() == k.numel() * self.width
-        N.check(N.cuda_lib().mvb_keys_add(C.byref(self._map), C.c_void_p(k.data_ptr()), C.c_void_p(v.data_ptr()),
-                                          C.c_int64(k.numel()), C.c_float(-1.0), C.c_void_p(N.stream_ptr())), "mvb_keys_add")
+        N.cuda_lib().mvb_keys_add(self._map, k, v, k.numel(), -1.0, N.stream_ptr())
         self._keep = (k, v)
 
     def get(self, keys=None):
@@ -148,16 +146,13 @@ class SparseDeviceTable(CustomDeviceTable):
         if keys is not None:
             k = self._keys(keys)
             out = torch.empty(k.numel(), self.width, device=self.rt.device)
-            N.check(lib.mvb_keys_get(C.byref(self._map), C.c_void_p(k.data_ptr()), C.c_void_p(out.data_ptr()),
-                                     C.c_int64(k.numel()), C.c_void_p(N.stream_ptr())), "mvb_keys_get")
+            lib.mvb_keys_get(self._map, k, out, k.numel(), N.stream_ptr())
             self._keep_get = k
             return out if self.width > 1 else out.view(-1)
         cap = self.size
         ok = torch.empty(cap, dtype=torch.int64, device=self.rt.device)
         ov = torch.empty(cap, self.width, device=self.rt.device)
-        N.check(lib.mvb_keys_collect(C.byref(self._map), C.c_void_p(ok.data_ptr()), C.c_void_p(ov.data_ptr()),
-                                     C.c_void_p(self._count.data_ptr()), C.c_int64(cap), C.c_void_p(N.stream_ptr())),
-                "mvb_keys_collect")
+        lib.mvb_keys_collect(self._map, ok, ov, self._count, cap, N.stream_ptr())
         n = int(self._count.item())
         order = torch.argsort(ok[:n])
         vals = ov[:n][order]

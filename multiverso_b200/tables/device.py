@@ -238,9 +238,7 @@ class DenseDeviceTable(_AsyncOps):
                 sl = (C.c_int64 * self.S)(*self.lens)
                 if self.updater in (N.UPD_DEFAULT, N.UPD_SGD) or self.dtype in (torch.int32, torch.int64):
                     sign = -1.0 if self.updater == N.UPD_SGD else 1.0
-                    N.check(lib.mvb_push_dense_red(self.dcode, C.c_void_p(src.data_ptr()), self.S, sp, so,
-                                                   sl, C.c_float(sign), C.c_void_p(N.stream_ptr())),
-                            "mvb_push_dense_red")
+                    lib.mvb_push_dense_red(self.dcode, src, self.S, sp, so, sl, sign, N.stream_ptr())
                 else:
                     ranks = [rt.server_id_to_rank(s) for s in range(self.S)]
                     s0 = (C.c_void_p * self.S)(*[self._state_bufs[0].ptrs[r] for r in ranks])
@@ -249,9 +247,8 @@ class DenseDeviceTable(_AsyncOps):
                     ss = (C.c_int64 * self.S)(*self.state_strides)
                     ao = _opt_struct(opt)
                     ao.worker_id = max(rt.worker_id(), 0)
-                    N.check(lib.mvb_push_dense_stateful(self.dcode, self.updater, C.c_void_p(src.data_ptr()),
-                                                        self.S, sp, s0, s1, so, sl, ss, C.byref(ao), rt.rank,
-                                                        C.c_void_p(N.stream_ptr())), "mvb_push_dense_stateful")
+                    lib.mvb_push_dense_stateful(self.dcode, self.updater, src, self.S, sp, s0, s1, so, sl, ss, ao,
+                                                rt.rank, N.stream_ptr())
                 self._keep = src
             if rt.is_worker():
                 self._note_add()
@@ -259,16 +256,12 @@ class DenseDeviceTable(_AsyncOps):
 
     def _note_add(self) -> None:
         if self._ver is not None:
-            N.check(N.cuda_lib().mvb_stale_on_add(self._ver_ptrs, self.S, C.c_void_p(self._ver_last.data_ptr()),
-                                                  C.c_void_p(self._ver_adds.data_ptr()),
-                                                  C.c_void_p(self.staleness_hist.data_ptr()), C.c_int(64),
-                                                  C.c_void_p(N.stream_ptr())), "mvb_stale_on_add")
+            N.cuda_lib().mvb_stale_on_add(self._ver_ptrs, self.S, self._ver_last, self._ver_adds,
+                                          self.staleness_hist, 64, N.stream_ptr())
 
     def _note_get(self) -> None:
         if self._ver is not None:
-            N.check(N.cuda_lib().mvb_stale_on_get(self._ver_ptrs, self.S, C.c_void_p(self._ver_last.data_ptr()),
-                                                  C.c_void_p(self._ver_adds.data_ptr()), C.c_void_p(N.stream_ptr())),
-                    "mvb_stale_on_get")
+            N.cuda_lib().mvb_stale_on_get(self._ver_ptrs, self.S, self._ver_last, self._ver_adds, N.stream_ptr())
 
     def _opt_box_buf(self):
         """Symmetric option boxes (2 generations x MAX_RANKS AddOptions per rank); allocated at the first
@@ -323,7 +316,7 @@ class DenseDeviceTable(_AsyncOps):
         a.fin_flag = self._fin.data_ptr()
         a.done_counter = self._done_counter
         a.timeout_s = float(FLAGS.get("barrier_timeout_s"))
-        N.check(lib.mvb_add_dense_fused(C.byref(a), C.c_void_p(N.stream_ptr())), "mvb_add_dense_fused")
+        lib.mvb_add_dense_fused(a, N.stream_ptr())
 
     # ------------------------------------------------------------------ Get (whole table)
     def get(self, out: Optional[torch.Tensor] = None, option: Optional[GetOption] = None) -> torch.Tensor:
@@ -342,10 +335,8 @@ class DenseDeviceTable(_AsyncOps):
             for s_ in range(self.S):
                 mask |= 1 << rt.server_id_to_rank(s_)
             with monitor("WORKER_TABLE_GET", cuda=True, nbytes=self.size * self.esz):
-                N.check(lib.mvb_wait(rt.pads_array(), rt.rank, rt.size, self.ch_done, C.c_uint64(self.add_epoch),
-                                     C.c_uint32(mask), C.c_void_p(rt.err_flag.data_ptr()),
-                                     C.c_double(float(FLAGS.get("barrier_timeout_s"))),
-                                     C.c_void_p(N.stream_ptr())), "mvb_wait")
+                lib.mvb_wait(rt.pads_array(), rt.rank, rt.size, self.ch_done, self.add_epoch, mask, rt.err_flag,
+                             float(FLAGS.get("barrier_timeout_s")), N.stream_ptr())
                 rep = self._replica.tensor(self.dtype, self.size)
                 if out is None:
                     out = rep.clone()
@@ -371,7 +362,7 @@ class DenseDeviceTable(_AsyncOps):
         g.timeout_s = float(FLAGS.get("barrier_timeout_s"))
         self._note_get()        # versions as of the start of the pull (a conservative read point)
         with monitor("WORKER_TABLE_GET", cuda=True, nbytes=self.size * self.esz):
-            N.check(lib.mvb_get_dense(C.byref(g), C.c_void_p(N.stream_ptr())), "mvb_get_dense")
+            lib.mvb_get_dense(g, N.stream_ptr())
         return self._record(), out
 
     # ------------------------------------------------------------------ BSP shutdown
@@ -393,15 +384,12 @@ class DenseDeviceTable(_AsyncOps):
                 mask = 0
                 for s_ in range(self.S):
                     mask |= 1 << rt.server_id_to_rank(s_)
-                N.check(lib.mvb_wait(rt.pads_array(), rt.rank, rt.size, self.ch_done, C.c_uint64(self.add_epoch),
-                                     C.c_uint32(mask), C.c_void_p(rt.err_flag.data_ptr()),
-                                     C.c_double(float(FLAGS.get("barrier_timeout_s"))),
-                                     C.c_void_p(N.stream_ptr())), "mvb_wait")
+                lib.mvb_wait(rt.pads_array(), rt.rank, rt.size, self.ch_done, self.add_epoch, mask, rt.err_flag,
+                             float(FLAGS.get("barrier_timeout_s")), N.stream_ptr())
             for b in self._stage:
                 b.tensor(torch.uint8).zero_()
         if rt.is_worker():
-            N.check(lib.mvb_signal(rt.pads_array(), rt.rank, rt.size, self.ch_ready,
-                                   C.c_uint64(N.EPOCH_FIN), C.c_void_p(N.stream_ptr())), "mvb_signal")
+            lib.mvb_signal(rt.pads_array(), rt.rank, rt.size, self.ch_ready, N.EPOCH_FIN, N.stream_ptr())
 
     def drain_step(self, pads_host) -> str:
         """One polling step of the owner-side drain: 'done' when every worker finished,
@@ -468,10 +456,8 @@ class RowMailbox:
         S = table.S
         self.cap = max(hi - lo for lo, hi in zip(table.row_lo, table.row_hi))
         lib = N.cuda_lib()
-        lib.mvb_rowbox_slot_bytes.restype = C.c_int64
-        self.slot_bytes = int(lib.mvb_rowbox_slot_bytes(C.c_int64(self.cap), C.c_int64(table.num_col)))
-        self.slot_bytes = (self.slot_bytes + 255) // 256 * 256
-        self.nslots = int(lib.mvb_rowbox_slots())
+        self.slot_bytes = (lib.mvb_rowbox_slot_bytes(self.cap, table.num_col) + 255) // 256 * 256
+        self.nslots = lib.mvb_rowbox_slots()
         self.box = rt.alloc_symm(S * self.nslots * self.slot_bytes)
         self.ack = rt.alloc_symm(8 * N.MAX_RANKS)
         self.box.tensor(torch.uint8)[:].view(S * self.nslots, self.slot_bytes)[:, :128].zero_()   # headers: seq = 0
@@ -509,20 +495,15 @@ class RowMailbox:
         """rows[ids] += (cur - old) * scale at their owners (ids ascending int32; count read on the device)."""
         self.epoch += 1
         ao = _opt_struct(option or AddOption())
-        N.check(N.cuda_lib().mvb_rowbox_push_delta(
-            C.byref(self.c), C.c_void_p(ids32.data_ptr()), C.c_void_p(n_ptr), C.c_int64(n_max),
-            C.c_void_p(cur.data_ptr()), C.c_void_p(old.data_ptr()), C.c_int64(cur.stride(0)), C.c_float(scale),
-            C.c_uint64(self.epoch), C.byref(ao), C.c_int(ctas_per_sm), C.c_void_p(N.stream_ptr())),
-            "mvb_rowbox_push_delta")
+        N.cuda_lib().mvb_rowbox_push_delta(self.c, ids32, n_ptr, n_max, cur, old, cur.stride(0), scale, self.epoch, ao,
+                                           ctas_per_sm, N.stream_ptr())
 
     def push_vals(self, ids32: torch.Tensor, vals: torch.Tensor, option: Optional[AddOption] = None,
                   scale: float = 1.0, ctas_per_sm: int = 1) -> None:
         self.epoch += 1
         ao = _opt_struct(option or AddOption())
-        N.check(N.cuda_lib().mvb_rowbox_push_vals(
-            C.byref(self.c), C.c_void_p(ids32.data_ptr()), C.c_void_p(0), C.c_int64(ids32.numel()),
-            C.c_void_p(vals.data_ptr()), C.c_int64(vals.stride(0)), C.c_float(scale), C.c_uint64(self.epoch),
-            C.byref(ao), C.c_int(ctas_per_sm), C.c_void_p(N.stream_ptr())), "mvb_rowbox_push_vals")
+        N.cuda_lib().mvb_rowbox_push_vals(self.c, ids32, None, ids32.numel(), vals, vals.stride(0), scale, self.epoch,
+                                          ao, ctas_per_sm, N.stream_ptr())
 
     def drain(self, wait: bool = False, ctas_per_sm: int = 1, stream=None) -> None:
         """Owner side: apply what has arrived (wait=False) or the next push of every source (wait=True).
@@ -530,12 +511,11 @@ class RowMailbox:
         ack on the caller's stream can never block the drain that produces the peer's ack)."""
         t, lib = self.t, N.cuda_lib()
         st = stream if stream is not None else self.drain_stream
-        sp = C.c_void_p(st.cuda_stream)
-        N.check(lib.mvb_rowbox_poll(C.byref(self.c), C.c_int(-1), C.c_int(1 if wait else 0), sp), "mvb_rowbox_poll")
+        sp = st.cuda_stream
+        lib.mvb_rowbox_poll(self.c, -1, 1 if wait else 0, sp)
         for w in range(t.S):
-            N.check(lib.mvb_rowbox_apply(C.byref(self.c), C.c_int(t.updater), C.c_void_p(t.shard_buf.local_ptr),
-                                         t._sp(0), t._sp(1), C.c_int64(t.state_stride), C.c_int64(t.row_lo[t.sid]),
-                                         C.c_int(w), C.c_int(ctas_per_sm), sp), "mvb_rowbox_apply")
+            lib.mvb_rowbox_apply(self.c, t.updater, t.shard_buf.local_ptr, t._sp(0), t._sp(1), t.state_stride,
+                                 t.row_lo[t.sid], w, ctas_per_sm, sp)
 
     def launches_per_drain(self) -> int:
         return 1 + self.t.S
@@ -638,9 +618,7 @@ class MatrixDeviceTable(DenseDeviceTable):
         assert out.is_cuda and out.dtype == self.dtype and out.stride(-1) == 1
         ld = out.stride(0) if out.dim() == 2 else self.num_col
         with monitor("WORKER_TABLE_GET_ROWS", cuda=True, nbytes=k * self.num_col * self.esz):
-            N.check(lib.mvb_get_rows(self.dcode, C.byref(self._rowmap), C.c_void_p(ids.data_ptr()),
-                                     C.c_int64(k), C.c_void_p(out.data_ptr()), C.c_int64(ld),
-                                     C.c_void_p(N.stream_ptr())), "mvb_get_rows")
+            lib.mvb_get_rows(self.dcode, self._rowmap, ids, k, out, ld, N.stream_ptr())
         self._keep_ids = ids
         return self._record(), out
 
@@ -662,14 +640,10 @@ class MatrixDeviceTable(DenseDeviceTable):
             vals = vals.to(rt.device, non_blocking=True)
         vals = vals.contiguous().view(k, self.num_col)
         opt = option or AddOption()
-        st = C.c_void_p(N.stream_ptr())
         with monitor("WORKER_TABLE_ADD_ROWS", cuda=True, nbytes=k * self.num_col * self.esz):
             if self.updater in (N.UPD_DEFAULT, N.UPD_SGD):
                 sign = -1.0 if self.updater == N.UPD_SGD else 1.0
-                N.check(lib.mvb_add_rows_red(self.dcode, C.byref(self._rowmap),
-                                             C.c_void_p(ids.data_ptr()), C.c_int64(k),
-                                             C.c_void_p(vals.data_ptr()), C.c_int64(self.num_col),
-                                             C.c_float(sign), st), "mvb_add_rows_red")
+                lib.mvb_add_rows_red(self.dcode, self._rowmap, ids, k, vals, self.num_col, sign, N.stream_ptr())
             else:
                 self._add_rows_stateful(ids, vals, opt)
             if self.is_sparse:
@@ -685,11 +659,8 @@ class MatrixDeviceTable(DenseDeviceTable):
         k = ids.numel()
         sign = -1.0 if self.updater == N.UPD_SGD else 1.0
         with monitor("WORKER_TABLE_ADD_ROWS", cuda=True, nbytes=k * self.num_col * self.esz):
-            N.check(N.cuda_lib().mvb_add_rows_delta(C.byref(self._rowmap), C.c_void_p(ids.data_ptr()),
-                                                    C.c_int64(k), C.c_void_p(cur.data_ptr()),
-                                                    C.c_void_p(old.data_ptr()), C.c_int64(cur.stride(0)),
-                                                    C.c_float(sign * scale), C.c_void_p(N.stream_ptr())),
-                    "mvb_add_rows_delta")
+            N.cuda_lib().mvb_add_rows_delta(self._rowmap, ids, k, cur, old, cur.stride(0), sign * scale,
+                                            N.stream_ptr())
             if self.is_sparse:
                 self._mark_stale(ids)
         self._keep_rows = (ids, cur, old)
@@ -712,16 +683,13 @@ class MatrixDeviceTable(DenseDeviceTable):
             self._keep_push = (ids32,)
             self._mailbox.drain(wait=False)
             return
-        st = C.c_void_p(N.stream_ptr())
+        st = N.stream_ptr()
         ao = _opt_struct(opt)
         if rt.size == 1:
             ao.worker_id = 0
-            N.check(lib.mvb_add_rows_owner(self.dcode, self.updater, C.c_void_p(self.shard_buf.local_ptr),
-                                           self._sp(0), self._sp(1), C.c_int64(self.row_lo[0]),
-                                           C.c_int64(self.row_hi[0]), C.c_int64(self.num_col),
-                                           C.c_int64(self.state_stride), C.c_void_p(ids.data_ptr()),
-                                           C.c_int64(k), C.c_void_p(vals.data_ptr()),
-                                           C.c_int64(self.num_col), C.byref(ao), st), "mvb_add_rows_owner")
+            lib.mvb_add_rows_owner(self.dcode, self.updater, self.shard_buf.local_ptr, self._sp(0), self._sp(1),
+                                   self.row_lo[0], self.row_hi[0], self.num_col, self.state_stride, ids, k, vals,
+                                   self.num_col, ao, st)
             return
         counts = rt.all_gather_object(int(k))
         cap = max(max(counts), 1)
@@ -741,17 +709,14 @@ class MatrixDeviceTable(DenseDeviceTable):
                 if counts[r] == 0:
                     continue
                 ao.worker_id = w
-                N.check(lib.mvb_add_rows_owner(
-                    self.dcode, self.updater, C.c_void_p(self.shard_buf.local_ptr), self._sp(0),
-                    self._sp(1), C.c_int64(self.row_lo[self.sid]), C.c_int64(self.row_hi[self.sid]),
-                    C.c_int64(self.num_col), C.c_int64(self.state_stride),
-                    C.c_void_p(self._row_stage_ids.ptrs[r]), C.c_int64(counts[r]),
-                    C.c_void_p(self._row_stage_vals.ptrs[r]), C.c_int64(self.num_col), C.byref(ao), st),
-                    "mvb_add_rows_owner")
+                lib.mvb_add_rows_owner(self.dcode, self.updater, self.shard_buf.local_ptr, self._sp(0), self._sp(1),
+                                       self.row_lo[self.sid], self.row_hi[self.sid], self.num_col, self.state_stride,
+                                       self._row_stage_ids.ptrs[r], counts[r], self._row_stage_vals.ptrs[r],
+                                       self.num_col, ao, st)
         rt.barrier()
 
     def _sp(self, i):
-        return C.c_void_p(self.state[i].data_ptr()) if self.n_states > i else C.c_void_p(0)
+        return self.state[i] if self.n_states > i else None
 
     # ---- whole-table ops honour the sparse bookkeeping ----------------------------------
     def add_async(self, delta=None, option=None, staged=False) -> int:
@@ -759,10 +724,7 @@ class MatrixDeviceTable(DenseDeviceTable):
             lib = N.cuda_lib()
             d = self._as_device(delta)
             mask = torch.empty(self.num_row, dtype=torch.uint8, device=self.rt.device)
-            N.check(lib.mvb_row_nonzero_mask(self.dcode, C.c_void_p(d.data_ptr()), C.c_int64(self.num_row),
-                                             C.c_int64(self.num_col), C.c_int64(self.num_col),
-                                             C.c_void_p(mask.data_ptr()), C.c_void_p(N.stream_ptr())),
-                    "mvb_row_nonzero_mask")
+            lib.mvb_row_nonzero_mask(self.dcode, d, self.num_row, self.num_col, self.num_col, mask, N.stream_ptr())
             h = super().add_async(d, option, False)
             self._mark_stale(mask.nonzero().view(-1))
             return h
@@ -774,9 +736,7 @@ class MatrixDeviceTable(DenseDeviceTable):
         if k == 0:
             return
         for r in range(self.rt.size):
-            N.check(lib.mvb_stale_mark(C.c_void_p(self._stale_buf.ptrs[r]), C.c_int64(self.num_row),
-                                       self._nslots, C.c_void_p(ids.data_ptr()), C.c_int64(k),
-                                       C.c_void_p(N.stream_ptr())), "mvb_stale_mark")
+            lib.mvb_stale_mark(self._stale_buf.ptrs[r], self.num_row, self._nslots, ids, k, N.stream_ptr())
         self._keep_mark = ids
 
     def get_stale(self, option: Optional[GetOption] = None, slot: int = 0):
@@ -790,9 +750,7 @@ class MatrixDeviceTable(DenseDeviceTable):
         w = wid + (self.W if (self.is_pipeline and slot) else 0)
         mine = self._stale[w * self.num_row:(w + 1) * self.num_row]
         mask = torch.empty(self.num_row, dtype=torch.uint8, device=self.rt.device)
-        N.check(lib.mvb_stale_take(C.c_void_p(mine.data_ptr()), C.c_int64(self.num_row), None,
-                                   C.c_int64(-1), C.c_void_p(mask.data_ptr()),
-                                   C.c_void_p(N.stream_ptr())), "mvb_stale_take")
+        lib.mvb_stale_take(mine, self.num_row, None, -1, mask, N.stream_ptr())
         ids = mask.nonzero().view(-1)
         if ids.numel() == 0:
             return ids, torch.empty(0, self.num_col, dtype=self.dtype, device=self.rt.device)
@@ -840,8 +798,7 @@ class KVDeviceTable(_AsyncOps):
         self.capacity = cap
         self.keys_buf = rt.alloc_symm(cap * 8)
         self.vals_buf = rt.alloc_symm(cap * self.vsz)
-        N.check(lib.mvb_kv_init(C.c_void_p(self.keys_buf.local_ptr), C.c_int64(cap),
-                                C.c_void_p(N.stream_ptr())), "mvb_kv_init")
+        lib.mvb_kv_init(self.keys_buf.local_ptr, cap, N.stream_ptr())
         self.vals_buf.tensor(torch.uint8).zero_()
         kv = N.KV()
         kv.vtype, kv.nservers, kv.capacity = self.vcode, self.S, cap
@@ -854,8 +811,7 @@ class KVDeviceTable(_AsyncOps):
     # ---- growth -------------------------------------------------------------------------------
     def live_keys(self) -> int:
         """Keys stored in this rank's shard (synchronises the stream)."""
-        N.check(N.cuda_lib().mvb_kv_count(C.c_void_p(self.keys_buf.local_ptr), C.c_int64(self.capacity),
-                                          C.c_void_p(self._count.data_ptr()), C.c_void_p(N.stream_ptr())), "mvb_kv_count")
+        N.cuda_lib().mvb_kv_count(self.keys_buf.local_ptr, self.capacity, self._count, N.stream_ptr())
         return int(self._count.item())
 
     def reserve(self, keys_per_shard: int = 0) -> None:
@@ -874,10 +830,8 @@ class KVDeviceTable(_AsyncOps):
             rt.control_barrier()                 # nobody is still pushing into the old slabs
         old_keys, old_vals, old_cap = self.keys_buf, self.vals_buf, self.capacity
         self._alloc(cap)
-        N.check(lib.mvb_kv_rehash(self.vcode, C.c_void_p(old_keys.local_ptr), C.c_void_p(old_vals.local_ptr),
-                                  C.c_int64(old_cap), C.c_void_p(self.keys_buf.local_ptr),
-                                  C.c_void_p(self.vals_buf.local_ptr), C.c_int64(cap),
-                                  C.c_void_p(rt.err_flag.data_ptr()), C.c_void_p(N.stream_ptr())), "mvb_kv_rehash")
+        lib.mvb_kv_rehash(self.vcode, old_keys.local_ptr, old_vals.local_ptr, old_cap, self.keys_buf.local_ptr,
+                          self.vals_buf.local_ptr, cap, rt.err_flag, N.stream_ptr())
         torch.cuda.synchronize()
         rt.release_symm(old_keys)                # two-phase, collective
         rt.release_symm(old_vals)
@@ -908,9 +862,7 @@ class KVDeviceTable(_AsyncOps):
         k = self._keys([keys] if scalar else keys)
         v = torch.as_tensor([vals] if scalar else vals).to(self.vdtype).to(self.rt.device).contiguous().view(-1)
         assert k.numel() == v.numel()
-        N.check(lib.mvb_kv_add(C.byref(self._kv), C.c_void_p(k.data_ptr()), C.c_void_p(v.data_ptr()),
-                               C.c_int64(k.numel()), C.c_void_p(self.rt.err_flag.data_ptr()),
-                               C.c_void_p(N.stream_ptr())), "mvb_kv_add")
+        lib.mvb_kv_add(self._kv, k, v, k.numel(), self.rt.err_flag, N.stream_ptr())
         self._keep_add = (k, v)
         self._added_ub += k.numel()
         if self.rt.size == 1 and self._added_ub > self.MAX_LOAD * self.capacity:
@@ -922,8 +874,7 @@ class KVDeviceTable(_AsyncOps):
         scalar = not hasattr(keys, "__len__") and not torch.is_tensor(keys)
         k = self._keys([keys] if scalar else keys)
         out = torch.empty(k.numel(), dtype=self.vdtype, device=self.rt.device)
-        N.check(lib.mvb_kv_get(C.byref(self._kv), C.c_void_p(k.data_ptr()), C.c_void_p(out.data_ptr()),
-                               C.c_int64(k.numel()), C.c_void_p(N.stream_ptr())), "mvb_kv_get")
+        lib.mvb_kv_get(self._kv, k, out, k.numel(), N.stream_ptr())
         self._pending.append((k, out))
         if len(self._pending) > 64:
             self.raw()
@@ -942,10 +893,8 @@ class KVDeviceTable(_AsyncOps):
         ok = torch.empty(self.capacity, dtype=torch.int64, device=self.rt.device)
         ov = torch.empty(self.capacity, dtype=self.vdtype, device=self.rt.device)
         cnt = torch.zeros(1, dtype=torch.int64, device=self.rt.device)
-        N.check(lib.mvb_kv_dump(self.vcode, C.c_void_p(self.keys_buf.local_ptr),
-                                C.c_void_p(self.vals_buf.local_ptr), C.c_int64(self.capacity),
-                                C.c_void_p(ok.data_ptr()), C.c_void_p(ov.data_ptr()),
-                                C.c_void_p(cnt.data_ptr()), C.c_void_p(N.stream_ptr())), "mvb_kv_dump")
+        lib.mvb_kv_dump(self.vcode, self.keys_buf.local_ptr, self.vals_buf.local_ptr, self.capacity, ok, ov, cnt,
+                        N.stream_ptr())
         n = int(cnt.item())
         stream.write(struct.pack("<q", n))
         stream.write(ok[:n].cpu().numpy().tobytes())

@@ -260,7 +260,6 @@ def scenario_async():
         check(f"get_gemm_peer_scratch_M{Mrows}", err2 < 4e-3 * 18 * 4, str(err2))
     mv.barrier()
     # device-side block protocol across ranks: bulk-engine pull from peer shards, one-sided delta push
-    import ctypes as C
     from multiverso_b200 import _native as N
     bt = mv.MatrixTable(40000, 300, "float32", min_value=-1.0, max_value=1.0, seed=11)
     mv.barrier()
@@ -269,17 +268,13 @@ def scenario_async():
     kk = bids.numel()
     ndev = torch.tensor([kk], dtype=torch.int32, device="cuda")
     cache = torch.zeros(kk + 7, 300, device="cuda"); old = torch.zeros(kk + 7, 300, device="cuda")
-    lib, stp = N.cuda_lib(), C.c_void_p(N.stream_ptr())
-    N.check(lib.mvb_rows_pull_bulk(C.byref(bt._rowmap), C.c_int(4), C.c_void_p(bids.data_ptr()), C.c_void_p(ndev.data_ptr()),
-                                   C.c_int64(kk + 7), C.c_void_p(cache.data_ptr()), C.c_void_p(old.data_ptr()),
-                                   C.c_int64(300), C.c_int(6), stp), "pull")
+    lib, stp = N.cuda_lib(), N.stream_ptr()
+    lib.mvb_rows_pull_bulk(bt._rowmap, 4, bids, ndev, kk + 7, cache, old, 300, 6, stp)
     torch.cuda.synchronize()
     check("rows_pull_bulk_peer", torch.equal(cache[:kk], bfull[bids.long()]) and torch.equal(old[:kk], bfull[bids.long()]))
     mv.barrier()
     cache[:kk] += float(r + 1)
-    N.check(lib.mvb_rows_push_delta_bulk(C.byref(bt._rowmap), C.c_void_p(bids.data_ptr()), C.c_void_p(ndev.data_ptr()),
-                                         C.c_int64(kk + 7), C.c_void_p(cache.data_ptr()), C.c_void_p(old.data_ptr()),
-                                         C.c_int64(300), C.c_float(0.5), C.c_int(6), stp), "push")
+    lib.mvb_rows_push_delta_bulk(bt._rowmap, bids, ndev, kk + 7, cache, old, 300, 0.5, 6, stp)
     torch.cuda.synchronize()
     mv.barrier()
     bexp = bfull.clone()

@@ -90,14 +90,16 @@ def _c_kind(t: str) -> str:
     if "*" in t or "[" in t or t.split()[0] == "TableHandler":
         return "ptr"
     base = t.split()[0]
-    return {"int": "i32", "int64_t": "i64", "float": "f32", "double": "f64", "void": "void", "char": "i8"}[base]
+    return {"int": "i32", "int64_t": "i64", "uint32_t": "u32", "uint64_t": "u64", "float": "f32", "double": "f64",
+            "void": "void", "char": "i8"}[base]
 
 
-def _parse_c_decls(text: str):
-    """name -> (return kind, [parameter kinds]) for every MV_* prototype in a C declaration block."""
+def _parse_c_decls(text: str, prefix: str = "MV_"):
+    """name -> (return kind, [parameter kinds]) for every ``prefix``* prototype in a C declaration block."""
     out = {}
     text = re.sub(r"/\*.*?\*/", " ", text, flags=re.S)
-    for m in re.finditer(r"(?:DllExport\s+)?((?:const\s+)?\w+\s*\*?)\s*(MV_\w+)\s*\(([^)]*)\)\s*;", text):
+    text = re.sub(r"//[^\n]*", " ", text)
+    for m in re.finditer(r"(?:DllExport\s+)?((?:const\s+)?\w+\s*\*?)\s*(" + prefix + r"\w+)\s*\(([^)]*)\)\s*;", text):
         ret, name, params = m.group(1), m.group(2), m.group(3).strip()
         kinds = []
         if params and params != "void":

@@ -1,8 +1,6 @@
 """K8 numerics against plain PyTorch references: the sparse / dense CUDA-core kernels, FTRL, regularisers
 (csrc/cuda/logreg.cu) and the wide dense path whose two products run on the hand-written wgmma kernel
 (no library GEMM), each compared with fp32/fp64 torch on the same inputs."""
-import ctypes as C
-
 import pytest
 import torch
 
@@ -50,7 +48,7 @@ def test_dense_cuda_core_kernel(mv_device, n, dim, out, objective):
     a.x, a.labels, a.n, a.dim, a.out, a.objective = x.data_ptr(), labels.data_ptr(), n, dim, out, objective
     a.w, a.grad, a.loss_sum, a.correct = w.data_ptr(), grad.data_ptr(), loss.data_ptr(), correct.data_ptr()
     a.pred, a.err, a.compute_grad = pred.data_ptr(), err.data_ptr(), 1
-    N.check(N.cuda_lib().mvb_lr_dense_fwd_bwd(C.byref(a), C.c_void_p(N.stream_ptr())))
+    N.cuda_lib().mvb_lr_dense_fwd_bwd(a, N.stream_ptr())
     torch.cuda.synchronize()
     rl, rc, rp, rg = _ref_dense(x, labels, w, objective, out)
     assert abs(loss.item() - rl) / max(abs(rl), 1e-6) < 1e-3
@@ -100,7 +98,7 @@ def test_sparse_kernel_matches_reference(mv_device):
     a.objective, a.w, a.dim, a.out = 1, w.data_ptr(), dim, 1
     a.grad, a.loss_sum, a.correct, a.pred, a.err, a.compute_grad = (grad.data_ptr(), loss.data_ptr(), correct.data_ptr(),
                                                                       pred.data_ptr(), err.data_ptr(), 1)
-    N.check(N.cuda_lib().mvb_lr_sparse_fwd_bwd(C.byref(a), C.c_void_p(N.stream_ptr())))
+    N.cuda_lib().mvb_lr_sparse_fwd_bwd(a, N.stream_ptr())
     torch.cuda.synchronize()
     X = torch.zeros(n, dim, dtype=torch.float64, device="cuda")
     X.index_put_((torch.arange(n, device="cuda").repeat_interleave(nnz_per), keys), vals.double(), accumulate=True)
@@ -115,14 +113,13 @@ def test_sparse_kernel_matches_reference(mv_device):
 
 def test_ftrl_and_regularisers(mv_device):
     from multiverso_b200 import _native as N
-    lib, st = N.cuda_lib(), C.c_void_p(N.stream_ptr())
+    lib, st = N.cuda_lib(), N.stream_ptr()
     g = torch.Generator(device="cuda").manual_seed(5)
     L = 10007
     z = torch.randn(L, device="cuda", generator=g); nn = torch.rand(L, device="cuda", generator=g) * 4
     w = torch.zeros(L, device="cuda")
     alpha, beta, l1, l2 = 0.1, 1.0, 0.5, 0.2
-    N.check(lib.mvb_ftrl_weights(C.c_void_p(z.data_ptr()), C.c_void_p(nn.data_ptr()), C.c_void_p(w.data_ptr()),
-                                 C.c_int64(L), C.c_float(alpha), C.c_float(beta), C.c_float(l1), C.c_float(l2), st))
+    lib.mvb_ftrl_weights(z, nn, w, L, alpha, beta, l1, l2, st)
     ref = torch.where(z.abs() <= l1, torch.zeros_like(z),
                       -(z - torch.sign(z) * l1) / ((beta + nn.sqrt()) / alpha + l2))
     torch.cuda.synchronize()
@@ -130,7 +127,6 @@ def test_ftrl_and_regularisers(mv_device):
     grad = torch.randn(L, device="cuda", generator=g)
     for typ, fn in ((1, lambda w_: torch.sign(w_) * 0.01), (2, lambda w_: w_ * 0.01)):
         gg = grad.clone()
-        N.check(lib.mvb_regularize(C.c_void_p(gg.data_ptr()), C.c_void_p(w.data_ptr()), C.c_int64(L), C.c_int(typ),
-                                   C.c_float(0.01), st))
+        lib.mvb_regularize(gg, w, L, typ, 0.01, st)
         torch.cuda.synchronize()
         assert torch.allclose(gg, grad + fn(w), atol=1e-7)

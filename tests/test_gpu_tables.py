@@ -261,7 +261,6 @@ def test_checkpoint_roundtrip(mv_device, tmp_path):
 def test_watchdog_reports_dead_peer(mv_device):
     """Fault injection (SURVEY 5.3): a device-side wait on a flag that nobody will ever write must end
     with a diagnostic naming the channel / peer after -barrier_timeout_s, not hang the GPU."""
-    import ctypes as C
     import time
     from multiverso_b200 import _native as N
     from multiverso_b200.runtime import Runtime
@@ -271,9 +270,7 @@ def test_watchdog_reports_dead_peer(mv_device):
     kill, Log.kill_fatal = Log.kill_fatal, False
     try:
         t0 = time.time()
-        N.check(N.cuda_lib().mvb_wait(rt.pads_array(), rt.rank, rt.size, ch, C.c_uint64(7), C.c_uint32(1),
-                                      C.c_void_p(rt.err_flag.data_ptr()), C.c_double(0.05),
-                                      C.c_void_p(N.stream_ptr())), "mvb_wait")
+        N.cuda_lib().mvb_wait(rt.pads_array(), rt.rank, rt.size, ch, 7, 1, rt.err_flag, 0.05, N.stream_ptr())
         torch.cuda.synchronize()
         assert time.time() - t0 < 10.0                     # gave up after the budget, did not spin forever
         with pytest.raises(FatalError, match="watchdog"):

@@ -1,7 +1,5 @@
 """Device-side WordEmbedding block protocol (csrc/cuda/we_block.cu) against plain PyTorch references:
 PrepareData (bitmap-unique + prefix sum + negative pool), bulk-engine row pull and delta push."""
-import ctypes as C
-
 import pytest
 import torch
 
@@ -25,7 +23,7 @@ def _prep(tokens, V, K, prob, alias, cap_in, cap_out, seed=99):
     p.ids_in, p.ids_out = b["ids_in"].data_ptr(), b["ids_out"].data_ptr()
     p.neg_pool, p.pool_cap, p.counts = b["neg_pool"].data_ptr(), b["neg_pool"].numel(), b["counts"].data_ptr()
     p.cap_in, p.cap_out = cap_in, cap_out
-    N.check(N.cuda_lib().mvb_we_prepare(C.byref(p), C.c_void_p(N.stream_ptr())), "mvb_we_prepare")
+    N.cuda_lib().mvb_we_prepare(p, N.stream_ptr())
     torch.cuda.synchronize()
     return b
 
@@ -67,8 +65,7 @@ def test_we_prepare_pool_distribution(mv_device):
     V, K = 64, 5
     wts = np.arange(1, V + 1, dtype=np.float64)
     prob = np.empty(V, dtype=np.float32); alias = np.empty(V, dtype=np.int32)
-    assert N.cuda_lib().mvb_build_alias_table(wts.ctypes.data_as(C.c_void_p), C.c_int(V),
-                                               prob.ctypes.data_as(C.c_void_p), alias.ctypes.data_as(C.c_void_p)) == 0
+    assert N.cuda_lib().mvb_build_alias_table(wts.ctypes.data, V, prob.ctypes.data, alias.ctypes.data) == 0
     toks = torch.arange(200000, dtype=torch.int32, device="cuda") % V     # n_in = 64 -> 320 draws only
     b = _prep(toks, V, K, torch.from_numpy(prob).cuda(), torch.from_numpy(alias).cuda(), V, V)
     assert b["counts"][2].item() == K * V
@@ -98,10 +95,8 @@ def test_rows_pull_push_bulk(mv_device, rows, cols, k, lsu):
     n_dev = torch.tensor([k], dtype=torch.int32, device="cuda")
     cache = torch.full((cap, cols), 7.0, device="cuda")
     old = torch.full((cap, cols), 7.0, device="cuda")
-    lib, st = N.cuda_lib(), C.c_void_p(N.stream_ptr())
-    N.check(lib.mvb_rows_pull_bulk(C.byref(t._rowmap), C.c_int(4), C.c_void_p(ids_buf.data_ptr()),
-                                   C.c_void_p(n_dev.data_ptr()), C.c_int64(cap), C.c_void_p(cache.data_ptr()),
-                                   C.c_void_p(old.data_ptr()), C.c_int64(cols), C.c_int(-1 if lsu else 5), st), "pull")
+    lib, st = N.cuda_lib(), N.stream_ptr()
+    lib.mvb_rows_pull_bulk(t._rowmap, 4, ids_buf, n_dev, cap, cache, old, cols, -1 if lsu else 5, st)
     torch.cuda.synchronize()
     assert torch.equal(cache[:k], full0[ids.long()]) and torch.equal(old[:k], full0[ids.long()])
     assert bool((cache[k:] == 7.0).all()) and bool((old[k:] == 7.0).all())       # the device count bounds the copy
@@ -109,9 +104,7 @@ def test_rows_pull_push_bulk(mv_device, rows, cols, k, lsu):
     delta = torch.randn(k, cols, device="cuda", generator=torch.Generator(device="cuda").manual_seed(1))
     delta[::5] = 0
     cache[:k] += delta
-    N.check(lib.mvb_rows_push_delta_bulk(C.byref(t._rowmap), C.c_void_p(ids_buf.data_ptr()),
-                                         C.c_void_p(n_dev.data_ptr()), C.c_int64(cap), C.c_void_p(cache.data_ptr()),
-                                         C.c_void_p(old.data_ptr()), C.c_int64(cols), C.c_float(0.5), C.c_int(-2 if lsu else 3), st), "push")
+    lib.mvb_rows_push_delta_bulk(t._rowmap, ids_buf, n_dev, cap, cache, old, cols, 0.5, -2 if lsu else 3, st)
     torch.cuda.synchronize()
     exp = full0.clone()
     exp[ids.long()] += (cache[:k] - old[:k]) * 0.5
@@ -122,8 +115,6 @@ def test_rows_pull_push_bulk(mv_device, rows, cols, k, lsu):
     assert torch.equal(got[untouched], full0[untouched])
     # host-count variant (n_ptr = NULL)
     cache2 = torch.zeros(k, cols, device="cuda")
-    N.check(lib.mvb_rows_pull_bulk(C.byref(t._rowmap), C.c_int(4), C.c_void_p(ids.data_ptr()), C.c_void_p(0),
-                                   C.c_int64(k), C.c_void_p(cache2.data_ptr()), C.c_void_p(0), C.c_int64(cols),
-                                   C.c_int(0), st), "pull2")
+    lib.mvb_rows_pull_bulk(t._rowmap, 4, ids, None, k, cache2, None, cols, 0, st)
     torch.cuda.synchronize()
     assert torch.equal(cache2, got[ids.long()])

@@ -19,7 +19,6 @@ def test_sgns_fast_kernel_matches_reference(mv_device, variant):
     is only through red.add accumulation: warps may or may not observe each other's updates
     (Hogwild), an O(lr^2) effect, so the test uses a small lr and compares the UPDATES with a
     relative tolerance (a wrong sign / missing term would be off by >= 100%)."""
-    import ctypes as C
     from multiverso_b200 import _native as N
     V, D, K, lr = 64, 300, 5, 1e-3
     torch.manual_seed(0)
@@ -57,7 +56,7 @@ def test_sgns_fast_kernel_matches_reference(mv_device, variant):
     a.vocab, a.neg_pool, a.neg_pool_size = V, pool.data_ptr(), 1
     a.seed, a.loss_sum, a.pair_count = 1234, loss.data_ptr(), pairs.data_ptr()
     a.variant = variant
-    N.check(N.cuda_lib().mvb_sgns_train(C.byref(a), C.c_void_p(N.stream_ptr())))
+    N.cuda_lib().mvb_sgns_train(a, N.stream_ptr())
     torch.cuda.synchronize()
     assert int(pairs.item()) == 8
     d_in, d_out = w_in.double().cpu() - i0, w_out.double().cpu() - o0
@@ -148,7 +147,6 @@ def test_sgns_det_kernel_matches_schedule(mv_device, n_tok, dim):
 
 
 def _check_schedule(fn, n_tok, dim, tol):
-    import ctypes as C
     from multiverso_b200 import _native as N
     V, D, K, W, lr, seed = 4096, dim, 5, 5, 1e-4, 0xC0FFEE
     g = torch.Generator().manual_seed(1)
@@ -200,7 +198,7 @@ def _check_schedule(fn, n_tok, dim, tol):
     a.seed, a.loss_sum, a.pair_count = seed, loss.data_ptr(), pairs.data_ptr()
     si, so = s_in.cuda(), s_out.cuda()
     a.scale_in, a.scale_out = si.data_ptr(), so.data_ptr()
-    N.check(getattr(N.cuda_lib(), fn)(C.byref(a), C.c_void_p(N.stream_ptr())))
+    getattr(N.cuda_lib(), fn)(a, N.stream_ptr())
     torch.cuda.synchronize()
     assert int(pairs.item()) == n_pairs
     d_in, d_out = w_in.double().cpu() - i0, w_out.double().cpu() - o0
@@ -219,7 +217,6 @@ def test_sgns_window_kernel_maps_and_cta_cap(mv_device):
     """Block mode of variant 20: rows live in a compact cache addressed through id -> slot maps
     (world > 1), the grid is capped (max_ctas) and rows are padded (ld > dim); result must equal the
     identity-mapped full-grid run on the same data (same seed => same schedule) up to Hogwild noise."""
-    import ctypes as C
     from multiverso_b200 import _native as N
     V, D, LD, K, W, lr, seed = 3000, 300, 320, 5, 5, 1e-3, 77
     g = torch.Generator().manual_seed(3)
@@ -241,7 +238,7 @@ def test_sgns_window_kernel_maps_and_cta_cap(mv_device):
         a.vocab, a.alias_prob, a.alias_idx = V, prob.data_ptr(), alias.data_ptr()
         a.map_in, a.map_out = N.ptr(map_in), N.ptr(map_out)
         a.seed, a.pair_count, a.max_ctas = seed, pairs.data_ptr(), max_ctas
-        N.check(N.cuda_lib().mvb_sgns_train_win(C.byref(a), C.c_void_p(N.stream_ptr())))
+        N.cuda_lib().mvb_sgns_train_win(a, N.stream_ptr())
         torch.cuda.synchronize()
         return int(pairs.item())
 
@@ -264,7 +261,6 @@ def test_sgns_window_kernel_maps_and_cta_cap(mv_device):
 def test_sgns_det_kernel_maps_and_ld(mv_device):
     """Deterministic K7 over several waves on a cache through id -> slot maps with padded rows (ld > dim):
     same schedule and arithmetic, so it equals the identity-mapped run exactly; the padding is never written."""
-    import ctypes as C
     from multiverso_b200 import _native as N
     V, D, LD = 3000, 300, 320
     g = torch.Generator().manual_seed(3)
@@ -280,7 +276,7 @@ def test_sgns_det_kernel_maps_and_ld(mv_device):
         a.dim, a.ld, a.window, a.negative, a.lr, a.seed = D, w_in.stride(0), 5, 5, 1e-2, 77
         a.vocab, a.alias_prob, a.alias_idx, a.map_in, a.map_out = V, prob.data_ptr(), alias.data_ptr(), N.ptr(m), N.ptr(m)
         a.pair_count, a.loss_sum = out.data_ptr(), out.data_ptr() + 8
-        N.check(N.cuda_lib().mvb_sgns_train_det(C.byref(a), C.c_void_p(N.stream_ptr())))
+        N.cuda_lib().mvb_sgns_train_det(a, N.stream_ptr())
         return out.cpu()
 
     a_in, a_out = base[0].clone(), base[1].clone()

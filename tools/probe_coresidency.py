@@ -1,6 +1,5 @@
 """Probe: do the register-path row kernels co-reside with the persistent K7 CTAs?  (1 GPU)
 Times a row pull alone, and the same pull launched ~300 us after K7 started on another stream."""
-import ctypes as C
 import os
 import sys
 
@@ -25,9 +24,7 @@ main = torch.cuda.current_stream()
 
 
 def pull(mode):
-    N.check(lib.mvb_rows_pull_bulk(C.byref(t._rowmap), C.c_int(4), C.c_void_p(ids.data_ptr()), C.c_void_p(0), C.c_int64(k),
-                                   C.c_void_p(cache.data_ptr()), C.c_void_p(old.data_ptr()), C.c_int64(D), C.c_int(mode),
-                                   C.c_void_p(torch.cuda.current_stream().cuda_stream)), "pull")
+    lib.mvb_rows_pull_bulk(t._rowmap, 4, ids, None, k, cache, old, D, mode, torch.cuda.current_stream().cuda_stream)
 
 
 for mode in (-1, -2, 10):
