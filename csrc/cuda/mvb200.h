@@ -506,6 +506,62 @@ int mvb_embedding_bag_bwd(const MvbEmbBag* a, void* stream);
 /* dpsw[j] = s_bag * <dout[bag(j)], W[ids_j, :dim]> (ids in lookup order) */
 int mvb_embedding_bag_psw_grad(const MvbEmbBag* a, void* stream);
 
+/* ---- embedding-bag collection: F features over T row-sharded fp32 tables (emb_bag_coll.cu) -------- */
+/* Jagged input: ids holds feature 0's lookups for bags 0..B-1, then feature 1's, ...; offsets[g] (g = f B + b)
+ * is the exclusive scan of the [F x B] lengths. Feature f writes columns [col, col + round4(dim)) of out[b].
+ * Each feature's bags are summed exactly as mvb_embedding_bag_fwd sums them over its table. The backward sorts
+ * keys key_base[table] + id, so each table is one contiguous segment of the sorted order, cut into its own
+ * chunks: a table's gradient depends only on its own lookups. The table and feature descriptors live in device
+ * memory; they are built once and read by every call. The caller validates lengths and ids. */
+enum { MVB_EMB_NO_PUSH = 2 };  /* a collection table whose gradient is not pushed */
+typedef struct MvbEmbTable {
+  MvbRowMap wmap;            /* fp32 shards, row pitch wmap.num_col (% 4 == 0), rows_per_server >= 1       */
+  int64_t dim;               /* columns used, 1 <= dim <= min(512, wmap.num_col)                          */
+  int64_t key_base;          /* backward key of row id: key_base + id (exclusive scan of the num_row)     */
+  int mean;                  /* 0 sum, 1 mean                                                            */
+  int epilogue;              /* MVB_EMB_PUSH, MVB_EMB_COMPACT or MVB_EMB_NO_PUSH                         */
+  float scale;               /* the pushed value is scale * g                                            */
+  int64_t ldg;               /* compact: row pitch of the table's gradient, % 4 == 0, >= round4(dim)     */
+} MvbEmbTable;
+typedef struct MvbEmbFeature {
+  int table;                 /* index into the table descriptors                                         */
+  int64_t col;               /* first column of the feature in out / dout, % 4 == 0                      */
+} MvbEmbFeature;
+typedef struct MvbEmbColl {
+  const MvbEmbTable* tables;      /* device [T]                                                          */
+  const MvbEmbFeature* features;  /* device [F]                                                          */
+  const int* class_feats;         /* device [F]: the features grouped by register class (1..4 float4 per lane,
+                                     round4(dim) <= 128, 256, 384, 512)                                   */
+  int class_off[5];               /* class k holds class_feats[class_off[k - 1] .. class_off[k]), k = 1..4 */
+  int T, F;
+  int64_t B;                      /* bags per feature                                                    */
+  const int64_t* ids;             /* [L] row ids, feature-major                                          */
+  int64_t L;
+  const int64_t* offsets;         /* [F B]                                                               */
+  const float* psw;               /* [L] or NULL                                                         */
+  float* out;                     /* forward: [B x ldo], ldo % 4 == 0, 16-byte aligned                   */
+  int64_t ldo;
+  const float* dout;              /* backward, psw grad: [B x ldd], ldd % 4 == 0, 16-byte aligned        */
+  int64_t ldd;
+  int64_t* keys;                  /* [L], written by mvb_emb_coll_keys                                   */
+  const int64_t* skeys;           /* [L] keys sorted ascending, equal keys in ascending position         */
+  const int64_t* perm;            /* [L] lookup position of each sorted key                              */
+  int64_t* info;                  /* device int64 [4 T + 2]: per table {U, first unique, grads offset,
+                                     uniq offset}, then the total floats of grads and entries of uniq      */
+  float* grads;                   /* compact tables: table t's [U x ldg] gradient at grads + grads offset */
+  int64_t* uniq;                  /* compact tables: table t's [U] row ids at uniq + uniq offset         */
+  float* dpsw;                    /* psw grad: [L]                                                       */
+  void* scratch;                  /* mvb_emb_coll_scratch_bytes(L, T, max dim) bytes of device memory    */
+  int64_t scratch_bytes;
+} MvbEmbColl;
+int mvb_emb_coll_fwd(const MvbEmbColl* a, void* stream);
+int64_t mvb_emb_coll_scratch_bytes(int64_t L, int T, int64_t max_dim);
+/* backward, in order: keys (then sort them), count (unique ids per table into info), bwd (the epilogues) */
+int mvb_emb_coll_keys(const MvbEmbColl* a, void* stream);
+int mvb_emb_coll_count(const MvbEmbColl* a, void* stream);
+int mvb_emb_coll_bwd(const MvbEmbColl* a, void* stream);
+int mvb_emb_coll_psw_grad(const MvbEmbColl* a, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -155,6 +155,25 @@ class EmbBag(C.Structure):
                 ("uniq", vp), ("n_unique", vp), ("dpsw", vp), ("scratch", vp), ("scratch_bytes", i64)]
 
 
+EMB_NO_PUSH = 2
+
+
+class EmbTable(C.Structure):
+    _fields_ = [("wmap", RowMap), ("dim", i64), ("key_base", i64), ("mean", C.c_int), ("epilogue", C.c_int),
+                ("scale", C.c_float), ("ldg", i64)]
+
+
+class EmbFeature(C.Structure):
+    _fields_ = [("table", C.c_int), ("col", i64)]
+
+
+class EmbColl(C.Structure):
+    _fields_ = [("tables", vp), ("features", vp), ("class_feats", vp), ("class_off", C.c_int * 5), ("T", C.c_int),
+                ("F", C.c_int), ("B", i64), ("ids", vp), ("L", i64), ("offsets", vp), ("psw", vp), ("out", vp),
+                ("ldo", i64), ("dout", vp), ("ldd", i64), ("keys", vp), ("skeys", vp), ("perm", vp), ("info", vp),
+                ("grads", vp), ("uniq", vp), ("dpsw", vp), ("scratch", vp), ("scratch_bytes", i64)]
+
+
 class NativeError(RuntimeError):
     pass
 
@@ -270,6 +289,12 @@ _CUDA_FUNCS = {
     "mvb_embedding_bag_fwd": _status(C.POINTER(EmbBag), Ptr),
     "mvb_embedding_bag_bwd": _status(C.POINTER(EmbBag), Ptr),
     "mvb_embedding_bag_psw_grad": _status(C.POINTER(EmbBag), Ptr),
+    "mvb_emb_coll_scratch_bytes": _unchecked(i64, i64, i32, i64),
+    "mvb_emb_coll_fwd": _status(C.POINTER(EmbColl), Ptr),
+    "mvb_emb_coll_keys": _status(C.POINTER(EmbColl), Ptr),
+    "mvb_emb_coll_count": _status(C.POINTER(EmbColl), Ptr),
+    "mvb_emb_coll_bwd": _status(C.POINTER(EmbColl), Ptr),
+    "mvb_emb_coll_psw_grad": _status(C.POINTER(EmbColl), Ptr),
 }
 
 
