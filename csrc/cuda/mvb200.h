@@ -562,6 +562,36 @@ int mvb_emb_coll_count(const MvbEmbColl* a, void* stream);
 int mvb_emb_coll_bwd(const MvbEmbColl* a, void* stream);
 int mvb_emb_coll_psw_grad(const MvbEmbColl* a, void* stream);
 
+/* ---- sampled softmax over a row-sharded fp32 MatrixTable (sampled_softmax.cu) ---------------------------- */
+/* Example b has the true logit t_b = x_b . w_{y_b} - log(S q(y_b)) and the sampled logits
+ * s_bj = logits[b, j] - logq_c[j], -inf where cand[j] == y_b; loss_b = logsumexp(t_b, s_b.) - t_b. The row
+ * gathers and the products logits = X W_S^T, dX = E W_S, dW_S = E^T X are mvb_get_rows and mvb_get_gemm_fused. */
+typedef struct MvbSampledSoftmax {
+  const float* alias_prob;   /* [n] alias table of q (mvb_build_alias_table)                               */
+  const int* alias_idx;      /* [n]                                                                        */
+  const float* logq;         /* [n] log q(k)                                                               */
+  int64_t n;                 /* rows of the table, < 2^31                                                  */
+  uint64_t seed, step;       /* draw j of a call is a pure function of (seed, step, j)                     */
+  int64_t S, S_pad;          /* draws per call; S_pad = round4(S), the row pitch of logits                 */
+  float log_s;               /* log S in fp32                                                              */
+  int64_t* cand;             /* sample: [S] drawn row ids                                                  */
+  float* logq_c;             /* sample: [S] log_s + logq[cand]                                             */
+  const float* x;            /* [B x d] hidden, 16-byte aligned                                            */
+  const float* w_y;          /* [B x d] the label rows                                                     */
+  int64_t B, B_pad, d;       /* d % 4 == 0; B_pad = round4(B), the row pitch of e_t                        */
+  const int64_t* labels;     /* [B] in [0, n) (validated by the caller)                                    */
+  float* logits;             /* [B x S_pad]: X W_S^T in the forward; the backward overwrites it with E      */
+  float* loss;               /* forward: [B]                                                               */
+  float* lse;                /* forward: [B] logsumexp of the row                                          */
+  float* t_true;             /* forward: [B] the true logit                                                */
+  const float* g;            /* backward: [B] gradient of the loss                                         */
+  float* e_t;                /* backward: [S_pad x B_pad] E^T, zero on padding rows and columns            */
+  float* e_true;             /* backward: [B] g_b (exp(t_b - lse_b) - 1)                                   */
+} MvbSampledSoftmax;
+int mvb_ss_sample(const MvbSampledSoftmax* a, void* stream);
+int mvb_ss_fwd_epilogue(const MvbSampledSoftmax* a, void* stream);
+int mvb_ss_bwd_epilogue(const MvbSampledSoftmax* a, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

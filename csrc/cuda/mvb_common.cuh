@@ -224,6 +224,13 @@ struct Updater<MVB_UPD_DCASGDA, T> {
 };
 // int tables always use the plain add (reference: Updater<int>::GetUpdater).
 
+// 64-bit finaliser of MurmurHash3: the counter-based RNG of the on-device samplers (a draw is a pure
+// function of its seed and index, so every rank and every run draws the same ids).
+MVB_DEVINL uint64_t hash64(uint64_t x) {
+  x ^= x >> 33; x *= 0xff51afd7ed558ccdull; x ^= x >> 33; x *= 0xc4ceb9fe1a85ec53ull; x ^= x >> 33;
+  return x;
+}
+
 MVB_DEVINL float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

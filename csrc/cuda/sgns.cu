@@ -23,10 +23,6 @@
 namespace {
 
 MVB_DEVINL uint64_t lcg_next(uint64_t x) { return x * 25214903917ull + 11ull; }  // util.cpp:144-146
-MVB_DEVINL uint64_t hash64(uint64_t x) {
-  x ^= x >> 33; x *= 0xff51afd7ed558ccdull; x ^= x >> 33; x *= 0xc4ceb9fe1a85ec53ull; x ^= x >> 33;
-  return x;
-}
 MVB_DEVINL float sigmoidf_fast(float x) { return __fdividef(1.0f, 1.0f + __expf(-x)); }
 MVB_DEVINL float softplus_neg(float x) {  // -log(sigmoid(x)) = log(1+exp(-x))
   return fmaxf(-x, 0.f) + log1pf(__expf(-fabsf(x)));

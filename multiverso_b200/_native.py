@@ -174,6 +174,13 @@ class EmbColl(C.Structure):
                 ("grads", vp), ("uniq", vp), ("dpsw", vp), ("scratch", vp), ("scratch_bytes", i64)]
 
 
+class SampledSoftmax(C.Structure):
+    _fields_ = [("alias_prob", vp), ("alias_idx", vp), ("logq", vp), ("n", i64), ("seed", C.c_uint64),
+                ("step", C.c_uint64), ("S", i64), ("S_pad", i64), ("log_s", C.c_float), ("cand", vp), ("logq_c", vp),
+                ("x", vp), ("w_y", vp), ("B", i64), ("B_pad", i64), ("d", i64), ("labels", vp), ("logits", vp),
+                ("loss", vp), ("lse", vp), ("t_true", vp), ("g", vp), ("e_t", vp), ("e_true", vp)]
+
+
 class NativeError(RuntimeError):
     pass
 
@@ -295,6 +302,9 @@ _CUDA_FUNCS = {
     "mvb_emb_coll_count": _status(C.POINTER(EmbColl), Ptr),
     "mvb_emb_coll_bwd": _status(C.POINTER(EmbColl), Ptr),
     "mvb_emb_coll_psw_grad": _status(C.POINTER(EmbColl), Ptr),
+    "mvb_ss_sample": _status(C.POINTER(SampledSoftmax), Ptr),
+    "mvb_ss_fwd_epilogue": _status(C.POINTER(SampledSoftmax), Ptr),
+    "mvb_ss_bwd_epilogue": _status(C.POINTER(SampledSoftmax), Ptr),
 }
 
 

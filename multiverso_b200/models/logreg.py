@@ -22,6 +22,7 @@ from typing import Dict, Optional
 import torch
 
 from .. import _native as N
+from ..ops.get_gemm import gemm_nt
 from ..runtime import Runtime
 from ..tables.device import ArrayDeviceTable
 from ..tables.options import AddOption
@@ -132,22 +133,6 @@ def dense_gemm_step(x: torch.Tensor, labels: torch.Tensor, w: torch.Tensor, grad
     return loss, correct, p
 
 
-def _tc_gemm_nt(x: torch.Tensor, w: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
-    """out[M, N] = x[M, K] @ w[N, K]^T on the hand-written wgmma kernel (gemm_fused.cu: TMA-fed
-    wgmma, TF32 operands, fp32 accumulation in registers) -- `w` is presented as a one-server
-    row map, so the same kernel that streams table shards multiplies two local matrices.  K % 4 == 0."""
-    M, K = x.shape
-    Nr = w.shape[0]
-    g = N.GetGemm()
-    g.x, g.y, g.w_cache = x.data_ptr(), out.data_ptr(), None
-    g.M, g.N, g.K = M, Nr, K
-    g.wmap.num_row, g.wmap.num_col, g.wmap.nservers, g.wmap.rows_per_server = Nr, K, 1, Nr
-    g.wmap.shard_ptrs[0] = w.data_ptr()
-    g.local_server = 0
-    N.cuda_lib().mvb_get_gemm_fused(g, N.stream_ptr())
-    return out
-
-
 class LogRegModel:
     """Model (local) / PSModel (``use_ps``) on the device backend."""
 
@@ -247,7 +232,7 @@ class LogRegModel:
             x2 = x.view(n, self.dim)
             n_pad = (n + 3) // 4 * 4
             logits = torch.empty(n, self.out, device=dev)
-            _tc_gemm_nt(x2, self._weights().view(self.out, self.dim), logits)
+            gemm_nt(x2, self._weights().view(self.out, self.dim), logits)
             err_t = torch.empty(self.out, n_pad, device=dev)
             lib.mvb_lr_wide_epilogue(logits, labels, n, self.out, self.objective, err_t, n_pad, pred, self.loss,
                                      self.correct, st)
@@ -256,7 +241,7 @@ class LogRegModel:
                 x_t = torch.empty(self.dim, n_pad, device=dev)
                 lib.mvb_transpose_pad_f32(x2, n, self.dim, self.dim, x_t, n_pad, st)
                 dw = torch.empty(self.out, self.dim, device=dev)
-                _tc_gemm_nt(err_t, x_t, dw)                      # [out x n] . [dim x n]^T
+                gemm_nt(err_t, x_t, dw)                      # [out x n] . [dim x n]^T
                 lib.mvb_axpy_f32(self.grad, dw, self.out * self.dim, 1.0, st)
                 self.kernel_launches += 3
             return

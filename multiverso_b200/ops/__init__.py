@@ -1,9 +1,10 @@
 from .embedding import PSEmbedding, embedding_bag, embedding_bag_reference
 from .embedding_collection import EmbeddingBagConfig, PSEmbeddingCollection
-from .get_gemm import get_gemm, get_gemm_supported
+from .get_gemm import gemm_nt, get_gemm, get_gemm_supported
 from .ps_linear import PSLinear, ps_linear
+from .sampled_softmax import PSSampledSoftmax
 from .topk import TOPK_MAX, topk_cosine, topk_cosine_reference
 
 __all__ = ["get_gemm", "get_gemm_supported", "ps_linear", "PSLinear", "topk_cosine", "topk_cosine_reference",
            "TOPK_MAX", "embedding_bag", "embedding_bag_reference", "PSEmbedding",
-           "EmbeddingBagConfig", "PSEmbeddingCollection"]
+           "EmbeddingBagConfig", "PSEmbeddingCollection", "gemm_nt", "PSSampledSoftmax"]

@@ -51,3 +51,19 @@ def get_gemm(table, x: torch.Tensor, out: torch.Tensor = None) -> torch.Tensor:
     g.local_server = table.sid if table.S > 1 else 0
     N.cuda_lib().mvb_get_gemm_fused(g, N.stream_ptr())
     return out
+
+
+def gemm_nt(x: torch.Tensor, w: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
+    """out[M, N] = x[M, K] @ w[N, K]^T on the hand-written wgmma kernel (gemm_fused.cu: TMA-fed
+    wgmma, TF32 operands, fp32 accumulation in registers) -- `w` is presented as a one-server
+    row map, so the same kernel that streams table shards multiplies two local matrices.  K % 4 == 0."""
+    M, K = x.shape
+    Nr = w.shape[0]
+    g = N.GetGemm()
+    g.x, g.y, g.w_cache = x.data_ptr(), out.data_ptr(), None
+    g.M, g.N, g.K = M, Nr, K
+    g.wmap.num_row, g.wmap.num_col, g.wmap.nservers, g.wmap.rows_per_server = Nr, K, 1, Nr
+    g.wmap.shard_ptrs[0] = w.data_ptr()
+    g.local_server = 0
+    N.cuda_lib().mvb_get_gemm_fused(g, N.stream_ptr())
+    return out
