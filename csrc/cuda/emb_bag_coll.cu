@@ -8,109 +8,33 @@
 //            its table bit for bit. One launch per register class (1..4 float4 per lane) present.
 //  bwd       keys key_base[table] + id, sorted with their positions: each table becomes one contiguous segment
 //            ordered by (id, position). Every segment is cut into its own chunks of EMB_CHUNK starting at its
-//            first lookup, and the runs are summed and merged as emb_bwd_main / emb_bwd_merge do; a lookup's
-//            dout columns are those of its feature. A table's gradient therefore depends only on its own lookups
-//            and equals one mvb_embedding_bag_bwd over its features' bags stacked in feature order.
+//            first lookup, and the runs are summed and merged by emb_run_sum / emb_merge_run, as in emb_bag.cu;
+//            a lookup's dout columns are those of its feature. A table's gradient therefore depends only on its own
+//            lookups and equals one mvb_embedding_bag_bwd over its features' bags stacked in feature order.
 //              push     red.add.v4.f32 of scale * g into the owner's row (default / sgd tables)
 //              compact  table t's grads[u] = scale * g, uniq[u] = id, u = rank among t's unique ids
 //  psw_grad  dpsw_j = s_bag * <dout[bag(j), feature columns], W_table[ids_j, :dim]>, one warp per lookup.
+// The algorithms live in emb_bag.cuh and are the ones emb_bag.cu runs; the kernels here find each bag's table and
+// output columns and each chunk's table segment, and pass them on.
 #include "emb_bag.cuh"
 
 namespace {
-
-// float4 vectors per lane of a dim: emb_fwd_kernel's and emb_bwd_*'s template argument
-MVB_DEVINL int vpl_of(int nv) { return nv <= 32 ? 1 : (nv + 31) >> 5; }
-int vpl_of_host(int64_t dim) {
-  const int64_t nv = (dim + 3) / 4;
-  return nv <= 32 ? 1 : (int)((nv + 31) / 32);
-}
-
-// row r of a table: the address row_of gives for the same row map
-MVB_DEVINL float* trow(const MvbEmbTable* t, int64_t r) {
-  const int64_t rps = t->wmap.rows_per_server;
-  int64_t o = r / rps;
-  if (o > t->wmap.nservers - 1) o = t->wmap.nservers - 1;
-  return (float*)t->wmap.shard_ptrs[o] + (r - o * rps) * t->wmap.num_col;
-}
 
 // ------------------------------------------------------------------------------------------------ forward
 // flat bags of the nf features class_feats[k0 .. k0 + nf), all of register class VPL
 template <int VPL>
 __global__ void __launch_bounds__(256)
 emb_coll_fwd_kernel(const __grid_constant__ MvbEmbColl a, int k0, int nf) {
-  const int lane = threadIdx.x & 31;
   const int64_t FB = (int64_t)a.F * a.B;
-  const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
-  for (int64_t w = warp; w < (int64_t)nf * a.B; w += nwarps) {
+  for (int64_t w = warp_id(); w < (int64_t)nf * a.B; w += num_warps()) {
     const int f = __ldg(a.class_feats + k0 + w / a.B);
     const int64_t b = w % a.B, gb = (int64_t)f * a.B + b;
     const MvbEmbFeature* ft = a.features + f;
     const MvbEmbTable* tb = a.tables + ft->table;
-    const int dim = (int)tb->dim, nv = (dim + 3) >> 2;
-    int lg = 0;                                      // the lane groups mvb_embedding_bag_fwd picks for dim
-    while ((1 << lg) < nv && lg < 5) ++lg;
-    const int G = 1 << lg, NG = 32 >> lg;
-    const int grp = lane >> lg, gl = lane & (G - 1);
+    const int dim = (int)tb->dim;
     const int64_t lo = a.offsets[gb], hi = gb + 1 < FB ? a.offsets[gb + 1] : a.L;
-    float* out = a.out + b * a.ldo + ft->col;
-    for (int v0 = 0; v0 < nv; v0 += G * VPL) {
-      float4 acc[VPL];
-#pragma unroll
-      for (int k = 0; k < VPL; ++k) acc[k] = zero4();
-      for (int64_t w0 = lo; w0 < hi; w0 += 32) {
-        const int n = hi - w0 < 32 ? (int)(hi - w0) : 32;
-        const int64_t id_l = lane < n ? __ldg(a.ids + w0 + lane) : 0;
-        const float w_l = lane < n ? (a.psw ? __ldg(a.psw + w0 + lane) : 1.f) : 0.f;
-        for (int t0 = 0; t0 < n; t0 += EMB_INFLIGHT * NG) {
-          float4 x[EMB_INFLIGHT][VPL];
-          float wt[EMB_INFLIGHT];
-#pragma unroll
-          for (int u = 0; u < EMB_INFLIGHT; ++u) {
-            const int t = t0 + u * NG + grp;
-            const int64_t id = __shfl_sync(FULL, id_l, t & 31);
-            wt[u] = __shfl_sync(FULL, w_l, t & 31);
-#pragma unroll
-            for (int k = 0; k < VPL; ++k) x[u][k] = zero4();
-            if (t < n) {
-              const float* row = trow(tb, id);
-#pragma unroll
-              for (int k = 0; k < VPL; ++k) {
-                const int v = v0 + gl + k * G;
-                if (v < nv) x[u][k] = load_row4(row, 4 * v, dim);
-              }
-            }
-          }
-#pragma unroll
-          for (int u = 0; u < EMB_INFLIGHT; ++u)
-            if (t0 + u * NG + grp < n) {
-#pragma unroll
-              for (int k = 0; k < VPL; ++k) fma4(acc[k], wt[u], x[u][k]);
-            }
-        }
-      }
-      for (int o = G; o < 32; o <<= 1) {
-#pragma unroll
-        for (int k = 0; k < VPL; ++k) {
-          acc[k].x += __shfl_xor_sync(FULL, acc[k].x, o);
-          acc[k].y += __shfl_xor_sync(FULL, acc[k].y, o);
-          acc[k].z += __shfl_xor_sync(FULL, acc[k].z, o);
-          acc[k].w += __shfl_xor_sync(FULL, acc[k].w, o);
-        }
-      }
-      if (tb->mean && hi > lo) {
-        const float n = (float)(hi - lo);
-#pragma unroll
-        for (int k = 0; k < VPL; ++k) { acc[k].x /= n; acc[k].y /= n; acc[k].z /= n; acc[k].w /= n; }
-      }
-      if (grp == 0) {
-#pragma unroll
-        for (int k = 0; k < VPL; ++k) {
-          const int v = v0 + gl + k * G;
-          if (v < nv) *reinterpret_cast<float4*>(out + 4 * v) = acc[k];
-        }
-      }
-    }
+    emb_pool_bag<VPL>(tb->wmap, dim, emb_lane_group_log((dim + 3) >> 2), a.ids, a.psw, lo, hi, tb->mean,
+                      a.out + b * a.ldo + ft->col);
   }
 }
 
@@ -164,63 +88,32 @@ emb_coll_keys_kernel(const __grid_constant__ MvbEmbColl a, CollScratch s) {
   }
 }
 
-// the sorted positions [c0, c1) of chunk c < cb[T] and its table
-struct Chunk {
-  int t;
-  int64_t s1, c0, c1;
-};
-MVB_DEVINL Chunk chunk_of(const MvbEmbColl& a, const CollScratch& s, int64_t c) {
-  Chunk k;
-  k.t = (int)bag_of(s.cb, a.T, c);
-  k.s1 = s.seg[k.t + 1];
-  k.c0 = s.seg[k.t] + (c - s.cb[k.t]) * EMB_CHUNK;
-  k.c1 = k.c0 + EMB_CHUNK < k.s1 ? k.c0 + EMB_CHUNK : k.s1;
-  return k;
+// chunk c < cb[T]: its table t and its place in the table's segment of the sorted keys
+MVB_DEVINL EmbChunk chunk_of(const MvbEmbColl& a, const CollScratch& s, int64_t c, int& t) {
+  t = (int)bag_of(s.cb, a.T, c);
+  const int64_t s0 = s.seg[t], s1 = s.seg[t + 1], c0 = s0 + (c - s.cb[t]) * EMB_CHUNK;
+  return EmbChunk{s0, s1, s.cb[t], c, c0, c0 + EMB_CHUNK < s1 ? c0 + EMB_CHUNK : s1};
 }
 
 __global__ void __launch_bounds__(256)
 emb_coll_count_kernel(const __grid_constant__ MvbEmbColl a, CollScratch s, int64_t ncmax) {
-  const int lane = threadIdx.x & 31;
-  const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
   const int64_t nc = s.cb[a.T];
-  for (int64_t c = warp; c < ncmax; c += nwarps) {
+  for (int64_t c = warp_id(); c < ncmax; c += num_warps()) {
     int64_t n = 0;
     if (c < nc) {
-      const Chunk k = chunk_of(a, s, c);
-      for (int64_t i0 = k.c0; i0 < k.c1; i0 += 32) {
-        const int64_t i = i0 + lane;
-        n += __popc(__ballot_sync(FULL, i < k.c1 && run_start(a.skeys, i)));
-      }
+      int t;
+      const EmbChunk k = chunk_of(a, s, c, t);
+      n = emb_count_runs(a.skeys, k.c0, k.c1);
     }
-    if (lane == 0) s.base[c] = n;
+    if ((threadIdx.x & 31) == 0) s.base[c] = n;
   }
 }
 
 // in place: base[0..n) -> exclusive scan, base[n] = total (one CTA); then the per-table info
 __global__ void __launch_bounds__(1024)
 emb_coll_scan_kernel(const __grid_constant__ MvbEmbColl a, CollScratch s, int64_t n) {
-  __shared__ int64_t part[1024];
   int64_t* cnt = s.base;
-  const int64_t per = (n + 1023) / 1024;
-  const int64_t lo = (int64_t)threadIdx.x * per, hi = lo + per < n ? lo + per : n;
-  int64_t c = 0;
-  for (int64_t i = lo; i < hi; ++i) c += cnt[i];
-  part[threadIdx.x] = c;
-  __syncthreads();
-  for (int o = 1; o < 1024; o <<= 1) {
-    const int64_t t = threadIdx.x >= o ? part[threadIdx.x - o] : 0;
-    __syncthreads();
-    part[threadIdx.x] += t;
-    __syncthreads();
-  }
-  int64_t pos = part[threadIdx.x] - c;
-  for (int64_t i = lo; i < hi; ++i) {
-    const int64_t x = cnt[i];
-    cnt[i] = pos;
-    pos += x;
-  }
-  if (threadIdx.x == 1023) cnt[n] = part[1023];
+  emb_block_scan(cnt, n);
   __syncthreads();
   if (threadIdx.x == 0) {                            // {U, first unique, grads offset, uniq offset} per table
     int64_t g = 0, q = 0;
@@ -235,127 +128,38 @@ emb_coll_scan_kernel(const __grid_constant__ MvbEmbColl a, CollScratch s, int64_
   }
 }
 
-// the epilogue of one unique key of table tb for the vectors v0 + lane + 32 k of this lane
+// the epilogue of unique key u of table t; its compact rows start at info[4 t + 2] of grads, info[4 t + 3] of uniq
 template <int VPL>
-MVB_DEVINL void coll_epilogue(const MvbEmbColl& a, const MvbEmbTable* tb, int t, int64_t key, int64_t u, int v0,
-                              const float4* g) {
-  const int dim = (int)tb->dim, nv = (dim + 3) >> 2, lane = threadIdx.x & 31;
-  const int64_t id = key - tb->key_base;
-  const float scale = tb->scale;
-  if (tb->epilogue == MVB_EMB_PUSH) {
-    float* row = trow(tb, id);
-#pragma unroll
-    for (int k = 0; k < VPL; ++k) {
-      const int v = v0 + lane + 32 * k;
-      if (v >= nv) continue;
-      float4 x = g[k];
-      x.x *= scale; x.y *= scale; x.z *= scale; x.w *= scale;
-      const int c = 4 * v;
-      if (c + 4 <= dim) {
-        red_add_v4_f32(row + c, x);
-      } else {                                     // never touch the pitch padding
-        red_add_f32(row + c, x.x);
-        if (c + 1 < dim) red_add_f32(row + c + 1, x.y);
-        if (c + 2 < dim) red_add_f32(row + c + 2, x.z);
-      }
-    }
-  } else if (a.grads && a.uniq) {
+struct CollEpilogue {
+  const MvbEmbColl& a;
+  const MvbEmbTable* tb;
+  int t;
+  MVB_DEVINL void operator()(int64_t key, int64_t u, int v0, const float4* g) const {
+    const bool push = tb->epilogue == MVB_EMB_PUSH;
+    if (!push && (!a.grads || !a.uniq)) return;      // no compact destination: nothing to write
     const int64_t* in = a.info + 4 * t;
     const int64_t r = u - in[1];
-    float* gr = a.grads + in[2] + r * tb->ldg;
-#pragma unroll
-    for (int k = 0; k < VPL; ++k) {
-      const int v = v0 + lane + 32 * k;
-      if (v >= nv) continue;
-      float4 x = g[k];
-      x.x *= scale; x.y *= scale; x.z *= scale; x.w *= scale;
-      *reinterpret_cast<float4*>(gr + 4 * v) = x;
-    }
-    if (v0 == 0 && lane == 0) a.uniq[in[3] + r] = id;
+    emb_epilogue<VPL>(push, tb->wmap, key - tb->key_base, a.grads, in[2] + r * tb->ldg, a.uniq, in[3] + r,
+                      (int)tb->dim, tb->scale, v0, g);
   }
-}
+};
 
 template <int VPL>
 __global__ void __launch_bounds__(256)
 emb_coll_bwd_main_kernel(const __grid_constant__ MvbEmbColl a, CollScratch s) {
-  const int lane = threadIdx.x & 31;
-  const int ldp = s.ldp;
-  const int64_t* __restrict__ sid = a.skeys;
   const int64_t FB = (int64_t)a.F * a.B;
-  const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
   const int64_t nc = s.cb[a.T];
-  for (int64_t c = warp; c < nc; c += nwarps) {
-    const Chunk ch = chunk_of(a, s, c);
-    const MvbEmbTable* tb = a.tables + ch.t;
-    const int dim = (int)tb->dim, nv = (dim + 3) >> 2;
-    if (vpl_of(nv) != VPL || tb->epilogue == MVB_EMB_NO_PUSH) continue;
-    const bool mean = tb->mean;
-    const int64_t c0 = ch.c0, c1 = ch.c1;
-    const bool head_continues = c0 > s.seg[ch.t] && sid[c0 - 1] == sid[c0];
-    const bool tail_continues = c1 < ch.s1 && sid[c1] == sid[c1 - 1];
-    for (int v0 = 0; v0 < nv; v0 += 32 * VPL) {
-      float4 acc[VPL];
-#pragma unroll
-      for (int k = 0; k < VPL; ++k) acc[k] = zero4();
-      int64_t cur = -1, sg = c0, u = s.base[c] - 1;
-      auto flush = [&](int64_t end) {                // segment [sg, end) of key cur
-        const bool whole = (sg > c0 || !head_continues) && (end < c1 || !tail_continues);
-        if (whole) {
-          coll_epilogue<VPL>(a, tb, ch.t, cur, u, v0, acc);
-        } else {
-          float* p = s.part + (c * 2 + (sg == c0 ? 0 : 1)) * ldp;
-#pragma unroll
-          for (int k = 0; k < VPL; ++k) {
-            const int v = v0 + lane + 32 * k;
-            if (v < nv) *reinterpret_cast<float4*>(p + 4 * v) = acc[k];
-          }
-        }
-      };
-      for (int64_t i0 = c0; i0 < c1; i0 += 32) {
-        const int64_t i = i0 + lane;
-        const int n = c1 - i0 < 32 ? (int)(c1 - i0) : 32;
-        int64_t id_l = -1, drow_l = 0;
-        float sc_l = 0.f;
-        if (i < c1) {
-          id_l = sid[i];
-          const int64_t p = a.perm[i];
-          const int64_t g = bag_of(a.offsets, FB, p), f = g / a.B;
-          drow_l = (g - f * a.B) * a.ldd + a.features[f].col;
-          sc_l = a.psw ? __ldg(a.psw + p) : 1.f;
-          if (mean) sc_l /= (float)bag_len(a.offsets, FB, a.L, g);
-        }
-        for (int t = 0; t < n; t += EMB_INFLIGHT) {
-          float4 x[EMB_INFLIGHT][VPL];
-#pragma unroll
-          for (int q = 0; q < EMB_INFLIGHT; ++q) {
-            const int64_t drow = __shfl_sync(FULL, drow_l, (t + q) & 31);
-#pragma unroll
-            for (int k = 0; k < VPL; ++k) {
-              const int v = v0 + lane + 32 * k;
-              x[q][k] = (t + q < n && v < nv) ? f4(ld_nc_v4(a.dout + drow + 4 * v)) : zero4();
-            }
-          }
-#pragma unroll
-          for (int q = 0; q < EMB_INFLIGHT; ++q) {
-            const int64_t id = __shfl_sync(FULL, id_l, (t + q) & 31);
-            const float sc = __shfl_sync(FULL, sc_l, (t + q) & 31);
-            if (t + q >= n) continue;                // warp-uniform
-            if (id != cur) {
-              if (cur >= 0) flush(i0 + t + q);
-              cur = id;
-              sg = i0 + t + q;
-              if (sg > c0 || !head_continues) ++u;
-#pragma unroll
-              for (int k = 0; k < VPL; ++k) acc[k] = zero4();
-            }
-#pragma unroll
-            for (int k = 0; k < VPL; ++k) fma4(acc[k], sc, x[q][k]);
-          }
-        }
-      }
-      if (cur >= 0) flush(c1);
-    }
+  for (int64_t c = warp_id(); c < nc; c += num_warps()) {
+    int t;
+    const EmbChunk k = chunk_of(a, s, c, t);
+    const MvbEmbTable* tb = a.tables + t;
+    if (emb_vpl(tb->dim) != VPL || tb->epilogue == MVB_EMB_NO_PUSH) continue;
+    auto drow = [&](int64_t g) {                     // bag b of feature f: row b of dout, the feature's columns
+      const int64_t f = g / a.B;
+      return (g - f * a.B) * a.ldd + a.features[f].col;
+    };
+    emb_run_sum<VPL>(a.skeys, a.perm, a.offsets, FB, a.L, a.psw, tb->mean, a.dout, drow, (int)tb->dim, k, s.base,
+                     s.part, s.ldp, CollEpilogue<VPL>{a, tb, t});
   }
 }
 
@@ -363,82 +167,27 @@ emb_coll_bwd_main_kernel(const __grid_constant__ MvbEmbColl a, CollScratch s) {
 template <int VPL>
 __global__ void __launch_bounds__(256)
 emb_coll_bwd_merge_kernel(const __grid_constant__ MvbEmbColl a, CollScratch s) {
-  const int lane = threadIdx.x & 31;
-  const int ldp = s.ldp;
-  const int64_t* __restrict__ sid = a.skeys;
-  const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
   const int64_t nc = s.cb[a.T];
-  for (int64_t c = warp; c < nc; c += nwarps) {
-    const Chunk ch = chunk_of(a, s, c);
-    const MvbEmbTable* tb = a.tables + ch.t;
-    const int nv = ((int)tb->dim + 3) >> 2;
-    if (vpl_of(nv) != VPL || tb->epilogue == MVB_EMB_NO_PUSH) continue;
-    const int64_t s0 = s.seg[ch.t], c0 = ch.c0, c1 = ch.c1;
-    const int64_t id = sid[c1 - 1];
-    if (c1 >= ch.s1 || sid[c1] != id) continue;             // the chunk's last run ends in it
-    if (c0 > s0 && sid[c0 - 1] == id) continue;             // ... or started in an earlier chunk
-    int64_t lo = c1, hi = ch.s1;                             // end of the run: first sorted index past it
-    while (lo < hi) {
-      const int64_t mid = (lo + hi) >> 1;
-      if (sid[mid] == id) lo = mid + 1; else hi = mid;
-    }
-    const int64_t c_last = s.cb[ch.t] + (lo - 1 - s0) / EMB_CHUNK;
-    const int64_t u = s.base[c + 1] - 1;
-    const float* first = s.part + (c * 2 + (sid[c0] == id ? 0 : 1)) * ldp;
-    for (int v0 = 0; v0 < nv; v0 += 32 * VPL) {
-      float4 acc[VPL];
-#pragma unroll
-      for (int k = 0; k < VPL; ++k) {
-        const int v = v0 + lane + 32 * k;
-        acc[k] = v < nv ? *reinterpret_cast<const float4*>(first + 4 * v) : zero4();
-      }
-      for (int64_t cc = c + 1; cc <= c_last; cc += EMB_INFLIGHT) {
-        float4 x[EMB_INFLIGHT][VPL];
-#pragma unroll
-        for (int q = 0; q < EMB_INFLIGHT; ++q) {
-          const float* p = s.part + (cc + q) * 2 * ldp;
-#pragma unroll
-          for (int k = 0; k < VPL; ++k) {
-            const int v = v0 + lane + 32 * k;
-            x[q][k] = (cc + q <= c_last && v < nv) ? *reinterpret_cast<const float4*>(p + 4 * v) : zero4();
-          }
-        }
-#pragma unroll
-        for (int q = 0; q < EMB_INFLIGHT; ++q)
-          if (cc + q <= c_last) {
-#pragma unroll
-            for (int k = 0; k < VPL; ++k) add4(acc[k], x[q][k]);
-          }
-      }
-      coll_epilogue<VPL>(a, tb, ch.t, id, u, v0, acc);
-    }
+  for (int64_t c = warp_id(); c < nc; c += num_warps()) {
+    int t;
+    const EmbChunk k = chunk_of(a, s, c, t);
+    const MvbEmbTable* tb = a.tables + t;
+    if (emb_vpl(tb->dim) != VPL || tb->epilogue == MVB_EMB_NO_PUSH) continue;
+    emb_merge_run<VPL>(a.skeys, k, s.base, s.part, s.ldp, ((int)tb->dim + 3) >> 2, CollEpilogue<VPL>{a, tb, t});
   }
 }
 
 // ------------------------------------------------------------------------------------------------ psw grad
 __global__ void __launch_bounds__(256)
 emb_coll_psw_grad_kernel(const __grid_constant__ MvbEmbColl a) {
-  const int lane = threadIdx.x & 31;
   const int64_t FB = (int64_t)a.F * a.B;
-  const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
-  for (int64_t j = warp; j < a.L; j += nwarps) {
+  for (int64_t j = warp_id(); j < a.L; j += num_warps()) {
     const int64_t g = bag_of(a.offsets, FB, j), f = g / a.B;
     const MvbEmbFeature* ft = a.features + f;
     const MvbEmbTable* tb = a.tables + ft->table;
-    const int dim = (int)tb->dim, nv = (dim + 3) >> 2;
-    const float* row = trow(tb, __ldg(a.ids + j));
-    const float* d = a.dout + (g - f * a.B) * a.ldd + ft->col;
-    float dot = 0.f;
-    for (int v = lane; v < nv; v += 32) {
-      const float4 w = load_row4(row, 4 * v, dim);
-      const float4 x = f4(ld_nc_v4(d + 4 * v));
-      dot = fmaf(w.x, x.x, dot); dot = fmaf(w.y, x.y, dot);
-      dot = fmaf(w.z, x.z, dot); dot = fmaf(w.w, x.w, dot);
-    }
-    dot = warp_sum(dot);
-    if (lane == 0) a.dpsw[j] = tb->mean ? dot / (float)bag_len(a.offsets, FB, a.L, g) : dot;
+    const float dot = emb_psw_dot(row_of(tb->wmap, __ldg(a.ids + j)), a.dout + (g - f * a.B) * a.ldd + ft->col,
+                                  (int)tb->dim);
+    if ((threadIdx.x & 31) == 0) a.dpsw[j] = tb->mean ? dot / (float)bag_len(a.offsets, FB, a.L, g) : dot;
   }
 }
 
@@ -474,17 +223,14 @@ extern "C" int mvb_emb_coll_fwd(const MvbEmbColl* a, void* stream) {
     const int k0 = a->class_off[k - 1], nf = a->class_off[k] - k0;
     if (nf == 0) continue;
     const int grid = grid_for((int64_t)nf * a->B);
-    if (k == 1) emb_coll_fwd_kernel<1><<<grid, 256, 0, st>>>(*a, k0, nf);
-    else if (k == 2) emb_coll_fwd_kernel<2><<<grid, 256, 0, st>>>(*a, k0, nf);
-    else if (k == 3) emb_coll_fwd_kernel<3><<<grid, 256, 0, st>>>(*a, k0, nf);
-    else emb_coll_fwd_kernel<4><<<grid, 256, 0, st>>>(*a, k0, nf);
+    with_vpl(k, [&](auto V) { emb_coll_fwd_kernel<decltype(V)::value><<<grid, 256, 0, st>>>(*a, k0, nf); });
     MVB_CUDA_CHECK(cudaGetLastError());
   }
   return 0;
 }
 
 extern "C" int64_t mvb_emb_coll_scratch_bytes(int64_t L, int T, int64_t max_dim) {
-  return plan_bytes(T) + cbase_bytes(L, T) + cpart_bytes(L, T, vpl_of_host(max_dim));
+  return plan_bytes(T) + cbase_bytes(L, T) + cpart_bytes(L, T, emb_vpl(max_dim));
 }
 
 static int check_scratch(const MvbEmbColl* a) {
@@ -529,18 +275,14 @@ extern "C" int mvb_emb_coll_bwd(const MvbEmbColl* a, void* stream) {
   const int grid = grid_for(nc_max(a->L, a->T));
   for (int k = 1; k < 5; ++k) {
     if (a->class_off[k] == a->class_off[k - 1]) continue;
-#define MVB_COLL_BWD(V)                                                  \
-  do {                                                                   \
-    emb_coll_bwd_main_kernel<V><<<grid, 256, 0, st>>>(*a, s);            \
-    MVB_CUDA_CHECK(cudaGetLastError());                                  \
-    emb_coll_bwd_merge_kernel<V><<<grid, 256, 0, st>>>(*a, s);           \
-  } while (0)
-    if (k == 1) MVB_COLL_BWD(1);
-    else if (k == 2) MVB_COLL_BWD(2);
-    else if (k == 3) MVB_COLL_BWD(3);
-    else MVB_COLL_BWD(4);
-#undef MVB_COLL_BWD
-    MVB_CUDA_CHECK(cudaGetLastError());
+    if (int rc = with_vpl(k, [&](auto V) {
+          emb_coll_bwd_main_kernel<decltype(V)::value><<<grid, 256, 0, st>>>(*a, s);
+          MVB_CUDA_CHECK(cudaGetLastError());
+          emb_coll_bwd_merge_kernel<decltype(V)::value><<<grid, 256, 0, st>>>(*a, s);
+          MVB_CUDA_CHECK(cudaGetLastError());
+          return 0;
+        }))
+      return rc;
   }
   return 0;
 }

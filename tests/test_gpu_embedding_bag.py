@@ -45,7 +45,7 @@ def _close(out, ref, mag):
     assert (err <= TOL * mag + 1e-30).all(), (err / mag.clamp_min(1e-30)).max().item()
 
 
-@pytest.mark.parametrize("dim", [4, 16, 64, 128, 300])
+@pytest.mark.parametrize("dim", [4, 16, 64, 128, 300, 1000])
 @pytest.mark.parametrize("mode,weighted", [("sum", False), ("sum", True), ("mean", False)])
 def test_forward_matches_fp64(cuda, dim, mode, weighted):
     from multiverso_b200.ops import embedding_bag
@@ -111,7 +111,7 @@ def _step(rm, dim, ids, offsets, psw, mode, dout, updater, is_sparse=False, num_
     return out
 
 
-@pytest.mark.parametrize("dim", [64, 300])
+@pytest.mark.parametrize("dim", [64, 300, 1000])
 def test_sharded_bitwise_equal(cuda, dim):
     from multiverso_b200 import _native as N
     g = torch.Generator(device=cuda).manual_seed(11)
