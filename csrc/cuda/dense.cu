@@ -418,37 +418,6 @@ __global__ void __launch_bounds__(256) get_dense_kernel(const __grid_constant__ 
 constexpr int kBulkStages = 6;
 constexpr uint32_t kBulkChunk = 32 * 1024;
 
-MVB_DEVINL uint32_t dg_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-MVB_DEVINL void dg_mbar_init(uint64_t* bar, int count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(dg_smem_u32(bar)), "r"(count));
-}
-MVB_DEVINL void dg_mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(dg_smem_u32(bar)), "r"(bytes) : "memory");
-}
-MVB_DEVINL void dg_mbar_wait(uint64_t* bar, uint32_t parity) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "DG_WAIT_LOOP:\n"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-      "@p bra DG_DONE;\n"
-      "bra DG_WAIT_LOOP;\n"
-      "DG_DONE:\n"
-      "}\n" ::"r"(dg_smem_u32(bar)), "r"(parity)
-      : "memory");
-}
-MVB_DEVINL void dg_bulk_g2s(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                   dg_smem_u32(smem_dst)),
-               "l"(gsrc), "r"(bytes), "r"(dg_smem_u32(bar))
-               : "memory");
-}
-MVB_DEVINL void dg_bulk_s2g(void* gdst, const void* smem_src, uint32_t bytes) {
-  asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gdst), "r"(dg_smem_u32(smem_src)),
-               "r"(bytes)
-               : "memory");
-}
-
 // ---------------------------------------------------------------------------
 // K1, bulk-copy variant: the owner pulls its tile of EVERY worker's staging buffer with cp.async.bulk
 // (peer HBM -> shared memory, ~190 KB in flight per SM, no registers on the transfer path), four compute warps
@@ -472,7 +441,7 @@ add_dense_bulk_kernel(const __grid_constant__ DenseAddDev<float> a, int stages) 
   if (threadIdx.x == 0) smask = a.mask;
   if (threadIdx.x < MVB_MAX_RANKS) sopt[threadIdx.x] = a.opts[threadIdx.x];
   if (threadIdx.x == 0) {
-    for (int i = 0; i < stages; ++i) { dg_mbar_init(&full[i], 1); dg_mbar_init(&empty[i], kAddComputeWarps); }
+    for (int i = 0; i < stages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], kAddComputeWarps); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -517,16 +486,16 @@ add_dense_bulk_kernel(const __grid_constant__ DenseAddDev<float> a, int stages) 
       const int64_t off = (blockIdx.x + j * gridDim.x) * (int64_t)kAddChunk;
       const uint32_t len = (uint32_t)((body - off) < kAddChunk ? (body - off) : kAddChunk);
       if (lane == 0) {
-        dg_mbar_wait(&empty[st], (uint32_t)(((j / stages) & 1) ^ 1));
-        dg_mbar_expect_tx(&full[st], len * (uint32_t)(nact + 1));
+        mbar_wait(&empty[st], (uint32_t)(((j / stages) & 1) ^ 1));
+        mbar_arrive_expect_tx(&full[st], len * (uint32_t)(nact + 1));
       }
       __syncwarp();
       if (lane < a.W && ((mask >> lane) & 1u))
-        dg_bulk_g2s(ring + ((size_t)st * kAddSlots + lane) * kAddChunk,
-                    reinterpret_cast<const char*>(a.delta[lane] + a.shard_off) + off, len, &full[st]);
+        bulk_g2s(ring + ((size_t)st * kAddSlots + lane) * kAddChunk,
+                 reinterpret_cast<const char*>(a.delta[lane] + a.shard_off) + off, len, &full[st]);
       if (lane == MVB_MAX_RANKS)
-        dg_bulk_g2s(ring + ((size_t)st * kAddSlots + MVB_MAX_RANKS) * kAddChunk,
-                    reinterpret_cast<const char*>(a.shard) + off, len, &full[st]);
+        bulk_g2s(ring + ((size_t)st * kAddSlots + MVB_MAX_RANKS) * kAddChunk,
+                 reinterpret_cast<const char*>(a.shard) + off, len, &full[st]);
     }
   } else {
     // -------- compute warps: sum of the W copies + updater + shard / state write --------
@@ -535,7 +504,7 @@ add_dense_bulk_kernel(const __grid_constant__ DenseAddDev<float> a, int stages) 
       const int st = (int)(j % stages);
       const int64_t off = (blockIdx.x + j * gridDim.x) * (int64_t)kAddChunk;
       const int len = (int)((body - off) < kAddChunk ? (body - off) : kAddChunk);
-      dg_mbar_wait(&full[st], (uint32_t)((j / stages) & 1));
+      mbar_wait(&full[st], (uint32_t)((j / stages) & 1));
       const unsigned char* sb = ring + (size_t)st * kAddSlots * kAddChunk;
       for (int v = tid; v < len / 16; v += 32 * kAddComputeWarps) {
         const int64_t i = (off >> 2) + (int64_t)v * 4;                  // element index inside the shard
@@ -565,7 +534,7 @@ add_dense_bulk_kernel(const __grid_constant__ DenseAddDev<float> a, int stages) 
       }
       __syncwarp();
       if (lane == 0) {
-        asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(dg_smem_u32(&empty[st])) : "memory");
+        mbar_arrive(&empty[st]);
       }
     }
     // scalar tail (shard_len % 4): first compute threads of block 0
@@ -640,7 +609,7 @@ __global__ void __launch_bounds__(32) get_dense_bulk_kernel(const __grid_constan
     __syncthreads();
   }
   if (threadIdx.x != 0) return;
-  for (int i = 0; i < kBulkStages; ++i) dg_mbar_init(&full[i], 1);
+  for (int i = 0; i < kBulkStages; ++i) mbar_init(&full[i], 1);
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   const int groups = g.S;
@@ -662,14 +631,14 @@ __global__ void __launch_bounds__(32) get_dense_bulk_kernel(const __grid_constan
   };
   auto load = [&](int64_t j) {
     const int st = (int)(j % kBulkStages);
-    dg_mbar_expect_tx(&full[st], chunk_len(j));
-    dg_bulk_g2s(ring + (size_t)st * kBulkChunk, src + chunk_off(j), chunk_len(j), &full[st]);
+    mbar_arrive_expect_tx(&full[st], chunk_len(j));
+    bulk_g2s(ring + (size_t)st * kBulkChunk, src + chunk_off(j), chunk_len(j), &full[st]);
   };
   for (int64_t j = 0; j < mine && j < kBulkStages; ++j) load(j);
   for (int64_t j = 0; j < mine; ++j) {
     const int st = (int)(j % kBulkStages);
-    dg_mbar_wait(&full[st], (uint32_t)((j / kBulkStages) & 1));
-    dg_bulk_s2g(dst + chunk_off(j), ring + (size_t)st * kBulkChunk, chunk_len(j));
+    mbar_wait(&full[st], (uint32_t)((j / kBulkStages) & 1));
+    bulk_s2g(dst + chunk_off(j), ring + (size_t)st * kBulkChunk, chunk_len(j));
     asm volatile("cp.async.bulk.commit_group;" ::: "memory");
     if (j + kBulkStages < mine) {
       // the stage is refilled only after the store has finished READING it; the other stages' loads

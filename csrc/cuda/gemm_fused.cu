@@ -90,7 +90,7 @@ get_gemm_fused_kernel(const __grid_constant__ CUtensorMap map_x,
         for (int kb = 0; kb < num_kb; ++kb) {
           mbar_wait(&empty[st], ph ^ 1u);
           // out-of-range rows / columns are zero-filled and still counted in the transaction bytes
-          mbar_expect_tx(&full[st], X_BYTES + W_BYTES);
+          mbar_arrive_expect_tx(&full[st], X_BYTES + W_BYTES);
           tma_load_2d(x_tiles + st * X_BYTES, &map_x, kb * BK, mt * BM, &full[st]);
           tma_load_2d(w_tiles + st * W_BYTES, map_w, kb * BK, (int)t.n_local, &full[st]);   // peer HBM
           if (++st == STAGES) { st = 0; ph ^= 1u; }

@@ -1,9 +1,9 @@
 // multiverso-b200 :: Hopper (sm_90a) building blocks of the TMA + wgmma kernels
 // (gemm_fused.cu: fused Get+GEMM, topk_cos.cu: fused cosine top-k).
 //
-// mbarrier ring primitives, 2-D TMA loads, K-major 128B-swizzled shared-memory descriptors, the tf32
-// wgmma m64n128k8 with its register accumulator, and the host-side tensor-map encoder. Internal to the
-// kernel sources: every .cu that includes it gets its own copy.
+// 2-D TMA loads, K-major 128B-swizzled shared-memory descriptors, the tf32 wgmma m64n128k8 with its
+// register accumulator, and the host-side tensor-map encoder (the mbarrier primitives are in
+// mvb_common.cuh). Internal to the kernel sources: every .cu that includes it gets its own copy.
 #pragma once
 #include <cuda.h>
 #include "mvb_common.cuh"
@@ -13,22 +13,6 @@ namespace {
 constexpr int BK = 32;           // fp32 elements per k-block = 128 bytes = one swizzle row
 constexpr int UK = 8;                        // wgmma K for tf32
 
-MVB_DEVINL uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-MVB_DEVINL void mbar_init(uint64_t* bar, int count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-MVB_DEVINL void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-MVB_DEVINL void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-MVB_DEVINL void mbar_wait(uint64_t* bar, uint32_t parity) {
-  asm volatile(
-      "{\n.reg .pred p;\nLAB_WAIT:\n"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-      "@p bra LAB_DONE;\nbra LAB_WAIT;\nLAB_DONE:\n}\n" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
-}
 MVB_DEVINL void tma_load_2d(void* smem_dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
   asm volatile(
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"

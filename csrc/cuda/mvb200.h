@@ -273,18 +273,19 @@ typedef struct MvbSgns {
   uint64_t seed;
   float* loss_sum;           /* optional: += sum of -log sigma(..)         */
   unsigned long long* pair_count;  /* optional: += trained (input,target) samples */
-  int variant;               /* kernel variant: 0 auto, 1..5 = negatives held in registers, 10 = TMA pipeline
-                                (pair at a time), 20 = window-batched TMA pipeline (one centre per warp) */
+  int hogwild;               /* one device, skip-gram + NS: 0 = deterministic waves, 1 = the Hogwild
+                                window-batched kernel (one centre per warp)                          */
   int max_ctas;              /* 0 = one CTA per SM; > 0 caps the persistent grid (leaves SMs to the
                                 row pull / push kernels of the pipelined multi-GPU step)            */
-  /* optional per-WORD step scales in (0,1] (variant 20): caps the summed step of the Zipf-head rows
-     that collect more concurrent stale updates than plain SGD tolerates; NULL = 1 everywhere      */
+  /* optional per-WORD step scales in (0,1] (deterministic and window kernels): caps the summed step of
+     the Zipf-head rows that collect more concurrent stale updates than plain SGD tolerates;
+     NULL = 1 everywhere                                                                              */
   const float* scale_in;
   const float* scale_out;
   const int* neg_pool_size_ptr;  /* optional: pool size read on the DEVICE (mvb_we_prepare counts[2]);
-                                    variant 20 only, overrides neg_pool_size                          */
-  /* direct mode (variant 20, nservers > 1): train IN the row-sharded tables over NVLink -- rows are loaded
-     from and reduced into their owners' shards (owner = id / rows_per_server, last server takes the
+                                    deterministic and window kernels, overrides neg_pool_size          */
+  /* direct mode (nservers > 1, window kernel only): train IN the row-sharded tables over NVLink -- rows
+     are loaded from and reduced into their owners' shards (owner = id / rows_per_server, last server takes the
      remainder) through the peer mappings; no block cache, no maps (Hogwild across GPUs)                 */
   int nservers;
   int64_t rows_per_server;
@@ -292,7 +293,6 @@ typedef struct MvbSgns {
   void* w_out_peers[MVB_MAX_RANKS];
 } MvbSgns;
 int mvb_sgns_train(const MvbSgns* a, void* stream);
-int mvb_sgns_train_tma(const MvbSgns* a, void* stream);   /* TMA bulk-copy pipeline variant */
 int mvb_sgns_train_win(const MvbSgns* a, void* stream);   /* window-batched TMA pipeline      */
 int mvb_sgns_train_det(const MvbSgns* a, void* stream);   /* deterministic waves (default)    */
 int mvb_sgns_last_launches(void);   /* kernel launches of the last mvb_sgns_train call */

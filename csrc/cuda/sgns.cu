@@ -16,17 +16,12 @@
 //   sgns_fast_kernel    : skip-gram + negative sampling, plain SGD, D % 4 == 0, D <= 512
 //   w2v_generic_kernel  : CBOW / hierarchical softmax / AdaGrad / any D (smem staged)
 #include <cmath>
-#include <cstdlib>
 #include <vector>
 #include "mvb_common.cuh"
 
 namespace {
 
 MVB_DEVINL uint64_t lcg_next(uint64_t x) { return x * 25214903917ull + 11ull; }  // util.cpp:144-146
-MVB_DEVINL float sigmoidf_fast(float x) { return __fdividef(1.0f, 1.0f + __expf(-x)); }
-MVB_DEVINL float softplus_neg(float x) {  // -log(sigmoid(x)) = log(1+exp(-x))
-  return fmaxf(-x, 0.f) + log1pf(__expf(-fabsf(x)));
-}
 
 struct SgnsDev {
   const int* tokens;
@@ -174,7 +169,7 @@ sgns_fast_kernel(const __grid_constant__ SgnsDev a) {
       // positive sample (label 1) against the register-resident centre row
       {
         float f = warp_sum(row_dot<VPL>(h, crow));
-        float g = (1.f - sigmoidf_fast(f)) * a.lr;
+        float g = (1.f - sigm_fast(f)) * a.lr;
         if (a.loss_sum) loss_acc += softplus_neg(f);
         row_axpy<VPL>(herr, g, crow);
         row_axpy<VPL>(crow, g, h);
@@ -212,7 +207,7 @@ sgns_fast_kernel(const __grid_constant__ SgnsDev a) {
 #pragma unroll
         for (int d = 0; d < KB; ++d) {
           if (tgt[d] >= 0) {
-            float g = (0.f - sigmoidf_fast(f[d])) * a.lr;
+            float g = (0.f - sigm_fast(f[d])) * a.lr;
             if (a.loss_sum) loss_acc += softplus_neg(-f[d]);
             row_axpy<VPL>(herr, g, nrow[d]);
             row_red_add<VPL>(nptr[d], row_scaled<VPL>(g, h), nvec, lane);
@@ -311,7 +306,7 @@ __global__ void __launch_bounds__(128) w2v_generic_kernel(const __grid_constant_
         float f = 0.f;
         for (int c = lane; c < D; c += 32) f = fmaf(hid[c], wrow[c], f);
         f = warp_sum(f);
-        float sg = sigmoidf_fast(f);
+        float sg = sigm_fast(f);
         // BPOutputLayer: hs error = 1 - label - f ; ns error = label - f
         float err = a.hs ? (1.f - (float)label - sg) : ((float)label - sg);
         if (a.loss_sum) {
@@ -387,19 +382,24 @@ SgnsDev to_dev(const MvbSgns* h) {
 
 }  // namespace
 
-extern "C" int mvb_sgns_train_tma(const MvbSgns* h, void* stream);
 extern "C" int mvb_sgns_train_win(const MvbSgns* h, void* stream);
 extern "C" int mvb_sgns_train_det(const MvbSgns* h, void* stream);
 
 int mvb_sgns_launches = 1;   // kernel launches of the last mvb_sgns_train call
 extern "C" int mvb_sgns_last_launches(void) { return mvb_sgns_launches; }
 
+// One kernel per input:
+//   nservers > 1 (direct mode)           the window kernel, or its error code (only it addresses peer shards)
+//   skip-gram + NS, register-row shapes  the deterministic waves (hogwild = 0) or the window kernel
+//                                        (hogwild = 1) where it covers the input, else the register kernel
+//   anything else                        the generic kernel
 extern "C" int mvb_sgns_train(const MvbSgns* h, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   mvb_sgns_launches = 1;
   if (h->n_tokens <= 0) return 0;
   if (h->window < 1) return -5;
   if (!h->hs && h->negative > 0 && !h->neg_pool && !(h->alias_prob && h->alias_idx)) return -6;
+  if (h->nservers > 1) return mvb_sgns_train_win(h, stream);
   SgnsDev d = to_dev(h);
   const bool fast = !h->cbow && !h->hs && !h->use_adagrad && h->negative > 0 && (h->dim % 4 == 0) &&
                     (h->ld % 4 == 0) && h->dim <= 512 && h->window <= 15 &&
@@ -407,6 +407,9 @@ extern "C" int mvb_sgns_train(const MvbSgns* h, void* stream) {
                     ((reinterpret_cast<uintptr_t>(h->w_out) & 15) == 0);
   const int sms = mvb_num_sms();
   if (fast) {
+    // -20 / -21 / -22: the kernel does not cover this input (K >= 8; vocab <= 0 for the deterministic one)
+    const int rc = h->hogwild ? mvb_sgns_train_win(h, stream) : mvb_sgns_train_det(h, stream);
+    if (rc != -20 && rc != -21 && rc != -22) return rc;
     const int nvec = h->dim / 4;
     const int vpl = (nvec + 31) / 32;
     // persistent-style grid: 4 CTAs of 4 warps per SM, warps stride over positions
@@ -414,33 +417,11 @@ extern "C" int mvb_sgns_train(const MvbSgns* h, void* stream) {
     int64_t blocks = (warps_needed + 3) / 4;
     int64_t cap = (int64_t)sms * 16;
     if (blocks > cap) blocks = cap;
-    int variant = h->variant;
-    if (const char* e = getenv("MVB_SGNS_VARIANT")) variant = atoi(e);
-    // default: deterministic; the Hogwild kernels below by variant (window-batched: also direct mode)
-    if (variant == 0 && h->nservers <= 1) {
-      int rc = mvb_sgns_train_det(h, stream);
-      if (rc != -20 && rc != -21) return rc;
-    }
-    // window-batched pipeline (one centre position per warp, negatives shared by the position's contexts)
-    if ((variant == 20 || variant == 0) && h->negative <= 7 && h->window <= 15) {
-      int rc = mvb_sgns_train_win(h, stream);
-      if (rc != -22 && rc != -20 && rc != -21) return rc;   // else: rows do not fit the smem rings
-    }
-    // pair-at-a-time TMA pipeline before the register variants
-    if ((variant == 10 || variant == 0 || variant == 20) && h->negative <= 6 && h->window <= 15) {
-      int rc = mvb_sgns_train_tma(h, stream);
-      if (rc != -22 && rc != -20 && rc != -21) return rc;   // else: rows do not fit the smem ring
-    }
+    // register/occupancy trade-off per row width: KB rows of 4 * VPL registers each stay live per warp
     switch (vpl) {
       case 1: sgns_fast_kernel<1, 5, 4><<<(int)blocks, 128, 0, st>>>(d); break;
       case 2: sgns_fast_kernel<2, 5, 3><<<(int)blocks, 128, 0, st>>>(d); break;
-      case 3:
-        // register/occupancy trade-off: KB rows of 12 registers each stay live per warp
-        if (variant == 5) sgns_fast_kernel<3, 5, 3><<<(int)blocks, 128, 0, st>>>(d);
-        else if (variant == 3) sgns_fast_kernel<3, 3, 4><<<(int)blocks, 128, 0, st>>>(d);
-        else if (variant == 2) sgns_fast_kernel<3, 2, 5><<<(int)blocks, 128, 0, st>>>(d);
-        else sgns_fast_kernel<3, 1, 6><<<(int)blocks, 128, 0, st>>>(d);
-        break;
+      case 3: sgns_fast_kernel<3, 1, 6><<<(int)blocks, 128, 0, st>>>(d); break;
       default: sgns_fast_kernel<4, 2, 4><<<(int)blocks, 128, 0, st>>>(d); break;
     }
   } else {
@@ -454,7 +435,6 @@ extern "C" int mvb_sgns_train(const MvbSgns* h, void* stream) {
     // with thousands of samples in flight those rows see stale values and the accumulated
     // step overshoots (the reference's Hogwild runs <= 16 threads). Bound the concurrency.
     int64_t cap = h->hs ? (int64_t)sms / 4 : (int64_t)sms * 8;
-    if (const char* e = getenv("MVB_W2V_BLOCKS")) cap = atoi(e) > 0 ? atoi(e) : cap;
     if (blocks > cap) blocks = cap;
     w2v_generic_kernel<<<(int)blocks, 128, smem, st>>>(d);
   }

@@ -1,7 +1,7 @@
 // multiverso-b200 :: K7 (window-batched variant) -- skip-gram negative sampling, one CENTRE POSITION
 // per consumer warp, row traffic on the bulk-copy (TMA) engine.
 //
-// The pair-at-a-time kernels (sgns.cu, sgns_tma.cu) move 7 rows in and 7 rows out for every
+// The pair-at-a-time register kernel (sgns.cu) moves 7 rows in and 7 rows out for every
 // (context, centre) pair: the centre row and the K negatives are re-fetched and re-reduced for each
 // of the ~6 contexts of a position and every input row is fetched once per centre it is a context of.
 // This variant keeps the reference's sample schedule (ParseSentence, wordembedding.cpp:216-257: random
@@ -30,7 +30,6 @@
 // Synchronisation is mbarrier only (no __syncthreads after init): in_full/in_empty per ring slot
 // (empty counts 2W+1 arrivals: the centres whose window covers the slot), out_full/out_empty per
 // consumer stage.  Virtual positions [a-2W, b+2W) make every count uniform at the range ends.
-#include <cstdlib>
 #include "mvb_common.cuh"
 
 namespace {
@@ -93,52 +92,10 @@ struct OutMeta {
 };
 static_assert(sizeof(OutMeta) == 128, "OutMeta size");
 
-MVB_DEVINL uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-MVB_DEVINL void mbar_init(uint64_t* bar, int count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-MVB_DEVINL void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes)
-               : "memory");
-}
-MVB_DEVINL void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-MVB_DEVINL void mbar_wait(uint64_t* bar, uint32_t parity) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "WAIT_LOOP:\n"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-      "@p bra DONE;\n"
-      "bra WAIT_LOOP;\n"
-      "DONE:\n"
-      "}\n" ::"r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-}
-MVB_DEVINL void bulk_g2s(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-               ::"r"(smem_u32(smem_dst)), "l"(gsrc), "r"(bytes), "r"(smem_u32(bar))
-               : "memory");
-}
-MVB_DEVINL void bulk_reduce_add_s2g(void* gdst, const void* smem_src, uint32_t bytes) {
-  asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.f32 [%0], [%1], %2;"
-               ::"l"(gdst), "r"(smem_u32(smem_src)), "r"(bytes)
-               : "memory");
-}
-MVB_DEVINL void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-template <int N>
-MVB_DEVINL void bulk_wait_read() {
-  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
-}
-MVB_DEVINL void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-
 // fp32 pair math: sm_90 has no packed FFMA2, so each lane is one round-to-nearest FFMA
 MVB_DEVINL float2 ffma2(float2 a, float2 b, float2 c) {
   return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
 }
-MVB_DEVINL float sigm_fast(float x) { return __fdividef(1.0f, 1.0f + __expf(-x)); }
-MVB_DEVINL float softplus_neg(float x) { return fmaxf(-x, 0.f) + log1pf(__expf(-fabsf(x))); }
 
 struct F4 {
   float2 lo, hi;
@@ -264,8 +221,8 @@ sgns_win_kernel(const __grid_constant__ WinDev a) {
   const int R = a.ring;
   const int NW = a.nw;
 
-  // Work units are chunks of `a.chunk` consecutive token positions, chunk c on CTA c mod gridDim.x (one chunk
-  // per CTA unless MVB_WIN_CHUNK says otherwise).  Inside a CTA the chunks form ONE
+  // Work units are chunks of `a.chunk` consecutive token positions, chunk c on CTA c mod gridDim.x (the host
+  // launcher makes one chunk per CTA).  Inside a CTA the chunks form ONE
   // stream of virtual positions G = 0, 1, 2, ...: chunk [ra, rb) contributes rb - ra + 4W of them (local index
   // i <-> centre token ra - 2W + i, ring entry i <-> input token ra - W + i, empty beyond the chunk), so ring
   // slots, stages and barrier phases simply continue across chunks.
@@ -629,7 +586,7 @@ sgns_win_kernel(const __grid_constant__ WinDev a) {
       if (j >= 0) mbar_arrive(in_empty + (int)(j % R));
     }
   }
-  if (lane < kRelLanes) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // adds performed
+  if (lane < kRelLanes) bulk_wait_all();   // adds performed
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) loss_acc += __shfl_xor_sync(0xffffffffu, loss_acc, o);   // lanes hold different rows
   if (lane == 0) {
@@ -859,7 +816,7 @@ extern "C" int mvb_sgns_win_inflight(int dim, int negative, int window, int max_
 }
 
 // Window-batched K7. Returns -20/-21 for configurations it does not cover, -22 when the rows
-// do not fit the shared-memory rings (the caller falls back to the pair-at-a-time kernels).
+// do not fit the shared-memory rings (not reached on an H100 for dim <= 512).
 extern "C" int mvb_sgns_train_win(const MvbSgns* h, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   if (h->n_tokens <= 0) return 0;
@@ -900,28 +857,16 @@ extern "C" int mvb_sgns_train_win(const MvbSgns* h, void* stream) {
     if (L.total <= max_smem) break;
   }
   if (nw < 2) return -22;
-  if (const char* e = getenv("MVB_WIN_NW")) {
-    const int v = atoi(e);
-    if (v >= 2 && v < nw) {
-      nw = v;
-      a.ring = 2 * nw + 2 * h->window + 2;
-      L = make_layout(a.ring, nw, a.ko, a.row_bytes);
-    }
-  }
   a.nw = nw;
   int blocks = mvb_num_sms();
   if (h->max_ctas > 0 && h->max_ctas < blocks) blocks = h->max_ctas;
   // tiny inputs use fewer CTAs (>= 64 positions each)
   const int64_t by_len = (h->n_tokens + 63) / 64;
   if ((int64_t)blocks > by_len) blocks = (int)by_len;
-  // One chunk per CTA by default (a static partition: every chunk boundary drains and refills the rings, and
-  // the imbalance between CTAs is smaller than that: on 1M-token blocks, chunks of 256 / 512 / 1024 tokens
-  // handed out by an atomic ticket ran slower than one chunk per CTA).  MVB_WIN_CHUNK=n deals n-token chunks round-robin instead.
+  // One chunk per CTA (a static partition: every chunk boundary drains and refills the rings, and the
+  // imbalance between CTAs is smaller than that: on 1M-token blocks, chunks of 256 / 512 / 1024 tokens
+  // handed out by an atomic ticket ran slower than one chunk per CTA).
   a.chunk = (int)((h->n_tokens + blocks - 1) / blocks);
-  if (const char* e = getenv("MVB_WIN_CHUNK")) {
-    const int v = atoi(e);
-    if (v >= 32 && v <= (1 << 20)) a.chunk = v;
-  }
   const int64_t n_chunks = (h->n_tokens + a.chunk - 1) / a.chunk;
   if ((int64_t)blocks > n_chunks) blocks = (int)n_chunks;
   // register layout of a row: full float4 chunks (+ a partial one) or a float2 tail (Row<NF4, TAIL>)

@@ -160,7 +160,7 @@ topk_cos_kernel(const __grid_constant__ CUtensorMap map_x,
                                    : s == 4 ? &map_w4 : s == 5 ? &map_w5 : s == 6 ? &map_w6 : &map_w7;
           for (int kb = 0; kb < num_kb; ++kb) {
             mbar_wait(&empty[st], ph ^ 1u);
-            mbar_expect_tx(&full[st], X_BYTES + W_BYTES);
+            mbar_arrive_expect_tx(&full[st], X_BYTES + W_BYTES);
             tma_load_2d(x_tiles + st * X_BYTES, &map_x, kb * BK, mt * BM, &full[st]);
             tma_load_2d(w_tiles + st * W_BYTES, map_w, kb * BK, (int)t.n_local, &full[st]);   // peer HBM
             if (++st == STAGES) { st = 0; ph ^= 1u; }

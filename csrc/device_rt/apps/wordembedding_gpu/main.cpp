@@ -249,7 +249,7 @@ struct DeviceModel {
     a.seed = (0x5DEECE66DULL * static_cast<uint64_t>(dev::Rank() + 1)) ^ (step * 0x9E3779B97F4A7C15ULL);
     a.loss_sum = loss_sum;
     a.pair_count = pair_count;
-    a.variant = 0;
+    a.hogwild = 0;
     KERNEL_CHECK(mvb_sgns_train(&a, nullptr));
     ++launches;
   }

@@ -92,7 +92,7 @@ class Sgns(C.Structure):
         ("alias_prob", vp), ("alias_idx", vp), ("vocab", C.c_int), ("neg_pool", vp),
         ("neg_pool_size", C.c_int), ("hs_points", vp), ("hs_codes", vp), ("hs_len", vp),
         ("hs_max_code", C.c_int), ("map_in", vp), ("map_out", vp), ("seed", C.c_uint64),
-        ("loss_sum", vp), ("pair_count", vp), ("variant", C.c_int), ("max_ctas", C.c_int),
+        ("loss_sum", vp), ("pair_count", vp), ("hogwild", C.c_int), ("max_ctas", C.c_int),
         ("scale_in", vp), ("scale_out", vp), ("neg_pool_size_ptr", vp),
         ("nservers", C.c_int), ("rows_per_server", i64), ("w_in_peers", VP8), ("w_out_peers", VP8),
     ]

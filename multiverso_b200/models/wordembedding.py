@@ -104,20 +104,14 @@ class WordEmbedding:
         self.dev = rt.device
         self.W = max(rt.num_workers(), 1)
         D = self.D
-        # Row pitch of the tables. Experiment knob (off by default, to be measured): MVB_WE_ROW_PAD=32 pads
-        # every row to a multiple of 32 floats (300 -> 320: 1280-byte rows, so the TMA bulk loads / reductions
-        # of K7 are 128-byte aligned); the kernels take `dim` and `ld` separately, the padding is never read.
-        pad = int(os.environ.get("MVB_WE_ROW_PAD", "0"))
-        self.LD = (D + pad - 1) // pad * pad if pad > 1 else D
-        LD = self.LD
         # PrepareParameterTables (communicator.cpp:17-32)
-        self.input_table = MatrixDeviceTable(self.V, LD, "float32", updater="default",
+        self.input_table = MatrixDeviceTable(self.V, D, "float32", updater="default",
                                              min_value=-0.5 / D, max_value=0.5 / D, seed=seed)
-        self.output_table = MatrixDeviceTable(self.V, LD, "float32", updater="default", init_value=0.0)
+        self.output_table = MatrixDeviceTable(self.V, D, "float32", updater="default", init_value=0.0)
         self.g2_in = self.g2_out = None
         if option.use_adagrad:
-            self.g2_in = MatrixDeviceTable(self.V, LD, "float32", updater="default", init_value=0.0)
-            self.g2_out = MatrixDeviceTable(self.V, LD, "float32", updater="default", init_value=0.0)
+            self.g2_in = MatrixDeviceTable(self.V, D, "float32", updater="default", init_value=0.0)
+            self.g2_out = MatrixDeviceTable(self.V, D, "float32", updater="default", init_value=0.0)
         self.wordcount_table = KVDeviceTable("int64", "int64", capacity=1024)
         if word_counts is None:
             word_counts = 1.0 / np.arange(1, self.V + 1, dtype=np.float64)   # Zipf
@@ -144,7 +138,7 @@ class WordEmbedding:
         self._prefetched = None
         self._pending_side = False
         self.kernel_launches = 0
-        self.kernel_variant = 0     # 0 auto | 1,2,3,5 register kernel | 10 TMA pipeline (pair at a time) | 20 window-batched
+        self.hogwild = False        # one GPU, skip-gram + NS: the Hogwild window kernel instead of the deterministic waves
         self.max_ctas = 0           # > 0: cap K7's persistent grid (SMs left to the row pull / push kernels)
         # pull / push kernels of the block protocol (world > 1):
         #   "lsu" (default)   register-path pull + one-sided red.add push: 128-thread CTAs with <= 56 registers and no
@@ -161,7 +155,9 @@ class WordEmbedding:
         self.mode = os.environ.get("MVB_WE_MODE", "block")
         self.side_mode = os.environ.get("MVB_WE_SIDE_MODE", "lsu")
         self.side_ctas = int(os.environ.get("MVB_WE_SIDE_CTAS", "10" if self.side_mode == "bulk" else "1"))
-        if self.mode == "direct" and not (rt.size > 1 and self._dev_block_ok()):
+        # direct mode runs only on the window kernel: dim <= 512, window <= 15
+        if self.mode == "direct" and not (rt.size > 1 and self._dev_block_ok() and D <= 512
+                                          and option.window_size <= 15):
             self.mode = "block"
         if self.side_mode == "mbox" and rt.size > 1 and self._dev_block_ok() and self.input_table.S == rt.size:
             self.input_table.enable_row_mailbox()          # collective
@@ -242,14 +238,13 @@ class WordEmbedding:
         a.seed = ((0x5DEECE66D * (self.rt.rank + 1)) ^ (self._step * 0x9E3779B97F4A7C15)) & 0xFFFFFFFFFFFFFFFF
         a.loss_sum = self.loss.data_ptr() if compute_loss else None
         a.pair_count = self.pairs.data_ptr()
-        a.variant = self.kernel_variant
+        a.hogwild = int(self.hogwild)
         a.max_ctas = self.max_ctas if max_ctas is None else max_ctas
         if direct:
             ti, to = self.input_table, self.output_table
             a.nservers, a.rows_per_server = ti.S, ti.rps
             for s_ in range(ti.S):
                 a.w_in_peers[s_], a.w_out_peers[s_] = ti.shard_ptrs[s_], to.shard_ptrs[s_]
-            a.variant = 20
         a.scale_in, a.scale_out = N.ptr(self.scale_in), N.ptr(self.scale_out)
         N.cuda_lib().mvb_sgns_train(a, N.stream_ptr())
         self.kernel_launches += N.cuda_lib().mvb_sgns_last_launches()
@@ -272,12 +267,12 @@ class WordEmbedding:
             with monitor("WE_TRAIN_BLOCK", cuda=True):
                 self._launch(tokens, self.input_table.shard, self.output_table.shard,
                              None if self.g2_in is None else self.g2_in.shard,
-                             None if self.g2_out is None else self.g2_out.shard, self.LD,
+                             None if self.g2_out is None else self.g2_out.shard, self.D,
                              compute_loss=compute_loss)
             return
         if self.mode == "direct":
             with monitor("WE_TRAIN_BLOCK", cuda=True):
-                self._launch(tokens, self.input_table.shard, self.output_table.shard, None, None, self.LD,
+                self._launch(tokens, self.input_table.shard, self.output_table.shard, None, None, self.D,
                              compute_loss=compute_loss, direct=True)
             return
         if next_tokens is None and self._prefetched is None:
@@ -335,7 +330,7 @@ class WordEmbedding:
         if os.environ.get("MVB_WE_DEV_BLOCK", "1") == "0":
             return False
         return (not o.hs and not o.cbow and not o.use_adagrad and o.negative_num >= 1 and o.negative_num <= 7
-                and self.D % 4 == 0 and self.LD % 4 == 0 and self.kernel_variant in (0, 20))
+                and self.D % 4 == 0)
 
     def _block_buffers(self, slot: int, n_tokens: int) -> dict:
         """Fixed-capacity buffers of one in-flight block: nothing is allocated or sized on the host per
@@ -344,7 +339,7 @@ class WordEmbedding:
         cap_in = min(self.V, max(int(n_tokens), 1))
         if b is not None and b["cap_in"] >= cap_in:
             return b
-        o, dev, V, LD = self.opt, self.dev, self.V, self.LD
+        o, dev, V, D = self.opt, self.dev, self.V, self.D
         cap_out = min(V, cap_in * (1 + o.negative_num))
         words = (V + 31) // 32
         i32 = dict(dtype=torch.int32, device=dev)
@@ -354,8 +349,8 @@ class WordEmbedding:
                  map_in=torch.empty(V, **i32), map_out=torch.empty(V, **i32),
                  ids_in=torch.empty(cap_in, **i32), ids_out=torch.empty(cap_out, **i32),
                  neg_pool=torch.empty(max(cap_in * o.negative_num, 1), **i32), counts=torch.zeros(4, **i32),
-                 cache_in=torch.empty(cap_in, LD, device=dev), old_in=torch.empty(cap_in, LD, device=dev),
-                 cache_out=torch.empty(cap_out, LD, device=dev), old_out=torch.empty(cap_out, LD, device=dev))
+                 cache_in=torch.empty(cap_in, D, device=dev), old_in=torch.empty(cap_in, D, device=dev),
+                 cache_out=torch.empty(cap_out, D, device=dev), old_out=torch.empty(cap_out, D, device=dev))
         b["n_pool"] = b["counts"][2:]
         self._bufs[slot] = b
         return b
@@ -385,7 +380,7 @@ class WordEmbedding:
         with monitor("WE_REQUEST_PARAMETER", cuda=True):
             for tab, ids, ci, cache, old, cap in ((self.input_table, b["ids_in"], 0, b["cache_in"], b["old_in"], b["cap_in"]),
                                                   (self.output_table, b["ids_out"], 1, b["cache_out"], b["old_out"], b["cap_out"])):
-                lib.mvb_rows_pull_bulk(tab._rowmap, 4, ids, cnt + 4 * ci, cap, cache, old, self.LD, ctas, st)
+                lib.mvb_rows_pull_bulk(tab._rowmap, 4, ids, cnt + 4 * ci, cap, cache, old, self.D, ctas, st)
         self.kernel_launches += 2
         return b
 
@@ -410,7 +405,7 @@ class WordEmbedding:
         with monitor("WE_ADD_DELTA", cuda=True):
             for tab, ids, ci, cache, old, cap in ((self.input_table, b["ids_in"], 0, b["cache_in"], b["old_in"], b["cap_in"]),
                                                   (self.output_table, b["ids_out"], 1, b["cache_out"], b["old_out"], b["cap_out"])):
-                lib.mvb_rows_push_delta_bulk(tab._rowmap, ids, cnt + 4 * ci, cap, cache, old, self.LD, 1.0 / self.W,
+                lib.mvb_rows_push_delta_bulk(tab._rowmap, ids, cnt + 4 * ci, cap, cache, old, self.D, 1.0 / self.W,
                                              ctas, st)
         self.kernel_launches += 2
 
@@ -475,10 +470,10 @@ class WordEmbedding:
             if st.get("dev"):
                 # pipelined: leave `side_ctas` SMs to the pull / push kernels running on the side stream
                 cap = max(1, self.num_sms - self.side_ctas) if (pipelined and self.side_mode == "bulk") else None
-                self._launch(tokens, st["cache_in"], st["cache_out"], None, None, self.LD, st["map_in"], st["map_out"],
+                self._launch(tokens, st["cache_in"], st["cache_out"], None, None, self.D, st["map_in"], st["map_out"],
                              st["neg_pool"], compute_loss, neg_pool_size_ptr=st["n_pool"], max_ctas=cap)
             else:
-                self._launch(tokens, st["cache_in"], st["cache_out"], st["g2i"], st["g2o"], self.LD,
+                self._launch(tokens, st["cache_in"], st["cache_out"], st["g2i"], st["g2o"], self.D,
                              st["map_in"], st["map_out"], st["neg_pool"], compute_loss)
 
     def _add_delta(self, st: dict, side: bool = False) -> None:
@@ -486,7 +481,7 @@ class WordEmbedding:
         if st.get("dev"):
             self._add_delta_dev(st, side)
             return
-        o, D = self.opt, self.LD
+        o, D = self.opt, self.D
         inv = 1.0 / self.W
         in_ids, out_ids = st["in_ids"], st["out_ids"]
         if D % 4 == 0:
@@ -517,10 +512,10 @@ class WordEmbedding:
         row mailboxes a worker's last deltas are applied by their owners at the next MV_Barrier (the
         reference's SaveEmbedding is preceded by one, distributed_wordembedding.cpp:232-237)."""
         self.flush()
-        return self.input_table.get().view(self.V, self.LD)[:, :self.D]
+        return self.input_table.get().view(self.V, self.D)
 
     def _input_rows(self, ids: torch.Tensor) -> torch.Tensor:
-        return self.input_table.get_rows(ids)[:, :self.D]
+        return self.input_table.get_rows(ids)
 
     def most_similar(self, word_ids, k: int = 10, rows: Optional[int] = None):
         """Nearest input-embedding rows by cosine (word2vec's ``distance``) of each word in ``word_ids``,
@@ -554,7 +549,7 @@ class WordEmbedding:
             f.write(f"{self.V} {self.D}\n".encode())
             for lo in range(0, self.V, batch):
                 hi = min(self.V, lo + batch)
-                rows = self.input_table.get_rows(torch.arange(lo, hi, device=self.dev))[:, :self.D].cpu().numpy()
+                rows = self.input_table.get_rows(torch.arange(lo, hi, device=self.dev)).cpu().numpy()
                 for i in range(hi - lo):
                     w = words[lo + i] if words is not None else str(lo + i)
                     if binary:

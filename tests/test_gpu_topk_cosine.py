@@ -210,7 +210,7 @@ def test_model_search_planted(mv_device):
     E = rng.normal(size=(2000, 64)).astype(np.float32)
     r = rng.normal(size=64).astype(np.float32)
     E[1000:1020] = E[0:20] + r + 0.05 * rng.normal(size=(20, 64)).astype(np.float32)   # capital_i = country_i + r
-    we.input_table.shard.view(2000, we.LD)[:, :64].copy_(torch.from_numpy(E))
+    we.input_table.shard.view(2000, 64).copy_(torch.from_numpy(E))
     Et = torch.from_numpy(E)
     ids = torch.arange(0, 40)
     s, i = we.most_similar(ids, k=10)

@@ -11,16 +11,18 @@ def _sig(x):
     return 1.0 / (1.0 + torch.exp(-x))
 
 
-@pytest.mark.parametrize("variant", [5, 1, 10, 20])
-def test_sgns_fast_kernel_matches_reference(mv_device, variant):
-    """window=1 (no random shrink) and a one-word negative pool make the sample schedule
+@pytest.mark.parametrize("D,K,hogwild", [(64, 8, 0), (200, 8, 0), (300, 8, 0), (512, 8, 0), (300, 5, 1)])
+def test_sgns_fast_kernel_matches_reference(mv_device, D, K, hogwild):
+    """The Hogwild kernels through the default dispatch: K = 8 runs the register kernel (one
+    instantiation per row width: D 64 / 200 / 300 / 512), hogwild = 1 the window kernel.
+    window=1 (no random shrink) and a one-word negative pool make the sample schedule
     deterministic: centre p trains (ctx p-1 -> p) then (ctx p+1 -> p), each with K draws of
     the pool word evaluated on pre-update rows. All words distinct, so cross-warp coupling
     is only through red.add accumulation: warps may or may not observe each other's updates
     (Hogwild), an O(lr^2) effect, so the test uses a small lr and compares the UPDATES with a
     relative tolerance (a wrong sign / missing term would be off by >= 100%)."""
     from multiverso_b200 import _native as N
-    V, D, K, lr = 64, 300, 5, 1e-3
+    V, lr = 64, 1e-3
     torch.manual_seed(0)
     w_in = (torch.rand(V, D, device="cuda") - 0.5) * 0.2
     w_out = (torch.rand(V, D, device="cuda") - 0.5) * 0.2
@@ -55,7 +57,7 @@ def test_sgns_fast_kernel_matches_reference(mv_device, variant):
     a.window, a.negative, a.lr = 1, K, lr
     a.vocab, a.neg_pool, a.neg_pool_size = V, pool.data_ptr(), 1
     a.seed, a.loss_sum, a.pair_count = 1234, loss.data_ptr(), pairs.data_ptr()
-    a.variant = variant
+    a.hogwild = hogwild
     N.cuda_lib().mvb_sgns_train(a, N.stream_ptr())
     torch.cuda.synchronize()
     assert int(pairs.item()) == 8
@@ -68,19 +70,17 @@ def test_sgns_fast_kernel_matches_reference(mv_device, variant):
     assert float(loss.item()) > 0
 
 
-@pytest.mark.parametrize("mode", ["sg_ns", "cbow_ns", "sg_hs", "cbow_hs", "sg_ns_adagrad", "sg_ns_d100", "sg_ns_tma", "sg_ns_win"])
+@pytest.mark.parametrize("mode", ["sg_ns", "cbow_ns", "sg_hs", "cbow_hs", "sg_ns_adagrad", "sg_ns_d100", "sg_ns_k8", "sg_ns_win"])
 def test_wordembedding_loss_decreases(mv_device, mode):
     from multiverso_b200.models.wordembedding import (WordEmbedding, WordEmbeddingOption,
                                                       synthetic_zipf_corpus)
     V = 2000
-    opt = WordEmbeddingOption(embeding_size=100 if mode.endswith("d100") else 64, window_size=5, negative_num=5,
+    opt = WordEmbeddingOption(embeding_size=100 if mode.endswith("d100") else 64, window_size=5,
+                              negative_num=8 if mode.endswith("k8") else 5,
                               cbow="cbow" in mode, hs="hs" in mode, use_adagrad="adagrad" in mode,
                               init_learning_rate=0.025 if "hs" in mode else 0.05)
     we = WordEmbedding(opt, V)
-    if mode.endswith("tma"):
-        we.kernel_variant = 10
-    if mode.endswith("win"):
-        we.kernel_variant = 20
+    we.hogwild = mode.endswith("win")
     # a learnable corpus: word 2i is always followed by word 2i+1
     rng = np.random.default_rng(0)
     base = rng.integers(0, V // 2, size=40000) * 2
@@ -130,7 +130,7 @@ def _hash64(x):
 
 @pytest.mark.parametrize("n_tok,dim", [(60, 300), (1500, 300), (700, 64), (400, 200)])
 def test_sgns_window_kernel_matches_schedule(mv_device, n_tok, dim):
-    """The window-batched K7 (variant 20) against a plain fp64 re-implementation of ITS sample
+    """The window-batched K7 against a plain fp64 re-implementation of ITS sample
     schedule: per centre p the hash RNG gives the window shrink and K pool draws shared by the
     position's contexts; scores on pre-update rows; input delta sum_k g_ck out_k, output delta
     sum_c g_ck in_c.  All tokens are distinct and the pool words are not tokens, so rows only couple
@@ -214,7 +214,7 @@ def _check_schedule(fn, n_tok, dim, tol):
 
 
 def test_sgns_window_kernel_maps_and_cta_cap(mv_device):
-    """Block mode of variant 20: rows live in a compact cache addressed through id -> slot maps
+    """Block mode of the window kernel: rows live in a compact cache addressed through id -> slot maps
     (world > 1), the grid is capped (max_ctas) and rows are padded (ld > dim); result must equal the
     identity-mapped full-grid run on the same data (same seed => same schedule) up to Hogwild noise."""
     from multiverso_b200 import _native as N
@@ -288,6 +288,31 @@ def test_sgns_det_kernel_maps_and_ld(mv_device):
     assert torch.equal(r1, r2) and r1[0] > 0 and r1[1] != 0       # pairs, loss (float bits)
     assert torch.equal(c_in[perm, :D], a_in) and torch.equal(c_out[perm, :D], a_out)
     assert (c_in[:, D:] == 0).all() and (c_out[:, D:] == 0).all() and not torch.equal(a_in, base[0])
+
+
+def test_direct_mode_declines_what_the_window_kernel_does_not_cover(mv_device):
+    """Direct mode (nservers > 1) runs on the window kernel alone.  With dim 516 it declines, and the call
+    raises without touching either table instead of running a kernel that ignores the peer shards."""
+    from multiverso_b200 import _native as N
+    V, D = 64, 516
+    g = torch.Generator().manual_seed(5)
+    w_in = ((torch.rand(V, D, generator=g) - 0.5) * 0.4).cuda()
+    w_out = ((torch.rand(V, D, generator=g) - 0.5) * 0.4).cuda()
+    i0, o0 = w_in.clone(), w_out.clone()
+    toks = torch.randint(0, V, (500,), generator=g).to(torch.int32).cuda()
+    prob, alias = torch.ones(V, device="cuda"), torch.arange(V, dtype=torch.int32, device="cuda")
+    a = N.Sgns()
+    a.tokens, a.n_tokens = toks.data_ptr(), toks.numel()
+    a.w_in, a.w_out, a.dim, a.ld = w_in.data_ptr(), w_out.data_ptr(), D, D
+    a.window, a.negative, a.lr, a.seed = 5, 5, 0.05, 11
+    a.vocab, a.alias_prob, a.alias_idx = V, prob.data_ptr(), alias.data_ptr()
+    a.nservers, a.rows_per_server = 2, V // 2
+    for s_ in range(2):                                   # the two halves of one table as the two shards
+        a.w_in_peers[s_], a.w_out_peers[s_] = w_in[s_ * V // 2].data_ptr(), w_out[s_ * V // 2].data_ptr()
+    with pytest.raises(N.NativeError):
+        N.cuda_lib().mvb_sgns_train(a, N.stream_ptr())
+    torch.cuda.synchronize()
+    assert torch.equal(w_in, i0) and torch.equal(w_out, o0)
 
 
 def test_synthetic_corpus_shape():

@@ -29,7 +29,6 @@ mp)
   fi
   ;;
 ncu)
-  timeout 600 ncu --set full --clock-control none --import-source on -k regex:sgns_fast -s 3 -c 1 -f -o gpurun_out/sgns_fast python bench.py --steps 2 --warmup 3 --no-table-bw > gpurun_out/ncu_sgns.log 2>&1; echo "ncu rc=$?"; tail -3 gpurun_out/ncu_sgns.log
   timeout 600 ncu --metrics gpu__time_duration.sum --clock-control none -c 60 --csv --log-file gpurun_out/launches.csv python bench.py --steps 2 --warmup 3 > gpurun_out/ncu_launches.log 2>&1; echo "launches rc=$?"
   ;;
 ncu_dense)
@@ -37,14 +36,6 @@ ncu_dense)
 import torch, multiverso_b200 as mv
 mv.init(); t = mv.MatrixTable(1000000, 512, 'float32', updater='sgd'); d = torch.ones(512000000, device='cuda')
 t.add(d); t.get(); t.add(d); t.get(); mv.shutdown()" > gpurun_out/ncu_dense.log 2>&1; echo "ncu_dense rc=$?"
-  ;;
-sweep)
-  for v in ${SWEEP_VARIANTS:-5 3 2 1 10}; do
-    MVB_SGNS_VARIANT=$v timeout 300 python bench.py --steps 6 --warmup 3 --no-table-bw > gpurun_out/sweep_v$v.json 2> gpurun_out/sweep_v$v.err; echo "variant $v rc=$? $(python -c "import json;d=json.load(open('gpurun_out/sweep_v$v.json'));print(d['value']/1e6,'Mwords/s',d['ms_per_step'],'ms', 'loss',d['config']['loss_per_pair'])" 2>&1 | tail -1)"
-  done
-  for st in ${SWEEP_STAGES:-}; do
-    MVB_SGNS_STAGES=$st MVB_SGNS_VARIANT=10 timeout 300 python bench.py --steps 6 --warmup 3 --no-table-bw > gpurun_out/sweep_v10_s$st.json 2> gpurun_out/sweep_v10_s$st.err; echo "tma stages $st rc=$? $(python -c "import json;d=json.load(open('gpurun_out/sweep_v10_s$st.json'));print(d['value']/1e6,'Mwords/s',d['ms_per_step'],'ms')" 2>&1 | tail -1)"
-  done
   ;;
 extra)
   if [ "$NG" -gt 1 ]; then L="python -m torch.distributed.run --nnodes=1 --nproc-per-node $NG --master-addr 127.0.0.1 --master-port $((PORT+5))"; else L="python"; fi
@@ -78,20 +69,15 @@ perf)
   timeout 300 $L bench/matrix_perf.py --sparse > gpurun_out/matrix_perf_sparse.log 2>&1; echo "matrix_perf sparse rc=$?"; grep '^{' gpurun_out/matrix_perf_sparse.log | tail -1 | cut -c1-500
   ;;
 win)
-  # round 2: window-batched K7 (variant 20): numerics, 1-GPU bench vs the pair-at-a-time TMA kernel, ncu
+  # round 2: window-batched K7: numerics, 1-GPU bench, ncu
   timeout 600 python -m pytest tests/test_gpu_wordembedding.py -x -q > gpurun_out/pytest_we.log 2>&1; echo "pytest we rc=$?"; tail -8 gpurun_out/pytest_we.log
   timeout 300 python bench.py --steps 10 --warmup 3 > gpurun_out/bench_n1_win.json 2> gpurun_out/bench_n1_win.err; echo "bench win rc=$?"; cut -c1-700 gpurun_out/bench_n1_win.json; tail -3 gpurun_out/bench_n1_win.err
-  MVB_SGNS_VARIANT=10 timeout 300 python bench.py --steps 6 --warmup 3 --no-table-bw > gpurun_out/bench_n1_tma.json 2> gpurun_out/bench_n1_tma.err; echo "bench tma rc=$?"; cut -c1-300 gpurun_out/bench_n1_tma.json
-  for nw in ${WIN_NW:-6 8}; do
-    MVB_WIN_NW=$nw timeout 300 python bench.py --steps 6 --warmup 3 --no-table-bw > gpurun_out/bench_n1_win_nw$nw.json 2> gpurun_out/bench_n1_win_nw$nw.err; echo "bench win nw=$nw rc=$?"; cut -c1-200 gpurun_out/bench_n1_win_nw$nw.json
-  done
   timeout 600 ncu --set full --clock-control none --import-source on -k regex:sgns_win -s 3 -c 1 -f -o gpurun_out/sgns_win python bench.py --steps 2 --warmup 3 --no-table-bw > gpurun_out/ncu_sgns_win.log 2>&1; echo "ncu rc=$?"; tail -3 gpurun_out/ncu_sgns_win.log
   ;;
 cap)
-  # hot-row step cap sweep: loss after the same number of blocks vs the pair-at-a-time kernel
+  # hot-row step cap sweep: loss after the same number of blocks
   timeout 600 python -m pytest tests/test_gpu_wordembedding.py -x -q > gpurun_out/pytest_we.log 2>&1; echo "pytest we rc=$?"; tail -5 gpurun_out/pytest_we.log
   for st in ${CAP_STEPS:-6 22}; do
-  MVB_SGNS_VARIANT=10 timeout 300 python bench.py --steps $st --warmup 3 --no-table-bw > gpurun_out/cap_tma_s$st.json 2>/dev/null; python -c "import json;d=json.load(open('gpurun_out/cap_tma_s$st.json'));print('tma steps $st', round(d['value']/1e6,1), d['config']['loss_per_pair'])"
   for c in ${CAPS:-32 64 128 256 512}; do
     MVB_WE_HOT_CAP=$c timeout 300 python bench.py --steps $st --warmup 3 --no-table-bw > gpurun_out/cap_${c}_s$st.json 2>/dev/null; python -c "import json;d=json.load(open('gpurun_out/cap_${c}_s$st.json'));print('cap $c steps $st', round(d['value']/1e6,1), d['config']['loss_per_pair'])"
   done
@@ -132,14 +118,6 @@ r2final)
   ;;
 refarm)
   timeout 1500 python bench.py --impl reference --gpus 1 > gpurun_out/bench_ref_n1.json 2> gpurun_out/bench_ref_n1.err; echo "ref rc=$?"; cut -c1-300 gpurun_out/bench_ref_n1.json
-  ;;
-tma_debug)
-  for dbg in 0 1 2; do
-    MVB_TMA_DEBUG=$dbg MVB_SGNS_VARIANT=10 timeout 300 python bench.py --steps 6 --warmup 3 --no-table-bw > gpurun_out/tma_dbg$dbg.json 2> gpurun_out/tma_dbg$dbg.err; echo "tma debug $dbg rc=$? $(python -c "import json;d=json.load(open('gpurun_out/tma_dbg$dbg.json'));print(d['value']/1e6,'Mwords/s',d['ms_per_step'],'ms')" 2>&1 | tail -1)"
-  done
-  ;;
-ncu_tma)
-  MVB_SGNS_VARIANT=10 timeout 600 ncu --set full --clock-control none --import-source on -k regex:sgns_tma -s 3 -c 1 -f -o gpurun_out/sgns_tma python bench.py --steps 2 --warmup 3 --no-table-bw > gpurun_out/ncu_sgns_tma.log 2>&1; echo "ncu_tma rc=$?"; tail -2 gpurun_out/ncu_sgns_tma.log
   ;;
 bulk)
   # EXPERIMENT: dense Get through the bulk-copy engine (MVB_GET_BULK=1) -- correctness first, then time it

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Summarise an .ncu-rep (read on the CPU box) into <name>.md: key raw metrics, the
 top stall locations of the source page, and the occupancy / roofline lines of the details page.
-    python tools/ncu_summary.py sgns_tma.ncu-rep sgns_tma_ncu.md "title" """
+    python tools/ncu_summary.py sgns_win.ncu-rep sgns_win_ncu.md "title" """
 import csv
 import io
 import subprocess
