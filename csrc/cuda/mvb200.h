@@ -467,6 +467,32 @@ typedef struct MvbTopkCos {
 int64_t mvb_topk_cos_scratch_bytes(int64_t M, int k, int64_t n_rows);
 int mvb_topk_cosine(const MvbTopkCos* a, void* stream);
 
+/* Full softmax of an output layer whose classes are the rows [0, n_rows) of the table (topk_cos.cu, the
+ * same one-pass search with the dot product z = q . w as the score): for each query row
+ *   lse  = log sum_n exp(z_n)   (tf32 logits, fp32 accumulation, folded in a fixed tile / range order)
+ *   loss = lse - z_label        (label logit in fp64; not clamped)
+ * and / or the k rows with the largest z, sorted by score descending, ties by the smaller id (the fp64 dot
+ * products of k + 8 tf32 candidates, rounded to fp32; missing slots id -1, score -inf). The [M x n_rows]
+ * logits are never written. lse NULL: top-k only (k >= 1). labels and loss go together and need lse.
+ * The caller validates labels (in [0, n_rows)). Errors: -40 k, -41 row map, -42 pitches, -43 dim,
+ * -44 n_rows (1 <= n_rows <= num_row), -45 M or scratch, -46 outputs. */
+typedef struct MvbFullSoftmax {
+  const float* q;            /* [M x ldq] fp32, ldq % 4 == 0, columns >= dim unused             */
+  int64_t M, ldq;            /* M <= 65535 per call                                             */
+  int64_t dim, n_rows;       /* columns used (<= wmap.num_col); classes                         */
+  MvbRowMap wmap;            /* the table's shards, row pitch wmap.num_col (% 4 == 0)           */
+  int k;                     /* 0 <= k <= MVB_TOPK_MAX                                          */
+  const int64_t* labels;     /* [M] or NULL                                                     */
+  float* lse;                /* [M] out or NULL                                                 */
+  float* loss;               /* [M] out, with labels                                            */
+  float* scores;             /* [M x k] out, k > 0                                              */
+  int64_t* ids;              /* [M x k] out, k > 0                                              */
+  void* scratch;             /* device, mvb_full_softmax_scratch_bytes(M, k, n_rows) bytes      */
+  int64_t scratch_bytes;
+} MvbFullSoftmax;
+int64_t mvb_full_softmax_scratch_bytes(int64_t M, int k, int64_t n_rows);
+int mvb_full_softmax(const MvbFullSoftmax* a, void* stream);
+
 /* ---- embedding bag over a row-sharded fp32 MatrixTable (emb_bag.cu) ---------------------------- */
 /* Bag b holds the lookups [offsets[b], offsets[b + 1]) (the last bag ends at L); its output row is the sum
  * (mean: the sum over the bag length) of psw_j * W[ids_j, :dim]; an empty bag gives zeros. Rows are read

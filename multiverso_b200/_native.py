@@ -145,6 +145,12 @@ class TopkCos(C.Structure):
                 ("k", C.c_int), ("scores", vp), ("ids", vp), ("scratch", vp), ("scratch_bytes", i64)]
 
 
+class FullSoftmax(C.Structure):
+    _fields_ = [("q", vp), ("M", i64), ("ldq", i64), ("dim", i64), ("n_rows", i64), ("wmap", RowMap),
+                ("k", C.c_int), ("labels", vp), ("lse", vp), ("loss", vp), ("scores", vp), ("ids", vp),
+                ("scratch", vp), ("scratch_bytes", i64)]
+
+
 EMB_PUSH, EMB_COMPACT = 0, 1
 
 
@@ -292,6 +298,8 @@ _CUDA_FUNCS = {
     "mvb_get_gemm_last_config": _unchecked(i32),
     "mvb_topk_cos_scratch_bytes": _unchecked(i64, i64, i32, i64),
     "mvb_topk_cosine": _status(C.POINTER(TopkCos), Ptr),
+    "mvb_full_softmax_scratch_bytes": _unchecked(i64, i64, i32, i64),
+    "mvb_full_softmax": _status(C.POINTER(FullSoftmax), Ptr),
     "mvb_embedding_bag_scratch_bytes": _unchecked(i64, i64, i64),
     "mvb_embedding_bag_fwd": _status(C.POINTER(EmbBag), Ptr),
     "mvb_embedding_bag_bwd": _status(C.POINTER(EmbBag), Ptr),

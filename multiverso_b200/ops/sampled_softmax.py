@@ -43,6 +43,12 @@ graph raises. An empty batch returns an empty loss and pushes nothing.
 
 On the host backend the same call draws the same ids, reads ``get_rows`` of the unique rows, evaluates the formula
 in torch fp32 with autograd for ``dL/dhidden`` and pushes the row gradients with one coalesced ``add_rows``.
+
+The sampled loss is an estimate for training. ``ssm.evaluate(hidden, labels, k=0)`` is the exact full softmax over
+every row of the table (:func:`~multiverso_b200.ops.full_softmax`): ``r.lse``, the cross-entropy ``r.loss`` (the
+perplexity is ``exp(r.loss.mean())``) and, for ``k > 0``, the top-k classes by logit in ``r.scores`` / ``r.ids``. It
+has no log-Q correction and no accidental-hit mask, draws nothing, leaves ``ssm.steps`` alone, pushes nothing, and
+on the device never writes the ``[B, N]`` logits.
 """
 from __future__ import annotations
 
@@ -56,6 +62,7 @@ from .. import _native as N
 from ..tables.options import AddOption
 from ..utils import monitor
 from .embedding import _INT, _device_of, _dtype_of, _host_rows, _push_device
+from .full_softmax import FullSoftmaxResult, full_softmax
 from .get_gemm import gemm_nt
 from .topk import _rowmap_of
 
@@ -253,6 +260,18 @@ class PSSampledSoftmax(torch.nn.Module):
                 table.add_rows(uniq.numpy(), (g * float(scale)).numpy(), option)
         rows.register_hook(push)
         return loss.to(hidden.device)
+
+    # ------------------------------------------------------------------------------------------------ evaluation
+    def evaluate(self, hidden: torch.Tensor, labels, k: int = 0) -> FullSoftmaxResult:
+        """The exact full softmax of ``hidden`` [B, in_features] over all ``num_classes`` rows: ``lse``, ``loss`` and,
+        for ``k > 0``, the top-k classes (see :func:`~multiverso_b200.ops.full_softmax`). Evaluation only: nothing
+        is drawn, ``steps`` does not advance and nothing is pushed."""
+        h = torch.as_tensor(hidden)
+        if h.dim() == 2 and h.shape[1] != self.in_features:
+            raise ValueError(f"{_WHAT}: hidden has {h.shape[1]} columns, the table rows {self.in_features}")
+        if self._device is not None and isinstance(h, torch.Tensor) and not h.is_cuda:
+            raise ValueError(f"{_WHAT}: the table is on the GPU, hidden must be too")
+        return full_softmax(self.table, h, labels, k)
 
     def extra_repr(self) -> str:
         src = f"counts^{self.power}" if self.sampler == "counts" else repr(self.sampler)

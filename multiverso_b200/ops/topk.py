@@ -76,18 +76,25 @@ def topk_cosine_reference(weights: torch.Tensor, queries: torch.Tensor, k: int,
     for lo in range(0, n, row_chunk):
         hi = min(n, lo + row_chunk)
         wc = _unit_rows(w[lo:hi, :dim].to(device=q.device, dtype=torch.float32))
-        s = q @ wc.t()
-        kk = min(k, hi - lo)
-        v, _ = s.topk(kk, dim=1)
-        # every row scoring at least the kk-th value is a candidate: ties at the boundary resolve by id
-        cand = s >= v[:, -1:]
-        width = int(cand.sum(1).max())
-        cs = torch.where(cand, s, torch.full_like(s, float("-inf")))
-        cv, ci = cs.topk(width, dim=1)
-        ci = torch.where(cv > float("-inf"), ci + lo, torch.full_like(ci, torch.iinfo(torch.int64).max))
-        best_s, best_i = _sorted_topk(torch.cat([best_s, cv], 1),
-                                      torch.cat([torch.where(best_i < 0, torch.full_like(best_i, torch.iinfo(torch.int64).max), best_i), ci], 1), k)
-        best_i = torch.where(best_i == torch.iinfo(torch.int64).max, torch.full_like(best_i, -1), best_i)
+        best_s, best_i = merge_topk(best_s, best_i, q @ wc.t(), lo, k)
+    return best_s, best_i
+
+
+def merge_topk(best_s: torch.Tensor, best_i: torch.Tensor, s: torch.Tensor, lo: int,
+               k: int) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Fold the scores ``s`` [M, c] of rows [lo, lo + c) into a running top-k (``best_s``, ``best_i``) [M, k]
+    under (score desc, id asc); empty slots hold -inf / -1."""
+    kk = min(k, s.shape[1])
+    v, _ = s.topk(kk, dim=1)
+    # every row scoring at least the kk-th value is a candidate: ties at the boundary resolve by id
+    cand = s >= v[:, -1:]
+    width = int(cand.sum(1).max())
+    cs = torch.where(cand, s, torch.full_like(s, float("-inf")))
+    cv, ci = cs.topk(width, dim=1)
+    ci = torch.where(cv > float("-inf"), ci + lo, torch.full_like(ci, torch.iinfo(torch.int64).max))
+    best_s, best_i = _sorted_topk(torch.cat([best_s, cv], 1),
+                                  torch.cat([torch.where(best_i < 0, torch.full_like(best_i, torch.iinfo(torch.int64).max), best_i), ci], 1), k)
+    best_i = torch.where(best_i == torch.iinfo(torch.int64).max, torch.full_like(best_i, -1), best_i)
     return best_s, best_i
 
 
@@ -113,27 +120,40 @@ def _rowmap_of(table, what: str = "topk_cosine") -> Tuple[N.RowMap, int, int]:
     return rm, table.num_row, table.num_col
 
 
+def check_queries(rm: N.RowMap, width: int, queries: torch.Tensor, name: str,
+                  what: str = "topk_cosine") -> None:
+    """The kernel's demands on a query batch ``[M, dim]`` and on the table's row map."""
+    if queries.dtype != torch.float32 or queries.dim() != 2:
+        raise TypeError(f"{what}: {name} must be a 2-D float32 tensor, got {queries.dtype} {tuple(queries.shape)}")
+    if not queries.is_cuda:
+        raise ValueError(f"{what}: the table is on the GPU, the {name} must be too")
+    dim = queries.shape[1]
+    if dim < 1 or dim > width:
+        raise ValueError(f"{what}: {name} have {dim} columns, the table rows {width}")
+    if rm.num_col % 4 != 0:
+        raise ValueError(f"{what}: the table's row pitch ({rm.num_col} floats) must be a multiple of 4 "
+                         "(16-byte rows for TMA)")
+
+
+def padded_queries(q: torch.Tensor) -> torch.Tensor:
+    """``q`` [M, dim] in a fresh zero-padded [M, ldq] buffer, ldq = dim rounded up to 4 (16-byte TMA rows)."""
+    M, dim = q.shape
+    out = torch.zeros(M, (dim + 3) // 4 * 4, dtype=torch.float32, device=q.device)
+    out[:, :dim] = q
+    return out
+
+
 def _topk_device(rm: N.RowMap, width: int, queries: torch.Tensor, k: int,
                  rows: Optional[int]) -> Tuple[torch.Tensor, torch.Tensor]:
     """Kernel path over an explicit row map (``width``: usable columns of a row)."""
-    if queries.dtype != torch.float32 or queries.dim() != 2:
-        raise TypeError(f"topk_cosine: queries must be a 2-D float32 tensor, got {queries.dtype} "
-                        f"{tuple(queries.shape)}")
-    if not queries.is_cuda:
-        raise ValueError("topk_cosine: the table is on the GPU, the queries must be too")
+    check_queries(rm, width, queries, "queries")
     M, dim = queries.shape
-    if dim < 1 or dim > width:
-        raise ValueError(f"topk_cosine: queries have {dim} columns, the table rows {width}")
-    if rm.num_col % 4 != 0:
-        raise ValueError(f"topk_cosine: the table's row pitch ({rm.num_col} floats) must be a multiple of 4 "
-                         "(16-byte rows for TMA)")
     n = rm.num_row if rows is None else int(rows)
     if not 0 <= n <= rm.num_row:
         raise ValueError(f"topk_cosine: rows={n} outside [0, {rm.num_row}]")
     dev = queries.device
-    ldq = (dim + 3) // 4 * 4
-    q = torch.zeros(M, ldq, dtype=torch.float32, device=dev)
-    q[:, :dim] = _unit_rows(queries)
+    q = padded_queries(_unit_rows(queries))
+    ldq = q.shape[1]
     scores = torch.empty(M, k, dtype=torch.float32, device=dev)
     ids = torch.empty(M, k, dtype=torch.int64, device=dev)
     lib = N.cuda_lib()
