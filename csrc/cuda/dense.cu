@@ -383,7 +383,8 @@ __global__ void __launch_bounds__(256) get_dense_kernel(const __grid_constant__ 
   const T* __restrict__ src = g.shard[s];
   T* __restrict__ dst = g.out + g.off[s];
   const int64_t len = g.len[s];
-  const bool vec_ok = (g.off[s] % VEC == 0);
+  // `out` may be a view at any element offset: 16-byte accesses only where both ends are aligned
+  const bool vec_ok = ((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst)) & 15) == 0;
   const int64_t tid = gidx * blockDim.x + threadIdx.x;
   const int64_t stride = gcount * blockDim.x;
   if (vec_ok) {

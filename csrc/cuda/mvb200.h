@@ -179,7 +179,9 @@ int mvb_add_rows_red(int dtype, const MvbRowMap* m, const int64_t* row_ids, int6
 int mvb_add_rows_delta(const MvbRowMap* m, const int64_t* row_ids, int64_t k, const float* cur,
                        const float* old, int64_t ld, float scale, void* stream);
 /* Stateful row add applied by the OWNER on its local shard for rows in its range:
- * ids/vals may be another rank's (peer-mapped) staging. */
+ * ids/vals may be another rank's (peer-mapped) staging.  A repeated row is updated once per
+ * occurrence, in list order, when its occurrences are adjacent (sort the request stably by id);
+ * occurrences that are not adjacent race. */
 int mvb_add_rows_owner(int dtype, int updater, void* shard, void* state0, void* state1,
                        int64_t row_lo, int64_t row_hi, int64_t num_col, int64_t state_stride,
                        const int64_t* row_ids, int64_t k, const void* vals, int64_t vals_ld,

@@ -126,6 +126,9 @@ add_rows_delta_kernel(const __grid_constant__ RowMapDev m, const int64_t* __rest
   }
 }
 
+// Repeated rows must be applied one after the other, in list order (MatrixServerTable::ProcessAdd), so
+// the caller passes the ids with equal ids adjacent (a stable sort) and the warp that meets the START of
+// a run of equal ids applies the whole run in order, keeping the element and its state in registers.
 template <int UPD, typename T>
 __global__ void __launch_bounds__(256)
 add_rows_owner_kernel(T* __restrict__ shard, T* __restrict__ st0, T* __restrict__ st1,
@@ -139,14 +142,16 @@ add_rows_owner_kernel(T* __restrict__ shard, T* __restrict__ st0, T* __restrict_
   const int64_t woff = U::kPerWorker ? (int64_t)opt.worker_id * state_stride : 0;
   for (int64_t i = warp; i < k; i += nwarps) {
     const int64_t r = ids[i];
+    if (i > 0 && ids[i - 1] == r) continue;  // inside a run: applied by the run's first warp
     if (r < row_lo || r >= row_hi) continue;
+    int64_t end = i + 1;
+    while (end < k && ids[end] == r) ++end;
     const int64_t base = (r - row_lo) * num_col;
-    const T* src = vals + i * vals_ld;
     for (int64_t c = lane; c < num_col; c += 32) {
       T d = shard[base + c], s0 = (T)0, s1 = (T)0;
       if constexpr (U::kStates >= 1) s0 = st0[woff + base + c];
       if constexpr (U::kStates >= 2) s1 = st1[woff + base + c];
-      U::Apply(d, src[c], s0, s1, opt);
+      for (int64_t j = i; j < end; ++j) U::Apply(d, vals[j * vals_ld + c], s0, s1, opt);
       if constexpr (U::kStates >= 1) st0[woff + base + c] = s0;
       if constexpr (U::kStates >= 2) st1[woff + base + c] = s1;
       shard[base + c] = d;

@@ -77,6 +77,9 @@ class DenseDeviceTable(_AsyncOps):
         self.num_row, self.num_col = int(num_row), int(num_col)
         self.size = self.num_row * self.num_col
         self.dtype = _torch_dtype(dtype)
+        if self.dtype not in (torch.float32, torch.float64, torch.int32):
+            # the dense, push and row kernels serve these three (as the host backend and the reference do)
+            Log.fatal("device tables support float32/float64/int32, got %s", dtype)
         self.dcode = N.dtype_code(self.dtype)
         self.esz = torch.empty((), dtype=self.dtype).element_size()
         name = updater or str(FLAGS.get("updater_type"))
@@ -683,6 +686,12 @@ class MatrixDeviceTable(DenseDeviceTable):
             self._keep_push = (ids32,)
             self._mailbox.drain(wait=False)
             return
+        # a repeated row is applied once per occurrence, in list order (MatrixServerTable::ProcessAdd): the
+        # owner kernel walks each run of equal ids on one warp, so make the runs adjacent without reordering
+        # them (stable sort); staged requests are sorted too, so every owner sees the same order
+        ids, order = torch.sort(ids, stable=True)
+        vals = vals[order]
+        self._keep_sorted = (ids, vals)
         st = N.stream_ptr()
         ao = _opt_struct(opt)
         if rt.size == 1:
