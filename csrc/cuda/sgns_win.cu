@@ -596,7 +596,7 @@ sgns_win_kernel(const __grid_constant__ WinDev a) {
 }
 
 // ---- deterministic K7 (DESIGN.md §11): the maths above in waves of its in-flight count; reads see the tables as
-// the last wave left them, deltas / loss are summed in 64-bit fixed point, then applied.  Warp per centre.
+// the last wave left them, deltas / loss are summed in 64-bit fixed point, then applied.
 constexpr float kFixScale = 0x1p40f;              // 2^-40 resolution, +-2^23 range
 constexpr float kLossScale = 0x1p32f;
 
@@ -633,16 +633,6 @@ MVB_DEVINL void det_touch(const DetDev& a, int t, int r) {
   if (atomicExch(a.flag[t] + r, 1) == 0) a.list[t][atomicAdd(a.count + t, 1)] = r;
 }
 template <int NJ>
-MVB_DEVINL void det_add(const DetDev& a, int t, int r, const float (&v)[NJ], int lane) {
-  unsigned long long* dst = a.acc[t] + (int64_t)r * a.dim;
-#pragma unroll
-  for (int u = 0; u < NJ; ++u) {
-    const int j = lane + 32 * u;
-    if (j < a.dim) atomicAdd(dst + j, (unsigned long long)__float2ll_rn(v[u] * kFixScale));
-  }
-  if (lane == 0) det_touch(a, t, r);
-}
-template <int NJ>
 MVB_DEVINL void det_load(float (&v)[NJ], const float* row, int dim, int lane, bool on) {
 #pragma unroll
   for (int u = 0; u < NJ; ++u) v[u] = (on && lane + 32 * u < dim) ? row[lane + 32 * u] : 0.f;
@@ -657,139 +647,249 @@ MVB_DEVINL float det_dot(const float (&x)[NJ], const float (&y)[NJ]) {
   return s;
 }
 
+// Centres per CTA (one warp each) that the registers of a <NJ, KO> warp allow: its output rows stay in
+// registers, KO * NJ of them (60 at dim 300 with 5 negatives), so wide rows get fewer, fatter warps per SM.
+__host__ __device__ constexpr int det_max_s(int nj, int ko) { return nj * ko <= 64 ? 20 : nj * ko <= 96 ? 12 : 8; }
+
+// Shared memory of a CTA of S centres: per staged position (S + 2W of them) an int64 accumulator row, the input
+// row and its id / scale / "is a context" word; per (centre, output row) its id and scale; per (centre, offset,
+// output row) the pair's error term.
+__host__ __device__ inline size_t det_smem_bytes(int S, int W, int dim, int ko) {
+  return (size_t)(S + 2 * W) * ((size_t)dim * 12 + 12) + (size_t)S * ko * 8 + (size_t)S * (2 * W + 1) * ko * 4;
+}
+
+// One CTA owns S consecutive centres [s0, s0 + S) of the wave, one warp per centre.  All S samplings are done
+// up front, one thread per (centre, output row) and per staged position; the input rows of the positions
+// [s0 - W, s0 + S + W) are staged once in shared memory, and each position's input delta is summed there over
+// all its centres before one row of REDs sends it to the wave's accumulator.  The float arithmetic of every
+// (centre, context) pair does not depend on the tiling (element j on lane j % 32, register j / 32, fixed FMA
+// chains and butterflies, one conversion to fixed point per pair and per (centre, k)); only the grouping of the
+// exact int64 sums does, so the result is bitwise independent of S.
 template <int NJ, int KO>
-__global__ void __launch_bounds__(256)
+__global__ void __launch_bounds__(32 * det_max_s(NJ, KO))
 sgns_det_kernel(const __grid_constant__ DetDev a) {
-  const int lane = threadIdx.x & 31;
-  const int64_t warp0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
-  const int W = a.window;
+  extern __shared__ __align__(16) unsigned char smem[];
+  const int S = blockDim.x >> 5, W = a.window, dim = a.dim;
+  const int c = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int64_t s0 = a.p0 + (int64_t)blockIdx.x * S;
+  const int ns = (int)(a.p1 - s0 < S ? a.p1 - s0 : S);   // centres of this slice
+  const int np = ns + 2 * W;                               // staged positions: i <-> token s0 - W + i
+  unsigned long long* hacc = reinterpret_cast<unsigned long long*>(smem);
+  float* hrow = reinterpret_cast<float*>(hacc + (size_t)(S + 2 * W) * dim);
+  int* crid = reinterpret_cast<int*>(hrow + (size_t)(S + 2 * W) * dim);
+  float* csc = reinterpret_cast<float*>(crid + S + 2 * W);
+  int* need = reinterpret_cast<int*>(csc + S + 2 * W);
+  int* orid = need + S + 2 * W;
+  float* osc = reinterpret_cast<float*>(orid + S * KO);
+  float* gsm = osc + S * KO;
+
+  // ---- sampling of the whole slice: one thread per staged position, one per (centre, output row) ----------
   const int pool_n = a.neg_pool_size_ptr ? __ldg(a.neg_pool_size_ptr) : a.neg_pool_size;
-  float loss = 0.f;
-  unsigned long long pairs = 0ull;
-  for (int64_t p = a.p0 + warp0; p < a.p1; p += nwarps) {
-    const int tp = __ldg(a.tokens + p);
-    if (tp < 0) continue;
-    // centre + negatives (lane k < ko holds output row k), exactly as the window kernel samples them
-    const uint64_t prng = hash64(a.seed ^ (uint64_t)(p + 1) * 0x9E3779B97F4A7C15ull);
+  for (int t = threadIdx.x; t < np + ns * KO; t += blockDim.x) {
     int rid = -1;
-    float osc = 1.f;
-    if (lane == 0) {
-      rid = a.map_out ? __ldg(a.map_out + tp) : tp;
-      if (a.scale_out) osc = __ldg(a.scale_out + tp);
-    } else if (lane < a.ko) {
-      const uint64_t r = hash64(prng ^ ((uint64_t)lane * 0xD6E8FEB86659FD93ull));
-      int t;
-      if (a.neg_pool) {
-        t = pool_n > 0 ? __ldg(a.neg_pool + (r >> 8) % (uint64_t)pool_n) : -1;
-      } else {
-        const uint32_t idx = (uint32_t)((r >> 32) % (uint64_t)a.vocab);
-        const float u = (float)(r & 0xFFFFFF) * (1.0f / 16777216.0f);
-        t = (u < __ldg(a.alias_prob + idx)) ? (int)idx : __ldg(a.alias_idx + idx);
-      }
-      if (t == tp) t = -1;                         // Parse(): target == word_idx is skipped
-      if (t >= 0) {
-        rid = a.map_out ? __ldg(a.map_out + t) : t;
-        if (a.scale_out) osc = __ldg(a.scale_out + t);
-      }
-    }
-    if (__shfl_sync(0xffffffffu, rid, 0) < 0) continue;
-    const uint32_t used = __ballot_sync(0xffffffffu, rid >= 0) & ((1u << a.ko) - 1u);
-    // window (ParseSentence): lane l <-> offset d = l - hw; contexts stop at the first break on either side
-    const int hw = W - (int)((prng >> 16) % (uint64_t)W);
-    int crid = -1;
-    float csc = 1.f;
-    if (lane <= 2 * hw && lane != hw) {
-      const int64_t q = p + (lane - hw);
+    float sc = 1.f;
+    if (t < np) {
+      const int64_t q = s0 - W + t;
       if (q >= 0 && q < a.n_tokens) {
         const int tq = __ldg(a.tokens + q);
         if (tq >= 0) {
-          crid = a.map_in ? __ldg(a.map_in + tq) : tq;
-          if (a.scale_in) csc = __ldg(a.scale_in + tq);
+          rid = a.map_in ? __ldg(a.map_in + tq) : tq;
+          if (a.scale_in) sc = __ldg(a.scale_in + tq);
         }
       }
+      crid[t] = rid;
+      csc[t] = sc;
+      need[t] = 0;
+    } else {
+      const int ck = t - np, k = ck % KO;
+      const int64_t p = s0 + ck / KO;
+      const int tp = __ldg(a.tokens + p);
+      if (tp >= 0 && k == 0) {
+        rid = a.map_out ? __ldg(a.map_out + tp) : tp;
+        if (a.scale_out) sc = __ldg(a.scale_out + tp);
+      } else if (tp >= 0 && k < a.ko) {
+        const uint64_t prng = hash64(a.seed ^ (uint64_t)(p + 1) * 0x9E3779B97F4A7C15ull);
+        const uint64_t r = hash64(prng ^ ((uint64_t)k * 0xD6E8FEB86659FD93ull));
+        int tk;
+        if (a.neg_pool) {
+          tk = pool_n > 0 ? __ldg(a.neg_pool + (r >> 8) % (uint64_t)pool_n) : -1;
+        } else {
+          const uint32_t idx = (uint32_t)((r >> 32) % (uint64_t)a.vocab);
+          const float u = (float)(r & 0xFFFFFF) * (1.0f / 16777216.0f);
+          tk = (u < __ldg(a.alias_prob + idx)) ? (int)idx : __ldg(a.alias_idx + idx);
+        }
+        if (tk == tp) tk = -1;                       // Parse(): target == word_idx is skipped
+        if (tk >= 0) {
+          rid = a.map_out ? __ldg(a.map_out + tk) : tk;
+          if (a.scale_out) sc = __ldg(a.scale_out + tk);
+        }
+      }
+      orid[ck] = rid;
+      osc[ck] = sc;
     }
-    const uint32_t isnull = __ballot_sync(0xffffffffu, lane <= 2 * hw && lane != hw && crid < 0);
+  }
+  for (int e = threadIdx.x; e < np * dim; e += blockDim.x) hacc[e] = 0ull;
+  __syncthreads();
+
+  // ---- this warp's centre: window (ParseSentence), lane l <-> offset l - hw, staged position c + W + l - hw ----
+  const int64_t p = s0 + c;
+  const bool on = c < ns && orid[c * KO] >= 0;        // a break or an unmapped centre trains nothing
+  const int rid = on && lane < KO ? orid[c * KO + lane] : -1;
+  const uint32_t used = __ballot_sync(0xffffffffu, rid >= 0);
+  const int hw = W - (int)((hash64(a.seed ^ (uint64_t)(p + 1) * 0x9E3779B97F4A7C15ull) >> 16) % (uint64_t)W);
+  uint32_t ctx = 0;
+  if (on) {
+    const uint32_t isnull =
+        __ballot_sync(0xffffffffu, lane <= 2 * hw && lane != hw && crid[c + W + lane - hw] < 0);
     const uint32_t left_null = isnull & ((1u << hw) - 1u);
     const int lo = left_null ? (32 - __clz(left_null)) : 0;
     const uint32_t right_null = isnull >> (hw + 1);
     const int hi = right_null ? (hw + __ffs(right_null) - 1) : 2 * hw;
-    const uint32_t ctx = (((hi >= 31) ? 0xffffffffu : ((1u << (hi + 1)) - 1u)) & ~((1u << lo) - 1u)) & ~(1u << hw);
-    if (!ctx) continue;
-    float O[KO][NJ];
+    ctx = (((hi >= 31) ? 0xffffffffu : ((1u << (hi + 1)) - 1u)) & ~((1u << lo) - 1u)) & ~(1u << hw);
+  }
+  if ((ctx >> lane) & 1u) need[c + W + lane - hw] = 1;   // every writer stores the same value
+  if (ctx && ((used >> lane) & 1u)) det_touch(a, 1, rid);
+  float O[KO][NJ];
 #pragma unroll
-    for (int k = 0; k < KO; ++k) {
-      const int r = __shfl_sync(0xffffffffu, rid, k);
-      det_load(O[k], a.w_out + (int64_t)(r < 0 ? 0 : r) * a.ld, a.dim, lane, (used >> k) & 1u);
-    }
-    // phase 1: per context 1+K dots on the rows as the wave found them, input-row delta
-    float gs[KO];                                  // lane t keeps the error terms of context t
+  for (int k = 0; k < KO; ++k) {
+    const int r = __shfl_sync(0xffffffffu, rid, k);
+    det_load(O[k], a.w_out + (int64_t)(r < 0 ? 0 : r) * a.ld, dim, lane, ctx && ((used >> k) & 1u));
+  }
+  __syncthreads();
+
+  // ---- stage the input rows that are a context of some centre of the slice ----------------------------------
+  for (int i = c; i < np; i += S) {
+    if (!need[i]) continue;
+    float h[NJ];
+    det_load(h, a.w_in + (int64_t)crid[i] * a.ld, dim, lane, true);
 #pragma unroll
-    for (int k = 0; k < KO; ++k) gs[k] = 0.f;
-    const bool want_loss = a.want_loss && (p & 7) == 0;
-    for (uint32_t m = ctx; m; m &= m - 1) {
-      const int t = __ffs(m) - 1;
-      const int r = __shfl_sync(0xffffffffu, crid, t);
-      const float isc = __shfl_sync(0xffffffffu, csc, t);
-      float h[NJ], e[NJ] = {};
-      det_load(h, a.w_in + (int64_t)r * a.ld, a.dim, lane, true);
+    for (int u = 0; u < NJ; ++u)
+      if (lane + 32 * u < dim) hrow[(size_t)i * dim + lane + 32 * u] = h[u];
+  }
+  __syncthreads();
+
+  // ---- phase 1 in offset rounds: 1+K dots per (centre, context) on the rows as the wave found them; the
+  // pair's input delta goes to position p + d's accumulator row.  Within a round the centres of the slice hit
+  // distinct positions, so a plain read-add-write is exact; rounds are ordered by the barrier.
+  float* gs = gsm + (size_t)c * (2 * W + 1) * KO;    // [offset + hw][k]: error terms of this centre's pairs
+  const bool want_loss = a.want_loss && (p & 7) == 0;
+  float loss = 0.f;
+  int pairs = 0;
+  for (int d = -W; d <= W; ++d) {
+    const int t = hw + d;
+    if (d != 0 && t >= 0 && ((ctx >> t) & 1u)) {
+      const int i = c + W + d;
+      const float isc = csc[i];
+      {
+        float h[NJ];
+        det_load(h, hrow + (size_t)i * dim, dim, lane, true);
+#pragma unroll
+        for (int k = 0; k < KO; ++k) {
+          float g = 0.f;
+          if ((used >> k) & 1u) {
+            const float f = det_dot(h, O[k]);
+            g = ((k == 0 ? 1.f : 0.f) - sigm_fast(f)) * a.lr;
+            if (want_loss && lane == 0) loss += 8.f * softplus_neg(k == 0 ? f : -f);
+          }
+          if (lane == k) gs[t * KO + k] = g;              // every lane holds the same butterfly sums
+        }
+      }
+      __syncwarp();
+      // h is dead before e is live: the registers hold the output rows plus one row
+      float e[NJ] = {};
 #pragma unroll
       for (int k = 0; k < KO; ++k) {
         if (!((used >> k) & 1u)) continue;
-        const float f = det_dot(h, O[k]);
-        const float g = ((k == 0 ? 1.f : 0.f) - sigm_fast(f)) * a.lr;
-        if (want_loss && lane == 0) loss += 8.f * softplus_neg(k == 0 ? f : -f);
-        if (lane == t) gs[k] = g;
+        const float g = gs[t * KO + k];
 #pragma unroll
         for (int u = 0; u < NJ; ++u) e[u] = __fmaf_rn(g * isc, O[k][u], e[u]);
       }
-      det_add(a, 0, r, e, lane);
+      unsigned long long* dst = hacc + (size_t)i * dim;
+#pragma unroll
+      for (int u = 0; u < NJ; ++u)
+        if (lane + 32 * u < dim) dst[lane + 32 * u] += (unsigned long long)__float2ll_rn(e[u] * kFixScale);
       ++pairs;
     }
-    // phase 2: output-row deltas sum_c g_ck * in_c
+    if (d != 0) __syncthreads();
+  }
+
+  // ---- flush: one row of REDs per staged position that is a context (halo rows carry partial sums) ---------
+  for (int i = c; i < np; i += S) {
+    if (!need[i]) continue;
+    const int r = crid[i];
+    unsigned long long* dst = a.acc[0] + (int64_t)r * dim;
+    for (int j = lane; j < dim; j += 32) {
+      const unsigned long long v = hacc[(size_t)i * dim + j];
+      if (v) atomicAdd(dst + j, v);
+    }
+    if (lane == 0) det_touch(a, 0, r);
+  }
+
+  // ---- phase 2: output-row deltas sum_c g_ck * in_c in registers, one row of REDs per (centre, k) -----------
+  if (ctx) {
 #pragma unroll
     for (int k = 0; k < KO; ++k)
 #pragma unroll
       for (int u = 0; u < NJ; ++u) O[k][u] = 0.f;
     for (uint32_t m = ctx; m; m &= m - 1) {
       const int t = __ffs(m) - 1;
-      const int r = __shfl_sync(0xffffffffu, crid, t);
       float h[NJ];
-      det_load(h, a.w_in + (int64_t)r * a.ld, a.dim, lane, true);
+      det_load(h, hrow + (size_t)(c + W + t - hw) * dim, dim, lane, true);
 #pragma unroll
       for (int k = 0; k < KO; ++k) {
-        const float gk = __shfl_sync(0xffffffffu, gs[k], t) * __shfl_sync(0xffffffffu, osc, k);
+        const float gk = gs[t * KO + k] * osc[c * KO + k];
 #pragma unroll
         for (int u = 0; u < NJ; ++u) O[k][u] = __fmaf_rn(gk, h[u], O[k][u]);
       }
     }
 #pragma unroll
-    for (int k = 0; k < KO; ++k)
-      if ((used >> k) & 1u) det_add(a, 1, __shfl_sync(0xffffffffu, rid, k), O[k], lane);
+    for (int k = 0; k < KO; ++k) {
+      if (!((used >> k) & 1u)) continue;
+      unsigned long long* dst = a.acc[1] + (int64_t)orid[c * KO + k] * dim;
+#pragma unroll
+      for (int u = 0; u < NJ; ++u)
+        if (lane + 32 * u < dim) atomicAdd(dst + lane + 32 * u, (unsigned long long)__float2ll_rn(O[k][u] * kFixScale));
+    }
   }
   if (lane == 0) {
     if (a.want_loss && loss != 0.f) atomicAdd(a.loss_acc, (unsigned long long)__float2ll_rn(loss * kLossScale));
-    if (a.pair_count && pairs) atomicAdd(a.pair_count, pairs);
+    if (a.pair_count && pairs) atomicAdd(a.pair_count, (unsigned long long)pairs);
   }
 }
 
-// adds each touched row's sum to its table, clears the wave; resets the NEXT wave's (idle) counters
-template <typename I>                              // element index: int below 2^31 elements
-__global__ void sgns_det_apply(float* w_in, float* w_out, int dim, int64_t ld, unsigned long long* acc_in,
-                               unsigned long long* acc_out, int* flag_in, int* flag_out, const int* list_in,
-                               const int* list_out, const int* count, int* next, unsigned long long* loss_acc,
-                               float* loss_sum) {
-  const I n_in = (I)count[0] * dim, n_all = n_in + (I)count[1] * dim;
-  for (I i = (I)blockIdx.x * blockDim.x + threadIdx.x; i < n_all; i += (I)gridDim.x * blockDim.x) {
-    const bool in = i < n_in;
-    const I k = in ? i : i - n_in;
-    const int r = (in ? list_in : list_out)[k / dim];
-    const int j = (int)(k - (k / dim) * dim);
-    unsigned long long* q = (in ? acc_in : acc_out) + (int64_t)r * dim + j;
-    const long long v = (long long)*q;
-    if (v) (in ? w_in : w_out)[(int64_t)r * ld + j] += (float)((double)v * (1.0 / (double)kFixScale));
-    *q = 0ull;
-    if (j == 0) (in ? flag_in : flag_out)[r] = 0;
+// Adds each touched row's sum to its table and clears it, a warp per listed row (input rows, then output rows);
+// resets the NEXT wave's (idle) counters and rolls the wave's loss into loss_sum.
+__global__ void __launch_bounds__(256)
+sgns_det_apply(float* __restrict__ w_in, float* __restrict__ w_out, int dim, int64_t ld,
+               unsigned long long* __restrict__ acc_in, unsigned long long* __restrict__ acc_out, int* flag_in,
+               int* flag_out, const int* list_in, const int* list_out, const int* count, int* next,
+               unsigned long long* loss_acc, float* loss_sum) {
+  const int lane = threadIdx.x & 31;
+  const int n_in = count[0], n_all = n_in + count[1];
+  const int nwarps = (gridDim.x * blockDim.x) >> 5;
+  for (int w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; w < n_all; w += nwarps) {
+    const bool in = w < n_in;
+    const int r = in ? list_in[w] : list_out[w - n_in];
+    unsigned long long* q = (in ? acc_in : acc_out) + (int64_t)r * dim;
+    float* row = (in ? w_in : w_out) + (int64_t)r * ld;
+    for (int j0 = 0; j0 < dim; j0 += 128) {          // 4 elements per lane in flight
+      long long v[4];
+      float x[4];
+#pragma unroll
+      for (int u = 0; u < 4; ++u) {
+        const int j = j0 + lane + 32 * u;
+        v[u] = j < dim ? (long long)q[j] : 0;
+        x[u] = j < dim ? row[j] : 0.f;
+      }
+#pragma unroll
+      for (int u = 0; u < 4; ++u) {
+        const int j = j0 + lane + 32 * u;
+        if (j >= dim) continue;
+        if (v[u]) row[j] = x[u] + (float)((double)v[u] * (1.0 / (double)kFixScale));
+        q[j] = 0ull;
+      }
+    }
+    if (lane == 0) (in ? flag_in : flag_out)[r] = 0;
   }
   if (blockIdx.x == 0 && threadIdx.x == 0) {
     next[0] = next[1] = 0;
@@ -904,7 +1004,8 @@ extern "C" int mvb_sgns_train_win(const MvbSgns* h, void* stream) {
 }
 
 extern int mvb_sgns_launches;
-// Deterministic K7 on local tables or block caches; -20/-21: not covered (the caller falls back).
+// Deterministic K7 on local tables or block caches; -20/-21: not covered (the caller falls back); -22: one centre's
+// slice does not fit the shared memory (not reached on an H100 for dim <= 512, window <= 15).
 extern "C" int mvb_sgns_train_det(const MvbSgns* h, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   if (h->n_tokens <= 0) return 0;
@@ -946,29 +1047,39 @@ extern "C" int mvb_sgns_train_det(const MvbSgns* h, void* stream) {
   a.loss_acc = loss_acc;
   int wave = mvb_sgns_win_inflight(h->dim, h->negative, h->window, h->max_ctas);
   if (wave <= 0) wave = 2 * mvb_num_sms() * kNW;
-  const int det_blocks = (wave + 7) / 8;           // a warp per centre
+  // the <NJ, KO> instance, and as many centres per CTA as its registers and the opt-in shared memory allow
+  void (*kern)(DetDev) = nullptr;
+  int S = 0;
+  const int ko = a.ko <= 6 ? 6 : 8;
+#define MVB_DET_KERNEL(NJ)                                              \
+  case NJ:                                                              \
+    kern = ko == 6 ? sgns_det_kernel<NJ, 6> : sgns_det_kernel<NJ, 8>;   \
+    S = det_max_s(NJ, ko);                                              \
+    break;
+  switch ((h->dim + 31) / 32) {
+    MVB_DET_KERNEL(1) MVB_DET_KERNEL(2) MVB_DET_KERNEL(3) MVB_DET_KERNEL(4)
+    MVB_DET_KERNEL(5) MVB_DET_KERNEL(6) MVB_DET_KERNEL(7) MVB_DET_KERNEL(8)
+    MVB_DET_KERNEL(9) MVB_DET_KERNEL(10) MVB_DET_KERNEL(11) MVB_DET_KERNEL(12)
+    MVB_DET_KERNEL(13) MVB_DET_KERNEL(14) MVB_DET_KERNEL(15) MVB_DET_KERNEL(16)
+    default: return -21;
+  }
+#undef MVB_DET_KERNEL
+  int dev = 0, max_smem = 0;
+  MVB_CUDA_CHECK(cudaGetDevice(&dev));
+  MVB_CUDA_CHECK(cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+  while (S > 1 && det_smem_bytes(S, h->window, h->dim, ko) > (size_t)max_smem) --S;
+  const size_t smem = det_smem_bytes(S, h->window, h->dim, ko);
+  if (smem > (size_t)max_smem) return -22;
+  MVB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const int apply_blocks = mvb_num_sms() * 4;
-  const int nj = (h->dim + 31) / 32;
   for (int64_t p0 = 0; p0 < h->n_tokens; p0 += wave) {
     a.p0 = p0;
     a.p1 = p0 + wave < h->n_tokens ? p0 + wave : h->n_tokens;
     a.count = counters + 2 * parity;
-#define MVB_LAUNCH_DET(NJ)                                                              \
-  case NJ:                                                                              \
-    if (a.ko <= 6) sgns_det_kernel<NJ, 6><<<det_blocks, 256, 0, st>>>(a);               \
-    else sgns_det_kernel<NJ, 8><<<det_blocks, 256, 0, st>>>(a);                         \
-    break;
-    switch (nj) {
-      MVB_LAUNCH_DET(1) MVB_LAUNCH_DET(2) MVB_LAUNCH_DET(3) MVB_LAUNCH_DET(4)
-      MVB_LAUNCH_DET(5) MVB_LAUNCH_DET(6) MVB_LAUNCH_DET(7) MVB_LAUNCH_DET(8)
-      MVB_LAUNCH_DET(9) MVB_LAUNCH_DET(10) MVB_LAUNCH_DET(11) MVB_LAUNCH_DET(12)
-      MVB_LAUNCH_DET(13) MVB_LAUNCH_DET(14) MVB_LAUNCH_DET(15) MVB_LAUNCH_DET(16)
-      default: return -21;
-    }
-#undef MVB_LAUNCH_DET
-    (elems < (1ll << 31) ? sgns_det_apply<int> : sgns_det_apply<int64_t>)<<<apply_blocks, 256, 0, st>>>(h->w_in, h->w_out, h->dim, h->ld, a.acc[0], a.acc[1], a.flag[0],
-                                                  a.flag[1], a.list[0], a.list[1], a.count,
-                                                  counters + 2 * (parity ^ 1), loss_acc, h->loss_sum);
+    kern<<<(int)((a.p1 - p0 + S - 1) / S), 32 * S, smem, st>>>(a);
+    sgns_det_apply<<<apply_blocks, 256, 0, st>>>(h->w_in, h->w_out, h->dim, h->ld, a.acc[0], a.acc[1], a.flag[0],
+                                                 a.flag[1], a.list[0], a.list[1], a.count,
+                                                 counters + 2 * (parity ^ 1), loss_acc, h->loss_sum);
     parity ^= 1;
     mvb_sgns_launches += 2;
   }
