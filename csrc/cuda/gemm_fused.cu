@@ -134,7 +134,9 @@ get_gemm_fused_kernel(const __grid_constant__ CUtensorMap map_x,
       // column 8j + 2 (lane % 4) + c
       const int64_t m_row = (int64_t)mt * BM + cw * 64 + warp * 16 + (lane >> 2);
       const int n_col = 2 * (lane & 3);
-      const bool pairs = ((g.ldy | t.n_global) & 1) == 0;    // float2 stores are 8-byte aligned
+      // float2 stores need an 8-byte aligned address: y itself (a caller's `out` may start one float off), the row
+      // pitch and the tile's first column all even in floats
+      const bool pairs = (((reinterpret_cast<uintptr_t>(g.y) >> 2) | g.ldy | t.n_global) & 1) == 0;
       float* yt = g.y + t.n_global;
 #pragma unroll
       for (int h = 0; h < 2; ++h) {

@@ -21,8 +21,18 @@ def get_gemm_supported() -> bool:
     return bool(N.cuda_lib().mvb_get_gemm_supported())
 
 
+def _check_out(what: str, out: torch.Tensor, M: int, Nrows: int, device: torch.device) -> None:
+    """The kernel writes M x Nrows floats at row pitch Nrows from out's first element: anything else in `out`
+    would be written out of bounds or into the wrong elements."""
+    if (out.dtype != torch.float32 or out.device != device or tuple(out.shape) != (M, Nrows)
+            or not out.is_contiguous()):
+        raise ValueError(f"{what}: out must be a contiguous float32 [{M}, {Nrows}] tensor on {device}, got "
+                         f"{out.dtype} {tuple(out.shape)} stride {out.stride()} on {out.device}")
+
+
 def get_gemm(table, x: torch.Tensor, out: torch.Tensor = None) -> torch.Tensor:
-    """``x``: [M, K] fp32 CUDA, ``table``: MatrixDeviceTable with num_col == K. Returns [M, num_row].
+    """``x``: [M, K] fp32 CUDA, ``table``: MatrixDeviceTable with num_col == K. Returns [M, num_row], written
+    into ``out`` when given (a contiguous fp32 [M, num_row] tensor on x's device, else ValueError).
     On the host backend (no GPU) the same call is a plain Get followed by a matmul."""
     from ..runtime import Runtime
     if Runtime.get().backend == "host":
@@ -40,6 +50,7 @@ def get_gemm(table, x: torch.Tensor, out: torch.Tensor = None) -> torch.Tensor:
     Nrows = table.num_row
     if out is None:
         out = torch.empty(M, Nrows, dtype=torch.float32, device=x.device)
+    _check_out("get_gemm", out, M, Nrows, x.device)
     g = N.GetGemm()
     g.x, g.y, g.w_cache = x.data_ptr(), out.data_ptr(), None
     g.M, g.N, g.K = M, Nrows, K
@@ -57,8 +68,16 @@ def gemm_nt(x: torch.Tensor, w: torch.Tensor, out: torch.Tensor) -> torch.Tensor
     """out[M, N] = x[M, K] @ w[N, K]^T on the hand-written wgmma kernel (gemm_fused.cu: TMA-fed
     wgmma, TF32 operands, fp32 accumulation in registers) -- `w` is presented as a one-server
     row map, so the same kernel that streams table shards multiplies two local matrices.  K % 4 == 0."""
+    for name, t in (("x", x), ("w", w)):
+        if not (t.is_cuda and t.dtype == torch.float32 and t.dim() == 2 and t.is_contiguous()):
+            raise ValueError(f"gemm_nt: {name} must be a contiguous 2-D float32 CUDA tensor")
     M, K = x.shape
     Nr = w.shape[0]
+    if w.shape[1] != K or w.device != x.device:
+        raise ValueError(f"gemm_nt: w {tuple(w.shape)} on {w.device} does not match x {tuple(x.shape)} on {x.device}")
+    if K % 4 != 0:
+        raise ValueError("gemm_nt needs K % 4 == 0 (16-byte row pitch for TMA)")
+    _check_out("gemm_nt", out, M, Nr, x.device)
     g = N.GetGemm()
     g.x, g.y, g.w_cache = x.data_ptr(), out.data_ptr(), None
     g.M, g.N, g.K = M, Nr, K
