@@ -14,7 +14,8 @@
 // the window and flushed once.
 //
 //   sgns_fast_kernel    : skip-gram + negative sampling, plain SGD, D % 4 == 0, D <= 512
-//   w2v_generic_kernel  : CBOW / hierarchical softmax / AdaGrad / any D (smem staged)
+//   w2v_generic_kernel  : CBOW / hierarchical softmax / AdaGrad / any D (smem staged); AdaGrad accumulates
+//                         G^2 with atomicAdd and steps with red.add, as neighbouring centres share rows
 #include <cmath>
 #include <vector>
 #include "mvb_common.cuh"
@@ -314,14 +315,14 @@ __global__ void __launch_bounds__(128) w2v_generic_kernel(const __grid_constant_
           loss_acc += softplus_neg(pos ? f : -f);
         }
         if (a.use_adagrad) {
+          // other warps update the same rows and G^2 sums: accumulate both atomically, and step
+          // with the G this sample's own increment produced
           float* g2 = a.g2_out + (int64_t)oid * a.ld;
           for (int c = lane; c < D; c += 32) {
-            float w = wrow[c];
-            herr[c] += err * w;
+            herr[c] += err * wrow[c];
             float g = err * hid[c];
-            float s = g2[c] + g * g;
-            g2[c] = s;
-            if (s > 1e-10f) wrow[c] = w + g * a.lr * rsqrtf(s);
+            float s = atomicAdd(g2 + c, g * g) + g * g;
+            if (s > 1e-10f) red_add_f32(wrow + c, g * a.lr * rsqrtf(s));
           }
         } else {
           float g = err * a.lr;
@@ -345,9 +346,8 @@ __global__ void __launch_bounds__(128) w2v_generic_kernel(const __grid_constant_
               float* g2 = a.g2_in + (int64_t)rid * a.ld;
               for (int c = lane; c < D; c += 32) {
                 float e = herr[c];
-                float s = g2[c] + e * e;
-                g2[c] = s;
-                if (s > 1e-10f) row[c] += e * a.lr * rsqrtf(s);
+                float s = atomicAdd(g2 + c, e * e) + e * e;
+                if (s > 1e-10f) red_add_f32(row + c, e * a.lr * rsqrtf(s));
               }
             } else {
               for (int c = lane; c < D; c += 32) red_add_f32(row + c, herr[c] * a.lr);
@@ -390,8 +390,10 @@ extern "C" int mvb_sgns_last_launches(void) { return mvb_sgns_launches; }
 
 // One kernel per input:
 //   nservers > 1 (direct mode)           the window kernel, or its error code (only it addresses peer shards)
-//   skip-gram + NS, register-row shapes  the deterministic waves (hogwild = 0) or the window kernel
-//                                        (hogwild = 1) where it covers the input, else the register kernel
+//   skip-gram + NS, hogwild = 0          the deterministic waves where they cover the input (any dim <= 512,
+//                                        any ld and alignment)
+//   skip-gram + NS, register-row shapes  otherwise the window kernel (hogwild = 1) where it covers the input,
+//                                        else the register kernel
 //   anything else                        the generic kernel
 extern "C" int mvb_sgns_train(const MvbSgns* h, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
@@ -400,16 +402,25 @@ extern "C" int mvb_sgns_train(const MvbSgns* h, void* stream) {
   if (h->window < 1) return -5;
   if (!h->hs && h->negative > 0 && !h->neg_pool && !(h->alias_prob && h->alias_idx)) return -6;
   if (h->nservers > 1) return mvb_sgns_train_win(h, stream);
+  // -20 / -21 / -22 from the deterministic or window kernel: it does not cover this input (K >= 8; vocab <= 0
+  // for the deterministic one)
+  const auto declined = [](int rc) { return rc == -20 || rc == -21 || rc == -22; };
+  const bool sg_ns = !h->cbow && !h->hs && !h->use_adagrad && h->negative > 0;
+  if (sg_ns && !h->hogwild) {
+    const int rc = mvb_sgns_train_det(h, stream);
+    if (!declined(rc)) return rc;
+    mvb_sgns_launches = 1;
+  }
   SgnsDev d = to_dev(h);
-  const bool fast = !h->cbow && !h->hs && !h->use_adagrad && h->negative > 0 && (h->dim % 4 == 0) &&
-                    (h->ld % 4 == 0) && h->dim <= 512 && h->window <= 15 &&
+  const bool fast = sg_ns && (h->dim % 4 == 0) && (h->ld % 4 == 0) && h->dim <= 512 && h->window <= 15 &&
                     ((reinterpret_cast<uintptr_t>(h->w_in) & 15) == 0) &&
                     ((reinterpret_cast<uintptr_t>(h->w_out) & 15) == 0);
   const int sms = mvb_num_sms();
   if (fast) {
-    // -20 / -21 / -22: the kernel does not cover this input (K >= 8; vocab <= 0 for the deterministic one)
-    const int rc = h->hogwild ? mvb_sgns_train_win(h, stream) : mvb_sgns_train_det(h, stream);
-    if (rc != -20 && rc != -21 && rc != -22) return rc;
+    if (h->hogwild) {
+      const int rc = mvb_sgns_train_win(h, stream);
+      if (!declined(rc)) return rc;
+    }
     const int nvec = h->dim / 4;
     const int vpl = (nvec + 31) / 32;
     // persistent-style grid: 4 CTAs of 4 warps per SM, warps stride over positions

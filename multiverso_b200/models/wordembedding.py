@@ -72,11 +72,25 @@ class HuffmanTables:
     native encoder (csrc/host/applib/wordembedding_data.cpp)."""
 
     MAX_CODE = 64
+    FREQ_TOTAL_MAX = 1 << 62     # the encoder sums frequencies in int64: the root's weight is their total
+
+    @classmethod
+    def int_frequencies(cls, counts: np.ndarray) -> np.ndarray:
+        """Integer encoder frequencies for `counts`: the counts themselves when they are whole numbers,
+        fractional weights (the default Zipf 1/rank) scaled by 1e9; scaled down further while the
+        total would overflow the encoder's int64 sums.  Every word gets at least 1."""
+        c = np.asarray(counts, dtype=np.float64)
+        if not np.all(c == np.floor(c)):
+            c = c * 1e9
+        total = float(np.maximum(c, 1.0).sum())
+        if total >= cls.FREQ_TOTAL_MAX:
+            c = c * (cls.FREQ_TOTAL_MAX / 4 / total)
+        return np.ascontiguousarray(np.maximum(np.floor(c), 1.0).astype(np.int64))
 
     def __init__(self, counts: np.ndarray, device):
         from ..apps._applib import lib
         V = len(counts)
-        freq = np.ascontiguousarray(np.maximum(np.asarray(counts, dtype=np.float64), 1.0).astype(np.int64))
+        freq = self.int_frequencies(counts)
         P = np.zeros((V, self.MAX_CODE), dtype=np.int32)
         Cd = np.zeros((V, self.MAX_CODE), dtype=np.int8)
         lens = np.zeros(V, dtype=np.int32)
@@ -126,7 +140,7 @@ class WordEmbedding:
             self.alias_idx = torch.from_numpy(alias).to(self.dev)
         else:
             self.alias_prob = self.alias_idx = None
-        self.huffman = HuffmanTables(self.counts * 1e9, self.dev) if option.hs else None
+        self.huffman = HuffmanTables(self.counts, self.dev) if option.hs else None
         self.loss = torch.zeros(1, dtype=torch.float32, device=self.dev)
         self.pairs = torch.zeros(1, dtype=torch.int64, device=self.dev)
         self.word_count_actual = 0

@@ -117,6 +117,61 @@ def test_default_kernel_is_deterministic(mv_device):
     assert torch.equal(i0, i1) and torch.equal(o0, o1)
 
 
+def test_default_kernel_is_deterministic_at_dim_50(mv_device):
+    """A row width that is not a multiple of 4 also runs on the deterministic waves."""
+    from multiverso_b200.models.wordembedding import (WordEmbedding, WordEmbeddingOption,
+                                                      synthetic_zipf_corpus)
+    V = 5000
+    toks = torch.from_numpy(synthetic_zipf_corpus(200000, V, 1000, seed=3)).cuda()
+    runs = []
+    for _ in range(2):
+        we = WordEmbedding(WordEmbeddingOption(embeding_size=50, window_size=5, negative_num=5), V, seed=1)
+        for _ in range(2):
+            we.train_block(toks)
+        torch.cuda.synchronize()
+        runs.append((we.input_table.get().clone(), we.output_table.get().clone(), we.loss.item(), we.pairs.item(),
+                     we.kernel_launches))
+    (i0, o0, l0, p0, k0), (i1, o1, l1, p1, k1) = runs
+    assert p0 == p1 and p0 > 0 and l0 == l1 and k0 == k1 and k0 >= 4     # two launches per wave
+    assert torch.equal(i0, i1) and torch.equal(o0, o1) and not torch.equal(i0, torch.zeros_like(i0))
+
+
+@pytest.mark.parametrize("dim,pad", [(37, 0), (37, 3), (50, 0), (50, 14), (300, 0)])
+def test_dispatch_runs_the_deterministic_kernel_at_any_width(mv_device, dim, pad):
+    """`mvb_sgns_train` sends skip-gram + NS (hogwild = 0) to the deterministic waves at any dim <= 512 and any
+    row pitch: the same bits as a direct `mvb_sgns_train_det` call, and two launches per wave (the generic
+    kernel would make one)."""
+    from multiverso_b200 import _native as N
+    V, ld = 3000, dim + pad
+    g = torch.Generator().manual_seed(dim + pad)
+    toks = torch.randint(0, V, (20000,), generator=g).to(torch.int32)
+    toks[200::201] = -1
+    toks = toks.cuda()
+    prob, alias = torch.ones(V, device="cuda"), torch.arange(V, dtype=torch.int32, device="cuda")
+    base = [torch.zeros(V, ld) for _ in range(2)]
+    for b in base:
+        b[:, :dim] = (torch.rand(V, dim, generator=g) - 0.5) * 0.4
+
+    def run(fn):
+        w_in, w_out = base[0].cuda(), base[1].cuda()
+        a, out = N.Sgns(), torch.zeros(2, dtype=torch.int64, device="cuda")
+        a.tokens, a.n_tokens, a.w_in, a.w_out = toks.data_ptr(), toks.numel(), w_in.data_ptr(), w_out.data_ptr()
+        a.dim, a.ld, a.window, a.negative, a.lr, a.seed = dim, ld, 5, 5, 1e-2, 77
+        a.vocab, a.alias_prob, a.alias_idx = V, prob.data_ptr(), alias.data_ptr()
+        a.pair_count, a.loss_sum = out.data_ptr(), out.data_ptr() + 8
+        getattr(N.cuda_lib(), fn)(a, N.stream_ptr())
+        launches = N.cuda_lib().mvb_sgns_last_launches()
+        torch.cuda.synchronize()
+        return w_in, w_out, out.cpu(), launches
+
+    i1, o1, r1, n1 = run("mvb_sgns_train")
+    i2, o2, r2, n2 = run("mvb_sgns_train_det")
+    assert n1 == n2 and n1 >= 2 and n1 % 2 == 0
+    assert torch.equal(r1, r2) and r1[0] > 0
+    assert torch.equal(i1, i2) and torch.equal(o1, o2) and not torch.equal(i1.cpu(), base[0])
+    assert (i1[:, dim:] == 0).all() and (o1[:, dim:] == 0).all()
+
+
 M64 = (1 << 64) - 1
 
 
