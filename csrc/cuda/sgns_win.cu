@@ -596,13 +596,23 @@ sgns_win_kernel(const __grid_constant__ WinDev a) {
 }
 
 // ---- deterministic K7 (DESIGN.md §11): the maths above in waves of its in-flight count; reads see the tables as
-// the last wave left them, deltas / loss are summed in 64-bit fixed point, then applied.
+// the last wave left them, deltas / loss are summed in 64-bit fixed point, then applied.  A row that only one
+// reader of the wave reads (one (centre, k) of the output table, one staged (CTA, position) of the input table)
+// is applied in place by that reader, with the same bits the apply would give it.
 constexpr float kFixScale = 0x1p40f;              // 2^-40 resolution, +-2^23 range
 constexpr float kLossScale = 0x1p32f;
 
+// Readers per row of one wave, counted by the apply of the wave before it: [input table, output table].
+struct DetOwn {
+  int* cnt[2];                                    // [rows] readers (a superset is safe: > 1 takes the accumulator)
+  int* list[2];                                   // rows with a nonzero count, to reset them
+  int* n;                                         // [2] rows listed
+};
+
 struct DetDev {
   const int* tokens;
-  int64_t n_tokens, p0, p1;                       // centres of this wave
+  int64_t n_tokens, p0, p1, p2;                   // centres of this wave [p0, p1) and of the next one [p1, p2)
+  int S;                                          // centres per CTA of the wave kernel
   float* w_in;
   float* w_out;
   int dim;
@@ -626,12 +636,63 @@ struct DetDev {
   int* flag[2];                                   // row touched in this wave
   int* list[2];                                   // touched rows (any order)
   int* count;                                     // [2]
+  int* count_next;                                // [2] the next wave's, reset by this wave's apply
   unsigned long long* loss_acc;
+  float* loss_sum;
+  bool counted;                                   // own holds this wave's readers (false: the first wave of a call)
+  DetOwn own, own_next;                           // readers of this wave / of the next one
 };
 
 MVB_DEVINL void det_touch(const DetDev& a, int t, int r) {
   if (atomicExch(a.flag[t] + r, 1) == 0) a.list[t][atomicAdd(a.count + t, 1)] = r;
 }
+
+// The row of the input table staged for token position q, and its step scale; -1: none.  The wave kernel and the
+// reader count of the apply before it both sample through det_in_row / det_out_row, so they see the same rows.
+MVB_DEVINL int det_in_row(const DetDev& a, int64_t q, float& sc) {
+  int rid = -1;
+  sc = 1.f;
+  if (q >= 0 && q < a.n_tokens) {
+    const int tq = __ldg(a.tokens + q);
+    if (tq >= 0) {
+      rid = a.map_in ? __ldg(a.map_in + tq) : tq;
+      if (a.scale_in) sc = __ldg(a.scale_in + tq);
+    }
+  }
+  return rid;
+}
+
+// The row of the output table that output k of centre p reads (k = 0 the centre, 1.. its negatives), and its
+// step scale; -1: none.
+MVB_DEVINL int det_out_row(const DetDev& a, int64_t p, int k, int pool_n, float& sc) {
+  int rid = -1;
+  sc = 1.f;
+  const int tp = __ldg(a.tokens + p);
+  if (tp >= 0 && k == 0) {
+    rid = a.map_out ? __ldg(a.map_out + tp) : tp;
+    if (a.scale_out) sc = __ldg(a.scale_out + tp);
+  } else if (tp >= 0 && k < a.ko) {
+    const uint64_t prng = hash64(a.seed ^ (uint64_t)(p + 1) * 0x9E3779B97F4A7C15ull);
+    const uint64_t r = hash64(prng ^ ((uint64_t)k * 0xD6E8FEB86659FD93ull));
+    int tk;
+    if (a.neg_pool) {
+      tk = pool_n > 0 ? __ldg(a.neg_pool + (r >> 8) % (uint64_t)pool_n) : -1;
+    } else {
+      const uint32_t idx = (uint32_t)((r >> 32) % (uint64_t)a.vocab);
+      const float u = (float)(r & 0xFFFFFF) * (1.0f / 16777216.0f);
+      tk = (u < __ldg(a.alias_prob + idx)) ? (int)idx : __ldg(a.alias_idx + idx);
+    }
+    if (tk == tp) tk = -1;                       // Parse(): target == word_idx is skipped
+    if (tk >= 0) {
+      rid = a.map_out ? __ldg(a.map_out + tk) : tk;
+      if (a.scale_out) sc = __ldg(a.scale_out + tk);
+    }
+  }
+  return rid;
+}
+
+// x + the fixed-point sum v: what the apply writes for an element whose sum is nonzero
+MVB_DEVINL float det_fix_add(float x, long long v) { return x + (float)((double)v * (1.0 / (double)kFixScale)); }
 template <int NJ>
 MVB_DEVINL void det_load(float (&v)[NJ], const float* row, int dim, int lane, bool on) {
 #pragma unroll
@@ -686,49 +747,20 @@ sgns_det_kernel(const __grid_constant__ DetDev a) {
   // ---- sampling of the whole slice: one thread per staged position, one per (centre, output row) ----------
   const int pool_n = a.neg_pool_size_ptr ? __ldg(a.neg_pool_size_ptr) : a.neg_pool_size;
   for (int t = threadIdx.x; t < np + ns * KO; t += blockDim.x) {
-    int rid = -1;
-    float sc = 1.f;
+    float sc;
     if (t < np) {
-      const int64_t q = s0 - W + t;
-      if (q >= 0 && q < a.n_tokens) {
-        const int tq = __ldg(a.tokens + q);
-        if (tq >= 0) {
-          rid = a.map_in ? __ldg(a.map_in + tq) : tq;
-          if (a.scale_in) sc = __ldg(a.scale_in + tq);
-        }
-      }
-      crid[t] = rid;
+      crid[t] = det_in_row(a, s0 - W + t, sc);
       csc[t] = sc;
       need[t] = 0;
     } else {
-      const int ck = t - np, k = ck % KO;
-      const int64_t p = s0 + ck / KO;
-      const int tp = __ldg(a.tokens + p);
-      if (tp >= 0 && k == 0) {
-        rid = a.map_out ? __ldg(a.map_out + tp) : tp;
-        if (a.scale_out) sc = __ldg(a.scale_out + tp);
-      } else if (tp >= 0 && k < a.ko) {
-        const uint64_t prng = hash64(a.seed ^ (uint64_t)(p + 1) * 0x9E3779B97F4A7C15ull);
-        const uint64_t r = hash64(prng ^ ((uint64_t)k * 0xD6E8FEB86659FD93ull));
-        int tk;
-        if (a.neg_pool) {
-          tk = pool_n > 0 ? __ldg(a.neg_pool + (r >> 8) % (uint64_t)pool_n) : -1;
-        } else {
-          const uint32_t idx = (uint32_t)((r >> 32) % (uint64_t)a.vocab);
-          const float u = (float)(r & 0xFFFFFF) * (1.0f / 16777216.0f);
-          tk = (u < __ldg(a.alias_prob + idx)) ? (int)idx : __ldg(a.alias_idx + idx);
-        }
-        if (tk == tp) tk = -1;                       // Parse(): target == word_idx is skipped
-        if (tk >= 0) {
-          rid = a.map_out ? __ldg(a.map_out + tk) : tk;
-          if (a.scale_out) sc = __ldg(a.scale_out + tk);
-        }
-      }
-      orid[ck] = rid;
+      const int ck = t - np;
+      orid[ck] = det_out_row(a, s0 + ck / KO, ck % KO, pool_n, sc);
       osc[ck] = sc;
     }
   }
   for (int e = threadIdx.x; e < np * dim; e += blockDim.x) hacc[e] = 0ull;
+  // the next wave's readers are counted from zero by this wave's apply
+  if (blockIdx.x == 0 && threadIdx.x == 0) a.own_next.n[0] = a.own_next.n[1] = 0;
   __syncthreads();
 
   // ---- this warp's centre: window (ParseSentence), lane l <-> offset l - hw, staged position c + W + l - hw ----
@@ -748,7 +780,9 @@ sgns_det_kernel(const __grid_constant__ DetDev a) {
     ctx = (((hi >= 31) ? 0xffffffffu : ((1u << (hi + 1)) - 1u)) & ~((1u << lo) - 1u)) & ~(1u << hw);
   }
   if ((ctx >> lane) & 1u) need[c + W + lane - hw] = 1;   // every writer stores the same value
-  if (ctx && ((used >> lane) & 1u)) det_touch(a, 1, rid);
+  // output rows this (centre, k) alone reads in the wave: applied in place after phase 2
+  const uint32_t owned = __ballot_sync(0xffffffffu, a.counted && rid >= 0 && a.own.cnt[1][rid] == 1);
+  if (ctx && ((used & ~owned) >> lane) & 1u) det_touch(a, 1, rid);
   float O[KO][NJ];
 #pragma unroll
   for (int k = 0; k < KO; ++k) {
@@ -817,6 +851,14 @@ sgns_det_kernel(const __grid_constant__ DetDev a) {
   for (int i = c; i < np; i += S) {
     if (!need[i]) continue;
     const int r = crid[i];
+    if (a.counted && a.own.cnt[0][r] == 1) {          // no other staged position holds the row: apply in place
+      float* row = a.w_in + (int64_t)r * a.ld;
+      for (int j = lane; j < dim; j += 32) {
+        const long long v = (long long)hacc[(size_t)i * dim + j];
+        if (v) row[j] = det_fix_add(hrow[(size_t)i * dim + j], v);
+      }
+      continue;
+    }
     unsigned long long* dst = a.acc[0] + (int64_t)r * dim;
     for (int j = lane; j < dim; j += 32) {
       const unsigned long long v = hacc[(size_t)i * dim + j];
@@ -845,7 +887,22 @@ sgns_det_kernel(const __grid_constant__ DetDev a) {
 #pragma unroll
     for (int k = 0; k < KO; ++k) {
       if (!((used >> k) & 1u)) continue;
-      unsigned long long* dst = a.acc[1] + (int64_t)orid[c * KO + k] * dim;
+      const int r = orid[c * KO + k];
+      if ((owned >> k) & 1u) {
+        // the row as the wave found it (nothing else reads or writes it in this wave) plus the one term its
+        // fixed-point sum would hold; zero terms leave the element untouched, as in the apply
+        float* row = a.w_out + (int64_t)r * a.ld;
+        float x[NJ];
+#pragma unroll
+        for (int u = 0; u < NJ; ++u) x[u] = lane + 32 * u < dim ? row[lane + 32 * u] : 0.f;
+#pragma unroll
+        for (int u = 0; u < NJ; ++u) {
+          const long long v = __float2ll_rn(O[k][u] * kFixScale);
+          if (lane + 32 * u < dim && v != 0) row[lane + 32 * u] = det_fix_add(x[u], v);
+        }
+        continue;
+      }
+      unsigned long long* dst = a.acc[1] + (int64_t)r * dim;
 #pragma unroll
       for (int u = 0; u < NJ; ++u)
         if (lane + 32 * u < dim) atomicAdd(dst + lane + 32 * u, (unsigned long long)__float2ll_rn(O[k][u] * kFixScale));
@@ -858,18 +915,52 @@ sgns_det_kernel(const __grid_constant__ DetDev a) {
 }
 
 // Adds each touched row's sum to its table and clears it, a warp per listed row (input rows, then output rows);
-// resets the NEXT wave's (idle) counters and rolls the wave's loss into loss_sum.
+// resets this wave's reader counts and counts the next wave's readers: per row of the output table its
+// (centre, k), per row of the input table its staged (CTA, position), a halo position once per CTA that stages
+// it; resets the NEXT wave's (idle) counters and rolls the wave's loss into loss_sum.
 __global__ void __launch_bounds__(256)
-sgns_det_apply(float* __restrict__ w_in, float* __restrict__ w_out, int dim, int64_t ld,
-               unsigned long long* __restrict__ acc_in, unsigned long long* __restrict__ acc_out, int* flag_in,
-               int* flag_out, const int* list_in, const int* list_out, const int* count, int* next,
-               unsigned long long* loss_acc, float* loss_sum) {
+sgns_det_apply(const __grid_constant__ DetDev a) {
+  const int tid = blockIdx.x * blockDim.x + threadIdx.x, nthreads = gridDim.x * blockDim.x;
+  // listed rows go to the first warps and the counts to the last threads, so their latencies overlap
+  const int ctid = nthreads - 1 - tid;
+  if (a.counted) {
+    const int n0 = a.own.n[0], n01 = n0 + a.own.n[1];
+    for (int e = ctid; e < n01; e += nthreads) {
+      const int t = e < n0 ? 0 : 1;
+      a.own.cnt[t][a.own.list[t][e - (t ? n0 : 0)]] = 0;
+    }
+  }
+  if (a.p2 > a.p1) {
+    const int pool_n = a.neg_pool_size_ptr ? __ldg(a.neg_pool_size_ptr) : a.neg_pool_size;
+    const int W = a.window, span = a.S + 2 * W;
+    const int64_t n_out = (a.p2 - a.p1) * a.ko, n_slices = (a.p2 - a.p1 + a.S - 1) / a.S;
+    for (int64_t e = ctid; e < n_out + n_slices * span; e += nthreads) {
+      int t, r;
+      float sc;
+      if (e < n_out) {
+        t = 1;
+        r = det_out_row(a, a.p1 + e / a.ko, (int)(e % a.ko), pool_n, sc);
+      } else {
+        t = 0;
+        const int64_t s0 = a.p1 + (e - n_out) / span * a.S;     // the slice's first centre
+        const int i = (int)((e - n_out) % span);
+        r = (i < (a.p2 - s0 < a.S ? a.p2 - s0 : a.S) + 2 * W) ? det_in_row(a, s0 - W + i, sc) : -1;
+      }
+      if (r >= 0 && atomicAdd(a.own_next.cnt[t] + r, 1) == 0) a.own_next.list[t][atomicAdd(a.own_next.n + t, 1)] = r;
+    }
+  }
+  float* __restrict__ w_in = a.w_in;
+  float* __restrict__ w_out = a.w_out;
+  unsigned long long* __restrict__ acc_in = a.acc[0];
+  unsigned long long* __restrict__ acc_out = a.acc[1];
+  const int dim = a.dim;
+  const int64_t ld = a.ld;
   const int lane = threadIdx.x & 31;
-  const int n_in = count[0], n_all = n_in + count[1];
+  const int n_in = a.count[0], n_all = n_in + a.count[1];
   const int nwarps = (gridDim.x * blockDim.x) >> 5;
-  for (int w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; w < n_all; w += nwarps) {
+  for (int w = tid >> 5; w < n_all; w += nwarps) {
     const bool in = w < n_in;
-    const int r = in ? list_in[w] : list_out[w - n_in];
+    const int r = in ? a.list[0][w] : a.list[1][w - n_in];
     unsigned long long* q = (in ? acc_in : acc_out) + (int64_t)r * dim;
     float* row = (in ? w_in : w_out) + (int64_t)r * ld;
     for (int j0 = 0; j0 < dim; j0 += 128) {          // 4 elements per lane in flight
@@ -885,16 +976,17 @@ sgns_det_apply(float* __restrict__ w_in, float* __restrict__ w_out, int dim, int
       for (int u = 0; u < 4; ++u) {
         const int j = j0 + lane + 32 * u;
         if (j >= dim) continue;
-        if (v[u]) row[j] = x[u] + (float)((double)v[u] * (1.0 / (double)kFixScale));
+        if (v[u]) row[j] = det_fix_add(x[u], v[u]);
         q[j] = 0ull;
       }
     }
-    if (lane == 0) (in ? flag_in : flag_out)[r] = 0;
+    if (lane == 0) a.flag[in ? 0 : 1][r] = 0;
   }
-  if (blockIdx.x == 0 && threadIdx.x == 0) {
-    next[0] = next[1] = 0;
-    if (loss_sum && *loss_acc) *loss_sum += (float)((double)(long long)*loss_acc * (1.0 / (double)kLossScale));
-    *loss_acc = 0ull;
+  if (tid == 0) {
+    a.count_next[0] = a.count_next[1] = 0;
+    if (a.loss_sum && *a.loss_acc)
+      *a.loss_sum += (float)((double)(long long)*a.loss_acc * (1.0 / (double)kLossScale));
+    *a.loss_acc = 0ull;
   }
 }
 
@@ -1012,12 +1104,14 @@ extern "C" int mvb_sgns_train_det(const MvbSgns* h, void* stream) {
   if (h->cbow || h->hs || h->use_adagrad || h->negative < 1 || h->negative > kKO - 1) return -20;
   if (h->nservers > 1 || h->dim < 1 || h->dim > 512 || h->window < 1 || h->window > 15 || h->vocab <= 0) return -21;
   mvb_sgns_launches = 0;
-  // rows are word ids or cache slots (< vocab).  Scratch (one stream): counters [4] | loss | acc [2 x rows x dim] |
-  // flags, lists [2 x rows]; grown on demand, cleared when its layout changes (a wave leaves it clear but for counters)
+  // rows are word ids or cache slots (< vocab).  Scratch (one stream): counters [4] | listed rows of the reader
+  // counts [2 parities x 2] | loss | acc [2 x rows x dim] | flags, lists [2 x rows] | reader counts, their lists
+  // [2 parities x 2 x rows]; grown on demand, cleared when its layout changes (a wave leaves it clear but for
+  // counters, and a call leaves every reader count zero)
   static unsigned char* buf = nullptr;
   static int64_t cap = 0, last_elems = -1;
   static int parity = 0;
-  const int64_t rows = h->vocab, elems = rows * h->dim, bytes = 16 + 8 + 2 * elems * 8 + 4 * rows * 4;
+  const int64_t rows = h->vocab, elems = rows * h->dim, bytes = 32 + 8 + 2 * elems * 8 + 12 * rows * 4;
   if (bytes > cap) {
     MVB_CUDA_CHECK(cudaDeviceSynchronize());
     if (buf) MVB_CUDA_CHECK(cudaFree(buf));
@@ -1031,9 +1125,17 @@ extern "C" int mvb_sgns_train_det(const MvbSgns* h, void* stream) {
     parity = 0;
   }
   int* counters = reinterpret_cast<int*>(buf);
-  unsigned long long* loss_acc = reinterpret_cast<unsigned long long*>(buf + 16);
+  unsigned long long* loss_acc = reinterpret_cast<unsigned long long*>(buf + 32);
   unsigned long long* acc = loss_acc + 1;
   int* ints = reinterpret_cast<int*>(acc + 2 * elems);
+  DetOwn own[2];                                  // by wave parity within the call
+  for (int q = 0; q < 2; ++q) {
+    for (int t = 0; t < 2; ++t) {
+      own[q].cnt[t] = ints + (4 + 2 * q + t) * rows;
+      own[q].list[t] = ints + (8 + 2 * q + t) * rows;
+    }
+    own[q].n = counters + 4 + 2 * q;
+  }
   DetDev a{};
   a.tokens = h->tokens; a.n_tokens = h->n_tokens; a.w_in = h->w_in; a.w_out = h->w_out;
   a.dim = h->dim; a.ld = h->ld; a.window = h->window; a.ko = 1 + h->negative; a.lr = h->lr;
@@ -1044,7 +1146,7 @@ extern "C" int mvb_sgns_train_det(const MvbSgns* h, void* stream) {
   a.acc[0] = acc; a.acc[1] = acc + elems;
   a.flag[0] = ints; a.flag[1] = ints + rows;
   a.list[0] = ints + 2 * rows; a.list[1] = ints + 3 * rows;
-  a.loss_acc = loss_acc;
+  a.loss_acc = loss_acc; a.loss_sum = h->loss_sum;
   int wave = mvb_sgns_win_inflight(h->dim, h->negative, h->window, h->max_ctas);
   if (wave <= 0) wave = 2 * mvb_num_sms() * kNW;
   // the <NJ, KO> instance, and as many centres per CTA as its registers and the opt-in shared memory allow
@@ -1072,14 +1174,20 @@ extern "C" int mvb_sgns_train_det(const MvbSgns* h, void* stream) {
   if (smem > (size_t)max_smem) return -22;
   MVB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const int apply_blocks = mvb_num_sms() * 4;
-  for (int64_t p0 = 0; p0 < h->n_tokens; p0 += wave) {
+  a.S = S;
+  // the first wave has no reader counts and sends every row through the accumulator; the last one counts none,
+  // so the call leaves every count zero
+  for (int64_t p0 = 0, w = 0; p0 < h->n_tokens; p0 += wave, ++w) {
     a.p0 = p0;
     a.p1 = p0 + wave < h->n_tokens ? p0 + wave : h->n_tokens;
+    a.p2 = a.p1 + wave < h->n_tokens ? a.p1 + wave : h->n_tokens;
     a.count = counters + 2 * parity;
+    a.count_next = counters + 2 * (parity ^ 1);
+    a.counted = w > 0;
+    a.own = own[w & 1];
+    a.own_next = own[(w & 1) ^ 1];
     kern<<<(int)((a.p1 - p0 + S - 1) / S), 32 * S, smem, st>>>(a);
-    sgns_det_apply<<<apply_blocks, 256, 0, st>>>(h->w_in, h->w_out, h->dim, h->ld, a.acc[0], a.acc[1], a.flag[0],
-                                                 a.flag[1], a.list[0], a.list[1], a.count,
-                                                 counters + 2 * (parity ^ 1), loss_acc, h->loss_sum);
+    sgns_det_apply<<<apply_blocks, 256, 0, st>>>(a);
     parity ^= 1;
     mvb_sgns_launches += 2;
   }
