@@ -6,9 +6,10 @@
 Builds the configuration `bench.py` measures (skip-gram, dim 300, vocab 1M, 5 negatives, window 5,
 synthetic Zipf corpus of 1M-word blocks, the default deterministic K7), trains the warm-up blocks
 untraced, then traces each timed block on its own under torch.profiler with CUDA activities.  Per
-block it prints one JSON line: the device time of the deterministic K7 wave kernels
-(`sgns_det_kernel*`) and of their apply kernels (`sgns_det_apply*`), the time of every other kernel,
-and the idle time between kernels inside the block's device span.  The first line names the card,
+block it prints one JSON line: the device time of the deterministic K7 plan (its `sgns_det_plan*`
+kernels and the radix sort of its readers, whose kernels carry `sgns_det_plan_reader` in their
+names), of its wave kernels (`sgns_det_kernel*`) and of their apply kernels (`sgns_det_apply*`), the
+time of every other kernel, and the idle time between kernels inside the block's device span.  The first line names the card,
 its power limit and SM clock, read in this process.  Tracing slows the host, so take words/s from
 `bench.py`, not from here.
 """
@@ -50,10 +51,13 @@ def block_profile(prof):
     ks = sorted(((e.time_range.start, e.time_range.end, e.name) for e in prof.events()
                  if e.device_type == DeviceType.CUDA and not e.name.startswith("Memcpy")
                  and not e.name.startswith("Memset")), key=lambda k: k[0])
-    out = {"det_kernel_us": 0.0, "det_apply_us": 0.0, "other_kernels_us": 0.0,
-           "n_det_kernel": 0, "n_det_apply": 0, "n_other": 0}
+    out = {"det_plan_us": 0.0, "det_kernel_us": 0.0, "det_apply_us": 0.0, "other_kernels_us": 0.0,
+           "n_det_plan": 0, "n_det_kernel": 0, "n_det_apply": 0, "n_other": 0}
     for s, e, name in ks:
-        if "sgns_det_kernel" in name:
+        if "sgns_det_plan" in name:
+            out["det_plan_us"] += e - s
+            out["n_det_plan"] += 1
+        elif "sgns_det_kernel" in name:
             out["det_kernel_us"] += e - s
             out["n_det_kernel"] += 1
         elif "sgns_det_apply" in name:

@@ -30,6 +30,10 @@
 // Synchronisation is mbarrier only (no __syncthreads after init): in_full/in_empty per ring slot
 // (empty counts 2W+1 arrivals: the centres whose window covers the slot), out_full/out_empty per
 // consumer stage.  Virtual positions [a-2W, b+2W) make every count uniform at the range ends.
+#include <cub/block/block_reduce.cuh>
+#include <cub/block/block_scan.cuh>
+#include <cub/device/device_radix_sort.cuh>
+
 #include "mvb_common.cuh"
 
 namespace {
@@ -597,21 +601,29 @@ sgns_win_kernel(const __grid_constant__ WinDev a) {
 
 // ---- deterministic K7 (DESIGN.md §11): the maths above in waves of its in-flight count; reads see the tables as
 // the last wave left them, deltas / loss are summed in 64-bit fixed point, then applied.  A row that only one
-// reader of the wave reads (one (centre, k) of the output table, one staged (CTA, position) of the input table)
+// reader of the wave reads (one (centre, k) of the output table, one staged (slice, position) of the input table)
 // is applied in place by that reader, with the same bits the apply would give it.
+//
+// Which rows a wave reads depends on the tokens, the seed, the sampler, the maps and the scales only, never on
+// table values, so the whole call is planned before its first wave: the rows and scales of every position and
+// centre, every centre's window, and per reader of every wave its slot -- -2 it reads nothing, -1 it is its row's
+// only reader in the wave, else the row's entry in the wave's compact list of shared rows, whose sums go through
+// the accumulator.
 constexpr float kFixScale = 0x1p40f;              // 2^-40 resolution, +-2^23 range
 constexpr float kLossScale = 0x1p32f;
+constexpr int kPlanThreads = 256;
+constexpr int kPlanItems = 8;                     // sorted readers per thread of the run classification
+constexpr int kPlanTile = kPlanThreads * kPlanItems;
 
-// Readers per row of one wave, counted by the apply of the wave before it: [input table, output table].
-struct DetOwn {
-  int* cnt[2];                                    // [rows] readers (a superset is safe: > 1 takes the accumulator)
-  int* list[2];                                   // rows with a nonzero count, to reset them
-  int* n;                                         // [2] rows listed
+// The value sorted with each reader's key: its reader index (named so that the sort's kernels carry the plan's
+// name in profiles).
+struct sgns_det_plan_reader {
+  int i;
 };
 
 struct DetDev {
   const int* tokens;
-  int64_t n_tokens, p0, p1, p2;                   // centres of this wave [p0, p1) and of the next one [p1, p2)
+  int64_t n_tokens, p0, p1;                       // centres of this wave [p0, p1)
   int S;                                          // centres per CTA of the wave kernel
   float* w_in;
   float* w_out;
@@ -632,23 +644,29 @@ struct DetDev {
   uint64_t seed;
   bool want_loss;
   unsigned long long* pair_count;
-  unsigned long long* acc[2];                     // [rows x dim] deltas of the input / output table
-  int* flag[2];                                   // row touched in this wave
-  int* list[2];                                   // touched rows (any order)
-  int* count;                                     // [2]
-  int* count_next;                                // [2] the next wave's, reset by this wave's apply
   unsigned long long* loss_acc;
   float* loss_sum;
-  bool counted;                                   // own holds this wave's readers (false: the first wave of a call)
-  DetOwn own, own_next;                           // readers of this wave / of the next one
+  // the plan.  Readers: (centre p, output k) is p * ko + k; staged position i of slice b of wave w is
+  // n_tokens * ko + ((w * spw + b) * (S + 2W) + i).
+  int64_t wave;                                   // centres per wave
+  int n_waves, spw;                               // waves of the call, slices per wave
+  int wi;                                         // the wave [p0, p1) is wave wi
+  int64_t n_readers;
+  int* in_rid;                                    // [n_tokens] input row of each position (-1 none) ...
+  float* in_sc;                                   // ... and its step scale
+  int* out_rid;                                   // [n_tokens x ko] output rows of each centre (-1 none) ...
+  float* out_sc;                                  // ... and their step scales
+  int2* chw;                                      // [n_tokens] context mask and half window of each centre
+  unsigned long long* key;                        // [n_readers] (wave, table, row) of each reader; none: n_waves
+  sgns_det_plan_reader* reader;                   // [n_readers] reader indices, sorted with the keys
+  int* tile_off;                                  // shared rows starting in earlier tiles of the sorted readers
+  int* slot;                                      // [n_readers] -2 / -1 / index into list
+  unsigned* list;                                 // shared rows of every wave, wave by wave: row | table << 31
+  int* off;                                       // [n_waves + 1] first entry of each wave in list
+  unsigned long long* acc;                        // [shared rows of a wave x dim] their fixed-point sums
 };
 
-MVB_DEVINL void det_touch(const DetDev& a, int t, int r) {
-  if (atomicExch(a.flag[t] + r, 1) == 0) a.list[t][atomicAdd(a.count + t, 1)] = r;
-}
-
-// The row of the input table staged for token position q, and its step scale; -1: none.  The wave kernel and the
-// reader count of the apply before it both sample through det_in_row / det_out_row, so they see the same rows.
+// The row of the input table staged for token position q, and its step scale; -1: none.
 MVB_DEVINL int det_in_row(const DetDev& a, int64_t q, float& sc) {
   int rid = -1;
   sc = 1.f;
@@ -691,6 +709,146 @@ MVB_DEVINL int det_out_row(const DetDev& a, int64_t p, int k, int pool_n, float&
   return rid;
 }
 
+MVB_DEVINL unsigned long long det_key(const DetDev& a, int64_t w, int t, int r) {
+  return ((unsigned long long)w * 2 + t) * (unsigned long long)a.vocab + (unsigned)r;
+}
+
+// ---- plan, step 1: input row and scale of every token position --------------------------------------------
+__global__ void __launch_bounds__(kPlanThreads) sgns_det_plan_tokens(const __grid_constant__ DetDev a) {
+  const int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (q >= a.n_tokens) return;
+  float sc;
+  a.in_rid[q] = det_in_row(a, q, sc);
+  a.in_sc[q] = sc;
+}
+
+// ---- plan, step 2: per centre its output rows and scales, its window (ParseSentence: a random shrink, contexts
+// stop at the first break on either side; bit hw + d <-> offset d) and a reader key per (centre, k) it reads ---
+__global__ void __launch_bounds__(kPlanThreads) sgns_det_plan_centres(const __grid_constant__ DetDev a) {
+  const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= a.n_tokens) return;
+  const int pool_n = a.neg_pool_size_ptr ? __ldg(a.neg_pool_size_ptr) : a.neg_pool_size;
+  const int W = a.window;
+  const int hw = W - (int)((hash64(a.seed ^ (uint64_t)(p + 1) * 0x9E3779B97F4A7C15ull) >> 16) % (uint64_t)W);
+  float sc;
+  const int r0 = det_out_row(a, p, 0, pool_n, sc);
+  uint32_t ctx = 0;
+  if (r0 >= 0) {                                  // a break or an unmapped centre trains nothing
+    int nl = 0, nr = 0;
+    while (nl < hw && p - 1 - nl >= 0 && a.in_rid[p - 1 - nl] >= 0) ++nl;
+    while (nr < hw && p + 1 + nr < a.n_tokens && a.in_rid[p + 1 + nr] >= 0) ++nr;
+    ctx = (((1u << nl) - 1u) << (hw - nl)) | (((1u << nr) - 1u) << (hw + 1));
+  }
+  a.chw[p] = make_int2((int)ctx, hw);
+  const int64_t w = p / a.wave;
+  const unsigned long long none = det_key(a, a.n_waves, 0, 0);
+  for (int k = 0; k < a.ko; ++k) {
+    const int r = k == 0 ? r0 : det_out_row(a, p, k, pool_n, sc);
+    const int64_t e = p * a.ko + k;
+    a.out_rid[e] = r;
+    a.out_sc[e] = sc;
+    a.key[e] = (ctx && r >= 0) ? det_key(a, w, 1, r) : none;
+    a.reader[e].i = (int)e;
+  }
+}
+
+// ---- plan, step 3: a reader key per staged (slice, position) that is a context of some centre of its slice ---
+__global__ void __launch_bounds__(kPlanThreads) sgns_det_plan_staged(const __grid_constant__ DetDev a) {
+  const int W = a.window, span = a.S + 2 * W;
+  const int64_t n_out = a.n_tokens * a.ko;
+  const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= a.n_readers - n_out) return;
+  const int64_t g = e / span, w = g / a.spw;
+  const int i = (int)(e % span);
+  const int64_t s0 = w * a.wave + (g % a.spw) * a.S;
+  const int64_t p1 = (w + 1) * a.wave < a.n_tokens ? (w + 1) * a.wave : a.n_tokens;
+  const int ns = s0 < p1 ? (int)(p1 - s0 < a.S ? p1 - s0 : a.S) : 0;
+  bool need = false;
+  // centre c of the slice sits at staged position c + W: position i is its context at offset i - c - W
+  for (int c = (i - 2 * W > 0 ? i - 2 * W : 0); c < ns && c <= i && !need; ++c) {
+    const int d = i - c - W;
+    const int2 cx = a.chw[s0 + c];
+    need = d != 0 && d >= -cx.y && d <= cx.y && ((cx.x >> (cx.y + d)) & 1);
+  }
+  a.key[n_out + e] = need ? det_key(a, w, 0, a.in_rid[s0 - W + i]) : det_key(a, a.n_waves, 0, 0);
+  a.reader[n_out + e].i = (int)(n_out + e);
+}
+
+// ---- plan, steps 5-7: classify the sorted readers.  A run of equal keys is the readers of one row in one wave:
+// a run of one reads alone; a longer one is a shared row and gets the next entry of the list.
+struct DetRun {
+  bool shared, alone, first;                      // starts a shared run / is a run of one / first key of its wave
+};
+MVB_DEVINL DetRun det_run(const DetDev& a, int64_t j, unsigned long long none) {
+  const unsigned long long k = a.key[j];
+  const unsigned long long prev = j > 0 ? a.key[j - 1] : ~0ull, next = j + 1 < a.n_readers ? a.key[j + 1] : ~0ull;
+  const unsigned long long wv = 2ull * (unsigned)a.vocab;
+  DetRun r;
+  r.shared = k < none && k != prev && k == next;
+  r.alone = k != prev && k != next;
+  r.first = j == 0 || prev / wv != k / wv;
+  return r;
+}
+
+// shared rows starting in each tile of kPlanTile sorted readers
+__global__ void __launch_bounds__(kPlanThreads) sgns_det_plan_runs(const __grid_constant__ DetDev a) {
+  using BlockReduce = cub::BlockReduce<int, kPlanThreads>;
+  __shared__ typename BlockReduce::TempStorage tmp;
+  const unsigned long long none = det_key(a, a.n_waves, 0, 0);
+  const int64_t j0 = (int64_t)blockIdx.x * kPlanTile + threadIdx.x * kPlanItems;
+  int n = 0;
+  for (int u = 0; u < kPlanItems; ++u)
+    if (j0 + u < a.n_readers) n += det_run(a, j0 + u, none).shared;
+  n = BlockReduce(tmp).Sum(n);
+  if (threadIdx.x == 0) a.tile_off[blockIdx.x] = n;
+}
+
+// exclusive sum of the tiles' counts, in place (one CTA)
+__global__ void __launch_bounds__(1024) sgns_det_plan_scan(int* tile_off, int n_tiles) {
+  using BlockScan = cub::BlockScan<int, 1024>;
+  __shared__ typename BlockScan::TempStorage tmp;
+  int carry = 0;
+  for (int t0 = 0; t0 < n_tiles; t0 += 1024) {
+    const int t = t0 + threadIdx.x;
+    const int v = t < n_tiles ? tile_off[t] : 0;
+    int x, total;
+    BlockScan(tmp).ExclusiveSum(v, x, total);
+    if (t < n_tiles) tile_off[t] = carry + x;
+    carry += total;
+    __syncthreads();
+  }
+}
+
+// every reader's slot, the list of shared rows and each wave's first entry in it
+__global__ void __launch_bounds__(kPlanThreads) sgns_det_plan_slots(const __grid_constant__ DetDev a) {
+  using BlockScan = cub::BlockScan<int, kPlanThreads>;
+  __shared__ typename BlockScan::TempStorage tmp;
+  const unsigned long long none = det_key(a, a.n_waves, 0, 0), wv = 2ull * (unsigned)a.vocab;
+  const int64_t j0 = (int64_t)blockIdx.x * kPlanTile + threadIdx.x * kPlanItems;
+  int n = 0;
+  for (int u = 0; u < kPlanItems; ++u)
+    if (j0 + u < a.n_readers) n += det_run(a, j0 + u, none).shared;
+  int before;
+  BlockScan(tmp).ExclusiveSum(n, before);
+  int incl = a.tile_off[blockIdx.x] + before;     // shared rows started up to and including reader j
+  for (int u = 0; u < kPlanItems; ++u) {
+    const int64_t j = j0 + u;
+    if (j >= a.n_readers) break;
+    const DetRun r = det_run(a, j, none);
+    const unsigned long long k = a.key[j];
+    incl += r.shared;
+    a.slot[a.reader[j].i] = k == none ? -2 : r.alone ? -1 : incl - 1;
+    if (r.shared) a.list[incl - 1] = (unsigned)(k % (unsigned)a.vocab) | (unsigned)((k / (unsigned)a.vocab) & 1) << 31;
+    if (r.first) {                                // waves before this key's without a key start here too
+      const int64_t w = (int64_t)(k / wv);
+      const int64_t wp = j > 0 ? (int64_t)(a.key[j - 1] / wv) : -1;
+      for (int64_t x = wp + 1; x <= w; ++x) a.off[x] = incl - r.shared;
+    }
+    if (j == a.n_readers - 1)
+      for (int64_t x = (int64_t)(k / wv) + 1; x <= a.n_waves; ++x) a.off[x] = incl;
+  }
+}
+
 // x + the fixed-point sum v: what the apply writes for an element whose sum is nonzero
 MVB_DEVINL float det_fix_add(float x, long long v) { return x + (float)((double)v * (1.0 / (double)kFixScale)); }
 template <int NJ>
@@ -713,19 +871,19 @@ MVB_DEVINL float det_dot(const float (&x)[NJ], const float (&y)[NJ]) {
 __host__ __device__ constexpr int det_max_s(int nj, int ko) { return nj * ko <= 64 ? 20 : nj * ko <= 96 ? 12 : 8; }
 
 // Shared memory of a CTA of S centres: per staged position (S + 2W of them) an int64 accumulator row, the input
-// row and its id / scale / "is a context" word; per (centre, output row) its id and scale; per (centre, offset,
-// output row) the pair's error term.
+// row and its id / scale / slot; per (centre, output row) its id and scale; per (centre, offset, output row) the
+// pair's error term.
 __host__ __device__ inline size_t det_smem_bytes(int S, int W, int dim, int ko) {
   return (size_t)(S + 2 * W) * ((size_t)dim * 12 + 12) + (size_t)S * ko * 8 + (size_t)S * (2 * W + 1) * ko * 4;
 }
 
-// One CTA owns S consecutive centres [s0, s0 + S) of the wave, one warp per centre.  All S samplings are done
-// up front, one thread per (centre, output row) and per staged position; the input rows of the positions
-// [s0 - W, s0 + S + W) are staged once in shared memory, and each position's input delta is summed there over
-// all its centres before one row of REDs sends it to the wave's accumulator.  The float arithmetic of every
-// (centre, context) pair does not depend on the tiling (element j on lane j % 32, register j / 32, fixed FMA
-// chains and butterflies, one conversion to fixed point per pair and per (centre, k)); only the grouping of the
-// exact int64 sums does, so the result is bitwise independent of S.
+// One CTA owns S consecutive centres [s0, s0 + S) of the wave, one warp per centre.  The slice's rows, scales,
+// windows and slots come from the plan; the input rows of the positions [s0 - W, s0 + S + W) that are a context
+// are staged once in shared memory, and each position's input delta is summed there over all its centres before
+// one row of REDs sends it to its accumulator slot.  The float arithmetic of every (centre, context) pair does not
+// depend on the tiling (element j on lane j % 32, register j / 32, fixed FMA chains and butterflies, one
+// conversion to fixed point per pair and per (centre, k)); only the grouping of the exact int64 sums does, so the
+// result is bitwise independent of S.
 template <int NJ, int KO>
 __global__ void __launch_bounds__(32 * det_max_s(NJ, KO))
 sgns_det_kernel(const __grid_constant__ DetDev a) {
@@ -739,61 +897,55 @@ sgns_det_kernel(const __grid_constant__ DetDev a) {
   float* hrow = reinterpret_cast<float*>(hacc + (size_t)(S + 2 * W) * dim);
   int* crid = reinterpret_cast<int*>(hrow + (size_t)(S + 2 * W) * dim);
   float* csc = reinterpret_cast<float*>(crid + S + 2 * W);
-  int* need = reinterpret_cast<int*>(csc + S + 2 * W);
-  int* orid = need + S + 2 * W;
+  int* cslot = reinterpret_cast<int*>(csc + S + 2 * W);
+  int* orid = cslot + S + 2 * W;
   float* osc = reinterpret_cast<float*>(orid + S * KO);
   float* gsm = osc + S * KO;
 
-  // ---- sampling of the whole slice: one thread per staged position, one per (centre, output row) ----------
-  const int pool_n = a.neg_pool_size_ptr ? __ldg(a.neg_pool_size_ptr) : a.neg_pool_size;
+  // ---- the slice's plan: one thread per staged position, one per (centre, output row) ----------------------
+  const int base = __ldg(a.off + a.wi);                   // the wave's first entry in the list of shared rows
+  const int* pslot = a.slot + a.n_tokens * a.ko + ((int64_t)a.wi * a.spw + blockIdx.x) * (S + 2 * W);
   for (int t = threadIdx.x; t < np + ns * KO; t += blockDim.x) {
-    float sc;
     if (t < np) {
-      crid[t] = det_in_row(a, s0 - W + t, sc);
-      csc[t] = sc;
-      need[t] = 0;
+      const int64_t q = s0 - W + t;
+      const bool in = q >= 0 && q < a.n_tokens;
+      const int sl = __ldg(pslot + t);
+      crid[t] = in ? __ldg(a.in_rid + q) : -1;
+      csc[t] = in ? __ldg(a.in_sc + q) : 1.f;
+      cslot[t] = sl >= 0 ? sl - base : sl;
     } else {
-      const int ck = t - np;
-      orid[ck] = det_out_row(a, s0 + ck / KO, ck % KO, pool_n, sc);
-      osc[ck] = sc;
+      const int ck = t - np, k = ck % KO;
+      const int64_t e = (s0 + ck / KO) * a.ko + k;
+      orid[ck] = k < a.ko ? __ldg(a.out_rid + e) : -1;
+      osc[ck] = k < a.ko ? __ldg(a.out_sc + e) : 1.f;
     }
   }
+  const int64_t p = s0 + c;
+  const int2 cx = c < ns ? __ldg(a.chw + p) : make_int2(0, 0);
+  const uint32_t ctx = (uint32_t)cx.x;                    // lane l <-> offset l - hw, staged position c + W + l - hw
+  const int hw = cx.y;
+  int oslot = -2;                                         // this lane's (centre, k = lane)
+  if (ctx && lane < a.ko) {
+    oslot = __ldg(a.slot + p * a.ko + lane);
+    if (oslot >= 0) oslot -= base;
+  }
   for (int e = threadIdx.x; e < np * dim; e += blockDim.x) hacc[e] = 0ull;
-  // the next wave's readers are counted from zero by this wave's apply
-  if (blockIdx.x == 0 && threadIdx.x == 0) a.own_next.n[0] = a.own_next.n[1] = 0;
   __syncthreads();
 
-  // ---- this warp's centre: window (ParseSentence), lane l <-> offset l - hw, staged position c + W + l - hw ----
-  const int64_t p = s0 + c;
-  const bool on = c < ns && orid[c * KO] >= 0;        // a break or an unmapped centre trains nothing
-  const int rid = on && lane < KO ? orid[c * KO + lane] : -1;
+  const int rid = ctx && lane < KO ? orid[c * KO + lane] : -1;
   const uint32_t used = __ballot_sync(0xffffffffu, rid >= 0);
-  const int hw = W - (int)((hash64(a.seed ^ (uint64_t)(p + 1) * 0x9E3779B97F4A7C15ull) >> 16) % (uint64_t)W);
-  uint32_t ctx = 0;
-  if (on) {
-    const uint32_t isnull =
-        __ballot_sync(0xffffffffu, lane <= 2 * hw && lane != hw && crid[c + W + lane - hw] < 0);
-    const uint32_t left_null = isnull & ((1u << hw) - 1u);
-    const int lo = left_null ? (32 - __clz(left_null)) : 0;
-    const uint32_t right_null = isnull >> (hw + 1);
-    const int hi = right_null ? (hw + __ffs(right_null) - 1) : 2 * hw;
-    ctx = (((hi >= 31) ? 0xffffffffu : ((1u << (hi + 1)) - 1u)) & ~((1u << lo) - 1u)) & ~(1u << hw);
-  }
-  if ((ctx >> lane) & 1u) need[c + W + lane - hw] = 1;   // every writer stores the same value
   // output rows this (centre, k) alone reads in the wave: applied in place after phase 2
-  const uint32_t owned = __ballot_sync(0xffffffffu, a.counted && rid >= 0 && a.own.cnt[1][rid] == 1);
-  if (ctx && ((used & ~owned) >> lane) & 1u) det_touch(a, 1, rid);
+  const uint32_t owned = __ballot_sync(0xffffffffu, rid >= 0 && oslot == -1);
   float O[KO][NJ];
 #pragma unroll
   for (int k = 0; k < KO; ++k) {
     const int r = __shfl_sync(0xffffffffu, rid, k);
-    det_load(O[k], a.w_out + (int64_t)(r < 0 ? 0 : r) * a.ld, dim, lane, ctx && ((used >> k) & 1u));
+    det_load(O[k], a.w_out + (int64_t)(r < 0 ? 0 : r) * a.ld, dim, lane, (used >> k) & 1u);
   }
-  __syncthreads();
 
   // ---- stage the input rows that are a context of some centre of the slice ----------------------------------
   for (int i = c; i < np; i += S) {
-    if (!need[i]) continue;
+    if (cslot[i] < -1) continue;
     float h[NJ];
     det_load(h, a.w_in + (int64_t)crid[i] * a.ld, dim, lane, true);
 #pragma unroll
@@ -847,24 +999,23 @@ sgns_det_kernel(const __grid_constant__ DetDev a) {
     if (d != 0) __syncthreads();
   }
 
-  // ---- flush: one row of REDs per staged position that is a context (halo rows carry partial sums) ---------
+  // ---- flush: one row per staged position that is a context (halo rows carry partial sums) ------------------
   for (int i = c; i < np; i += S) {
-    if (!need[i]) continue;
-    const int r = crid[i];
-    if (a.counted && a.own.cnt[0][r] == 1) {          // no other staged position holds the row: apply in place
-      float* row = a.w_in + (int64_t)r * a.ld;
+    const int sl = cslot[i];
+    if (sl < -1) continue;
+    if (sl == -1) {                                   // no other staged position reads the row: apply in place
+      float* row = a.w_in + (int64_t)crid[i] * a.ld;
       for (int j = lane; j < dim; j += 32) {
         const long long v = (long long)hacc[(size_t)i * dim + j];
         if (v) row[j] = det_fix_add(hrow[(size_t)i * dim + j], v);
       }
       continue;
     }
-    unsigned long long* dst = a.acc[0] + (int64_t)r * dim;
+    unsigned long long* dst = a.acc + (int64_t)sl * dim;
     for (int j = lane; j < dim; j += 32) {
       const unsigned long long v = hacc[(size_t)i * dim + j];
       if (v) atomicAdd(dst + j, v);
     }
-    if (lane == 0) det_touch(a, 0, r);
   }
 
   // ---- phase 2: output-row deltas sum_c g_ck * in_c in registers, one row of REDs per (centre, k) -----------
@@ -886,12 +1037,12 @@ sgns_det_kernel(const __grid_constant__ DetDev a) {
     }
 #pragma unroll
     for (int k = 0; k < KO; ++k) {
+      const int sl = __shfl_sync(0xffffffffu, oslot, k);
       if (!((used >> k) & 1u)) continue;
-      const int r = orid[c * KO + k];
       if ((owned >> k) & 1u) {
         // the row as the wave found it (nothing else reads or writes it in this wave) plus the one term its
         // fixed-point sum would hold; zero terms leave the element untouched, as in the apply
-        float* row = a.w_out + (int64_t)r * a.ld;
+        float* row = a.w_out + (int64_t)orid[c * KO + k] * a.ld;
         float x[NJ];
 #pragma unroll
         for (int u = 0; u < NJ; ++u) x[u] = lane + 32 * u < dim ? row[lane + 32 * u] : 0.f;
@@ -902,7 +1053,7 @@ sgns_det_kernel(const __grid_constant__ DetDev a) {
         }
         continue;
       }
-      unsigned long long* dst = a.acc[1] + (int64_t)r * dim;
+      unsigned long long* dst = a.acc + (int64_t)sl * dim;
 #pragma unroll
       for (int u = 0; u < NJ; ++u)
         if (lane + 32 * u < dim) atomicAdd(dst + lane + 32 * u, (unsigned long long)__float2ll_rn(O[k][u] * kFixScale));
@@ -914,55 +1065,22 @@ sgns_det_kernel(const __grid_constant__ DetDev a) {
   }
 }
 
-// Adds each touched row's sum to its table and clears it, a warp per listed row (input rows, then output rows);
-// resets this wave's reader counts and counts the next wave's readers: per row of the output table its
-// (centre, k), per row of the input table its staged (CTA, position), a halo position once per CTA that stages
-// it; resets the NEXT wave's (idle) counters and rolls the wave's loss into loss_sum.
+// Adds each shared row's sum to its table and clears its slot, a warp per entry of the wave's list; rolls the
+// wave's loss into loss_sum.
 __global__ void __launch_bounds__(256)
 sgns_det_apply(const __grid_constant__ DetDev a) {
-  const int tid = blockIdx.x * blockDim.x + threadIdx.x, nthreads = gridDim.x * blockDim.x;
-  // listed rows go to the first warps and the counts to the last threads, so their latencies overlap
-  const int ctid = nthreads - 1 - tid;
-  if (a.counted) {
-    const int n0 = a.own.n[0], n01 = n0 + a.own.n[1];
-    for (int e = ctid; e < n01; e += nthreads) {
-      const int t = e < n0 ? 0 : 1;
-      a.own.cnt[t][a.own.list[t][e - (t ? n0 : 0)]] = 0;
-    }
-  }
-  if (a.p2 > a.p1) {
-    const int pool_n = a.neg_pool_size_ptr ? __ldg(a.neg_pool_size_ptr) : a.neg_pool_size;
-    const int W = a.window, span = a.S + 2 * W;
-    const int64_t n_out = (a.p2 - a.p1) * a.ko, n_slices = (a.p2 - a.p1 + a.S - 1) / a.S;
-    for (int64_t e = ctid; e < n_out + n_slices * span; e += nthreads) {
-      int t, r;
-      float sc;
-      if (e < n_out) {
-        t = 1;
-        r = det_out_row(a, a.p1 + e / a.ko, (int)(e % a.ko), pool_n, sc);
-      } else {
-        t = 0;
-        const int64_t s0 = a.p1 + (e - n_out) / span * a.S;     // the slice's first centre
-        const int i = (int)((e - n_out) % span);
-        r = (i < (a.p2 - s0 < a.S ? a.p2 - s0 : a.S) + 2 * W) ? det_in_row(a, s0 - W + i, sc) : -1;
-      }
-      if (r >= 0 && atomicAdd(a.own_next.cnt[t] + r, 1) == 0) a.own_next.list[t][atomicAdd(a.own_next.n + t, 1)] = r;
-    }
-  }
+  const int tid = blockIdx.x * blockDim.x + threadIdx.x;
+  const int base = a.off[a.wi], n = a.off[a.wi + 1] - base;
   float* __restrict__ w_in = a.w_in;
   float* __restrict__ w_out = a.w_out;
-  unsigned long long* __restrict__ acc_in = a.acc[0];
-  unsigned long long* __restrict__ acc_out = a.acc[1];
   const int dim = a.dim;
   const int64_t ld = a.ld;
   const int lane = threadIdx.x & 31;
-  const int n_in = a.count[0], n_all = n_in + a.count[1];
   const int nwarps = (gridDim.x * blockDim.x) >> 5;
-  for (int w = tid >> 5; w < n_all; w += nwarps) {
-    const bool in = w < n_in;
-    const int r = in ? a.list[0][w] : a.list[1][w - n_in];
-    unsigned long long* q = (in ? acc_in : acc_out) + (int64_t)r * dim;
-    float* row = (in ? w_in : w_out) + (int64_t)r * ld;
+  for (int w = tid >> 5; w < n; w += nwarps) {
+    const unsigned e = a.list[base + w];
+    unsigned long long* q = a.acc + (int64_t)w * dim;
+    float* row = ((e >> 31) ? w_out : w_in) + (int64_t)(e & 0x7fffffffu) * ld;
     for (int j0 = 0; j0 < dim; j0 += 128) {          // 4 elements per lane in flight
       long long v[4];
       float x[4];
@@ -980,10 +1098,8 @@ sgns_det_apply(const __grid_constant__ DetDev a) {
         q[j] = 0ull;
       }
     }
-    if (lane == 0) a.flag[in ? 0 : 1][r] = 0;
   }
   if (tid == 0) {
-    a.count_next[0] = a.count_next[1] = 0;
     if (a.loss_sum && *a.loss_acc)
       *a.loss_sum += (float)((double)(long long)*a.loss_acc * (1.0 / (double)kLossScale));
     *a.loss_acc = 0ull;
@@ -1097,56 +1213,21 @@ extern "C" int mvb_sgns_train_win(const MvbSgns* h, void* stream) {
 
 extern int mvb_sgns_launches;
 // Deterministic K7 on local tables or block caches; -20/-21: not covered (the caller falls back); -22: one centre's
-// slice does not fit the shared memory (not reached on an H100 for dim <= 512, window <= 15).
+// slice does not fit the shared memory (not reached on an H100 for dim <= 512, window <= 15), or the call has more
+// than 2^31 - 1 readers (some 250M tokens).
 extern "C" int mvb_sgns_train_det(const MvbSgns* h, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   if (h->n_tokens <= 0) return 0;
   if (h->cbow || h->hs || h->use_adagrad || h->negative < 1 || h->negative > kKO - 1) return -20;
   if (h->nservers > 1 || h->dim < 1 || h->dim > 512 || h->window < 1 || h->window > 15 || h->vocab <= 0) return -21;
   mvb_sgns_launches = 0;
-  // rows are word ids or cache slots (< vocab).  Scratch (one stream): counters [4] | listed rows of the reader
-  // counts [2 parities x 2] | loss | acc [2 x rows x dim] | flags, lists [2 x rows] | reader counts, their lists
-  // [2 parities x 2 x rows]; grown on demand, cleared when its layout changes (a wave leaves it clear but for
-  // counters, and a call leaves every reader count zero)
-  static unsigned char* buf = nullptr;
-  static int64_t cap = 0, last_elems = -1;
-  static int parity = 0;
-  const int64_t rows = h->vocab, elems = rows * h->dim, bytes = 32 + 8 + 2 * elems * 8 + 12 * rows * 4;
-  if (bytes > cap) {
-    MVB_CUDA_CHECK(cudaDeviceSynchronize());
-    if (buf) MVB_CUDA_CHECK(cudaFree(buf));
-    MVB_CUDA_CHECK(cudaMalloc(&buf, bytes));
-    cap = bytes;
-    last_elems = -1;
-  }
-  if (elems != last_elems) {
-    MVB_CUDA_CHECK(cudaMemsetAsync(buf, 0, bytes, st));
-    last_elems = elems;
-    parity = 0;
-  }
-  int* counters = reinterpret_cast<int*>(buf);
-  unsigned long long* loss_acc = reinterpret_cast<unsigned long long*>(buf + 32);
-  unsigned long long* acc = loss_acc + 1;
-  int* ints = reinterpret_cast<int*>(acc + 2 * elems);
-  DetOwn own[2];                                  // by wave parity within the call
-  for (int q = 0; q < 2; ++q) {
-    for (int t = 0; t < 2; ++t) {
-      own[q].cnt[t] = ints + (4 + 2 * q + t) * rows;
-      own[q].list[t] = ints + (8 + 2 * q + t) * rows;
-    }
-    own[q].n = counters + 4 + 2 * q;
-  }
   DetDev a{};
   a.tokens = h->tokens; a.n_tokens = h->n_tokens; a.w_in = h->w_in; a.w_out = h->w_out;
   a.dim = h->dim; a.ld = h->ld; a.window = h->window; a.ko = 1 + h->negative; a.lr = h->lr;
   a.alias_prob = h->alias_prob; a.alias_idx = h->alias_idx; a.vocab = h->vocab;
   a.neg_pool = h->neg_pool; a.neg_pool_size = h->neg_pool_size; a.neg_pool_size_ptr = h->neg_pool_size_ptr;
   a.map_in = h->map_in; a.map_out = h->map_out; a.scale_in = h->scale_in; a.scale_out = h->scale_out;
-  a.seed = h->seed; a.want_loss = h->loss_sum != nullptr; a.pair_count = h->pair_count;
-  a.acc[0] = acc; a.acc[1] = acc + elems;
-  a.flag[0] = ints; a.flag[1] = ints + rows;
-  a.list[0] = ints + 2 * rows; a.list[1] = ints + 3 * rows;
-  a.loss_acc = loss_acc; a.loss_sum = h->loss_sum;
+  a.seed = h->seed; a.want_loss = h->loss_sum != nullptr; a.pair_count = h->pair_count; a.loss_sum = h->loss_sum;
   int wave = mvb_sgns_win_inflight(h->dim, h->negative, h->window, h->max_ctas);
   if (wave <= 0) wave = 2 * mvb_num_sms() * kNW;
   // the <NJ, KO> instance, and as many centres per CTA as its registers and the opt-in shared memory allow
@@ -1173,22 +1254,95 @@ extern "C" int mvb_sgns_train_det(const MvbSgns* h, void* stream) {
   const size_t smem = det_smem_bytes(S, h->window, h->dim, ko);
   if (smem > (size_t)max_smem) return -22;
   MVB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  const int apply_blocks = mvb_num_sms() * 4;
+
+  // ---- the plan's shape: readers of every wave, sort key width, shared rows a wave can have -----------------
+  const int64_t N = h->n_tokens, span = S + 2 * h->window;
   a.S = S;
-  // the first wave has no reader counts and sends every row through the accumulator; the last one counts none,
-  // so the call leaves every count zero
-  for (int64_t p0 = 0, w = 0; p0 < h->n_tokens; p0 += wave, ++w) {
+  a.wave = wave;
+  a.n_waves = (int)((N + wave - 1) / wave);
+  a.spw = (wave + S - 1) / S;
+  a.n_readers = N * a.ko + (int64_t)a.n_waves * a.spw * span;
+  if (a.n_readers > INT32_MAX) return -22;
+  const int n_readers = (int)a.n_readers, n_tiles = (n_readers + kPlanTile - 1) / kPlanTile;
+  const unsigned long long none = (unsigned long long)a.n_waves * 2 * (unsigned long long)h->vocab;
+  int end_bit = 1;
+  while (end_bit < 64 && (none >> end_bit) != 0) ++end_bit;
+  // a shared row has two readers or more in its wave
+  const int64_t max_shared = ((int64_t)wave * a.ko + (int64_t)a.spw * span) / 2;
+
+  // ---- scratch (one stream), grown on demand: loss | acc | plan arrays | sort buffers | sort temp.  The
+  // accumulator is left clear by every wave's apply, so it is only cleared where it grows into bytes that held
+  // something else.
+  static unsigned char* buf = nullptr;
+  static size_t cap = 0, clear = 0;
+  const auto up = [](size_t x) { return (x + 255) / 256 * 256; };
+  const size_t R = (size_t)n_readers, NK = (size_t)N * a.ko;
+  cub::DoubleBuffer<unsigned long long> keys(nullptr, nullptr);
+  cub::DoubleBuffer<sgns_det_plan_reader> vals(nullptr, nullptr);
+  size_t sort_bytes = 0;
+  MVB_CUDA_CHECK(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, keys, vals, n_readers, 0, end_bit, st));
+  size_t o = 0;
+  const size_t o_loss = o;   o = up(o + 8);
+  const size_t o_acc = o;    o = up(o + (size_t)max_shared * h->dim * 8);
+  const size_t acc_end = o;
+  const size_t o_in = o;     o = up(o + (size_t)N * 8);                 // in_rid, in_sc
+  const size_t o_out = o;    o = up(o + NK * 8);                        // out_rid, out_sc
+  const size_t o_chw = o;    o = up(o + (size_t)N * 8);
+  const size_t o_slot = o;   o = up(o + R * 4);
+  const size_t o_list = o;   o = up(o + R / 2 * 4);
+  const size_t o_off = o;    o = up(o + ((size_t)a.n_waves + 1) * 4);
+  const size_t o_tile = o;   o = up(o + (size_t)n_tiles * 4);
+  const size_t o_keys = o;   o = up(o + 2 * R * 8);
+  const size_t o_vals = o;   o = up(o + 2 * R * 4);
+  const size_t o_temp = o;   o = up(o + sort_bytes);
+  if (o > cap) {
+    MVB_CUDA_CHECK(cudaDeviceSynchronize());
+    if (buf) MVB_CUDA_CHECK(cudaFree(buf));
+    MVB_CUDA_CHECK(cudaMalloc(&buf, o));
+    cap = o;
+    clear = 0;
+  }
+  if (acc_end > clear) MVB_CUDA_CHECK(cudaMemsetAsync(buf, 0, acc_end, st));
+  clear = acc_end;                                // the plan arrays overwrite whatever lies beyond
+  a.loss_acc = reinterpret_cast<unsigned long long*>(buf + o_loss);
+  a.acc = reinterpret_cast<unsigned long long*>(buf + o_acc);
+  a.in_rid = reinterpret_cast<int*>(buf + o_in);
+  a.in_sc = reinterpret_cast<float*>(a.in_rid + N);
+  a.out_rid = reinterpret_cast<int*>(buf + o_out);
+  a.out_sc = reinterpret_cast<float*>(a.out_rid + NK);
+  a.chw = reinterpret_cast<int2*>(buf + o_chw);
+  a.slot = reinterpret_cast<int*>(buf + o_slot);
+  a.list = reinterpret_cast<unsigned*>(buf + o_list);
+  a.off = reinterpret_cast<int*>(buf + o_off);
+  a.tile_off = reinterpret_cast<int*>(buf + o_tile);
+  keys = cub::DoubleBuffer<unsigned long long>(reinterpret_cast<unsigned long long*>(buf + o_keys),
+                                               reinterpret_cast<unsigned long long*>(buf + o_keys) + R);
+  vals = cub::DoubleBuffer<sgns_det_plan_reader>(reinterpret_cast<sgns_det_plan_reader*>(buf + o_vals),
+                                                 reinterpret_cast<sgns_det_plan_reader*>(buf + o_vals) + R);
+
+  // ---- the plan: rows, windows and reader keys; sort; slots, shared rows and wave offsets ------------------
+  const auto grid = [](int64_t n) { return (int)((n + kPlanThreads - 1) / kPlanThreads); };
+  a.key = keys.Current();
+  a.reader = vals.Current();
+  sgns_det_plan_tokens<<<grid(N), kPlanThreads, 0, st>>>(a);
+  sgns_det_plan_centres<<<grid(N), kPlanThreads, 0, st>>>(a);
+  sgns_det_plan_staged<<<grid(a.n_readers - (int64_t)NK), kPlanThreads, 0, st>>>(a);
+  MVB_CUDA_CHECK(cub::DeviceRadixSort::SortPairs(buf + o_temp, sort_bytes, keys, vals, n_readers, 0, end_bit, st));
+  a.key = keys.Current();
+  a.reader = vals.Current();
+  sgns_det_plan_runs<<<n_tiles, kPlanThreads, 0, st>>>(a);
+  sgns_det_plan_scan<<<1, 1024, 0, st>>>(a.tile_off, n_tiles);
+  sgns_det_plan_slots<<<n_tiles, kPlanThreads, 0, st>>>(a);
+  mvb_sgns_launches = 6;     // the plan's own kernels (the radix sort launches its own)
+
+  // ---- the waves ------------------------------------------------------------------------------------------
+  const int apply_blocks = mvb_num_sms() * 4;
+  for (int64_t p0 = 0, w = 0; p0 < N; p0 += wave, ++w) {
     a.p0 = p0;
-    a.p1 = p0 + wave < h->n_tokens ? p0 + wave : h->n_tokens;
-    a.p2 = a.p1 + wave < h->n_tokens ? a.p1 + wave : h->n_tokens;
-    a.count = counters + 2 * parity;
-    a.count_next = counters + 2 * (parity ^ 1);
-    a.counted = w > 0;
-    a.own = own[w & 1];
-    a.own_next = own[(w & 1) ^ 1];
+    a.p1 = p0 + wave < N ? p0 + wave : N;
+    a.wi = (int)w;
     kern<<<(int)((a.p1 - p0 + S - 1) / S), 32 * S, smem, st>>>(a);
     sgns_det_apply<<<apply_blocks, 256, 0, st>>>(a);
-    parity ^= 1;
     mvb_sgns_launches += 2;
   }
   MVB_CUDA_CHECK(cudaGetLastError());
