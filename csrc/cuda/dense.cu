@@ -260,10 +260,6 @@ bool aligned16(const void* p) {
   return (reinterpret_cast<uintptr_t>(p) & 15) == 0;
 }
 
-// bulk-copy-engine variant of K1 (defined below, next to the bulk Get it shares its helpers with)
-template <int UPD>
-int launch_add_bulk(const DenseAddDev<float>& a, cudaStream_t st);
-
 template <int UPD, typename T>
 int launch_add(const MvbDenseAdd* h, cudaStream_t st) {
   DenseAddDev<T> a{};
@@ -316,13 +312,6 @@ int launch_add(const MvbDenseAdd* h, cudaStream_t st) {
   int64_t cap = (int64_t)mvb_num_sms() * 4;
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
-  if constexpr (std::is_same<T, float>::value) {
-    // peer pulls on the bulk-copy engine (opt-in until measured everywhere: MVB_ADD_BULK=1)
-    static const int bulk_env = [] { const char* e = getenv("MVB_ADD_BULK"); return e ? atoi(e) : 0; }();
-    if (bulk_env >= 1 && vec_ok && a.delta_mc == nullptr && !a.has_replica && a.W > 1 &&
-        (bulk_env == 2 || h->shard_len * (int64_t)sizeof(T) >= (int64_t)(4 << 20)))     // 2: always (tests)
-      return launch_add_bulk<UPD>(a, st);
-  }
   if (vec_ok)
     add_dense_fused_kernel<UPD, T, VEC><<<(int)blocks, threads, 0, st>>>(a);
   else
@@ -418,184 +407,6 @@ __global__ void __launch_bounds__(256) get_dense_kernel(const __grid_constant__ 
 // ---------------------------------------------------------------------------
 constexpr int kBulkStages = 6;
 constexpr uint32_t kBulkChunk = 32 * 1024;
-
-// ---------------------------------------------------------------------------
-// K1, bulk-copy variant: the owner pulls its tile of EVERY worker's staging buffer with cp.async.bulk
-// (peer HBM -> shared memory, ~190 KB in flight per SM, no registers on the transfer path), four compute warps
-// sum the W copies out of shared memory, run the updater once per worker in worker order and write shard + state.
-// Same handshake, option boxes and finished-worker mask as add_dense_fused_kernel.
-// ---------------------------------------------------------------------------
-constexpr int kAddChunk = 4096;          // bytes of the shard per chunk (x W worker copies per stage)
-constexpr int kAddComputeWarps = 4;
-constexpr int kAddSlots = MVB_MAX_RANKS + 1;   // W worker copies + the owner's current shard chunk (prefetched too:
-                                               // with 128 compute threads per SM a dependent shard load per float4
-                                               // would bound the kernel by latency)
-
-template <int UPD>
-__global__ void __launch_bounds__(32 * (1 + kAddComputeWarps), 1)
-add_dense_bulk_kernel(const __grid_constant__ DenseAddDev<float> a, int stages) {
-  using U = Updater<UPD, float>;
-  extern __shared__ __align__(128) unsigned char ring[];
-  __shared__ uint64_t full[8], empty[8];
-  __shared__ unsigned int smask;
-  __shared__ MvbAddOpt sopt[MVB_MAX_RANKS];
-  if (threadIdx.x == 0) smask = a.mask;
-  if (threadIdx.x < MVB_MAX_RANKS) sopt[threadIdx.x] = a.opts[threadIdx.x];
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < stages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], kAddComputeWarps); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
-  if (a.has_pads) {
-    if (blockIdx.x == 0 && a.is_worker && threadIdx.x < a.world) {
-      if (a.opt_box[threadIdx.x] != nullptr && a.my_worker >= 0) {
-        MvbAddOpt mine = a.opts[a.my_worker];
-        a.opt_box[threadIdx.x][(a.epoch & 1) * MVB_MAX_RANKS + a.my_worker] = mine;
-      }
-      fence_sys();
-      uint64_t* slot = reinterpret_cast<uint64_t*>(a.pads.p[threadIdx.x]) + a.ch_ready * MVB_MAX_RANKS + a.me;
-      st_release_sys_u64(slot, a.epoch);
-    }
-    if (threadIdx.x < a.W && ((a.mask >> threadIdx.x) & 1u)) {
-      const uint64_t* slot = reinterpret_cast<const uint64_t*>(a.pads.p[a.me]) +
-                             a.ch_ready * MVB_MAX_RANKS + a.worker_rank[threadIdx.x];
-      if (!spin_wait_ge(slot, a.epoch, a.budget)) { if (a.err) atomicExch(a.err, 3000 + threadIdx.x); }
-      if (ld_acquire_sys_u64(slot) >= MVB_EPOCH_FIN) atomicAnd(&smask, ~(1u << threadIdx.x));
-      else if (a.opt_box[a.me] != nullptr) {
-        const volatile int* src = reinterpret_cast<const volatile int*>(
-            a.opt_box[a.me] + (a.epoch & 1) * MVB_MAX_RANKS + threadIdx.x);
-        int* dst = reinterpret_cast<int*>(&sopt[threadIdx.x]);
-#pragma unroll
-        for (int k = 0; k < (int)(sizeof(MvbAddOpt) / 4); ++k) dst[k] = src[k];
-        sopt[threadIdx.x].worker_id = threadIdx.x;
-      }
-    }
-    __syncthreads();
-  }
-  const unsigned int mask = smask;
-  if (a.fin_flag && blockIdx.x == 0 && threadIdx.x == 0 && mask == 0) *a.fin_flag = 1;
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int64_t body = (a.shard_len / 4) * 16;                          // bytes handled in 16-byte units
-  const int64_t n_chunks = (body + kAddChunk - 1) / kAddChunk;
-  const int64_t mine = n_chunks > blockIdx.x ? (n_chunks - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
-  const int nact = __popc(mask & ((1u << a.W) - 1u));
-  if (warp == 0) {
-    // -------- producer: lane w pulls worker w's copy of the chunk --------
-    for (int64_t j = 0; j < mine; ++j) {
-      const int st = (int)(j % stages);
-      const int64_t off = (blockIdx.x + j * gridDim.x) * (int64_t)kAddChunk;
-      const uint32_t len = (uint32_t)((body - off) < kAddChunk ? (body - off) : kAddChunk);
-      if (lane == 0) {
-        mbar_wait(&empty[st], (uint32_t)(((j / stages) & 1) ^ 1));
-        mbar_arrive_expect_tx(&full[st], len * (uint32_t)(nact + 1));
-      }
-      __syncwarp();
-      if (lane < a.W && ((mask >> lane) & 1u))
-        bulk_g2s(ring + ((size_t)st * kAddSlots + lane) * kAddChunk,
-                 reinterpret_cast<const char*>(a.delta[lane] + a.shard_off) + off, len, &full[st]);
-      if (lane == MVB_MAX_RANKS)
-        bulk_g2s(ring + ((size_t)st * kAddSlots + MVB_MAX_RANKS) * kAddChunk,
-                 reinterpret_cast<const char*>(a.shard) + off, len, &full[st]);
-    }
-  } else {
-    // -------- compute warps: sum of the W copies + updater + shard / state write --------
-    const int tid = threadIdx.x - 32;
-    for (int64_t j = 0; j < mine; ++j) {
-      const int st = (int)(j % stages);
-      const int64_t off = (blockIdx.x + j * gridDim.x) * (int64_t)kAddChunk;
-      const int len = (int)((body - off) < kAddChunk ? (body - off) : kAddChunk);
-      mbar_wait(&full[st], (uint32_t)((j / stages) & 1));
-      const unsigned char* sb = ring + (size_t)st * kAddSlots * kAddChunk;
-      for (int v = tid; v < len / 16; v += 32 * kAddComputeWarps) {
-        const int64_t i = (off >> 2) + (int64_t)v * 4;                  // element index inside the shard
-        float4 d = *reinterpret_cast<const float4*>(sb + (size_t)MVB_MAX_RANKS * kAddChunk + (size_t)v * 16);
-        float4 s0 = make_float4(0, 0, 0, 0), s1 = make_float4(0, 0, 0, 0);
-        if constexpr (U::kStates >= 1 && !U::kPerWorker) s0 = *reinterpret_cast<const float4*>(a.state0 + i);
-#pragma unroll
-        for (int w = 0; w < MVB_MAX_RANKS; ++w) {
-          if (w < a.W && ((mask >> w) & 1u)) {
-            const float4 g = *reinterpret_cast<const float4*>(sb + (size_t)w * kAddChunk + (size_t)v * 16);
-            if constexpr (U::kPerWorker) {
-              s0 = *reinterpret_cast<const float4*>(a.state0 + (int64_t)w * a.state_stride + i);
-              if constexpr (U::kStates >= 2) s1 = *reinterpret_cast<const float4*>(a.state1 + (int64_t)w * a.state_stride + i);
-            }
-            U::Apply(d.x, prep_delta<float>(g.x, a.scale, a.clip), s0.x, s1.x, sopt[w]);
-            U::Apply(d.y, prep_delta<float>(g.y, a.scale, a.clip), s0.y, s1.y, sopt[w]);
-            U::Apply(d.z, prep_delta<float>(g.z, a.scale, a.clip), s0.z, s1.z, sopt[w]);
-            U::Apply(d.w, prep_delta<float>(g.w, a.scale, a.clip), s0.w, s1.w, sopt[w]);
-            if constexpr (U::kPerWorker) {
-              *reinterpret_cast<float4*>(a.state0 + (int64_t)w * a.state_stride + i) = s0;
-              if constexpr (U::kStates >= 2) *reinterpret_cast<float4*>(a.state1 + (int64_t)w * a.state_stride + i) = s1;
-            }
-          }
-        }
-        if constexpr (U::kStates >= 1 && !U::kPerWorker) *reinterpret_cast<float4*>(a.state0 + i) = s0;
-        *reinterpret_cast<float4*>(a.shard + i) = d;
-      }
-      __syncwarp();
-      if (lane == 0) {
-        mbar_arrive(&empty[st]);
-      }
-    }
-    // scalar tail (shard_len % 4): first compute threads of block 0
-    if (blockIdx.x == 0) {
-      for (int64_t i = (a.shard_len / 4) * 4 + tid; i < a.shard_len; i += 32 * kAddComputeWarps) {
-        float d = a.shard[i], s0 = 0.f, s1 = 0.f;
-        if constexpr (U::kStates >= 1 && !U::kPerWorker) s0 = a.state0[i];
-        for (int w = 0; w < a.W; ++w) {
-          if (!((mask >> w) & 1u)) continue;
-          if constexpr (U::kPerWorker) {
-            s0 = a.state0[(int64_t)w * a.state_stride + i];
-            if constexpr (U::kStates >= 2) s1 = a.state1[(int64_t)w * a.state_stride + i];
-          }
-          U::Apply(d, prep_delta<float>(__ldg(a.delta[w] + a.shard_off + i), a.scale, a.clip), s0, s1, sopt[w]);
-          if constexpr (U::kPerWorker) {
-            a.state0[(int64_t)w * a.state_stride + i] = s0;
-            if constexpr (U::kStates >= 2) a.state1[(int64_t)w * a.state_stride + i] = s1;
-          }
-        }
-        if constexpr (U::kStates >= 1 && !U::kPerWorker) a.state0[i] = s0;
-        a.shard[i] = d;
-      }
-    }
-  }
-  // ---- fused "Reply_Add": last CTA publishes ch_done to every rank ------------
-  if (a.has_pads) {
-    __shared__ int is_last;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      __threadfence();
-      unsigned int prev = atomicAdd(a.done_counter, 1u);
-      is_last = (prev == gridDim.x - 1);
-      if (is_last) *a.done_counter = 0;
-    }
-    __syncthreads();
-    if (is_last && threadIdx.x < a.world) {
-      fence_sys();
-      uint64_t* slot = reinterpret_cast<uint64_t*>(a.pads.p[threadIdx.x]) + a.ch_done * MVB_MAX_RANKS + a.me;
-      st_release_sys_u64(slot, a.epoch);
-    }
-  }
-}
-
-template <int UPD>
-int launch_add_bulk(const DenseAddDev<float>& a, cudaStream_t st) {
-  int dev = 0, max_smem = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
-  int stages = (max_smem - 2048) / (kAddSlots * kAddChunk);
-  if (stages > 8) stages = 8;
-  if (stages < 2) return -22;
-  const size_t smem = (size_t)stages * kAddSlots * kAddChunk;
-  MVB_CUDA_CHECK(cudaFuncSetAttribute(add_dense_bulk_kernel<UPD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  int blocks = mvb_num_sms();
-  const int64_t n_chunks = ((a.shard_len / 4) * 16 + kAddChunk - 1) / kAddChunk;
-  if ((int64_t)blocks > n_chunks) blocks = (int)(n_chunks > 0 ? n_chunks : 1);
-  add_dense_bulk_kernel<UPD><<<blocks, 32 * (1 + kAddComputeWarps), smem, st>>>(a, stages);
-  MVB_CUDA_CHECK(cudaGetLastError());
-  return 0;
-}
 
 template <typename T>
 __global__ void __launch_bounds__(32) get_dense_bulk_kernel(const __grid_constant__ DenseGetDev<T> g) {

@@ -277,8 +277,6 @@ typedef struct MvbSgns {
   unsigned long long* pair_count;  /* optional: += trained (input,target) samples */
   int hogwild;               /* one device, skip-gram + NS: 0 = deterministic waves, 1 = the Hogwild
                                 window-batched kernel (one centre per warp)                          */
-  int max_ctas;              /* 0 = one CTA per SM; > 0 caps the persistent grid (leaves SMs to the
-                                row pull / push kernels of the pipelined multi-GPU step)            */
   /* optional per-WORD step scales in (0,1] (deterministic and window kernels): caps the summed step of
      the Zipf-head rows that collect more concurrent stale updates than plain SGD tolerates;
      NULL = 1 everywhere                                                                              */
@@ -298,7 +296,7 @@ int mvb_sgns_train(const MvbSgns* a, void* stream);
 int mvb_sgns_train_win(const MvbSgns* a, void* stream);   /* window-batched TMA pipeline      */
 int mvb_sgns_train_det(const MvbSgns* a, void* stream);   /* deterministic waves (default)    */
 int mvb_sgns_last_launches(void);   /* kernel launches of the last mvb_sgns_train call */
-int mvb_sgns_win_inflight(int dim, int negative, int window, int max_ctas);  /* centre positions in flight */
+int mvb_sgns_win_inflight(int dim, int negative, int window);  /* centre positions in flight */
 /* ---- key-addressed shards for application-defined tables (keys.cu): the device-side extension point ---- */
 typedef struct MvbKeyMap {
   int64_t size;                        /* keys 0 .. size-1                                   */
@@ -348,7 +346,7 @@ int mvb_rowbox_apply(const MvbRowBox* b, int updater, float* shard, float* st0, 
                      int64_t state_stride, int64_t row_lo, int src, int ctas_per_sm, void* stream);
 
 /* WordEmbedding block protocol on the device (we_block.cu): PrepareData without a host round trip,
-   row pull / delta push on the bulk-copy engine.  All counts live in device memory. */
+   row pull / delta push in ctas_per_sm (>= 1) register-only CTAs per SM.  All counts live in device memory. */
 typedef struct MvbWePrep {
   const int* tokens;         /* block of word ids, <0 = sentence break                          */
   int64_t n_tokens;
@@ -371,11 +369,11 @@ typedef struct MvbWePrep {
 } MvbWePrep;
 int mvb_we_prepare(const MvbWePrep* p, void* stream);
 int mvb_we_prepare_launches(int negative);      /* kernels + memset/memcpy nodes it enqueues */
-int mvb_rows_pull_bulk(const MvbRowMap* m, int esz, const int* ids, const int* n_ptr, int64_t n_max,
-                       void* dst_a, void* dst_b, int64_t dst_ld, int max_ctas, void* stream);
-int mvb_rows_push_delta_bulk(const MvbRowMap* m, const int* ids, const int* n_ptr, int64_t n_max,
-                             const float* cur, const float* old, int64_t ld, float scale, int max_ctas,
-                             void* stream);
+int mvb_rows_pull(const MvbRowMap* m, int esz, const int* ids, const int* n_ptr, int64_t n_max,
+                  void* dst_a, void* dst_b, int64_t dst_ld, int ctas_per_sm, void* stream);
+int mvb_rows_push_delta(const MvbRowMap* m, const int* ids, const int* n_ptr, int64_t n_max,
+                        const float* cur, const float* old, int64_t ld, float scale, int ctas_per_sm,
+                        void* stream);
 int mvb_build_alias_table(const double* weights_host, int n, float* prob_host, int* alias_host);
 
 /* ---- LogisticRegression (K8) ---------------------------------------------------- */

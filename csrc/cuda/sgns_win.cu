@@ -1110,7 +1110,7 @@ sgns_det_apply(const __grid_constant__ DetDev a) {
 
 // Centre positions the window-batched kernel keeps in flight on this device (every consumer warp owns
 // a double-buffered stage): the staleness window the hot-row step cap is computed from.
-extern "C" int mvb_sgns_win_inflight(int dim, int negative, int window, int max_ctas) {
+extern "C" int mvb_sgns_win_inflight(int dim, int negative, int window) {
   int dev = 0, max_smem = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
@@ -1118,9 +1118,7 @@ extern "C" int mvb_sgns_win_inflight(int dim, int negative, int window, int max_
   for (; nw >= 2; --nw)
     if (make_layout(2 * nw + 2 * window + 2, nw, 1 + negative, dim * 4).total <= max_smem) break;
   if (nw < 2) return 0;
-  int blocks = mvb_num_sms();
-  if (max_ctas > 0 && max_ctas < blocks) blocks = max_ctas;
-  return blocks * nw * 2;
+  return mvb_num_sms() * nw * 2;
 }
 
 // Window-batched K7. Returns -20/-21 for configurations it does not cover, -22 when the rows
@@ -1167,7 +1165,6 @@ extern "C" int mvb_sgns_train_win(const MvbSgns* h, void* stream) {
   if (nw < 2) return -22;
   a.nw = nw;
   int blocks = mvb_num_sms();
-  if (h->max_ctas > 0 && h->max_ctas < blocks) blocks = h->max_ctas;
   // tiny inputs use fewer CTAs (>= 64 positions each)
   const int64_t by_len = (h->n_tokens + 63) / 64;
   if ((int64_t)blocks > by_len) blocks = (int)by_len;
@@ -1228,7 +1225,7 @@ extern "C" int mvb_sgns_train_det(const MvbSgns* h, void* stream) {
   a.neg_pool = h->neg_pool; a.neg_pool_size = h->neg_pool_size; a.neg_pool_size_ptr = h->neg_pool_size_ptr;
   a.map_in = h->map_in; a.map_out = h->map_out; a.scale_in = h->scale_in; a.scale_out = h->scale_out;
   a.seed = h->seed; a.want_loss = h->loss_sum != nullptr; a.pair_count = h->pair_count; a.loss_sum = h->loss_sum;
-  int wave = mvb_sgns_win_inflight(h->dim, h->negative, h->window, h->max_ctas);
+  int wave = mvb_sgns_win_inflight(h->dim, h->negative, h->window);
   if (wave <= 0) wave = 2 * mvb_num_sms() * kNW;
   // the <NJ, KO> instance, and as many centres per CTA as its registers and the opt-in shared memory allow
   void (*kern)(DetDev) = nullptr;

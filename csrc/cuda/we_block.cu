@@ -13,14 +13,12 @@
 //                      drawn on the device from the unigram^0.75 alias table with a hash RNG, its words are
 //                      OR-ed into the output bitmap, second scan.  Counts stay on the device; every later
 //                      kernel reads them there, so nothing ever synchronises with the host.
-//   mvb_rows_pull_bulk row gather over NVLink on the bulk-copy engine: one warp per CTA, 32 rows per
-//                      mbarrier batch, cp.async.bulk peer HBM -> smem, then smem -> the block cache AND its
-//                      "pulled" copy (what clone() did) with bulk stores; ~190 KB in flight per SM, so a
-//                      handful of SMs saturates the link while K7 keeps the rest.
-//   mvb_rows_push_delta_bulk   (trained - pulled) * scale per row computed in smem by 4 warps, pushed into
-//                      the owner's shard with cp.reduce.async.bulk.add.f32 (one-sided, element-wise atomic
-//                      at the owner's L2: the async-PS Add for stateless updaters); untouched rows skipped.
-#include <cstdlib>
+//   mvb_rows_pull      row gather from the owners' shards (over NVLink for peer shards) into the block cache
+//                      AND its "pulled" copy (what clone() did): a warp per row, 128-bit loads and stores.
+//   mvb_rows_push_delta   (trained - pulled) * scale per row, reduced into the owner's shard with one-sided
+//                      red.add.v4.f32 (element-wise atomic at the owner: the async-PS Add for stateless
+//                      updaters); all-zero 16-byte deltas are skipped.
+// Pull and push run ctas_per_sm register-only CTAs per SM, co-resident with the persistent K7 (see below).
 #include "mvb_common.cuh"
 
 namespace {
@@ -168,7 +166,7 @@ prep_neg_pool_kernel(const int* __restrict__ n_in_ptr, int negative, int vocab, 
 }
 
 // ------------------------------------------------------------------------------------------------
-// row pull / delta push on the bulk-copy engine
+// row pull / delta push
 // ------------------------------------------------------------------------------------------------
 struct RowMapDev {
   int64_t num_row, rps;
@@ -184,112 +182,14 @@ MVB_DEVINL unsigned char* row_addr(const RowMapDev& m, int64_t r) {
 
 struct PullDev {
   RowMapDev m;
-  const int* ids;          // slot -> row id (ascending: consecutive ids are merged into one bulk copy)
+  const int* ids;          // slot -> row id
   const int* n_ptr;        // device count (nullptr: n_max rows)
   int64_t n_max;
   unsigned char* dst_a;    // [n x dst_ld_bytes]
   unsigned char* dst_b;    // optional second copy
   int64_t dst_ld_bytes;
   int row_bytes;
-  int q;                   // batches in flight
-  int br;                  // rows per batch (32; fewer for rows too large for the shared-memory ring)
 };
-
-// Row runs of one 32-row batch: lane `l` starts a run when its row does not continue lane l-1's
-// (id + 1, same owner).  The bulk engine is op-rate bound for 1.2 KB rows (~27 M ops/s per SM measured),
-// and the sorted id lists of a Zipf block are mostly runs, so merging them is what makes a handful
-// of SMs enough.  Returns the run length for start lanes, 0 otherwise; `hmask` = lanes with a row.
-MVB_DEVINL int row_runs(const RowMapDev& m, int64_t r, bool have, int lane, uint32_t& hmask) {
-  int64_t o = -1;
-  if (have) {
-    o = r / m.rps;
-    if (o > m.S - 1) o = m.S - 1;
-  }
-  const int64_t r_prev = __shfl_up_sync(0xffffffffu, r, 1);
-  const int64_t o_prev = __shfl_up_sync(0xffffffffu, o, 1);
-  const bool start = have && (lane == 0 || r != r_prev + 1 || o != o_prev);
-  hmask = __ballot_sync(0xffffffffu, have);
-  const uint32_t smask = __ballot_sync(0xffffffffu, start);
-  if (!start) return 0;
-  const uint32_t stop = (smask | ~hmask) & ~((2u << lane) - 1u);     // next run start / missing row above me
-  return stop ? (__ffs(stop) - 1 - lane) : (32 - lane);
-}
-
-__global__ void __launch_bounds__(32, 1)
-rows_pull_bulk_kernel(const __grid_constant__ PullDev a) {
-  extern __shared__ __align__(128) unsigned char smem[];
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem);
-  unsigned char* stage = smem + 128;
-  const int lane = threadIdx.x;
-  const int Q = a.q;
-  if (lane == 0) {
-    for (int s = 0; s < Q; ++s) mbar_init(full + s, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncwarp();
-  int64_t n = a.n_ptr ? (int64_t)*a.n_ptr : a.n_max;
-  if (n > a.n_max) n = a.n_max;
-  const int BR = a.br;
-  const int64_t n_batches = (n + BR - 1) / BR;
-  // batches of this CTA: b = blockIdx.x + t * gridDim.x
-  const int64_t mine = n_batches > blockIdx.x ? (n_batches - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
-  const size_t batch_bytes = (size_t)BR * a.row_bytes;
-  const bool dst_contig = a.dst_ld_bytes == a.row_bytes;
-
-  auto batch_row = [&](int64_t t, int64_t& s, int64_t& r) {
-    s = (blockIdx.x + t * gridDim.x) * BR + lane;
-    const bool in = lane < BR && s < n;
-    r = in ? (int64_t)__ldg(a.ids + s) : -1;
-    return in && r >= 0 && r < a.m.num_row;
-  };
-  auto issue_load = [&](int64_t t) {
-    const int q = (int)(t % Q);
-    int64_t s, r;
-    const bool have = batch_row(t, s, r);
-    uint32_t hmask;
-    const int len = row_runs(a.m, r, have, lane, hmask);
-    if (lane == 0) {
-      if (hmask) mbar_arrive_expect_tx(full + q, (uint32_t)__popc(hmask) * (uint32_t)a.row_bytes);
-      else mbar_arrive(full + q);
-    }
-    __syncwarp();
-    if (len > 0)
-      bulk_g2s(stage + q * batch_bytes + (size_t)lane * a.row_bytes, row_addr(a.m, r),
-               (uint32_t)len * (uint32_t)a.row_bytes, full + q);
-  };
-
-  // Q-2 loads in flight; a stage is re-filled two batches after its stores were committed, so the
-  // newest store group may still be reading shared memory (wait_group.read 1)
-  const int64_t pre = mine < Q - 2 ? mine : Q - 2;
-  for (int64_t t = 0; t < pre; ++t) issue_load(t);
-  for (int64_t t = 0; t < mine; ++t) {
-    const int64_t tn = t + Q - 2;
-    if (tn < mine) {
-      bulk_wait_read<1>();      // stage (tn % Q) was stored by batch t-2: its bulk stores have read the rows
-      __syncwarp();
-      issue_load(tn);
-    }
-    const int q = (int)(t % Q);
-    mbar_wait(full + q, (uint32_t)((t / Q) & 1));
-    int64_t s, r;
-    const bool have = batch_row(t, s, r);
-    const uint32_t hmask = __ballot_sync(0xffffffffu, have);
-    const unsigned char* src = stage + q * batch_bytes + (size_t)lane * a.row_bytes;
-    const bool prefix = hmask != 0 && (hmask & (hmask + 1u)) == 0;      // rows 0..m-1 present, no holes
-    if (dst_contig && prefix) {
-      if (lane == 0) {                                                  // one store per destination
-        const uint32_t bytes = (uint32_t)__popc(hmask) * (uint32_t)a.row_bytes;
-        bulk_s2g(a.dst_a + s * a.dst_ld_bytes, src, bytes);
-        if (a.dst_b) bulk_s2g(a.dst_b + s * a.dst_ld_bytes, src, bytes);
-      }
-    } else if (have) {
-      bulk_s2g(a.dst_a + s * a.dst_ld_bytes, src, (uint32_t)a.row_bytes);
-      if (a.dst_b) bulk_s2g(a.dst_b + s * a.dst_ld_bytes, src, (uint32_t)a.row_bytes);
-    }
-    bulk_commit();
-  }
-  bulk_wait_all();
-}
 
 struct PushDev {
   RowMapDev m;
@@ -301,127 +201,14 @@ struct PushDev {
   int64_t ld_bytes;
   int row_bytes;
   float scale;
-  int q;
-  int br;
 };
-constexpr int kPushComputeWarps = 4;
 
-__global__ void __launch_bounds__(32 * (1 + kPushComputeWarps), 1)
-rows_push_delta_bulk_kernel(const __grid_constant__ PushDev a) {
-  extern __shared__ __align__(128) unsigned char smem[];
-  const int Q = a.q;
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem);         // loads landed
-  uint64_t* ready = full + Q;                                 // deltas computed (kPushComputeWarps arrivals)
-  int* nz = reinterpret_cast<int*>(smem + 256);               // [Q][32] row has a non-zero delta
-  unsigned char* stage = smem + 256 + Q * 32 * 4;
-  stage = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(stage) + 127) / 128 * 128);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int BR = a.br;
-  const size_t batch_bytes = (size_t)BR * a.row_bytes;        // cur block, then old block
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < Q; ++s) {
-      mbar_init(full + s, 1);
-      mbar_init(ready + s, kPushComputeWarps);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
-  int64_t n = a.n_ptr ? (int64_t)*a.n_ptr : a.n_max;
-  if (n > a.n_max) n = a.n_max;
-  const int64_t n_batches = (n + BR - 1) / BR;
-  const int64_t mine = n_batches > blockIdx.x ? (n_batches - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
-  const bool contig = a.ld_bytes == a.row_bytes;
-
-  if (warp == 0) {
-    // ---------------- issuer: loads of batch t+Q-1, reductions of batch t ----------------
-    auto issue_load = [&](int64_t t) {
-      const int q = (int)(t % Q);
-      const int64_t s0 = (blockIdx.x + t * gridDim.x) * BR;
-      const int rows = (int)((n - s0) < BR ? (n - s0) : BR);
-      unsigned char* c0 = stage + (size_t)q * 2 * batch_bytes;
-      if (lane == 0) mbar_arrive_expect_tx(full + q, 2u * (uint32_t)rows * (uint32_t)a.row_bytes);
-      __syncwarp();
-      if (contig) {
-        if (lane == 0) {                                       // the batch is contiguous in both caches
-          bulk_g2s(c0, a.cur + s0 * a.ld_bytes, (uint32_t)rows * (uint32_t)a.row_bytes, full + q);
-          bulk_g2s(c0 + batch_bytes, a.old + s0 * a.ld_bytes, (uint32_t)rows * (uint32_t)a.row_bytes, full + q);
-        }
-      } else if (lane < rows) {
-        unsigned char* c = c0 + (size_t)lane * a.row_bytes;
-        bulk_g2s(c, a.cur + (s0 + lane) * a.ld_bytes, (uint32_t)a.row_bytes, full + q);
-        bulk_g2s(c + batch_bytes, a.old + (s0 + lane) * a.ld_bytes, (uint32_t)a.row_bytes, full + q);
-      }
-    };
-    const int64_t pre = mine < Q - 1 ? mine : Q - 1;
-    for (int64_t t = 0; t < pre; ++t) issue_load(t);
-    for (int64_t t = 0; t < mine; ++t) {
-      const int64_t tn = t + Q - 1;
-      if (tn < mine) {
-        if (tn >= Q) {
-          // stage (tn % Q) held batch tn-Q = t-1: its reductions must have read the deltas
-          bulk_wait_read<0>();
-          __syncwarp();
-        }
-        issue_load(tn);
-      }
-      const int q = (int)(t % Q);
-      mbar_wait(ready + q, (uint32_t)((t / Q) & 1));
-      const int64_t s = (blockIdx.x + t * gridDim.x) * BR + lane;
-      const bool in = lane < BR && s < n;
-      const int64_t r = in ? (int64_t)__ldg(a.ids + s) : -1;
-      const bool have = in && r >= 0 && r < a.m.num_row;
-      uint32_t hmask;
-      const int len = row_runs(a.m, r, have, lane, hmask);
-      const uint32_t nzmask = __ballot_sync(0xffffffffu, have && nz[q * 32 + lane] != 0);
-      if (len > 0) {
-        const uint32_t run = (len >= 32 ? 0xffffffffu : ((1u << len) - 1u)) << lane;
-        if (run & nzmask)                                       // an untouched run adds nothing: skip it
-          bulk_reduce_add_s2g(row_addr(a.m, r), stage + (size_t)q * 2 * batch_bytes + (size_t)lane * a.row_bytes,
-                              (uint32_t)len * (uint32_t)a.row_bytes);
-      }
-      bulk_commit();
-    }
-    bulk_wait_all();
-  } else {
-    // ---------------- compute warps: delta = (cur - old) * scale, in place over cur ----------------
-    const int cw = warp - 1;
-    const int nvec = a.row_bytes >> 4;
-    for (int64_t t = 0; t < mine; ++t) {
-      const int q = (int)(t % Q);
-      mbar_wait(full + q, (uint32_t)((t / Q) & 1));
-      unsigned char* cb = stage + (size_t)q * 2 * batch_bytes;
-      const int64_t s0 = (blockIdx.x + t * gridDim.x) * BR;
-      for (int row = cw; row < BR; row += kPushComputeWarps) {
-        if (s0 + row >= n) break;
-        float4* c = reinterpret_cast<float4*>(cb + (size_t)row * a.row_bytes);
-        const float4* o = reinterpret_cast<const float4*>(cb + batch_bytes + (size_t)row * a.row_bytes);
-        int any = 0;
-        for (int v = lane; v < nvec; v += 32) {
-          float4 x = c[v];
-          const float4 y = o[v];
-          x.x = (x.x - y.x) * a.scale; x.y = (x.y - y.y) * a.scale;
-          x.z = (x.z - y.z) * a.scale; x.w = (x.w - y.w) * a.scale;
-          any |= (x.x != 0.f) | (x.y != 0.f) | (x.z != 0.f) | (x.w != 0.f);
-          c[v] = x;
-        }
-        any = __any_sync(0xffffffffu, any);
-        if (lane == 0) nz[q * 32 + row] = any;
-      }
-      fence_proxy_async();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(ready + q);
-    }
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
-// Register-path variants (no shared memory, <= 40 registers): these CTAs co-reside with the persistent
-// K7 CTAs (which own the SMs' shared memory but leave threads and registers), so the pull of block i+1 and
-// the push of block i-1 use the memory-level parallelism of ALL SMs instead of a few reserved ones.
+// No shared memory and <= 56 registers: these CTAs co-reside with the persistent K7 CTAs (which own the
+// SMs' shared memory but leave threads and registers), so the pull of block i+1 and the push of block i-1
+// use the memory-level parallelism of ALL SMs while K7 trains block i.
 // Warp per row, 128-bit accesses, two rows in flight per warp.
-// ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(kSideThreads, 9)
-rows_pull_lsu_kernel(const __grid_constant__ PullDev a) {
+rows_pull_kernel(const __grid_constant__ PullDev a) {
   const int lane = threadIdx.x & 31;
   const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
@@ -462,7 +249,7 @@ rows_pull_lsu_kernel(const __grid_constant__ PullDev a) {
 }
 
 __global__ void __launch_bounds__(kSideThreads, 9)
-rows_push_delta_lsu_kernel(const __grid_constant__ PushDev a) {
+rows_push_delta_kernel(const __grid_constant__ PushDev a) {
   const int lane = threadIdx.x & 31;
   const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
@@ -510,13 +297,6 @@ RowMapDev to_dev(const MvbRowMap* m, int esz) {
   return d;
 }
 
-int max_optin_smem() {
-  int dev = 0, v = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&v, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
-  return v;
-}
-
 }  // namespace
 
 extern "C" int mvb_we_prepare(const MvbWePrep* p, void* stream) {
@@ -552,82 +332,42 @@ extern "C" int mvb_we_prepare(const MvbWePrep* p, void* stream) {
 }
 extern "C" int mvb_we_prepare_launches(int negative) { return negative > 0 ? 9 : 8; }
 
-// Gather rows ids[0..n) of a row-sharded fp32/any-4-byte table into dst_a (and dst_b) over the bulk-copy
-// engine.  n is read on the device from n_ptr when given (clamped to n_max).  Row bytes must be a
-// multiple of 16.  max_ctas bounds the grid (0: 16 CTAs).
-extern "C" int mvb_rows_pull_bulk(const MvbRowMap* m, int esz, const int* ids, const int* n_ptr, int64_t n_max,
-                                  void* dst_a, void* dst_b, int64_t dst_ld, int max_ctas, void* stream) {
+// Gather rows ids[0..n) of a row-sharded table of 4-byte elements into dst_a (and dst_b, when given).
+// n is read on the device from n_ptr when given (clamped to n_max).  Row bytes must be a multiple of 16.
+// The grid is ctas_per_sm (>= 1) CTAs per SM.
+extern "C" int mvb_rows_pull(const MvbRowMap* m, int esz, const int* ids, const int* n_ptr, int64_t n_max,
+                             void* dst_a, void* dst_b, int64_t dst_ld, int ctas_per_sm, void* stream) {
+  if (ctas_per_sm < 1) return -22;
   if (n_max <= 0) return 0;
   const int64_t row_bytes = m->num_col * esz;
-  if (row_bytes % 16 || (dst_ld * esz) % 16 || row_bytes > 16384) return -9;
+  if (row_bytes % 16 || (dst_ld * esz) % 16) return -9;
   if ((reinterpret_cast<uintptr_t>(dst_a) & 15) || (reinterpret_cast<uintptr_t>(dst_b) & 15)) return -9;
   PullDev a{};
   a.m = to_dev(m, esz);
   a.ids = ids; a.n_ptr = n_ptr; a.n_max = n_max;
   a.dst_a = (unsigned char*)dst_a; a.dst_b = (unsigned char*)dst_b; a.dst_ld_bytes = dst_ld * esz;
   a.row_bytes = (int)row_bytes;
-  if (max_ctas < 0) {          // register path: -max_ctas CTAs per SM, co-resident with K7
-    a.q = 0; a.br = 32;
-    const int g = mvb_num_sms() * (-max_ctas);
-    rows_pull_lsu_kernel<<<g, kSideThreads, 0, (cudaStream_t)stream>>>(a);
-    MVB_CUDA_CHECK(cudaGetLastError());
-    return 0;
-  }
-  const int budget = max_optin_smem() - 128;
-  int br = 32, q = 0;
-  for (; br >= 4; br >>= 1) {
-    q = (int)(budget / (br * row_bytes));
-    if (q >= 3) break;
-  }
-  if (q > 8) q = 8;
-  if (q < 3) return -22;
-  a.q = q; a.br = br;
-  const size_t smem = 128 + (size_t)q * br * row_bytes;
-  int grid = max_ctas > 0 ? max_ctas : 16;
-  const int64_t nb = (n_max + br - 1) / br;
-  if ((int64_t)grid > nb) grid = (int)nb;
-  MVB_CUDA_CHECK(cudaFuncSetAttribute(rows_pull_bulk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  rows_pull_bulk_kernel<<<grid, 32, smem, (cudaStream_t)stream>>>(a);
+  rows_pull_kernel<<<mvb_num_sms() * ctas_per_sm, kSideThreads, 0, (cudaStream_t)stream>>>(a);
   MVB_CUDA_CHECK(cudaGetLastError());
   return 0;
 }
 
-// rows[ids[s]] += (cur[s] - old[s]) * scale for s in [0, n): fused AddDeltaParameter on the bulk engine.
-extern "C" int mvb_rows_push_delta_bulk(const MvbRowMap* m, const int* ids, const int* n_ptr, int64_t n_max,
-                                        const float* cur, const float* old, int64_t ld, float scale, int max_ctas,
-                                        void* stream) {
+// rows[ids[s]] += (cur[s] - old[s]) * scale for s in [0, n): AddDeltaParameter as one-sided red.add into the
+// owners' shards; all-zero 16-byte deltas are skipped.  Same count and grid conventions as mvb_rows_pull.
+extern "C" int mvb_rows_push_delta(const MvbRowMap* m, const int* ids, const int* n_ptr, int64_t n_max,
+                                   const float* cur, const float* old, int64_t ld, float scale, int ctas_per_sm,
+                                   void* stream) {
+  if (ctas_per_sm < 1) return -22;
   if (n_max <= 0) return 0;
   const int64_t row_bytes = m->num_col * 4;
-  if (row_bytes % 16 || (ld * 4) % 16 || row_bytes > 16384) return -9;
+  if (row_bytes % 16 || (ld * 4) % 16) return -9;
   if ((reinterpret_cast<uintptr_t>(cur) & 15) || (reinterpret_cast<uintptr_t>(old) & 15)) return -9;
   PushDev a{};
   a.m = to_dev(m, 4);
   a.ids = ids; a.n_ptr = n_ptr; a.n_max = n_max;
   a.cur = (const unsigned char*)cur; a.old = (const unsigned char*)old; a.ld_bytes = ld * 4;
   a.row_bytes = (int)row_bytes; a.scale = scale;
-  if (max_ctas < 0) {
-    a.q = 0; a.br = 32;
-    const int g = mvb_num_sms() * (-max_ctas);
-    rows_push_delta_lsu_kernel<<<g, kSideThreads, 0, (cudaStream_t)stream>>>(a);
-    MVB_CUDA_CHECK(cudaGetLastError());
-    return 0;
-  }
-  const int budget = max_optin_smem() - 1024;
-  int br = 32, q = 0;
-  for (; br >= 4; br >>= 1) {
-    q = (int)(budget / (2 * br * row_bytes + 128));
-    if (q >= 2) break;
-  }
-  if (q > 4) q = 4;
-  if (q < 2) return -22;
-  a.q = q; a.br = br;
-  const size_t smem = 256 + (size_t)q * 32 * 4 + 128 + (size_t)q * 2 * br * row_bytes;
-  int grid = max_ctas > 0 ? max_ctas : 16;
-  const int64_t nb = (n_max + br - 1) / br;
-  if ((int64_t)grid > nb) grid = (int)nb;
-  MVB_CUDA_CHECK(cudaFuncSetAttribute(rows_push_delta_bulk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)smem));
-  rows_push_delta_bulk_kernel<<<grid, 32 * (1 + kPushComputeWarps), smem, (cudaStream_t)stream>>>(a);
+  rows_push_delta_kernel<<<mvb_num_sms() * ctas_per_sm, kSideThreads, 0, (cudaStream_t)stream>>>(a);
   MVB_CUDA_CHECK(cudaGetLastError());
   return 0;
 }

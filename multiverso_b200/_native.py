@@ -92,7 +92,7 @@ class Sgns(C.Structure):
         ("alias_prob", vp), ("alias_idx", vp), ("vocab", C.c_int), ("neg_pool", vp),
         ("neg_pool_size", C.c_int), ("hs_points", vp), ("hs_codes", vp), ("hs_len", vp),
         ("hs_max_code", C.c_int), ("map_in", vp), ("map_out", vp), ("seed", C.c_uint64),
-        ("loss_sum", vp), ("pair_count", vp), ("hogwild", C.c_int), ("max_ctas", C.c_int),
+        ("loss_sum", vp), ("pair_count", vp), ("hogwild", C.c_int),
         ("scale_in", vp), ("scale_out", vp), ("neg_pool_size_ptr", vp),
         ("nservers", C.c_int), ("rows_per_server", i64), ("w_in_peers", VP8), ("w_out_peers", VP8),
     ]
@@ -266,7 +266,7 @@ _CUDA_FUNCS = {
     "mvb_sgns_train_win": _status(C.POINTER(Sgns), Ptr),
     "mvb_sgns_train_det": _status(C.POINTER(Sgns), Ptr),
     "mvb_sgns_last_launches": _unchecked(i32),
-    "mvb_sgns_win_inflight": _unchecked(i32, i32, i32, i32, i32),
+    "mvb_sgns_win_inflight": _unchecked(i32, i32, i32, i32),
     "mvb_keys_add": _status(C.POINTER(KeyMap), Ptr, Ptr, i64, f32, Ptr),
     "mvb_keys_get": _status(C.POINTER(KeyMap), Ptr, Ptr, i64, Ptr),
     "mvb_keys_collect": _status(C.POINTER(KeyMap), Ptr, Ptr, Ptr, i64, Ptr),
@@ -281,8 +281,8 @@ _CUDA_FUNCS = {
     "mvb_rowbox_apply": _status(C.POINTER(RowBox), i32, Ptr, Ptr, Ptr, i64, i64, i32, i32, Ptr),
     "mvb_we_prepare": _status(C.POINTER(WePrep), Ptr),
     "mvb_we_prepare_launches": _unchecked(i32, i32),
-    "mvb_rows_pull_bulk": _status(C.POINTER(RowMap), i32, Ptr, Ptr, i64, Ptr, Ptr, i64, i32, Ptr),
-    "mvb_rows_push_delta_bulk": _status(C.POINTER(RowMap), Ptr, Ptr, i64, Ptr, Ptr, i64, f32, i32, Ptr),
+    "mvb_rows_pull": _status(C.POINTER(RowMap), i32, Ptr, Ptr, i64, Ptr, Ptr, i64, i32, Ptr),
+    "mvb_rows_push_delta": _status(C.POINTER(RowMap), Ptr, Ptr, i64, Ptr, Ptr, i64, f32, i32, Ptr),
     "mvb_build_alias_table": _status(Ptr, i32, Ptr, Ptr),
     "mvb_lr_sparse_fwd_bwd": _status(C.POINTER(LrSparse), Ptr),
     "mvb_lr_dense_fwd_bwd": _status(C.POINTER(LrDense), Ptr),

@@ -13,11 +13,12 @@ Device mapping
   ((trained - cur)/1 added back == trained) and the K7 kernel trains in place on the HBM
   resident shards -- no gather, no scatter.
 * ``world > 1`` (block mode = reference semantics): device-side PrepareData (``mvb_we_prepare``:
-  bitmap-unique + prefix sum + negative pool, counts stay on the device), bulk-engine row pull of
-  the needed rows over NVLink into a local block cache (``mvb_rows_pull_bulk``), K7 on the cache
-  through id->slot maps, bulk-engine push of (new - old)/W (``mvb_rows_push_delta_bulk``).  No
+  bitmap-unique + prefix sum + negative pool, counts stay on the device), row pull of the needed
+  rows over NVLink into a local block cache (``mvb_rows_pull``), K7 on the cache through id->slot
+  maps, one-sided push of (new - old)/W into the owners' shards (``mvb_rows_push_delta``).  No
   host synchronisation and no eager PyTorch op anywhere in the step; pipelined, the pull of block
-  i+1 and the push of block i-1 run on a few reserved SMs under block i's K7.
+  i+1 and the push of block i-1 run on a side stream in one register-only CTA per SM, co-resident
+  with block i's K7 on every SM.
 * learning-rate decay follows UpdateLearningRate (wordembedding.cpp:38-47) from the global
   word count kept in the KV table (constant.h: kWordCountId).
 """
@@ -37,6 +38,10 @@ from ..tables.device import KVDeviceTable, MatrixDeviceTable
 from ..utils import Log, monitor
 
 K_WORD_COUNT_ID = 4  # constant.h:16-20
+# Row pull / delta push CTAs per SM when nothing else runs (the non-pipelined step).  2 is the smallest
+# grid at which both beat the former bulk-copy kernels at 32 CTAs: pull 1.21 vs 1.50 ms, push 0.90 vs 1.52 ms
+# (both tables of a 1M-word Zipf block, dim 300, local shard; H100 80GB HBM3, 700 W power limit).
+_BLOCKING_CTAS_PER_SM = 2
 
 
 @dataclass
@@ -153,32 +158,15 @@ class WordEmbedding:
         self._pending_side = False
         self.kernel_launches = 0
         self.hogwild = False        # one GPU, skip-gram + NS: the Hogwild window kernel instead of the deterministic waves
-        self.max_ctas = 0           # > 0: cap K7's persistent grid (SMs left to the row pull / push kernels)
-        # pull / push kernels of the block protocol (world > 1):
-        #   "lsu" (default)   register-path pull + one-sided red.add push: 128-thread CTAs with <= 56 registers and no
-        #                     shared memory, co-resident with the persistent K7 CTA on every SM (measured at 2 GPUs:
-        #                     pull 2.2 ms + push 2.1 ms under a 9.7 ms K7, 0.96 weak-scaling efficiency)
-        #   "mbox"            register-path pull + row-mailbox push with owner-side apply (rowbox.cu; what the
-        #                     stateful updaters need -- 3x the memory traffic for the plain-add updater)
-        #   "bulk"            bulk-copy engine on `side_ctas` SMs reserved from K7's grid (op-rate bound:
-        #                     ~27 M bulk ops/s per SM)
         # world > 1 training mode: "block" (reference semantics: pull, train a block-local copy, push (new - old) / W)
         # or "direct": K7 trains IN the row-sharded tables, loading rows from and reducing deltas into their owners'
         # shards over NVLink (Hogwild across GPUs: no cache, no PrepareData, one kernel per block at any world size;
         # link bound: ~20 KB per word cross NVLink instead of ~2 KB in block mode)
         self.mode = os.environ.get("MVB_WE_MODE", "block")
-        self.side_mode = os.environ.get("MVB_WE_SIDE_MODE", "lsu")
-        self.side_ctas = int(os.environ.get("MVB_WE_SIDE_CTAS", "10" if self.side_mode == "bulk" else "1"))
         # direct mode runs only on the window kernel: dim <= 512, window <= 15
         if self.mode == "direct" and not (rt.size > 1 and self._dev_block_ok() and D <= 512
                                           and option.window_size <= 15):
             self.mode = "block"
-        if self.side_mode == "mbox" and rt.size > 1 and self._dev_block_ok() and self.input_table.S == rt.size:
-            self.input_table.enable_row_mailbox()          # collective
-            self.output_table.enable_row_mailbox()
-        elif self.side_mode == "mbox":
-            self.side_mode = "lsu"
-        self.num_sms = torch.cuda.get_device_properties(self.dev).multi_processor_count
         self._bufs = [None, None]   # device-side block protocol: two buffer sets (block i trains, i+1 is pulled)
         self.scale_in = self.scale_out = None
         self._build_hot_row_cap()
@@ -199,7 +187,7 @@ class WordEmbedding:
         cap = float(os.environ.get("MVB_WE_HOT_CAP", "128"))
         if cap <= 0 or o.cbow or o.hs or o.use_adagrad or o.negative_num < 1:
             return
-        pos = N.cuda_lib().mvb_sgns_win_inflight(self.D, o.negative_num, o.window_size, self.max_ctas)
+        pos = N.cuda_lib().mvb_sgns_win_inflight(self.D, o.negative_num, o.window_size)
         if pos <= 0:
             return
         f = self.counts / self.counts.sum()
@@ -226,7 +214,7 @@ class WordEmbedding:
 
     # ------------------------------------------------------------------ K7 launch
     def _launch(self, tokens: torch.Tensor, w_in, w_out, g2_in, g2_out, ld, map_in=None,
-                map_out=None, neg_pool=None, compute_loss=True, neg_pool_size_ptr=None, max_ctas=None,
+                map_out=None, neg_pool=None, compute_loss=True, neg_pool_size_ptr=None,
                 direct: bool = False) -> None:
         o = self.opt
         a = N.Sgns()
@@ -253,7 +241,6 @@ class WordEmbedding:
         a.loss_sum = self.loss.data_ptr() if compute_loss else None
         a.pair_count = self.pairs.data_ptr()
         a.hogwild = int(self.hogwild)
-        a.max_ctas = self.max_ctas if max_ctas is None else max_ctas
         if direct:
             ti, to = self.input_table, self.output_table
             a.nservers, a.rows_per_server = ti.S, ti.rps
@@ -309,7 +296,7 @@ class WordEmbedding:
             self._record_streams(st, main)
         inputs_ready = torch.cuda.Event()
         inputs_ready.record(main)                                 # next_tokens (e.g. an H2D copy) is complete here
-        self._train_prepared(tokens, st, compute_loss, pipelined=True)
+        self._train_prepared(tokens, st, compute_loss)
         trained = torch.cuda.Event()
         trained.record(main)
         with torch.cuda.stream(side):
@@ -341,8 +328,6 @@ class WordEmbedding:
     # ------------------------------------------------------------------ device-side block protocol
     def _dev_block_ok(self) -> bool:
         o = self.opt
-        if os.environ.get("MVB_WE_DEV_BLOCK", "1") == "0":
-            return False
         return (not o.hs and not o.cbow and not o.use_adagrad and o.negative_num >= 1 and o.negative_num <= 7
                 and self.D % 4 == 0)
 
@@ -389,12 +374,12 @@ class WordEmbedding:
         with monitor("WE_PREPARE_DATA", cuda=True):
             lib.mvb_we_prepare(p, st)
         self.kernel_launches += lib.mvb_we_prepare_launches(o.negative_num)
-        ctas = (self.side_ctas if self.side_mode == "bulk" else -self.side_ctas) if side else 32
+        ctas = 1 if side else _BLOCKING_CTAS_PER_SM      # side stream: one CTA per SM next to K7's
         cnt = b["counts"].data_ptr()
         with monitor("WE_REQUEST_PARAMETER", cuda=True):
             for tab, ids, ci, cache, old, cap in ((self.input_table, b["ids_in"], 0, b["cache_in"], b["old_in"], b["cap_in"]),
                                                   (self.output_table, b["ids_out"], 1, b["cache_out"], b["old_out"], b["cap_out"])):
-                lib.mvb_rows_pull_bulk(tab._rowmap, 4, ids, cnt + 4 * ci, cap, cache, old, self.D, ctas, st)
+                lib.mvb_rows_pull(tab._rowmap, 4, ids, cnt + 4 * ci, cap, cache, old, self.D, ctas, st)
         self.kernel_launches += 2
         return b
 
@@ -402,25 +387,11 @@ class WordEmbedding:
         """AddDeltaParameter (communicator.cpp:206-249): rows += (trained - pulled) / W, pushed one-sided."""
         lib, st = N.cuda_lib(), N.stream_ptr()
         cnt = b["counts"].data_ptr()
-        if self.side_mode == "mbox":
-            cur = torch.cuda.current_stream()
-            with monitor("WE_ADD_DELTA", cuda=True):
-                for tab, ids, ci, cache, old, cap in ((self.input_table, b["ids_in"], 0, b["cache_in"], b["old_in"], b["cap_in"]),
-                                                      (self.output_table, b["ids_out"], 1, b["cache_out"], b["old_out"], b["cap_out"])):
-                    tab._mailbox.push_delta(ids, cnt + 4 * ci, cap, cache, old, 1.0 / self.W, ctas_per_sm=self.side_ctas)
-                    self.kernel_launches += 2
-            with monitor("WE_APPLY_DELTA", cuda=True):
-                # serve my shards: whatever the other workers have pushed by now (async PS: no waiting)
-                for tab in (self.input_table, self.output_table):
-                    tab._mailbox.drain(wait=False, ctas_per_sm=self.side_ctas, stream=cur)
-                    self.kernel_launches += tab._mailbox.launches_per_drain()
-            return
-        ctas = (self.side_ctas if self.side_mode == "bulk" else -self.side_ctas) if side else 32
+        ctas = 1 if side else _BLOCKING_CTAS_PER_SM
         with monitor("WE_ADD_DELTA", cuda=True):
             for tab, ids, ci, cache, old, cap in ((self.input_table, b["ids_in"], 0, b["cache_in"], b["old_in"], b["cap_in"]),
                                                   (self.output_table, b["ids_out"], 1, b["cache_out"], b["old_out"], b["cap_out"])):
-                lib.mvb_rows_push_delta_bulk(tab._rowmap, ids, cnt + 4 * ci, cap, cache, old, self.D, 1.0 / self.W,
-                                             ctas, st)
+                lib.mvb_rows_push_delta(tab._rowmap, ids, cnt + 4 * ci, cap, cache, old, self.D, 1.0 / self.W, ctas, st)
         self.kernel_launches += 2
 
     def _prepare_block(self, tokens: torch.Tensor, wait: bool) -> dict:
@@ -468,24 +439,22 @@ class WordEmbedding:
             st["old_g2i"], st["old_g2o"] = st["g2i"].clone(), st["g2o"].clone()
         return st
 
-    def _train_prepared(self, tokens: torch.Tensor, st: dict, compute_loss: bool, pipelined: bool = False) -> None:
+    def _train_prepared(self, tokens: torch.Tensor, st: dict, compute_loss: bool) -> None:
         tr = getattr(self, "trace", None)
         if tr is not None:                 # benchmark tracing: K7 start / end events of every block
             e0 = torch.cuda.Event(enable_timing=True)
             e0.record()
-        self._train_prepared_inner(tokens, st, compute_loss, pipelined)
+        self._train_prepared_inner(tokens, st, compute_loss)
         if tr is not None:
             e1 = torch.cuda.Event(enable_timing=True)
             e1.record()
             tr.append((e0, e1))
 
-    def _train_prepared_inner(self, tokens: torch.Tensor, st: dict, compute_loss: bool, pipelined: bool) -> None:
+    def _train_prepared_inner(self, tokens: torch.Tensor, st: dict, compute_loss: bool) -> None:
         with monitor("WE_TRAIN_BLOCK", cuda=True):
             if st.get("dev"):
-                # pipelined: leave `side_ctas` SMs to the pull / push kernels running on the side stream
-                cap = max(1, self.num_sms - self.side_ctas) if (pipelined and self.side_mode == "bulk") else None
                 self._launch(tokens, st["cache_in"], st["cache_out"], None, None, self.D, st["map_in"], st["map_out"],
-                             st["neg_pool"], compute_loss, neg_pool_size_ptr=st["n_pool"], max_ctas=cap)
+                             st["neg_pool"], compute_loss, neg_pool_size_ptr=st["n_pool"])
             else:
                 self._launch(tokens, st["cache_in"], st["cache_out"], st["g2i"], st["g2o"], self.D,
                              st["map_in"], st["map_out"], st["neg_pool"], compute_loss)
@@ -522,9 +491,7 @@ class WordEmbedding:
 
     # ------------------------------------------------------------------ results
     def embeddings(self) -> torch.Tensor:
-        """Whole input-embedding matrix [V, D] (SaveEmbedding pulls it in 100k-row batches).  With the
-        row mailboxes a worker's last deltas are applied by their owners at the next MV_Barrier (the
-        reference's SaveEmbedding is preceded by one, distributed_wordembedding.cpp:232-237)."""
+        """Whole input-embedding matrix [V, D] (SaveEmbedding pulls it in 100k-row batches)."""
         self.flush()
         return self.input_table.get().view(self.V, self.D)
 

@@ -259,7 +259,7 @@ def scenario_async():
         err2 = (y2.double() - ref2).abs().max().item()
         check(f"get_gemm_peer_scratch_M{Mrows}", err2 < 4e-3 * 18 * 4, str(err2))
     mv.barrier()
-    # device-side block protocol across ranks: bulk-engine pull from peer shards, one-sided delta push
+    # device-side block protocol across ranks: row pull from peer shards, one-sided delta push
     from multiverso_b200 import _native as N
     bt = mv.MatrixTable(40000, 300, "float32", min_value=-1.0, max_value=1.0, seed=11)
     mv.barrier()
@@ -269,18 +269,18 @@ def scenario_async():
     ndev = torch.tensor([kk], dtype=torch.int32, device="cuda")
     cache = torch.zeros(kk + 7, 300, device="cuda"); old = torch.zeros(kk + 7, 300, device="cuda")
     lib, stp = N.cuda_lib(), N.stream_ptr()
-    lib.mvb_rows_pull_bulk(bt._rowmap, 4, bids, ndev, kk + 7, cache, old, 300, 6, stp)
+    lib.mvb_rows_pull(bt._rowmap, 4, bids, ndev, kk + 7, cache, old, 300, 1, stp)
     torch.cuda.synchronize()
-    check("rows_pull_bulk_peer", torch.equal(cache[:kk], bfull[bids.long()]) and torch.equal(old[:kk], bfull[bids.long()]))
+    check("rows_pull_peer", torch.equal(cache[:kk], bfull[bids.long()]) and torch.equal(old[:kk], bfull[bids.long()]))
     mv.barrier()
     cache[:kk] += float(r + 1)
-    lib.mvb_rows_push_delta_bulk(bt._rowmap, bids, ndev, kk + 7, cache, old, 300, 0.5, 6, stp)
+    lib.mvb_rows_push_delta(bt._rowmap, bids, ndev, kk + 7, cache, old, 300, 0.5, 2, stp)
     torch.cuda.synchronize()
     mv.barrier()
     bexp = bfull.clone()
     for w in range(W):
         bexp[torch.arange(w, 40000, 3, device="cuda")] += 0.5 * (w + 1)
-    check("rows_push_delta_bulk_peer", torch.allclose(bt.get().view(40000, 300), bexp, rtol=0, atol=1e-5))
+    check("rows_push_delta_peer", torch.allclose(bt.get().view(40000, 300), bexp, rtol=0, atol=1e-5))
     mv.barrier()
     # distributed WordEmbedding block (block mode)
     from multiverso_b200.models.wordembedding import WordEmbedding, WordEmbeddingOption, synthetic_zipf_corpus

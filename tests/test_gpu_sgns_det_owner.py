@@ -116,7 +116,7 @@ def test_sgns_det_owner_matches_wave_model(mv_device, case):
     cs = rec.make_case(case)
     c = cs["c"]
     D = c["D"]
-    wave = N.cuda_lib().mvb_sgns_win_inflight(D, c["K"], c["W"], 0)
+    wave = N.cuda_lib().mvb_sgns_win_inflight(D, c["K"], c["W"])
     assert c["n_tok"] > 3 * wave
     w_in, w_out, _, _ = rec.train(cs)
     IN, OUT, read_in, read_out = _model(cs, wave)

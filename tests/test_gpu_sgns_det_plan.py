@@ -32,7 +32,7 @@ def _load(name, path):
 
 def _wave(D, K, W):
     from multiverso_b200 import _native as N
-    return N.cuda_lib().mvb_sgns_win_inflight(D, K, W, 0)
+    return N.cuda_lib().mvb_sgns_win_inflight(D, K, W)
 
 
 def _case(tokens, rows, D, W=5, K=5, V=None, word_map=None, pool=None, scales=True, seed=0x5EED):

@@ -1,5 +1,5 @@
 """Device-side WordEmbedding block protocol (csrc/cuda/we_block.cu) against plain PyTorch references:
-PrepareData (bitmap-unique + prefix sum + negative pool), bulk-engine row pull and delta push."""
+PrepareData (bitmap-unique + prefix sum + negative pool), row pull and delta push."""
 import pytest
 import torch
 
@@ -79,16 +79,10 @@ def test_we_prepare_pool_distribution(mv_device):
     assert (emp - exp).abs().max().item() < 0.004
 
 
-@pytest.mark.parametrize("lsu", [False, True])
-@pytest.mark.parametrize("rows,cols,k", [(20000, 300, 7001), (5000, 64, 5000), (3000, 512, 33), (1000, 300, 1)])
-def test_rows_pull_push_bulk(mv_device, rows, cols, k, lsu):
-    """lsu=False: bulk-copy-engine kernels (max_ctas > 0); lsu=True: register-path kernels (max_ctas < 0)."""
-    import multiverso_b200 as mv
+def _pull_push(rowmap, full0, read_full, ids, cols, ctas):
+    """Pull ids through a device count, push (trained - pulled) / 2 back, pull again with a host count."""
     from multiverso_b200 import _native as N
-    t = mv.MatrixTable(rows, cols, "float32", min_value=-1.0, max_value=1.0, seed=5)
-    full0 = t.get().view(rows, cols).clone()
-    g = torch.Generator().manual_seed(rows)
-    ids = torch.randperm(rows, generator=g)[:k].sort().values.to(torch.int32).cuda()
+    k = ids.numel()
     cap = k + 100
     ids_buf = torch.full((cap,), -1, dtype=torch.int32, device="cuda")
     ids_buf[:k] = ids
@@ -96,7 +90,7 @@ def test_rows_pull_push_bulk(mv_device, rows, cols, k, lsu):
     cache = torch.full((cap, cols), 7.0, device="cuda")
     old = torch.full((cap, cols), 7.0, device="cuda")
     lib, st = N.cuda_lib(), N.stream_ptr()
-    lib.mvb_rows_pull_bulk(t._rowmap, 4, ids_buf, n_dev, cap, cache, old, cols, -1 if lsu else 5, st)
+    lib.mvb_rows_pull(rowmap, 4, ids_buf, n_dev, cap, cache, old, cols, ctas, st)
     torch.cuda.synchronize()
     assert torch.equal(cache[:k], full0[ids.long()]) and torch.equal(old[:k], full0[ids.long()])
     assert bool((cache[k:] == 7.0).all()) and bool((old[k:] == 7.0).all())       # the device count bounds the copy
@@ -104,17 +98,60 @@ def test_rows_pull_push_bulk(mv_device, rows, cols, k, lsu):
     delta = torch.randn(k, cols, device="cuda", generator=torch.Generator(device="cuda").manual_seed(1))
     delta[::5] = 0
     cache[:k] += delta
-    lib.mvb_rows_push_delta_bulk(t._rowmap, ids_buf, n_dev, cap, cache, old, cols, 0.5, -2 if lsu else 3, st)
+    lib.mvb_rows_push_delta(rowmap, ids_buf, n_dev, cap, cache, old, cols, 0.5, ctas, st)
     torch.cuda.synchronize()
     exp = full0.clone()
     exp[ids.long()] += (cache[:k] - old[:k]) * 0.5
-    got = t.get().view(rows, cols)
+    got = read_full()
     assert torch.allclose(got, exp, rtol=0, atol=1e-6)
-    untouched = torch.ones(rows, dtype=torch.bool, device="cuda")
+    untouched = torch.ones(full0.shape[0], dtype=torch.bool, device="cuda")
     untouched[ids.long()] = False
     assert torch.equal(got[untouched], full0[untouched])
     # host-count variant (n_ptr = NULL)
     cache2 = torch.zeros(k, cols, device="cuda")
-    lib.mvb_rows_pull_bulk(t._rowmap, 4, ids, None, k, cache2, None, cols, 0, st)
+    lib.mvb_rows_pull(rowmap, 4, ids, None, k, cache2, None, cols, ctas, st)
     torch.cuda.synchronize()
     assert torch.equal(cache2, got[ids.long()])
+
+
+@pytest.mark.parametrize("ctas", [1, 2])
+@pytest.mark.parametrize("rows,cols,k", [(20000, 300, 7001), (5000, 64, 5000), (3000, 512, 33), (1000, 300, 1)])
+def test_rows_pull_push(mv_device, rows, cols, k, ctas):
+    """Row pull and delta push at 1 and 2 CTAs per SM (the pipelined and the blocking grid)."""
+    import multiverso_b200 as mv
+    from multiverso_b200 import _native as N
+    t = mv.MatrixTable(rows, cols, "float32", min_value=-1.0, max_value=1.0, seed=5)
+    full0 = t.get().view(rows, cols).clone()
+    g = torch.Generator().manual_seed(rows)
+    ids = torch.randperm(rows, generator=g)[:k].sort().values.to(torch.int32).cuda()
+    _pull_push(t._rowmap, full0, lambda: t.get().view(rows, cols), ids, cols, ctas)
+    with pytest.raises(N.NativeError):           # the grid is a whole number of CTAs per SM
+        N.cuda_lib().mvb_rows_pull(t._rowmap, 4, ids, None, k, full0, None, cols, 0, N.stream_ptr())
+
+
+def test_rows_pull_push_three_servers(mv_device):
+    """Owner arithmetic: three servers of 6000, 6000 and 8000 rows (the last takes the remainder), laid out
+    out of order in one local buffer with sentinel gaps between them, so a row read from or added to the wrong
+    server, or past its end, changes a value."""
+    from multiverso_b200 import _native as N
+    rows, cols, rps, gap = 20000, 300, 6000, 16
+    lens = [rps, rps, rows - 2 * rps]
+    starts = [lens[2] + gap, lens[2] + lens[0] + 2 * gap, 0]          # server 2 first, then 0, then 1
+    buf = torch.full((rows + 3 * gap, cols), 7.0, device="cuda")
+    shards = [buf[s0:s0 + n] for s0, n in zip(starts, lens)]
+    g = torch.Generator(device="cuda").manual_seed(3)
+    for sh in shards:
+        sh.copy_(torch.rand(sh.shape, device="cuda", generator=g) * 2 - 1)
+    gaps = torch.ones(buf.shape[0], dtype=torch.bool, device="cuda")
+    for s0, n in zip(starts, lens):
+        gaps[s0:s0 + n] = False
+    rm = N.RowMap()
+    rm.num_row, rm.num_col, rm.nservers, rm.rows_per_server = rows, cols, 3, rps
+    for s, sh in enumerate(shards):
+        rm.shard_ptrs[s] = sh.data_ptr()
+    full0 = torch.cat(shards)
+    pick = torch.randperm(rows, generator=torch.Generator().manual_seed(7))[:5000]
+    edges = torch.tensor([0, rps - 1, rps, 2 * rps - 1, 2 * rps, rows - 1])
+    ids = torch.unique(torch.cat([pick, edges])).to(torch.int32).cuda()      # every owner, both ends of each
+    _pull_push(rm, full0, lambda: torch.cat(shards), ids, cols, 2)
+    assert bool((buf[gaps] == 7.0).all())

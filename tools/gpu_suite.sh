@@ -89,30 +89,22 @@ blk)
   if [ "$NG" -gt 1 ]; then
     timeout 500 python -m torch.distributed.run --nnodes=1 --nproc-per-node $NG --master-addr 127.0.0.1 --master-port $PORT tests/mp_device_check.py async > gpurun_out/mp_check_async.log 2>&1; echo "mp async rc=$?"; grep -E "PASS|FAIL|Error|error" gpurun_out/mp_check_async.log | head -12
     timeout 400 python -m torch.distributed.run --nnodes=1 --nproc-per-node $NG --master-addr 127.0.0.1 --master-port $((PORT+1)) bench.py --gpus $NG --steps 10 --warmup 3 > gpurun_out/bench_n$NG.json 2> gpurun_out/bench_n$NG.err; echo "bench$NG rc=$?"; cut -c1-1500 gpurun_out/bench_n$NG.json; tail -5 gpurun_out/bench_n$NG.err
-    for sc in ${SIDE_CTAS:-}; do
-      MVB_WE_SIDE_MODE=${SIDE_MODE:-bulk} MVB_WE_SIDE_CTAS=$sc timeout 400 python -m torch.distributed.run --nnodes=1 --nproc-per-node $NG --master-addr 127.0.0.1 --master-port $((PORT+2)) bench.py --gpus $NG --steps 10 --warmup 3 --no-table-bw > gpurun_out/bench_n${NG}_side$sc.json 2> gpurun_out/bench_n${NG}_side$sc.err; echo "bench$NG side=$sc rc=$?"; python -c "import json;d=json.load(open('gpurun_out/bench_n${NG}_side$sc.json'));print(round(d['value']/1e6,1), round(d['e2e']['value']/1e6,1), d['config']['loss_per_pair'], {k:round(v['avg_ms'],2) for k,v in d['extra']['monitors_device_arm'].items()})"
-    done
   fi
   ;;
 r2n8)
-  # round 2, one multi-GPU call: scenarios (async + sync), headline bench, side-CTA variant, dense Get bulk experiment
+  # round 2, one multi-GPU call: scenarios (async + sync), headline bench, dense Get bulk experiment
   for w in async sync; do
     timeout 500 python -m torch.distributed.run --nnodes=1 --nproc-per-node $NG --master-addr 127.0.0.1 --master-port $((PORT+20)) tests/mp_device_check.py $w > gpurun_out/mp_check_${w}_n$NG.log 2>&1; echo "mp $w rc=$?"; grep -cE "PASS" gpurun_out/mp_check_${w}_n$NG.log; grep -E "FAIL|Error|Traceback" gpurun_out/mp_check_${w}_n$NG.log | head -5 | cut -c1-600
   done
   timeout 500 python -m torch.distributed.run --nnodes=1 --nproc-per-node $NG --master-addr 127.0.0.1 --master-port $((PORT+21)) bench.py --gpus $NG --steps 20 --warmup 5 > gpurun_out/bench_n$NG.json 2> gpurun_out/bench_n$NG.err; echo "bench$NG rc=$?"; grep '^{' gpurun_out/bench_n$NG.json | cut -c1-1200; tail -3 gpurun_out/bench_n$NG.err
-  MVB_WE_SIDE_CTAS=2 timeout 400 python -m torch.distributed.run --nnodes=1 --nproc-per-node $NG --master-addr 127.0.0.1 --master-port $((PORT+22)) bench.py --gpus $NG --steps 10 --warmup 3 --no-table-bw > gpurun_out/bench_n${NG}_side2.json 2> gpurun_out/bench_n${NG}_side2.err; echo "bench$NG side2 rc=$?"
   L="python -m torch.distributed.run --nnodes=1 --nproc-per-node $NG --master-addr 127.0.0.1 --master-port $((PORT+23))"
   for v in 0 1; do
     MVB_GET_BULK=$v timeout 300 $L bench/matrix_bw.py > gpurun_out/matrix_bw_bulk${v}_n$NG.log 2>&1; echo "matrix_bw MVB_GET_BULK=$v rc=$?"; grep '^{' gpurun_out/matrix_bw_bulk${v}_n$NG.log | tail -1 | cut -c1-700
   done
   ;;
 r2final)
-  # round 2 final multi-GPU call: bulk Add correctness + timing, config-5 stress, headline bench
-  MVB_ADD_BULK=2 timeout 400 python -m torch.distributed.run --nnodes=1 --nproc-per-node $NG --master-addr 127.0.0.1 --master-port $((PORT+30)) tests/mp_device_check.py sync > gpurun_out/mp_check_sync_addbulk_n$NG.log 2>&1; echo "mp sync (bulk add) rc=$?"; grep -cE "PASS" gpurun_out/mp_check_sync_addbulk_n$NG.log; grep -E "FAIL|Error" gpurun_out/mp_check_sync_addbulk_n$NG.log | head -3 | cut -c1-400
+  # round 2 final multi-GPU call: config-5 stress, headline bench
   L="python -m torch.distributed.run --nnodes=1 --nproc-per-node $NG --master-addr 127.0.0.1 --master-port $((PORT+31))"
-  for v in 0 1; do
-    MVB_ADD_BULK=$v timeout 300 $L bench/matrix_bw.py > gpurun_out/matrix_bw_addbulk${v}_n$NG.log 2>&1; echo "matrix_bw MVB_ADD_BULK=$v rc=$?"; grep '^{' gpurun_out/matrix_bw_addbulk${v}_n$NG.log | tail -1 | python -c "import sys,json; d=json.loads(sys.stdin.read()); print({k:round(v,3) for k,v in d.items() if k.endswith('_ms')})"
-  done
   timeout 400 $L bench/array_async_stress.py > gpurun_out/array_async_stress_n$NG.log 2>&1; echo "stress rc=$?"; grep '^{' gpurun_out/array_async_stress_n$NG.log | tail -1 | cut -c1-900
   timeout 500 python -m torch.distributed.run --nnodes=1 --nproc-per-node $NG --master-addr 127.0.0.1 --master-port $((PORT+32)) bench.py --gpus $NG --steps 20 --warmup 5 > gpurun_out/bench_n$NG.json 2> gpurun_out/bench_n$NG.err; echo "bench$NG rc=$?"; grep '^{' gpurun_out/bench_n$NG.json | cut -c1-400; tail -3 gpurun_out/bench_n$NG.err
   ;;

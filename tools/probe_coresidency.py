@@ -23,29 +23,28 @@ side = torch.cuda.Stream()
 main = torch.cuda.current_stream()
 
 
-def pull(mode):
-    lib.mvb_rows_pull_bulk(t._rowmap, 4, ids, None, k, cache, old, D, mode, torch.cuda.current_stream().cuda_stream)
+def pull(ctas_per_sm):
+    lib.mvb_rows_pull(t._rowmap, 4, ids, None, k, cache, old, D, ctas_per_sm, torch.cuda.current_stream().cuda_stream)
 
 
-for mode in (-1, -2, 10):
+for ctas_per_sm in (1, 2):
     for _ in range(2):
-        pull(mode)
+        pull(ctas_per_sm)
     torch.cuda.synchronize()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record(); pull(mode); e1.record(); torch.cuda.synchronize()
+    e0.record(); pull(ctas_per_sm); e1.record(); torch.cuda.synchronize()
     alone = e0.elapsed_time(e1)
     we.train_block(toks); torch.cuda.synchronize()
     k0, k1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     s0, s1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    we.max_ctas = 138 if mode > 0 else 0
     k0.record(main)
     we.train_block(toks)
     k1.record(main)
     with torch.cuda.stream(side):
         side.wait_event(k0)
         torch.cuda._sleep(600_000)          # ~300 us: K7 is running by now
-        s0.record(side); pull(mode); s1.record(side)
+        s0.record(side); pull(ctas_per_sm); s1.record(side)
     torch.cuda.synchronize()
-    print(f"mode {mode}: pull alone {alone:.2f} ms, under K7 {s0.elapsed_time(s1):.2f} ms, K7 {k0.elapsed_time(k1):.2f} ms, "
+    print(f"{ctas_per_sm} CTAs/SM: pull alone {alone:.2f} ms, under K7 {s0.elapsed_time(s1):.2f} ms, K7 {k0.elapsed_time(k1):.2f} ms, "
           f"pull end - K7 start {k0.elapsed_time(s1):.2f} ms, carveout={os.environ.get('MVB_SIDE_CARVEOUT', '-')}", flush=True)
 mv.shutdown()
