@@ -76,12 +76,17 @@ struct Pk {
   T v[N];
 };
 
+// `bufs` are staging or symmetric memory on 16-byte boundaries; `out` is the caller's tensor, which may
+// be any view (t[1:]), so the 16-byte store to it is taken only when its address allows.
+MVB_DEVINL bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
 template <typename T>
 __global__ void __launch_bounds__(256) allreduce_oneshot_kernel(const __grid_constant__ ArDev<T> a) {
   constexpr int VEC = 16 / sizeof(T);
   handshake_begin(a);
   const int64_t nvec = a.n / VEC;
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  const bool out_aligned = aligned16(a.out);
   for (int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; v < nvec; v += stride) {
     Pk<T, VEC> g[MVB_MAX_RANKS];
 #pragma unroll
@@ -97,7 +102,12 @@ __global__ void __launch_bounds__(256) allreduce_oneshot_kernel(const __grid_con
 #pragma unroll
         for (int e = 0; e < VEC; ++e) s.v[e] = (T)(s.v[e] + g[r].v[e]);
       }
-    st_v4(a.out + v * VEC, *reinterpret_cast<uint4*>(&s));
+    if (out_aligned) {
+      st_v4(a.out + v * VEC, *reinterpret_cast<uint4*>(&s));
+    } else {
+#pragma unroll
+      for (int e = 0; e < VEC; ++e) a.out[v * VEC + e] = s.v[e];
+    }
   }
   if (blockIdx.x == 0) {
     for (int64_t i = nvec * VEC + threadIdx.x; i < a.n; i += blockDim.x) {
@@ -166,10 +176,14 @@ __global__ void __launch_bounds__(256) allreduce_twoshot_finish(const __grid_con
   const int64_t nvec = a.n / VEC;
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   const T* src = a.bufs[a.me];
-  for (int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; v < nvec; v += stride)
-    st_v4(a.out + v * VEC, ld_v4(src + v * VEC));
-  if (blockIdx.x == 0)
-    for (int64_t i = nvec * VEC + threadIdx.x; i < a.n; i += blockDim.x) a.out[i] = src[i];
+  const int64_t v0 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (aligned16(a.out)) {
+    for (int64_t v = v0; v < nvec; v += stride) st_v4(a.out + v * VEC, ld_v4(src + v * VEC));
+    if (blockIdx.x == 0)
+      for (int64_t i = nvec * VEC + threadIdx.x; i < a.n; i += blockDim.x) a.out[i] = src[i];
+  } else {
+    for (int64_t i = v0; i < a.n; i += stride) a.out[i] = src[i];
+  }
 }
 
 // NVLS two-shot: rank r reduces slice r IN THE SWITCH (multimem.ld_reduce on the multicast
@@ -210,7 +224,7 @@ allreduce_fused_kernel(const __grid_constant__ ArDev<T> a, const T* __restrict__
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   const int64_t v0 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   T* mine = a.bufs[a.me] + slot_off;
-  const bool aligned = (reinterpret_cast<uintptr_t>(src) & 15) == 0 && (reinterpret_cast<uintptr_t>(a.out) & 15) == 0;
+  const bool aligned = aligned16(src) && aligned16(a.out);
   if (aligned) {
     for (int64_t v = v0; v < nvec; v += stride) st_v4(mine + v * VEC, ld_v4(src + v * VEC));
     if (blockIdx.x == 0)

@@ -225,7 +225,7 @@ typedef struct MvbAllreduce {
   int dtype;
   int64_t n;
   void* bufs[MVB_MAX_RANKS];    /* symmetric staging, peer-mapped */
-  void* out;                    /* local result (may alias bufs[me] for two-shot) */
+  void* out;                    /* local result, any element alignment (may alias bufs[me] for two-shot) */
   void* const* pads;
   int me, world;
   int ch;
