@@ -19,19 +19,6 @@ struct KVDev {
   void* vals[MVB_MAX_RANKS];
 };
 
-MVB_DEVINL uint64_t mix64(uint64_t x) {
-  x ^= x >> 33;
-  x *= 0xff51afd7ed558ccdull;
-  x ^= x >> 33;
-  x *= 0xc4ceb9fe1a85ec53ull;
-  x ^= x >> 33;
-  return x;
-}
-MVB_DEVINL int owner_of(long long key, int S) {
-  long long m = key % S;
-  return (int)(m < 0 ? m + S : m);
-}
-
 template <typename V>
 MVB_DEVINL void atomic_add_sys(V* p, V v);
 template <>

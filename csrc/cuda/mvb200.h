@@ -217,6 +217,50 @@ int mvb_kv_get(const MvbKV* kv, const int64_t* keys, void* out_vals, int64_t n, 
 int mvb_kv_dump(int vtype, const void* keys, const void* vals, int64_t capacity,
                 int64_t* out_keys, void* out_vals, int64_t* out_count, void* stream);
 
+/* ---- hash index of a HashMatrixTable (hash_rows.cu) ---------------------------------------------------- */
+/* Rows keyed by any int64 except INT64_MIN. Server s = mod(key, nservers) owns the key; it has `slots` (P, a
+ * power of two) slots, probed linearly from mix64(key) & (P - 1). Slot j of server s is row s P + j of an fp32
+ * MatrixTable of nservers P + 1 rows (row pitch % 4 == 0); the last row is the zero row, never given to a key.
+ * A server holds at most floor(7 P / 8) keys. keys / ready / count are symmetric (peer-mapped) allocations. */
+enum { MVB_HASH_INIT_CONST = 0, MVB_HASH_INIT_UNIFORM = 1 };
+enum { MVB_HASH_FULL = 1, MVB_HASH_TIMEOUT = 2, MVB_HASH_BAD_KEY = 3 };
+typedef struct MvbHashRows {
+  int nservers;
+  int64_t slots;                   /* P per server                                                          */
+  void* keys[MVB_MAX_RANKS];       /* int64[P] per server, INT64_MIN = empty                                */
+  void* ready[MVB_MAX_RANKS];      /* uint32[P] per server: 1 once the slot's row holds its initial value,
+                                      2 for a key refused at the limit (it keeps the slot, never a row)     */
+  void* count[MVB_MAX_RANKS];      /* uint64 per server: live keys (ready == 1)                             */
+  MvbRowMap map;                   /* the rows                                                              */
+  int init;                        /* MVB_HASH_INIT_CONST: init_value; UNIFORM: lo + u (hi - lo), u from the key */
+  float init_value, lo, hi;
+  uint64_t seed;
+} MvbHashRows;
+typedef struct MvbHashLookup {
+  const MvbHashRows* tables;       /* device [T] index descriptors                                          */
+  const int64_t* keys;             /* [n]                                                                   */
+  int64_t n;
+  const int64_t* seg_end;          /* device [G]: key i belongs to the first segment g with i < seg_end[g];
+                                      NULL: every key belongs to table 0                                    */
+  const int* seg_table;            /* device [G]: the descriptor of segment g, or -1: the key is a row id,
+                                      copied unchanged                                                       */
+  int G;
+  int insert;                      /* 1: a missing key claims a slot; 0: it reads the zero row              */
+  const int64_t* insert_ok;        /* device int64 or NULL: when it holds 0, insert is treated as 0 (the
+                                      caller's device-side check of the segment layout failed)              */
+  int64_t* rows;                   /* [n] out                                                               */
+  int64_t* status;                 /* device int64, 0 on entry; the first error as kind << 40 | table << 8 | server */
+  double timeout_s;                /* watchdog of the wait for a slot another thread is initialising        */
+} MvbHashLookup;
+/* empty keys, zero ready flags and counter of one server's index */
+int mvb_hash_rows_init(void* keys, void* ready, void* count, int64_t slots, void* stream);
+int mvb_hash_rows_lookup(const MvbHashLookup* a, void* stream);
+/* *out = live keys over all servers of the (host) descriptor */
+int mvb_hash_rows_count(const MvbHashRows* h, int64_t* out, void* stream);
+/* (key, row) of every live slot (ready == 1) of server `server`, in no particular order; *out_count on the device */
+int mvb_hash_rows_dump(const MvbHashRows* h, int server, int64_t* out_keys, int64_t* out_rows, int64_t* out_count,
+                       void* stream);
+
 /* ---- all-reduce (K6) --------------------------------------------------------- */
 /* One-shot P2P: every rank reads all peers' symmetric buffers and reduces locally
  * in fixed rank order (deterministic, identical on all ranks). Two-shot: reduce own

@@ -231,6 +231,15 @@ MVB_DEVINL uint64_t hash64(uint64_t x) {
   return x;
 }
 
+// Keyed tables (the KVTable, the hash index of HashMatrixTable): server `owner_of(key, S)` = key mod S (the
+// reference KVTable rule) holds a key; its probe chain starts at mix64(key) & (capacity - 1). mix64 is hash64 under
+// the name the probe rule is known by.
+MVB_DEVINL uint64_t mix64(uint64_t x) { return hash64(x); }
+MVB_DEVINL int owner_of(long long key, int S) {
+  long long m = key % S;
+  return (int)(m < 0 ? m + S : m);
+}
+
 MVB_DEVINL float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

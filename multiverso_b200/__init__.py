@@ -6,7 +6,7 @@ from .api import (aggregate, barrier, dashboard_display, init, is_master_worker,
                   save_table, server_id_to_rank, set_flag, shutdown, size, symm_tensor, worker_id, worker_id_to_rank,
                   workers_num)
 from . import ops, runtime  # noqa: F401
-from .tables import (AddOption, ArrayTable, ArrayTableOption, GetOption, KVTable, KVTableOption,
+from .tables import (AddOption, ArrayTable, ArrayTableOption, GetOption, HashMatrixTable, KVTable, KVTableOption,
                      MatrixOption, MatrixTable, MatrixTableOption, SparseMatrixTable,
                      SparseMatrixTableOption, create_table)
 from .utils import FLAGS, Dashboard, Log

@@ -77,6 +77,21 @@ class KV(C.Structure):
                 ("vals", VP8)]
 
 
+HASH_INIT_CONST, HASH_INIT_UNIFORM = 0, 1
+HASH_FULL, HASH_TIMEOUT, HASH_BAD_KEY = 1, 2, 3
+
+
+class HashRows(C.Structure):
+    _fields_ = [("nservers", C.c_int), ("slots", i64), ("keys", VP8), ("ready", VP8), ("count", VP8),
+                ("map", RowMap), ("init", C.c_int), ("init_value", C.c_float), ("lo", C.c_float),
+                ("hi", C.c_float), ("seed", C.c_uint64)]
+
+
+class HashLookup(C.Structure):
+    _fields_ = [("tables", vp), ("keys", vp), ("n", i64), ("seg_end", vp), ("seg_table", vp), ("G", C.c_int),
+                ("insert", C.c_int), ("insert_ok", vp), ("rows", vp), ("status", vp), ("timeout_s", C.c_double)]
+
+
 class Allreduce(C.Structure):
     _fields_ = [("dtype", C.c_int), ("n", i64), ("bufs", VP8), ("out", vp),
                 ("pads", C.POINTER(vp)), ("me", C.c_int), ("world", C.c_int), ("ch", C.c_int),
@@ -258,6 +273,10 @@ _CUDA_FUNCS = {
     "mvb_kv_add": _status(C.POINTER(KV), Ptr, Ptr, i64, Ptr, Ptr),
     "mvb_kv_get": _status(C.POINTER(KV), Ptr, Ptr, i64, Ptr),
     "mvb_kv_dump": _status(i32, Ptr, Ptr, i64, Ptr, Ptr, Ptr, Ptr),
+    "mvb_hash_rows_init": _status(Ptr, Ptr, Ptr, i64, Ptr),
+    "mvb_hash_rows_lookup": _status(C.POINTER(HashLookup), Ptr),
+    "mvb_hash_rows_count": _status(C.POINTER(HashRows), Ptr, Ptr),
+    "mvb_hash_rows_dump": _status(C.POINTER(HashRows), i32, Ptr, Ptr, Ptr, Ptr),
     "mvb_allreduce_oneshot": _status(C.POINTER(Allreduce), Ptr),
     "mvb_allreduce_twoshot": _status(C.POINTER(Allreduce), Ptr),
     "mvb_allreduce_fused": _status(C.POINTER(Allreduce), Ptr, i64, Ptr),

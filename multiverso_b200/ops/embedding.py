@@ -21,6 +21,11 @@ coalesced gradient times ``push_scale``:
   stateful updaters on the owners, stale marking of ``is_sparse`` tables). Sizing that buffer reads the number of
   unique ids on the host: one synchronisation per backward.
 
+Over a :class:`~multiverso_b200.tables.device.HashMatrixTable` the ids are int64 keys: one ``mvb_hash_rows_lookup``
+translates them to rows before the input checks (its status word is read in the checks' one host read), then the
+same kernels run on the rows. ``PSEmbedding`` in training mode inserts missing keys; in eval mode, and in
+``embedding_bag``, they read the zero row, and a backward after such a forward raises.
+
 On the host backend the same calls run :func:`embedding_bag_reference` over ``get_rows`` of the unique ids, and the
 backward pushes the gradient coalesced in torch with ``add_rows``: the same semantics.
 """
@@ -33,6 +38,7 @@ import torch
 import torch.nn.functional as F
 
 from .. import _native as N
+from ..tables.device import HashMatrixTable, raise_hash_status
 from ..tables.options import AddOption
 from ..utils import monitor
 from .topk import _rowmap_of
@@ -77,8 +83,10 @@ def _bags(ids, offsets, per_sample_weights, mode: str) -> Tuple[torch.Tensor, to
     return ids.reshape(-1).to(torch.int64).contiguous(), offsets.to(torch.int64).contiguous(), psw
 
 
-def _check_values(ids: torch.Tensor, offsets: torch.Tensor, num_row: int) -> None:
-    """ids in [0, num_row) and offsets that start at 0, never decrease and stay within the ids (one host read)."""
+def _check_values(ids: torch.Tensor, offsets: torch.Tensor, num_row: int, status: Optional[torch.Tensor] = None,
+                  hash_table=None) -> None:
+    """ids in [0, num_row) and offsets that start at 0, never decrease and stay within the ids (one host read).
+    ``status``: the status word of the hash translation that produced ``ids``, read in the same copy."""
     L, B = ids.numel(), offsets.numel()
     if B == 0:
         if L:
@@ -87,7 +95,11 @@ def _check_values(ids: torch.Tensor, offsets: torch.Tensor, num_row: int) -> Non
     parts = [offsets[:1], (offsets[1:] < offsets[:-1]).any().view(1).to(torch.int64), offsets[-1:]]
     if L:
         parts += list(torch.aminmax(ids))
+    if status is not None:
+        parts.append(status)
     v = torch.cat([p.view(-1) for p in parts]).tolist()
+    if status is not None:
+        raise_hash_status(v.pop(), [hash_table])
     if v[0] != 0:
         raise ValueError(f"embedding_bag: offsets must start at 0, got {v[0]}")
     if v[1]:
@@ -231,8 +243,9 @@ def _host_backward(ctx, ids, offsets, psw, dout):
 # ------------------------------------------------------------------------------------------------ autograd
 class _EmbeddingBagFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, anchor, psw, table, ids, offsets, mode, push_scale, option):
+    def forward(ctx, anchor, psw, table, ids, offsets, mode, push_scale, option, frozen):
         ctx.table, ctx.mode, ctx.push_scale, ctx.option = table, mode, push_scale, option
+        ctx.frozen = frozen
         ctx.anchor = None if anchor is None else (anchor.shape, anchor.dtype, anchor.device)
         ctx.psw_like = None if psw is None else (psw.dtype, psw.device)
         dev = _device_of(table)
@@ -257,6 +270,9 @@ class _EmbeddingBagFn(torch.autograd.Function):
     def backward(ctx, dout):
         ids, offsets, psw = ctx.saved_tensors
         dpsw = None
+        if ctx.frozen and ctx.push_scale is not None:
+            raise RuntimeError("PSEmbedding: backward after a forward that inserted no keys (eval mode): missing keys "
+                               "share the zero row, which must not be pushed to; run the forward in training mode")
         if ctx.device:
             if ctx.needs_input_grad[1]:
                 dpsw = _psw_grad_device(ctx.rm, ctx.dim, ids, offsets, ctx.mode, dout)
@@ -270,10 +286,12 @@ class _EmbeddingBagFn(torch.autograd.Function):
         if ctx.anchor is not None:
             shape, dtype, device = ctx.anchor
             da = torch.zeros(shape, dtype=dtype, device=device)
-        return da, dpsw, None, None, None, None, None, None
+        return da, dpsw, None, None, None, None, None, None, None
 
 
-def _prepare(table, ids, offsets, per_sample_weights, mode):
+def _prepare(table, ids, offsets, per_sample_weights, mode, insert: bool = False):
+    """Checked (ids, offsets, weights) of a call; for a HashMatrixTable the ids are keys, translated to rows first
+    (``insert``: missing keys get rows; otherwise they read the zero row)."""
     if _dtype_of(table) != torch.float32:
         raise TypeError(f"embedding_bag: the table must be float32, got {_dtype_of(table)}")
     ids, offsets, psw = _bags(ids, offsets, per_sample_weights, mode)
@@ -284,19 +302,26 @@ def _prepare(table, ids, offsets, per_sample_weights, mode):
             raise ValueError(f"embedding_bag: the table's row pitch ({rm.num_col} floats) must be a multiple of 4 "
                              "(16-byte row loads)")
         ids, offsets = ids.to(dev), offsets.to(dev)
-    _check_values(ids, offsets, table.shape[0] if isinstance(table, torch.Tensor) else table.num_row)
+    num_row = table.shape[0] if isinstance(table, torch.Tensor) else table.num_row
+    if isinstance(table, HashMatrixTable):
+        rows, status = torch.empty_like(ids), torch.empty(1, dtype=torch.int64, device=dev)
+        table.lookup_call(ids, rows, status, insert)
+        _check_values(rows, offsets, num_row, status, table)
+        return rows, offsets, psw
+    _check_values(ids, offsets, num_row)
     return ids, offsets, psw
 
 
 def embedding_bag(table, ids, offsets=None, per_sample_weights=None, mode: str = "sum") -> torch.Tensor:
     """Bags of table rows: ``[B, dim]``. ``table``: MatrixTable (device or host backend) or a 2-D fp32 tensor
-    (a CUDA tensor may be a column slice of a wider pitch: only its columns are read); ``ids``: int32 / int64,
+    (a CUDA tensor may be a column slice of a wider pitch: only its columns are read), or a HashMatrixTable, whose
+    ids are keys (a missing key adds zeros and is not inserted); ``ids``: int32 / int64,
     1-D with ``offsets`` or 2-D ``[B, n]``; ``per_sample_weights``: the shape of ``ids``, ``mode="sum"`` only.
     Differentiable in ``per_sample_weights``; nothing is pushed to the table (see :class:`PSEmbedding`)."""
     ids, offsets, psw = _prepare(table, ids, offsets, per_sample_weights, mode)
     if isinstance(table, torch.Tensor) and not table.is_cuda:
         return F.embedding_bag(ids, table, offsets, mode=mode, per_sample_weights=psw)
-    return _EmbeddingBagFn.apply(None, psw, table, ids, offsets, mode, None, None)
+    return _EmbeddingBagFn.apply(None, psw, table, ids, offsets, mode, None, None, False)
 
 
 class PSEmbedding(torch.nn.Module):
@@ -318,9 +343,11 @@ class PSEmbedding(torch.nn.Module):
         self.anchor = torch.nn.Parameter(torch.zeros(0))
 
     def forward(self, ids, offsets=None, per_sample_weights=None) -> torch.Tensor:
-        ids, offsets, psw = _prepare(self.table, ids, offsets, per_sample_weights, self.mode)
+        # over a HashMatrixTable the ids are keys: training inserts the missing ones, eval reads them as zeros
+        frozen = isinstance(self.table, HashMatrixTable) and not self.training
+        ids, offsets, psw = _prepare(self.table, ids, offsets, per_sample_weights, self.mode, insert=self.training)
         return _EmbeddingBagFn.apply(self.anchor, psw, self.table, ids, offsets, self.mode, self.push_scale,
-                                     self.option)
+                                     self.option, frozen)
 
     def extra_repr(self) -> str:
         return (f"{self.num_embeddings}, {self.embedding_dim}, mode={self.mode!r}, "

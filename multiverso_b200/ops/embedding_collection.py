@@ -26,6 +26,10 @@ Host synchronisation: the input checks read the device once per forward, however
 backward does not synchronise when every pushing table takes the fused ``red.add`` push (``default`` / ``sgd``,
 not ``is_sparse``); otherwise it reads the unique-row counts of all compact tables in one copy.
 
+A config may name a ``HashMatrixTable``: its features' ids are then int64 keys, translated to rows by one launch per
+call that covers every hash feature (dense features' ids pass through unchanged), before the input checks and inside
+their one host read. In training mode missing keys are inserted; in eval mode they add zeros and a backward raises.
+
 On the host backend the same module runs ``get_rows`` of the unique ids of each table over all of its features,
 torch's ``embedding_bag`` per feature, and in the backward one coalesced ``add_rows`` per table: the same semantics.
 """
@@ -38,6 +42,7 @@ import torch
 import torch.nn.functional as F
 
 from .. import _native as N
+from ..tables.device import HashMatrixTable, raise_hash_status
 from ..tables.options import AddOption
 from ..utils import monitor
 from .embedding import MODES, _INT, _device_of, _dtype_of, _host_rows
@@ -122,8 +127,17 @@ class PSEmbeddingCollection(torch.nn.Module):
         # ids in range are checked against the table of each lookup's own feature
         self._rows_of_feature = torch.tensor([self._num_rows[t] for t in feat_table], dtype=torch.int64,
                                              device=self._device)
+        self._hash = [c.table for c in configs if isinstance(c.table, HashMatrixTable)]
         if self._device is not None:
             self._build_device()
+        if self._hash:
+            # one translation launch covers every hash feature: the index descriptors of the hash tables, and per
+            # feature the descriptor of its table (-1: a dense table, whose ids are copied unchanged)
+            slot = {id(t): k for k, t in enumerate(self._hash)}
+            descs = (N.HashRows * len(self._hash))(*[t._hash for t in self._hash])
+            self._d_hash = _device_array(descs, self._device)
+            self._seg_table = torch.tensor([slot.get(id(configs[t].table), -1) for t in feat_table],
+                                           dtype=torch.int32, device=self._device)
         # ids never require grad: without an input that does, autograd would skip the backward and so the push
         self.anchor = torch.nn.Parameter(torch.zeros(0))
 
@@ -206,13 +220,38 @@ class PSEmbeddingCollection(torch.nn.Module):
         dev = self._device if self._device is not None else torch.device("cpu")
         ids = ids.to(device=dev, dtype=torch.int64).contiguous()
         lengths = lengths.to(device=dev, dtype=torch.int64).contiguous()
-        self._check_values(ids, lengths)
+        status = None
+        if self._hash:
+            ids, status = self._translate(ids, lengths)
+        self._check_values(ids, lengths, status)
         flat = lengths.view(-1)
         offsets = torch.cumsum(flat, 0) - flat
         return ids, lengths, offsets, psw
 
-    def _check_values(self, ids: torch.Tensor, lengths: torch.Tensor) -> None:
-        """Non-negative lengths that sum to len(ids), and every id inside its own feature's table: one host read."""
+    def _translate(self, ids: torch.Tensor, lengths: torch.Tensor):
+        """The keys of the hash features as rows (training: missing keys get rows), the other ids unchanged: one
+        launch. Returns (rows, status word of the translation). The feature of a lookup comes from the lengths,
+        which are checked only afterwards: lengths that do not sum to len(ids) or hold a negative value would hand
+        keys to the wrong table, so with those nothing is inserted (a device-side test, no host read) and the checks
+        then raise."""
+        rows = torch.empty_like(ids)
+        status = torch.empty(1, dtype=torch.int64, device=ids.device)
+        if ids.numel():
+            seg_end = torch.cumsum(lengths.sum(1), 0)
+            ok = None
+            if self.training:
+                ok = (seg_end[-1:] == ids.numel()).to(torch.int64)
+                if lengths.numel():
+                    ok &= (lengths.view(-1).min().view(1) >= 0).to(torch.int64)
+            self._hash[0].lookup_call(ids, rows, status, self.training, seg_end, self._seg_table, self._d_hash,
+                                      insert_ok=ok)
+        else:
+            status.zero_()
+        return rows, status
+
+    def _check_values(self, ids: torch.Tensor, lengths: torch.Tensor, status: Optional[torch.Tensor] = None) -> None:
+        """Non-negative lengths that sum to len(ids), and every id inside its own feature's table: one host read.
+        ``status``: the status word of the hash translation, read in the same copy."""
         L, flat = ids.numel(), lengths.view(-1)
         zero = torch.zeros(1, dtype=torch.int64, device=ids.device)
         parts = [flat.sum().view(1), flat.min().view(1) if flat.numel() else zero]
@@ -223,7 +262,11 @@ class PSEmbeddingCollection(torch.nn.Module):
             bad = (ids < 0) | (ids >= self._rows_of_feature[feat])
             first = bad.to(torch.int32).argmax().view(1)
             parts += [bad.any().view(1).to(torch.int64), feat.index_select(0, first), ids.index_select(0, first)]
+        if status is not None:
+            parts.append(status)
         v = torch.cat(parts).tolist()
+        if status is not None:
+            raise_hash_status(v.pop(), self._hash)
         if v[1] < 0:
             raise ValueError(f"{_WHAT}: lengths must be non-negative, got {v[1]}")
         if v[0] != L:
@@ -238,7 +281,10 @@ class PSEmbeddingCollection(torch.nn.Module):
         """``ids`` 1-D int32 / int64, feature-major; ``lengths`` ``[F, B]``; ``per_sample_weights`` the shape of
         ``ids`` (every table ``mode="sum"``), differentiable. Returns ``[B, sum of feature dims]``."""
         ids, lengths, offsets, psw = self._inputs(ids, lengths, per_sample_weights)
-        return _CollectionFn.apply(self.anchor, psw, self, ids, lengths, offsets)
+        # a hash table looked up in eval mode inserted nothing: its missing keys share the zero row, never pushed to
+        frozen = not self.training and any(isinstance(c.table, HashMatrixTable) and c.push_scale is not None
+                                           for c in self.configs)
+        return _CollectionFn.apply(self.anchor, psw, self, ids, lengths, offsets, frozen)
 
     def split(self, out: torch.Tensor) -> Dict[str, torch.Tensor]:
         """The output of :meth:`forward` as ``{feature: [B, dim]}`` column views."""
@@ -366,8 +412,8 @@ class PSEmbeddingCollection(torch.nn.Module):
 
 class _CollectionFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, anchor, psw, coll, ids, lengths, offsets):
-        ctx.coll = coll
+    def forward(ctx, anchor, psw, coll, ids, lengths, offsets, frozen):
+        ctx.coll, ctx.frozen = coll, frozen
         ctx.anchor = (anchor.shape, anchor.dtype, anchor.device)
         ctx.psw_like = None if psw is None else (psw.dtype, psw.device)
         B = lengths.shape[1]
@@ -384,6 +430,9 @@ class _CollectionFn(torch.autograd.Function):
     def backward(ctx, dout):
         ids, offsets, psw = ctx.saved_tensors
         coll, need_dpsw, dpsw = ctx.coll, ctx.needs_input_grad[1], None
+        if ctx.frozen:
+            raise RuntimeError(f"{_WHAT}: backward after an eval-mode forward over a HashMatrixTable: it inserted no "
+                               "keys, and the missing ones share the zero row, which must not be pushed to")
         if coll._device is not None:
             d = coll._dout_device(dout)
             if need_dpsw:
@@ -396,4 +445,4 @@ class _CollectionFn(torch.autograd.Function):
         else:
             dpsw = None
         shape, dtype, device = ctx.anchor
-        return torch.zeros(shape, dtype=dtype, device=device), dpsw, None, None, None, None
+        return torch.zeros(shape, dtype=dtype, device=device), dpsw, None, None, None, None, None

@@ -42,6 +42,17 @@ def KVTable(key_dtype="int64", val_dtype="float32", capacity=None):
     return HostKVTable(key_dtype, val_dtype)
 
 
+def HashMatrixTable(capacity, num_col, dtype="float32", updater=None, init_value=None, min_value=None,
+                    max_value=None, seed=1):
+    """fp32 rows keyed by any int64, allocated on first lookup (device backend only; see
+    :class:`multiverso_b200.tables.device.HashMatrixTable`)."""
+    if not _device():
+        raise NotImplementedError("HashMatrixTable needs the device backend (a CUDA device): its index is a GPU "
+                                  "hash table; the host backend has no counterpart")
+    from .device import HashMatrixTable as _Hash
+    return _Hash(capacity, num_col, dtype, updater, init_value, min_value, max_value, seed)
+
+
 def create_table(option):
     """MV_CreateTable(option)."""
     if isinstance(option, MatrixOption):
@@ -74,6 +85,6 @@ def FTRLTable(size):
     return FTRLDeviceTable(size)
 
 
-__all__ = ["SparseTable", "FTRLTable", "ArrayTable", "MatrixTable", "SparseMatrixTable", "KVTable", "create_table", "AddOption",
-           "GetOption", "ArrayTableOption", "MatrixTableOption", "MatrixOption",
+__all__ = ["SparseTable", "FTRLTable", "ArrayTable", "MatrixTable", "HashMatrixTable", "SparseMatrixTable",
+           "KVTable", "create_table", "AddOption", "GetOption", "ArrayTableOption", "MatrixTableOption", "MatrixOption",
            "SparseMatrixTableOption", "KVTableOption"]

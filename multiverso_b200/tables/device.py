@@ -766,6 +766,193 @@ class MatrixDeviceTable(DenseDeviceTable):
         return ids, self.get_rows(ids)
 
 
+INT64_MIN = -(1 << 63)
+
+
+def raise_hash_status(code: int, tables: Sequence["HashMatrixTable"]) -> None:
+    """Raise the error of a non-zero status word of ``mvb_hash_rows_lookup`` (``tables``: by descriptor index)."""
+    if not code:
+        return
+    kind, t, server = code >> 40, (code >> 8) & 0xFFFFFFFF, code & 0xFF
+    tid = tables[t].table_id if t < len(tables) else "?"
+    if kind == N.HASH_BAD_KEY:
+        raise ValueError(f"HashMatrixTable #{tid}: key {INT64_MIN} (INT64_MIN) is reserved for empty slots")
+    if kind == N.HASH_FULL:
+        tab = tables[t] if t < len(tables) else None
+        limit = f" (at most {7 * tab.slots // 8} keys per server)" if tab is not None else ""
+        raise RuntimeError(f"HashMatrixTable #{tid}: table full on server {server}{limit}; keys inserted before "
+                           "stay valid")
+    if kind == N.HASH_TIMEOUT:
+        raise RuntimeError(f"HashMatrixTable #{tid}: timed out waiting for a row of server {server} to be "
+                           "initialised (-barrier_timeout_s)")
+    raise RuntimeError(f"HashMatrixTable #{tid}: lookup status {code:#x}")
+
+
+class HashMatrixTable(MatrixDeviceTable):
+    """Rows keyed by any int64 (but INT64_MIN), one row per distinct key, allocated on first lookup.
+
+    A ``MatrixDeviceTable`` of ``S P + 1`` fp32 rows plus a device hash index (``csrc/cuda/hash_rows.cu``): server
+    ``s = key mod S`` owns the key, and the ``P`` slots of server ``s`` are rows ``[s P, (s + 1) P)``. The last row is
+    the zero row, which every missing key reads and which no key ever gets. ``P`` is the smallest power of two with
+    ``floor(7 P / 8) >= ceil(capacity / S)``, so each server holds at most ``floor(7 P / 8)`` keys; an insert beyond
+    that raises "table full" and leaves the keys inserted before valid.
+
+    ``lookup`` translates keys to rows; the inherited row ops (``get_rows``, ``add_rows``, the updaters, row
+    mailboxes) then work on them unchanged. ``get`` and ``add`` take keys, like the KVTable's; the whole-table
+    dense ``get`` / ``add`` are not offered, because their layout is the slot layout.
+
+    A key's initial row depends on the key only: ``init_value`` (default 0) in every column, or, with
+    ``min_value`` and ``max_value``, ``lo + u (hi - lo)`` with ``u`` drawn from ``(key, seed, column)``. Which slot
+    (row id) a key gets depends on the order in which keys arrive, which may depend on timing; nothing else does."""
+
+    def __init__(self, capacity: int, num_col: int, dtype="float32", updater: Optional[str] = None,
+                 init_value=None, min_value=None, max_value=None, seed: int = 1):
+        rt = Runtime.get()
+        if not rt.started:
+            Log.fatal("MV_Init must be called before creating tables")
+        if _torch_dtype(dtype) != torch.float32:
+            raise TypeError(f"HashMatrixTable: rows are float32, got {dtype}")
+        capacity, num_col = int(capacity), int(num_col)
+        if capacity < 1:
+            raise ValueError(f"HashMatrixTable: capacity must be >= 1, got {capacity}")
+        if num_col < 1 or num_col % 4:
+            raise ValueError(f"HashMatrixTable: num_col must be a positive multiple of 4 (16-byte row "
+                             f"initialisation), got {num_col}")
+        S = max(rt.num_servers(), 1)
+        per_server = -(-capacity // S)
+        P = 2
+        while 7 * P // 8 < per_server:
+            P *= 2
+        self.capacity, self.slots = capacity, P
+        super().__init__(S * P + 1, num_col, "float32", updater)
+        lib = N.cuda_lib()
+        self._keys_buf = rt.alloc_symm(P * 8)
+        self._ready_buf = rt.alloc_symm(P * 4)
+        self._count_buf = rt.alloc_symm(8)
+        lib.mvb_hash_rows_init(self._keys_buf.local_ptr, self._ready_buf.local_ptr, self._count_buf.local_ptr, P,
+                               N.stream_ptr())
+        h = N.HashRows()
+        h.nservers, h.slots = self.S, P
+        for s in range(self.S):
+            r = rt.server_id_to_rank(s) if rt.num_servers() else rt.rank
+            h.keys[s], h.ready[s], h.count[s] = self._keys_buf.ptrs[r], self._ready_buf.ptrs[r], self._count_buf.ptrs[r]
+        h.map = self._rowmap
+        if min_value is not None and max_value is not None:
+            h.init, h.lo, h.hi = N.HASH_INIT_UNIFORM, float(min_value), float(max_value)
+        else:
+            h.init, h.init_value = N.HASH_INIT_CONST, float(init_value or 0.0)
+        h.seed = int(seed) & ((1 << 64) - 1)
+        self._hash = h
+        self._d_hash = torch.frombuffer(bytearray(h), dtype=torch.uint8).to(rt.device)
+        self.zero_row = self.S * P
+        torch.cuda.synchronize()
+        rt.barrier()            # every index is initialised before any rank inserts into it
+
+    # ---- keys -> rows ------------------------------------------------------------------
+    def _key_tensor(self, keys) -> torch.Tensor:
+        t = torch.as_tensor(keys)
+        if t.dtype not in (torch.int32, torch.int64):
+            raise TypeError(f"HashMatrixTable: keys must be int32 or int64, got {t.dtype}")
+        return t.to(device=self.rt.device, dtype=torch.int64).contiguous().view(-1)
+
+    def lookup_call(self, keys: torch.Tensor, rows: torch.Tensor, status: torch.Tensor, insert: bool,
+                    seg_end: Optional[torch.Tensor] = None, seg_table: Optional[torch.Tensor] = None,
+                    tables: Optional[torch.Tensor] = None, insert_ok: Optional[torch.Tensor] = None) -> None:
+        """Launch one translation of int64 device ``keys`` into ``rows`` (no host read). ``status`` (device int64,
+        zeroed here) receives the first error; ``raise_hash_status`` interprets it. ``seg_end`` / ``seg_table`` /
+        ``tables``: several indexes in one launch (see ``MvbHashLookup``). ``insert_ok``: device int64; when it
+        holds 0 nothing is inserted."""
+        a = N.HashLookup()
+        a.tables = (self._d_hash if tables is None else tables).data_ptr()
+        a.keys, a.n, a.rows, a.status = keys.data_ptr(), keys.numel(), rows.data_ptr(), status.data_ptr()
+        a.seg_end, a.seg_table = N.ptr(seg_end), N.ptr(seg_table)
+        a.G = 0 if seg_end is None else seg_end.numel()
+        a.insert, a.insert_ok = int(bool(insert)), N.ptr(insert_ok)
+        a.timeout_s = float(FLAGS.get("barrier_timeout_s"))
+        status.zero_()
+        with monitor("WORKER_TABLE_HASH_LOOKUP", cuda=True):
+            N.cuda_lib().mvb_hash_rows_lookup(a, N.stream_ptr())
+
+    def lookup(self, keys, insert: bool = True) -> torch.Tensor:
+        """int64 rows of ``keys`` (device tensor). ``insert``: a missing key gets a row, initialised; otherwise it
+        reads the zero row. INT64_MIN raises ValueError before anything is inserted."""
+        k = self._key_tensor(keys)
+        rows = torch.empty_like(k)
+        if k.numel():
+            if bool((k == INT64_MIN).any()):
+                raise ValueError(f"HashMatrixTable #{self.table_id}: key {INT64_MIN} (INT64_MIN) is reserved for "
+                                 "empty slots")
+            status = torch.empty(1, dtype=torch.int64, device=self.rt.device)
+            self.lookup_call(k, rows, status, insert)
+            raise_hash_status(int(status.item()), [self])
+        return rows
+
+    def get(self, keys, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Rows of ``keys`` ``[n, num_col]``; a missing key reads zeros and is not inserted."""
+        return self.get_rows(self.lookup(keys, insert=False), out)
+
+    def add(self, keys, values, option: Optional[AddOption] = None) -> None:
+        """Insert the missing keys, then ``add_rows`` of their rows (the table's updater, ``option``)."""
+        self.add_rows(self.lookup(keys, insert=True), values, option)
+
+    def get_async(self, *args, **kwargs):
+        raise TypeError("HashMatrixTable: the whole-table get is not offered (its layout is the slot layout); "
+                        "use get(keys) or export()")
+
+    def add_async(self, *args, **kwargs):
+        raise TypeError("HashMatrixTable: the whole-table add is not offered (its layout is the slot layout); "
+                        "use add(keys, values)")
+
+    def num_keys(self) -> int:
+        """Keys held over all servers (reads the device)."""
+        out = torch.empty(1, dtype=torch.int64, device=self.rt.device)
+        N.cuda_lib().mvb_hash_rows_count(self._hash, out, N.stream_ptr())
+        return int(out.item())
+
+    def _dump(self, server: int):
+        keys = torch.empty(self.slots, dtype=torch.int64, device=self.rt.device)
+        rows = torch.empty_like(keys)
+        cnt = torch.empty(1, dtype=torch.int64, device=self.rt.device)
+        N.cuda_lib().mvb_hash_rows_dump(self._hash, server, keys, rows, cnt, N.stream_ptr())
+        n = int(cnt.item())
+        return keys[:n], rows[:n]
+
+    def export(self):
+        """(keys ascending [K] int64, their rows' values [K, num_col]) over all servers, on the device."""
+        parts = [self._dump(s) for s in range(self.S)]
+        keys = torch.cat([k for k, _ in parts])
+        rows = torch.cat([r for _, r in parts])
+        keys, order = torch.sort(keys)
+        return keys, self.get_rows(rows[order])
+
+    def store(self, stream) -> None:
+        """This rank's shard and updater state (the slot layout), then its server's keys. A table of the same
+        capacity, width and number of servers loads it back with every key in its slot."""
+        super().store(stream)
+        torch.cuda.current_stream().synchronize()
+        stream.write(self._keys_buf.tensor(torch.int64, self.slots).cpu().numpy().tobytes())
+        stream.write(self._ready_buf.tensor(torch.int32, self.slots).cpu().numpy().tobytes())
+
+    def load(self, stream) -> None:
+        import numpy as np
+        super().load(stream)
+        raw = stream.read(self.slots * 12)
+        if len(raw) != self.slots * 12:
+            raise ValueError(f"HashMatrixTable #{self.table_id}: the stream holds no index of {self.slots} slots")
+        arr = np.frombuffer(raw, dtype=np.uint8)
+        keys = torch.from_numpy(arr[:self.slots * 8].view(np.int64).copy()).to(self.rt.device)
+        ready = torch.from_numpy(arr[self.slots * 8:].view(np.int32).copy()).to(self.rt.device)
+        self._keys_buf.tensor(torch.int64, self.slots).copy_(keys)
+        self._ready_buf.tensor(torch.int32, self.slots).copy_(ready)
+        self._count_buf.tensor(torch.int64, 1).fill_(int((ready == 1).sum()))     # refused slots hold no row
+        torch.cuda.synchronize()
+
+    def free(self) -> None:
+        super().free()
+        for b in (self._keys_buf, self._ready_buf, self._count_buf):
+            self.rt.release_symm(b)
+
+
 class KVDeviceTable(_AsyncOps):
     """KVTable<K,V>: hash-partitioned map (key % num_servers) as per-shard GPU hash tables.
 
