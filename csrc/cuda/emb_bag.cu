@@ -98,14 +98,14 @@ __global__ void __launch_bounds__(256)
 emb_psw_grad_kernel(const __grid_constant__ MvbEmbBag a) {
   for (int64_t j = warp_id(); j < a.L; j += num_warps()) {
     const int64_t b = bag_of(a.offsets, a.B, j);
-    const float dot = emb_psw_dot(row_of(a.wmap, __ldg(a.ids + j)), a.dout + b * a.ldd, (int)a.dim);
+    const float dot = emb_psw_dot(row_ptr<const float>(a.wmap, __ldg(a.ids + j)), a.dout + b * a.ldd, (int)a.dim);
     if ((threadIdx.x & 31) == 0) a.dpsw[j] = a.mean ? dot / (float)bag_len(a.offsets, a.B, a.L, b) : dot;
   }
 }
 
 int check_common(const MvbEmbBag* a, bool need_out) {
   const MvbRowMap& wm = a->wmap;
-  if (wm.nservers < 1 || wm.nservers > MVB_MAX_RANKS || wm.rows_per_server < 1) return -50;
+  if (!row_split_ok(wm.nservers, wm.rows_per_server)) return -50;
   if (wm.num_col % 4 != 0) return -51;
   if (a->dim < 1 || a->dim > wm.num_col) return -52;
   if (a->L < 0 || a->B < 0 || (a->B > 0 && !a->offsets)) return -53;

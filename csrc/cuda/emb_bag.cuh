@@ -55,13 +55,6 @@ auto with_vpl(int vpl, F&& f) {
   return f(std::integral_constant<int, 4>{});
 }
 
-// row r: owner = r / rows_per_server, the last server takes the remainder (matrix_table.cpp:270-273)
-MVB_DEVINL float* row_of(const MvbRowMap& m, int64_t r) {
-  int64_t o = r / m.rows_per_server;
-  if (o > m.nservers - 1) o = m.nservers - 1;
-  return (float*)m.shard_ptrs[o] + (r - o * m.rows_per_server) * m.num_col;
-}
-
 MVB_DEVINL float4 f4(uint4 u) {
   return make_float4(__uint_as_float(u.x), __uint_as_float(u.y), __uint_as_float(u.z), __uint_as_float(u.w));
 }
@@ -106,17 +99,6 @@ MVB_DEVINL int64_t bag_len(const int64_t* __restrict__ off, int64_t B, int64_t L
 
 MVB_DEVINL bool run_start(const int64_t* __restrict__ sid, int64_t i) { return i == 0 || sid[i] != sid[i - 1]; }
 
-// the warp's index and the number of warps of a grid-stride loop
-MVB_DEVINL int64_t warp_id() { return ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; }
-MVB_DEVINL int64_t num_warps() { return ((int64_t)gridDim.x * blockDim.x) >> 5; }
-
-int grid_for(int64_t warps) {
-  int64_t blocks = (warps * 32 + 255) / 256;
-  const int64_t cap = (int64_t)mvb_num_sms() * 8;
-  if (blocks > cap) blocks = cap;
-  return (int)(blocks < 1 ? 1 : blocks);
-}
-
 // ------------------------------------------------------------------------------------------------ forward
 // the lookups [lo, hi) of one bag pooled into out[0 .. dim), lane groups of 1 << lg lanes
 template <int VPL>
@@ -144,7 +126,7 @@ MVB_DEVINL void emb_pool_bag(const MvbRowMap& m, int dim, int lg, const int64_t*
 #pragma unroll
           for (int k = 0; k < VPL; ++k) x[u][k] = zero4();
           if (t < n) {
-            const float* row = row_of(m, id);
+            const float* row = row_ptr<const float>(m, id);
 #pragma unroll
             for (int k = 0; k < VPL; ++k) {
               const int v = v0 + gl + k * G;
@@ -234,7 +216,7 @@ MVB_DEVINL void emb_epilogue(bool push, const MvbRowMap& m, int64_t id, float* g
                              int64_t uoff, int dim, float scale, int v0, const float4* g) {
   const int nv = (dim + 3) >> 2, lane = threadIdx.x & 31;
   if (push) {
-    float* row = row_of(m, id);
+    float* row = row_ptr<float>(m, id);
 #pragma unroll
     for (int k = 0; k < VPL; ++k) {
       const int v = v0 + lane + 32 * k;

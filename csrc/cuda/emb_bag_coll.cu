@@ -185,7 +185,7 @@ emb_coll_psw_grad_kernel(const __grid_constant__ MvbEmbColl a) {
     const int64_t g = bag_of(a.offsets, FB, j), f = g / a.B;
     const MvbEmbFeature* ft = a.features + f;
     const MvbEmbTable* tb = a.tables + ft->table;
-    const float dot = emb_psw_dot(row_of(tb->wmap, __ldg(a.ids + j)), a.dout + (g - f * a.B) * a.ldd + ft->col,
+    const float dot = emb_psw_dot(row_ptr<const float>(tb->wmap, __ldg(a.ids + j)), a.dout + (g - f * a.B) * a.ldd + ft->col,
                                   (int)tb->dim);
     if ((threadIdx.x & 31) == 0) a.dpsw[j] = tb->mean ? dot / (float)bag_len(a.offsets, FB, a.L, g) : dot;
   }

@@ -170,10 +170,8 @@ int launch_get_gemm(const MvbGetGemm* h, cudaStream_t st) {
   if (rc) return rc;
   int tiles = 0;
   for (int s = 0; s < wm.nservers; ++s) {
-    int64_t lo = wm.rows_per_server * s;
-    int64_t hi = (s == wm.nservers - 1) ? wm.num_row : wm.rows_per_server * (s + 1);
-    if (lo > wm.num_row) lo = wm.num_row;
-    if (hi > wm.num_row) hi = wm.num_row;
+    const RowRange rs = server_rows(wm, s);
+    const int64_t lo = std::min(rs.lo, wm.num_row), hi = std::min(rs.hi, wm.num_row);
     g.row_begin[s] = lo;
     g.row_begin[s + 1] = hi;
     g.tile_begin[s] = tiles;
@@ -209,6 +207,6 @@ extern "C" int mvb_get_gemm_fused(const MvbGetGemm* h, void* stream) {
   // TMA needs 16-byte aligned row pitches
   if (h->K % 4 != 0) return -32;
   const MvbRowMap& wm = h->wmap;
-  if (wm.nservers < 1 || wm.nservers > MVB_MAX_RANKS || wm.num_col != h->K || wm.num_row != h->N) return -33;
+  if (!row_split_ok(wm.nservers, wm.rows_per_server) || wm.num_col != h->K || wm.num_row != h->N) return -33;
   return launch_get_gemm(h, st);
 }

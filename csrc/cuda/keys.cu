@@ -20,8 +20,7 @@ struct KeysDev {
   unsigned int* touched[MVB_MAX_RANKS];
 };
 MVB_DEVINL void locate(const KeysDev& m, int64_t key, int& o, int64_t& local) {
-  int64_t s = key / m.per;
-  if (s > m.S - 1) s = m.S - 1;
+  const int64_t s = row_server(key, m.per, m.S);
   o = (int)s;
   local = key - s * m.per;
 }
@@ -104,7 +103,7 @@ KeysDev to_dev(const MvbKeyMap* h) {
   KeysDev m{};
   m.size = h->size;
   m.S = h->nservers;
-  m.per = h->per_server > 0 ? h->per_server : 1;
+  m.per = h->per_server;
   m.width = h->width;
   for (int s = 0; s < MVB_MAX_RANKS; ++s) {
     m.shard[s] = s < h->nservers ? (float*)h->shard_ptrs[s] : nullptr;
@@ -122,6 +121,7 @@ int blocks_for(int64_t n) {
 
 extern "C" int mvb_keys_add(const MvbKeyMap* m, const int64_t* keys, const float* vals, int64_t n, float sign,
                             void* stream) {
+  if (!row_split_ok(m->nservers, m->per_server)) return MVB_BAD_ROW_MAP;
   if (n <= 0) return 0;
   if (m->width < 1 || m->width > 16) return -8;
   keys_add_kernel<<<blocks_for(n * m->width), 256, 0, (cudaStream_t)stream>>>(to_dev(m), (const long long*)keys, vals, n, sign);
@@ -129,6 +129,7 @@ extern "C" int mvb_keys_add(const MvbKeyMap* m, const int64_t* keys, const float
   return 0;
 }
 extern "C" int mvb_keys_get(const MvbKeyMap* m, const int64_t* keys, float* out, int64_t n, void* stream) {
+  if (!row_split_ok(m->nservers, m->per_server)) return MVB_BAD_ROW_MAP;
   if (n <= 0) return 0;
   keys_get_kernel<<<blocks_for(n * m->width), 256, 0, (cudaStream_t)stream>>>(to_dev(m), (const long long*)keys, out, n);
   MVB_CUDA_CHECK(cudaGetLastError());
@@ -137,6 +138,7 @@ extern "C" int mvb_keys_get(const MvbKeyMap* m, const int64_t* keys, float* out,
 // Every touched key (ascending inside a shard is NOT guaranteed) with its values; *count may exceed cap.
 extern "C" int mvb_keys_collect(const MvbKeyMap* m, int64_t* out_keys, float* out_vals, int64_t* count, int64_t cap,
                                 void* stream) {
+  if (!row_split_ok(m->nservers, m->per_server)) return MVB_BAD_ROW_MAP;
   cudaStream_t st = (cudaStream_t)stream;
   MVB_CUDA_CHECK(cudaMemsetAsync(count, 0, 8, st));
   keys_collect_kernel<<<blocks_for((m->size + 31) / 32 + m->nservers), 256, 0, st>>>(to_dev(m), (long long*)out_keys, out_vals,

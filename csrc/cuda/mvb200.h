@@ -165,6 +165,13 @@ int mvb_push_dense_stateful(int dtype, int updater, const void* delta, int nserv
                             const int64_t* state_strides, const MvbAddOpt* opt, int me, void* stream);
 
 /* ---- row-sparse Get / Add (K3, K4, K10) ------------------------------------ */
+/* Server min(r / rows_per_server, nservers - 1) holds row r, at local index r - server * rows_per_server.
+ * Every entry point that takes a row map, directly or inside another descriptor, needs
+ * 1 <= nservers <= MVB_MAX_RANKS and rows_per_server >= 1, and checks it before any CUDA call. A map that
+ * fails returns MVB_BAD_ROW_MAP, except from the entry points with an older code of their own:
+ * mvb_get_gemm_fused -33, mvb_topk_cosine and mvb_full_softmax -41, mvb_embedding_bag_* -50 and
+ * mvb_sgns_train_win -21. The mvb_keys_* entry points check their MvbKeyMap in the same way. */
+enum { MVB_BAD_ROW_MAP = -70 };
 typedef struct MvbRowMap {
   int64_t num_row, num_col;
   int nservers;
@@ -175,7 +182,8 @@ int mvb_get_rows(int dtype, const MvbRowMap* m, const int64_t* row_ids, int64_t 
                  int64_t out_ld, void* stream);
 int mvb_add_rows_red(int dtype, const MvbRowMap* m, const int64_t* row_ids, int64_t k,
                      const void* vals, int64_t vals_ld, float sign, void* stream);
-/* fused AddDeltaParameter: red.add of (cur - old) * scale per row (fp32, num_col % 4 == 0) */
+/* fused AddDeltaParameter: red.add of (cur - old) * scale per row (fp32, num_col % 4 == 0, ld % 4 == 0,
+ * cur and old 16-byte aligned, else -9); the same kernel as mvb_rows_push_delta */
 int mvb_add_rows_delta(const MvbRowMap* m, const int64_t* row_ids, int64_t k, const float* cur,
                        const float* old, int64_t ld, float scale, void* stream);
 /* Stateful row add applied by the OWNER on its local shard for rows in its range:

@@ -240,6 +240,42 @@ MVB_DEVINL int owner_of(long long key, int S) {
   return (int)(m < 0 ? m + S : m);
 }
 
+// Row-sharded tables (the reference's partition, matrix_table.cpp:266-273): server min(r / per, S - 1) holds row r,
+// at local index r - server * per, so the last server takes the remainder. Every kernel that addresses table rows
+// goes through these helpers; the entry points reject a map that fails row_split_ok before any CUDA call.
+// S is a reference so that, for a map read from global memory (the collection's table descriptors), nservers is
+// loaded after the division: the embedding-bag kernels keep the instruction schedule they were tuned with.
+__host__ __device__ __forceinline__ int64_t row_server(int64_t r, int64_t per, const int& S) {
+  const int64_t o = r / per;
+  return o > S - 1 ? S - 1 : o;
+}
+
+// row r of the table as a T* into its owner's shard (row pitch num_col elements of T)
+template <typename T>
+MVB_DEVINL T* row_ptr(const MvbRowMap& m, int64_t r) {
+  const int64_t o = row_server(r, m.rows_per_server, m.nservers);
+  return static_cast<T*>(m.shard_ptrs[o]) + (r - o * m.rows_per_server) * m.num_col;
+}
+// ... at a row pitch of ld elements of T (a byte pitch for T = unsigned char)
+template <typename T>
+MVB_DEVINL T* row_ptr(const MvbRowMap& m, int64_t r, int64_t ld) {
+  const int64_t o = row_server(r, m.rows_per_server, m.nservers);
+  return static_cast<T*>(m.shard_ptrs[o]) + (r - o * m.rows_per_server) * ld;
+}
+
+// the rows [lo, hi) server s holds; lo and hi may exceed num_row when S * rows_per_server does
+struct RowRange { int64_t lo, hi; };
+__host__ __device__ __forceinline__ RowRange server_rows(const MvbRowMap& m, int s) {
+  return {m.rows_per_server * s, s == m.nservers - 1 ? m.num_row : m.rows_per_server * (s + 1)};
+}
+
+// S servers of per rows (keys) each can be addressed: the shard pointers of a map hold at most MVB_MAX_RANKS
+static inline bool row_split_ok(int S, int64_t per) { return S >= 1 && S <= MVB_MAX_RANKS && per >= 1; }
+
+// the warp's index and the number of warps of a grid-stride loop
+MVB_DEVINL int64_t warp_id() { return ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; }
+MVB_DEVINL int64_t num_warps() { return ((int64_t)gridDim.x * blockDim.x) >> 5; }
+
 MVB_DEVINL float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -319,4 +355,12 @@ static inline int mvb_num_sms() {
     if (sms <= 0) sms = 132;
   }
   return sms;
+}
+
+// 256-thread CTAs for a grid-stride loop over `warps` items of a warp each, at most 8 CTAs per SM
+static inline int grid_for(int64_t warps) {
+  int64_t blocks = (warps * 32 + 255) / 256;
+  const int64_t cap = (int64_t)mvb_num_sms() * 8;
+  if (blocks > cap) blocks = cap;
+  return (int)(blocks < 1 ? 1 : blocks);
 }

@@ -41,8 +41,9 @@ struct BoxHdr {
 static_assert(sizeof(BoxHdr) <= kHdrBytes, "header");
 
 struct BoxDev {
+  MvbRowMap map;               // the table's rows
   int me, S;
-  int64_t num_row, rps, cap;
+  int64_t cap;
   int64_t ld_bytes;            // row pitch inside a slot == shard row pitch
   int64_t slot_bytes, ids_bytes;
   unsigned char* box[MVB_MAX_RANKS];     // rank r's mailbox slab (S slots: one per source)
@@ -62,11 +63,6 @@ constexpr int kSlots = 2;
 MVB_DEVINL unsigned char* slot_of(const BoxDev& b, int owner, int source, uint64_t epoch) {
   return b.box[owner] + ((size_t)source * kSlots + (size_t)(epoch & 1)) * b.slot_bytes;
 }
-MVB_DEVINL int owner_of(const BoxDev& b, int64_t r) {
-  int64_t o = r / b.rps;
-  if (o > b.S - 1) o = b.S - 1;
-  return (int)o;
-}
 
 // seg[o] = first position of the sorted id list that belongs to owner o
 __global__ void rowbox_seg_kernel(const __grid_constant__ BoxDev b, const int* __restrict__ ids,
@@ -76,7 +72,7 @@ __global__ void rowbox_seg_kernel(const __grid_constant__ BoxDev b, const int* _
   const int o = threadIdx.x;
   if (o > b.S) return;
   if (o == b.S) { b.seg[o] = (int)n; return; }
-  const int64_t key = (int64_t)o * b.rps;          // first row of owner o
+  const int64_t key = server_rows(b.map, o).lo;    // first row of owner o
   int64_t lo = 0, hi = n;
   while (lo < hi) {
     const int64_t mid = (lo + hi) >> 1;
@@ -117,15 +113,13 @@ rowbox_push_kernel(const __grid_constant__ BoxDev b, const __grid_constant__ Pus
   __syncthreads();
   if (s_flag) return;
   const int lane = threadIdx.x & 31;
-  const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
   int64_t n = a.n_ptr ? (int64_t)*a.n_ptr : a.n_max;
   if (n > a.n_max) n = a.n_max;
   const int nvec = a.row_bytes >> 4;
-  for (int64_t s = warp; s < n; s += nwarps) {
+  for (int64_t s = warp_id(); s < n; s += num_warps()) {
     const int64_t r = (int64_t)__ldg(a.ids + s);
-    if (r < 0 || r >= b.num_row) continue;
-    const int o = owner_of(b, r);
+    if (r < 0 || r >= b.map.num_row) continue;
+    const int o = (int)row_server(r, b.map.rows_per_server, b.map.nservers);
     const int64_t idx = s - b.seg[o];
     if (idx < 0 || idx >= b.cap) {
       if (lane == 0 && b.err) atomicExch(b.err, 3100 + o);
@@ -234,11 +228,9 @@ rowbox_apply_kernel(const __grid_constant__ BoxDev b, const __grid_constant__ Ap
   const int* ids = reinterpret_cast<const int*>(slot + kHdrBytes);
   const unsigned char* vals = slot + kHdrBytes + b.ids_bytes;
   const int lane = threadIdx.x & 31;
-  const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
   const int64_t woff = U::kPerWorker ? (int64_t)a.src * a.state_stride : 0;
   const int nvec = a.row_floats >> 2;
-  for (int64_t i = warp; i < count; i += nwarps) {
+  for (int64_t i = warp_id(); i < count; i += num_warps()) {
     const int64_t r = (int64_t)__ldcg(ids + i);
     const int64_t base = (r - a.row_lo) * (int64_t)a.row_floats;
     if (r < a.row_lo || base < 0) continue;
@@ -277,10 +269,9 @@ rowbox_apply_kernel(const __grid_constant__ BoxDev b, const __grid_constant__ Ap
 
 BoxDev to_dev(const MvbRowBox* h) {
   BoxDev b{};
+  b.map = h->map;
   b.me = h->me;
   b.S = h->map.nservers;
-  b.num_row = h->map.num_row;
-  b.rps = h->map.rows_per_server > 0 ? h->map.rows_per_server : 1;
   b.cap = h->cap;
   b.ld_bytes = h->map.num_col * 4;
   b.ids_bytes = (h->cap * 4 + 127) / 128 * 128;
@@ -315,6 +306,7 @@ extern "C" int64_t mvb_rowbox_slot_bytes(int64_t cap, int64_t num_col) {
 static int push_common(const MvbRowBox* h, bool delta, const int* ids, const int* n_ptr, int64_t n_max,
                        const float* cur, const float* old, int64_t ld, float scale, uint64_t epoch,
                        const MvbAddOpt* opt, int ctas_per_sm, void* stream) {
+  if (!row_split_ok(h->map.nservers, h->map.rows_per_server)) return MVB_BAD_ROW_MAP;
   if (h->map.num_col % 4 || ld % 4) return -9;
   cudaStream_t st = (cudaStream_t)stream;
   BoxDev b = to_dev(h);
@@ -351,6 +343,7 @@ extern "C" int mvb_rowbox_push_vals(const MvbRowBox* h, const int* ids, const in
 // Owner side, step 1: for every source (src < 0) or one source decide whether its next push is complete
 // (wait = 1: spin for it with the watchdog; wait = 0: just look).  Step 2: mvb_rowbox_apply per source.
 extern "C" int mvb_rowbox_poll(const MvbRowBox* h, int src, int wait, void* stream) {
+  if (!row_split_ok(h->map.nservers, h->map.rows_per_server)) return MVB_BAD_ROW_MAP;
   BoxDev b = to_dev(h);
   rowbox_poll_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(b, wait, src);
   MVB_CUDA_CHECK(cudaGetLastError());
@@ -361,6 +354,7 @@ extern "C" int mvb_rowbox_poll(const MvbRowBox* h, int src, int wait, void* stre
 extern "C" int mvb_rowbox_apply(const MvbRowBox* h, int updater, float* shard, float* st0, float* st1,
                                 int64_t state_stride, int64_t row_lo, int src, int ctas_per_sm,
                                 void* stream) {
+  if (!row_split_ok(h->map.nservers, h->map.rows_per_server)) return MVB_BAD_ROW_MAP;
   if (h->map.num_col % 4) return -9;
   BoxDev b = to_dev(h);
   ApplyArgs a{};

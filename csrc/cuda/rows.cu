@@ -6,43 +6,28 @@
 //                        128-bit peer loads straight from the owner's shard.
 //  K3 add_rows_red    -- row Add for stateless updaters: one-sided vector red.add into
 //                        the owner shard (commutative => race-free async-PS semantics).
+//     add_rows_delta  -- AddDeltaParameter: red.add of (trained - pulled) * scale per row, behind
+//                        mvb_add_rows_delta and the WordEmbedding block push mvb_rows_push_delta.
 //     add_rows_owner  -- row Add for stateful updaters, applied by the OWNER exactly once
 //                        per (worker,row), reading ids/values from (peer) staging.
 //  K10 row_nonzero_mask, stale bitmap -- zero-row skip and delta-pull bookkeeping of the
 //                        sparse Matrix tables (src/table/matrix.cpp:151-164, 516-572).
+#include <algorithm>
 #include <type_traits>
 #include "mvb_common.cuh"
 
 namespace {
 
-struct RowMapDev {
-  int64_t num_row, num_col, rps;
-  int S;
-  void* shard[MVB_MAX_RANKS];
-};
-
-MVB_DEVINL void locate_row(const RowMapDev& m, int64_t r, int& owner, int64_t& local) {
-  int64_t o = r / m.rps;
-  if (o > m.S - 1) o = m.S - 1;  // last server takes the remainder (matrix_table.cpp:270-273)
-  owner = (int)o;
-  local = r - o * m.rps;
-}
-
 template <typename T, bool VECOK>
 __global__ void __launch_bounds__(256)
-get_rows_kernel(const __grid_constant__ RowMapDev m, const int64_t* __restrict__ ids, int64_t k,
+get_rows_kernel(const __grid_constant__ MvbRowMap m, const int64_t* __restrict__ ids, int64_t k,
                 T* __restrict__ out, int64_t out_ld) {
   constexpr int VEC = VecOf<T>::N;
   const int lane = threadIdx.x & 31;
-  const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
-  for (int64_t i = warp; i < k; i += nwarps) {
+  for (int64_t i = warp_id(); i < k; i += num_warps()) {
     const int64_t r = ids[i];
     if (r < 0 || r >= m.num_row) continue;
-    int owner;
-    int64_t local;
-    locate_row(m, r, owner, local);
-    const T* src = reinterpret_cast<const T*>(m.shard[owner]) + local * m.num_col;
+    const T* src = row_ptr<const T>(m, r);
     T* dst = out + i * out_ld;
     if constexpr (VECOK) {
       const int nvec = (int)(m.num_col / VEC);
@@ -73,18 +58,13 @@ get_rows_kernel(const __grid_constant__ RowMapDev m, const int64_t* __restrict__
 
 template <typename T, bool VECOK>
 __global__ void __launch_bounds__(256)
-add_rows_red_kernel(const __grid_constant__ RowMapDev m, const int64_t* __restrict__ ids,
+add_rows_red_kernel(const __grid_constant__ MvbRowMap m, const int64_t* __restrict__ ids,
                     int64_t k, const T* __restrict__ vals, int64_t vals_ld, float sign) {
   const int lane = threadIdx.x & 31;
-  const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
-  for (int64_t i = warp; i < k; i += nwarps) {
+  for (int64_t i = warp_id(); i < k; i += num_warps()) {
     const int64_t r = ids[i];
     if (r < 0 || r >= m.num_row) continue;
-    int owner;
-    int64_t local;
-    locate_row(m, r, owner, local);
-    T* dst = reinterpret_cast<T*>(m.shard[owner]) + local * m.num_col;
+    T* dst = row_ptr<T>(m, r);
     const T* src = vals + i * vals_ld;
     if constexpr (VECOK && std::is_same<T, float>::value) {
       const int nvec = (int)(m.num_col / 4);
@@ -99,29 +79,61 @@ add_rows_red_kernel(const __grid_constant__ RowMapDev m, const int64_t* __restri
   }
 }
 
-// AddDeltaParameter fused (Applications/WordEmbedding/src/communicator.cpp:157-203): push
-// (trained - pulled) * scale for every cached row straight into the owners, no delta tensor.
-__global__ void __launch_bounds__(256)
-add_rows_delta_kernel(const __grid_constant__ RowMapDev m, const int64_t* __restrict__ ids, int64_t k,
-                      const float* __restrict__ cur, const float* __restrict__ old, int64_t ld, float scale) {
+// AddDeltaParameter fused (Applications/WordEmbedding/src/communicator.cpp:157-203, 206-249): push
+// (trained - pulled) * scale for every cached row straight into its owner with one-sided red.add.v4.f32 (the
+// async-PS Add of a stateless updater), no delta tensor; all-zero 16-byte deltas are skipped. The row count is
+// n_max, or read on the device from n_ptr (clamped to n_max).
+template <typename Id>
+struct DeltaArgs {
+  MvbRowMap m;
+  const Id* ids;           // row ids
+  const int* n_ptr;        // device count (nullptr: n_max rows)
+  int64_t n_max;
+  const unsigned char* cur;   // trained rows [n x ld_bytes]
+  const unsigned char* old;   // pulled rows  [n x ld_bytes]
+  int64_t ld_bytes;
+  int row_bytes;              // == the shards' row pitch
+  float scale;
+};
+
+// 128-thread CTAs, no shared memory, <= 56 registers: the WordEmbedding block push runs these co-resident with
+// the persistent K7 CTAs (which own the SMs' shared memory but leave threads and registers; we_block.cu).
+// Warp per row, 3 vectors per lane in flight.
+constexpr int kDeltaThreads = 128;
+
+template <typename Id>
+__global__ void __launch_bounds__(kDeltaThreads, 9)
+add_rows_delta_kernel(const __grid_constant__ DeltaArgs<Id> a) {
   const int lane = threadIdx.x & 31;
-  const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
-  const int nvec = (int)(m.num_col / 4);
-  for (int64_t i = warp; i < k; i += nwarps) {
-    const int64_t r = ids[i];
-    if (r < 0 || r >= m.num_row) continue;
-    int owner;
-    int64_t local;
-    locate_row(m, r, owner, local);
-    float* dst = reinterpret_cast<float*>(m.shard[owner]) + local * m.num_col;
-    const float4* a = reinterpret_cast<const float4*>(cur + i * ld);
-    const float4* b = reinterpret_cast<const float4*>(old + i * ld);
-    for (int v = lane; v < nvec; v += 32) {
-      float4 x = a[v], y = b[v];
-      x.x = (x.x - y.x) * scale; x.y = (x.y - y.y) * scale;
-      x.z = (x.z - y.z) * scale; x.w = (x.w - y.w) * scale;
-      if (x.x != 0.f || x.y != 0.f || x.z != 0.f || x.w != 0.f) red_add_v4_f32(dst + (int64_t)v * 4, x);
+  int64_t n = a.n_ptr ? (int64_t)*a.n_ptr : a.n_max;
+  if (n > a.n_max) n = a.n_max;
+  const int nvec = a.row_bytes >> 4;
+  for (int64_t s = warp_id(); s < n; s += num_warps()) {
+    const int64_t r = (int64_t)__ldg(a.ids + s);
+    if (r < 0 || r >= a.m.num_row) continue;
+    float* dst = reinterpret_cast<float*>(row_ptr<unsigned char>(a.m, r, a.row_bytes));
+    const unsigned char* c = a.cur + s * a.ld_bytes;
+    const unsigned char* o = a.old + s * a.ld_bytes;
+    for (int v0 = 0; v0 < nvec; v0 += 96) {
+      float4 x[3], y[3];
+#pragma unroll
+      for (int j = 0; j < 3; ++j) {
+        const int v = v0 + lane + 32 * j;
+        if (v < nvec) {
+          x[j] = *reinterpret_cast<const float4*>(c + (size_t)v * 16);
+          y[j] = *reinterpret_cast<const float4*>(o + (size_t)v * 16);
+        }
+      }
+#pragma unroll
+      for (int j = 0; j < 3; ++j) {
+        const int v = v0 + lane + 32 * j;
+        if (v < nvec) {
+          float4 d;
+          d.x = (x[j].x - y[j].x) * a.scale; d.y = (x[j].y - y[j].y) * a.scale;
+          d.z = (x[j].z - y[j].z) * a.scale; d.w = (x[j].w - y[j].w) * a.scale;
+          if (d.x != 0.f || d.y != 0.f || d.z != 0.f || d.w != 0.f) red_add_v4_f32(dst + (size_t)v * 4, d);
+        }
+      }
     }
   }
 }
@@ -137,10 +149,8 @@ add_rows_owner_kernel(T* __restrict__ shard, T* __restrict__ st0, T* __restrict_
                       int64_t vals_ld, MvbAddOpt opt) {
   using U = Updater<UPD, T>;
   const int lane = threadIdx.x & 31;
-  const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
   const int64_t woff = U::kPerWorker ? (int64_t)opt.worker_id * state_stride : 0;
-  for (int64_t i = warp; i < k; i += nwarps) {
+  for (int64_t i = warp_id(); i < k; i += num_warps()) {
     const int64_t r = ids[i];
     if (i > 0 && ids[i - 1] == r) continue;  // inside a run: applied by the run's first warp
     if (r < row_lo || r >= row_hi) continue;
@@ -164,9 +174,7 @@ __global__ void __launch_bounds__(256)
 row_nonzero_kernel(const T* __restrict__ data, int64_t rows, int64_t cols, int64_t ld,
                    uint8_t* __restrict__ mask) {
   const int lane = threadIdx.x & 31;
-  const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
-  for (int64_t r = warp; r < rows; r += nwarps) {
+  for (int64_t r = warp_id(); r < rows; r += num_warps()) {
     const T* row = data + r * ld;
     int nz = 0;
     for (int64_t c = lane; c < cols; c += 32) nz |= (row[c] != (T)0);
@@ -224,35 +232,16 @@ mask_compact_kernel(const uint8_t* __restrict__ mask, int64_t n, int64_t* __rest
   if (threadIdx.x == 1023) *count = part[1023];
 }
 
-RowMapDev to_dev(const MvbRowMap* m) {
-  RowMapDev d{};
-  d.num_row = m->num_row;
-  d.num_col = m->num_col;
-  d.S = m->nservers;
-  d.rps = m->rows_per_server > 0 ? m->rows_per_server : 1;
-  for (int s = 0; s < MVB_MAX_RANKS; ++s) d.shard[s] = s < m->nservers ? m->shard_ptrs[s] : nullptr;
-  return d;
-}
-
-int grid_for_warps(int64_t warps_needed, int threads) {
-  int64_t blocks = (warps_needed * 32 + threads - 1) / threads;
-  int64_t cap = (int64_t)mvb_num_sms() * 8;
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
-  return (int)blocks;
-}
-
 template <typename T>
 int get_rows_t(const MvbRowMap* m, const int64_t* ids, int64_t k, void* out, int64_t out_ld,
                cudaStream_t st) {
-  RowMapDev d = to_dev(m);
   bool vec = (m->num_col % VecOf<T>::N == 0) && (out_ld % VecOf<T>::N == 0) &&
              ((reinterpret_cast<uintptr_t>(out) & 15) == 0);
-  int grid = grid_for_warps(k, 256);
+  int grid = grid_for(k);
   if (vec)
-    get_rows_kernel<T, true><<<grid, 256, 0, st>>>(d, ids, k, (T*)out, out_ld);
+    get_rows_kernel<T, true><<<grid, 256, 0, st>>>(*m, ids, k, (T*)out, out_ld);
   else
-    get_rows_kernel<T, false><<<grid, 256, 0, st>>>(d, ids, k, (T*)out, out_ld);
+    get_rows_kernel<T, false><<<grid, 256, 0, st>>>(*m, ids, k, (T*)out, out_ld);
   MVB_CUDA_CHECK(cudaGetLastError());
   return 0;
 }
@@ -260,14 +249,13 @@ int get_rows_t(const MvbRowMap* m, const int64_t* ids, int64_t k, void* out, int
 template <typename T>
 int add_rows_red_t(const MvbRowMap* m, const int64_t* ids, int64_t k, const void* vals,
                    int64_t vals_ld, float sign, cudaStream_t st) {
-  RowMapDev d = to_dev(m);
   bool vec = (m->num_col % 4 == 0) && (vals_ld % 4 == 0) &&
              ((reinterpret_cast<uintptr_t>(vals) & 15) == 0) && sizeof(T) == 4;
-  int grid = grid_for_warps(k, 256);
+  int grid = grid_for(k);
   if (vec)
-    add_rows_red_kernel<T, true><<<grid, 256, 0, st>>>(d, ids, k, (const T*)vals, vals_ld, sign);
+    add_rows_red_kernel<T, true><<<grid, 256, 0, st>>>(*m, ids, k, (const T*)vals, vals_ld, sign);
   else
-    add_rows_red_kernel<T, false><<<grid, 256, 0, st>>>(d, ids, k, (const T*)vals, vals_ld, sign);
+    add_rows_red_kernel<T, false><<<grid, 256, 0, st>>>(*m, ids, k, (const T*)vals, vals_ld, sign);
   MVB_CUDA_CHECK(cudaGetLastError());
   return 0;
 }
@@ -276,7 +264,7 @@ template <typename T>
 int add_rows_owner_t(int upd, void* shard, void* s0, void* s1, int64_t lo, int64_t hi,
                      int64_t cols, int64_t sstride, const int64_t* ids, int64_t k,
                      const void* vals, int64_t vld, const MvbAddOpt* opt, cudaStream_t st) {
-  int grid = grid_for_warps(k, 256);
+  int grid = grid_for(k);
 #define MVB_ROWS_OWNER(U)                                                                  \
   add_rows_owner_kernel<U, T><<<grid, 256, 0, st>>>((T*)shard, (T*)s0, (T*)s1, lo, hi, cols, \
                                                     sstride, ids, k, (const T*)vals, vld, *opt)
@@ -298,10 +286,24 @@ int add_rows_owner_t(int upd, void* shard, void* s0, void* s1, int64_t lo, int64
   return 0;
 }
 
+template <typename Id>
+int add_rows_delta_t(const MvbRowMap* m, const Id* ids, const int* n_ptr, int64_t n_max, const float* cur,
+                     const float* old, int64_t ld, float scale, int64_t ctas, cudaStream_t st) {
+  // whole float4 vectors: a 16-byte row pitch and 16-byte aligned rows
+  if (m->num_col % 4 || ld % 4) return -9;
+  if ((reinterpret_cast<uintptr_t>(cur) & 15) || (reinterpret_cast<uintptr_t>(old) & 15)) return -9;
+  const DeltaArgs<Id> a{*m, ids, n_ptr, n_max, reinterpret_cast<const unsigned char*>(cur),
+                        reinterpret_cast<const unsigned char*>(old), ld * 4, (int)(m->num_col * 4), scale};
+  add_rows_delta_kernel<Id><<<(unsigned)ctas, kDeltaThreads, 0, st>>>(a);
+  MVB_CUDA_CHECK(cudaGetLastError());
+  return 0;
+}
+
 }  // namespace
 
 extern "C" int mvb_get_rows(int dtype, const MvbRowMap* m, const int64_t* row_ids, int64_t k,
                             void* out, int64_t out_ld, void* stream) {
+  if (!row_split_ok(m->nservers, m->rows_per_server)) return MVB_BAD_ROW_MAP;
   if (k <= 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
   switch (dtype) {
@@ -313,6 +315,7 @@ extern "C" int mvb_get_rows(int dtype, const MvbRowMap* m, const int64_t* row_id
 }
 extern "C" int mvb_add_rows_red(int dtype, const MvbRowMap* m, const int64_t* row_ids, int64_t k,
                                 const void* vals, int64_t vals_ld, float sign, void* stream) {
+  if (!row_split_ok(m->nservers, m->rows_per_server)) return MVB_BAD_ROW_MAP;
   if (k <= 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
   switch (dtype) {
@@ -324,12 +327,22 @@ extern "C" int mvb_add_rows_red(int dtype, const MvbRowMap* m, const int64_t* ro
 }
 extern "C" int mvb_add_rows_delta(const MvbRowMap* m, const int64_t* row_ids, int64_t k, const float* cur,
                                   const float* old, int64_t ld, float scale, void* stream) {
+  if (!row_split_ok(m->nservers, m->rows_per_server)) return MVB_BAD_ROW_MAP;
   if (k <= 0) return 0;
-  if (m->num_col % 4 || ld % 4) return -9;
-  RowMapDev d = to_dev(m);
-  add_rows_delta_kernel<<<grid_for_warps(k, 256), 256, 0, (cudaStream_t)stream>>>(d, row_ids, k, cur, old, ld, scale);
-  MVB_CUDA_CHECK(cudaGetLastError());
-  return 0;
+  // a warp per row, at most 8 x 256 threads per SM
+  const int64_t ctas = std::min<int64_t>((k * 32 + kDeltaThreads - 1) / kDeltaThreads, (int64_t)mvb_num_sms() * 16);
+  return add_rows_delta_t<int64_t>(m, row_ids, nullptr, k, cur, old, ld, scale, ctas, (cudaStream_t)stream);
+}
+// rows[ids[s]] += (cur[s] - old[s]) * scale for s in [0, n), n read on the device from n_ptr when given (clamped to
+// n_max); the grid is ctas_per_sm (>= 1) CTAs per SM.
+extern "C" int mvb_rows_push_delta(const MvbRowMap* m, const int* ids, const int* n_ptr, int64_t n_max,
+                                   const float* cur, const float* old, int64_t ld, float scale, int ctas_per_sm,
+                                   void* stream) {
+  if (!row_split_ok(m->nservers, m->rows_per_server)) return MVB_BAD_ROW_MAP;
+  if (ctas_per_sm < 1) return -22;
+  if (n_max <= 0) return 0;
+  return add_rows_delta_t<int>(m, ids, n_ptr, n_max, cur, old, ld, scale, (int64_t)mvb_num_sms() * ctas_per_sm,
+                               (cudaStream_t)stream);
 }
 extern "C" int mvb_add_rows_owner(int dtype, int updater, void* shard, void* state0, void* state1,
                                   int64_t row_lo, int64_t row_hi, int64_t num_col,
@@ -355,7 +368,7 @@ extern "C" int mvb_row_nonzero_mask(int dtype, const void* data, int64_t rows, i
                                     int64_t ld, uint8_t* mask, void* stream) {
   if (rows <= 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
-  int grid = grid_for_warps(rows, 256);
+  int grid = grid_for(rows);
   switch (dtype) {
     case MVB_F32: row_nonzero_kernel<float><<<grid, 256, 0, st>>>((const float*)data, rows, cols, ld, mask); break;
     case MVB_F64: row_nonzero_kernel<double><<<grid, 256, 0, st>>>((const double*)data, rows, cols, ld, mask); break;

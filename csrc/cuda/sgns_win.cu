@@ -81,8 +81,7 @@ struct WinDev {
 
 MVB_DEVINL float* row_of(float* const* peers, int S, int64_t rps, int64_t ld, float* local_base, int64_t rid) {
   if (S <= 0) return local_base + rid * ld;
-  int64_t o = rid / rps;
-  if (o > S - 1) o = S - 1;
+  const int64_t o = row_server(rid, rps, S);
   return peers[o] + (rid - o * rps) * ld;
 }
 
@@ -1140,7 +1139,7 @@ extern "C" int mvb_sgns_train_win(const MvbSgns* h, void* stream) {
   a.scale_in = h->scale_in; a.scale_out = h->scale_out;
   a.S = 0;
   if (h->nservers > 1) {
-    if (h->map_in || h->map_out || h->rows_per_server <= 0) return -21;
+    if (h->map_in || h->map_out || !row_split_ok(h->nservers, h->rows_per_server)) return -21;
     a.S = h->nservers;
     a.rps = h->rows_per_server;
     for (int s = 0; s < MVB_MAX_RANKS; ++s) {

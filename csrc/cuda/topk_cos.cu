@@ -464,17 +464,6 @@ topk_merge_kernel(const float* __restrict__ in_s, const int* __restrict__ in_i, 
   }
 }
 
-struct RowsDev {
-  const float* shard[MVB_MAX_RANKS];
-  int64_t rps, ld;
-  int S;
-};
-
-MVB_DEVINL const float* row_ptr(const RowsDev& rows, int64_t id) {
-  const int s = (int)min(id / rows.rps, (int64_t)rows.S - 1);
-  return rows.shard[s] + (id - s * rows.rps) * rows.ld;
-}
-
 struct LseDev {
   const float2* part;        // [M][ranges] (m, s) in base 2
   int ranges;
@@ -489,7 +478,7 @@ struct LseDev {
 template <bool kCos, bool kLse, bool kTopk>
 __global__ void __launch_bounds__(128)
 topk_finish_kernel(const float* __restrict__ in_s, const int* __restrict__ in_i, const float* __restrict__ q,
-                   int64_t ldq, int64_t dim, const __grid_constant__ RowsDev rows, int kp, int k,
+                   int64_t ldq, int64_t dim, const __grid_constant__ MvbRowMap rows, int kp, int k,
                    float* __restrict__ out_s, int64_t* __restrict__ out_i, const __grid_constant__ LseDev e) {
   __shared__ float fs[KP_MAX];
   __shared__ int fi[KP_MAX];
@@ -500,7 +489,7 @@ topk_finish_kernel(const float* __restrict__ in_s, const int* __restrict__ in_i,
     if (warp == 0) {
       double t = 0.0;
       if (e.labels) {
-        const float* wr = row_ptr(rows, e.labels[m]);
+        const float* wr = row_ptr<const float>(rows, e.labels[m]);
         for (int64_t x = lane; x < dim; x += 32) t += (double)qr[x] * wr[x];
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
@@ -535,7 +524,7 @@ topk_finish_kernel(const float* __restrict__ in_s, const int* __restrict__ in_i,
         if (lane == 0) { fs[c] = -FLT_MAX; fi[c] = INT_MAX; }
         continue;
       }
-      const float* wr = row_ptr(rows, id);
+      const float* wr = row_ptr<const float>(rows, id);
       double d = 0.0, wn = 0.0;
       for (int64_t x = lane; x < dim; x += 32) {
         const double wv = wr[x];
@@ -615,10 +604,8 @@ int launch_search(const Search* a, cudaStream_t st) {
   if (rc) return rc;
   int tiles = 0;
   for (int s = 0; s < wm.nservers; ++s) {
-    int64_t lo = wm.rows_per_server * s;
-    int64_t hi = (s == wm.nservers - 1) ? wm.num_row : wm.rows_per_server * (s + 1);
-    lo = std::min(lo, a->n_rows);
-    hi = std::min(hi, a->n_rows);
+    const RowRange rs = server_rows(wm, s);
+    const int64_t lo = std::min(rs.lo, a->n_rows), hi = std::min(rs.hi, a->n_rows);
     g.lo[s] = lo;
     g.hi[s] = hi;
     g.tile_begin[s] = tiles;
@@ -661,15 +648,10 @@ int launch_search(const Search* a, cudaStream_t st) {
     std::swap(i0, i1);
     r_in = r_out;
   }
-  RowsDev rows{};
-  for (int s = 0; s < wm.nservers; ++s) rows.shard[s] = reinterpret_cast<const float*>(wm.shard_ptrs[s]);
-  rows.rps = wm.rows_per_server;
-  rows.ld = wm.num_col;
-  rows.S = wm.nservers;
   LseDev e{part_lse, g.ranges, a->labels, a->lse, a->loss};
   // without top-k only warp 0 has work
   topk_finish_kernel<kCos, kLse, kTopk><<<(unsigned)a->M, kTopk ? 128 : 32, 0, st>>>(
-      s0, i0, a->q, a->ldq, a->dim, rows, kp, a->k, a->scores, a->ids, e);
+      s0, i0, a->q, a->ldq, a->dim, wm, kp, a->k, a->scores, a->ids, e);
   MVB_CUDA_CHECK(cudaGetLastError());
   return 0;
 }
@@ -677,7 +659,7 @@ int launch_search(const Search* a, cudaStream_t st) {
 // the checks both entry points share
 int check_search(const Search& a, int64_t scratch_bytes_given, int64_t scratch_bytes_needed) {
   const MvbRowMap& wm = a.wmap;
-  if (wm.nservers < 1 || wm.nservers > MVB_MAX_RANKS || wm.rows_per_server < 1) return -41;
+  if (!row_split_ok(wm.nservers, wm.rows_per_server)) return -41;
   // TMA needs 16-byte aligned row pitches
   if (a.ldq % 4 != 0 || wm.num_col % 4 != 0) return -42;
   if (a.dim < 1 || a.dim > a.ldq || a.dim > wm.num_col) return -43;

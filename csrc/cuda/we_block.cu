@@ -15,9 +15,9 @@
 //                      kernel reads them there, so nothing ever synchronises with the host.
 //   mvb_rows_pull      row gather from the owners' shards (over NVLink for peer shards) into the block cache
 //                      AND its "pulled" copy (what clone() did): a warp per row, 128-bit loads and stores.
-//   mvb_rows_push_delta   (trained - pulled) * scale per row, reduced into the owner's shard with one-sided
-//                      red.add.v4.f32 (element-wise atomic at the owner: the async-PS Add for stateless
-//                      updaters); all-zero 16-byte deltas are skipped.
+//   mvb_rows_push_delta   (rows.cu) (trained - pulled) * scale per row, reduced into the owner's shard with
+//                      one-sided red.add.v4.f32 (element-wise atomic at the owner: the async-PS Add for
+//                      stateless updaters); all-zero 16-byte deltas are skipped.
 // Pull and push run ctas_per_sm register-only CTAs per SM, co-resident with the persistent K7 (see below).
 #include "mvb_common.cuh"
 
@@ -166,41 +166,17 @@ prep_neg_pool_kernel(const int* __restrict__ n_in_ptr, int negative, int vocab, 
 }
 
 // ------------------------------------------------------------------------------------------------
-// row pull / delta push
+// row pull (the delta push is rows.cu's add_rows_delta_kernel)
 // ------------------------------------------------------------------------------------------------
-struct RowMapDev {
-  int64_t num_row, rps;
-  int64_t ld_bytes;        // row pitch of the shards
-  int S;
-  unsigned char* shard[MVB_MAX_RANKS];
-};
-MVB_DEVINL unsigned char* row_addr(const RowMapDev& m, int64_t r) {
-  int64_t o = r / m.rps;
-  if (o > m.S - 1) o = m.S - 1;            // last server takes the remainder (matrix_table.cpp:270-273)
-  return m.shard[o] + (r - o * m.rps) * m.ld_bytes;
-}
-
 struct PullDev {
-  RowMapDev m;
+  MvbRowMap m;
   const int* ids;          // slot -> row id
   const int* n_ptr;        // device count (nullptr: n_max rows)
   int64_t n_max;
   unsigned char* dst_a;    // [n x dst_ld_bytes]
   unsigned char* dst_b;    // optional second copy
   int64_t dst_ld_bytes;
-  int row_bytes;
-};
-
-struct PushDev {
-  RowMapDev m;
-  const int* ids;
-  const int* n_ptr;
-  int64_t n_max;
-  const unsigned char* cur;   // trained rows  [n x ld_bytes]
-  const unsigned char* old;   // pulled rows
-  int64_t ld_bytes;
-  int row_bytes;
-  float scale;
+  int row_bytes;           // == the shards' row pitch
 };
 
 // No shared memory and <= 56 registers: these CTAs co-reside with the persistent K7 CTAs (which own the
@@ -210,19 +186,17 @@ struct PushDev {
 __global__ void __launch_bounds__(kSideThreads, 9)
 rows_pull_kernel(const __grid_constant__ PullDev a) {
   const int lane = threadIdx.x & 31;
-  const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
   int64_t n = a.n_ptr ? (int64_t)*a.n_ptr : a.n_max;
   if (n > a.n_max) n = a.n_max;
   const int nvec = a.row_bytes >> 4;
-  for (int64_t s = warp * 2; s < n; s += nwarps * 2) {
+  for (int64_t s = warp_id() * 2; s < n; s += num_warps() * 2) {
     const unsigned char* src[2];
 #pragma unroll
     for (int u = 0; u < 2; ++u) {
       src[u] = nullptr;
       if (s + u < n) {
         const int64_t r = (int64_t)__ldg(a.ids + s + u);
-        if (r >= 0 && r < a.m.num_row) src[u] = row_addr(a.m, r);
+        if (r >= 0 && r < a.m.num_row) src[u] = row_ptr<const unsigned char>(a.m, r, a.row_bytes);
       }
     }
     for (int v0 = 0; v0 < nvec; v0 += 64) {
@@ -246,55 +220,6 @@ rows_pull_kernel(const __grid_constant__ PullDev a) {
         }
     }
   }
-}
-
-__global__ void __launch_bounds__(kSideThreads, 9)
-rows_push_delta_kernel(const __grid_constant__ PushDev a) {
-  const int lane = threadIdx.x & 31;
-  const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
-  int64_t n = a.n_ptr ? (int64_t)*a.n_ptr : a.n_max;
-  if (n > a.n_max) n = a.n_max;
-  const int nvec = a.row_bytes >> 4;
-  for (int64_t s = warp; s < n; s += nwarps) {
-    const int64_t r = (int64_t)__ldg(a.ids + s);
-    if (r < 0 || r >= a.m.num_row) continue;
-    float* dst = reinterpret_cast<float*>(row_addr(a.m, r));
-    const unsigned char* c = a.cur + s * a.ld_bytes;
-    const unsigned char* o = a.old + s * a.ld_bytes;
-    for (int v0 = 0; v0 < nvec; v0 += 96) {
-      float4 x[3], y[3];
-#pragma unroll
-      for (int j = 0; j < 3; ++j) {
-        const int v = v0 + lane + 32 * j;
-        if (v < nvec) {
-          x[j] = *reinterpret_cast<const float4*>(c + (size_t)v * 16);
-          y[j] = *reinterpret_cast<const float4*>(o + (size_t)v * 16);
-        }
-      }
-#pragma unroll
-      for (int j = 0; j < 3; ++j) {
-        const int v = v0 + lane + 32 * j;
-        if (v < nvec) {
-          float4 d;
-          d.x = (x[j].x - y[j].x) * a.scale; d.y = (x[j].y - y[j].y) * a.scale;
-          d.z = (x[j].z - y[j].z) * a.scale; d.w = (x[j].w - y[j].w) * a.scale;
-          if (d.x != 0.f || d.y != 0.f || d.z != 0.f || d.w != 0.f) red_add_v4_f32(dst + (size_t)v * 4, d);
-        }
-      }
-    }
-  }
-}
-
-RowMapDev to_dev(const MvbRowMap* m, int esz) {
-  RowMapDev d{};
-  d.num_row = m->num_row;
-  d.S = m->nservers;
-  d.rps = m->rows_per_server > 0 ? m->rows_per_server : 1;
-  d.ld_bytes = m->num_col * esz;
-  for (int s = 0; s < MVB_MAX_RANKS; ++s)
-    d.shard[s] = s < m->nservers ? reinterpret_cast<unsigned char*>(m->shard_ptrs[s]) : nullptr;
-  return d;
 }
 
 }  // namespace
@@ -337,37 +262,18 @@ extern "C" int mvb_we_prepare_launches(int negative) { return negative > 0 ? 9 :
 // The grid is ctas_per_sm (>= 1) CTAs per SM.
 extern "C" int mvb_rows_pull(const MvbRowMap* m, int esz, const int* ids, const int* n_ptr, int64_t n_max,
                              void* dst_a, void* dst_b, int64_t dst_ld, int ctas_per_sm, void* stream) {
+  if (!row_split_ok(m->nservers, m->rows_per_server)) return MVB_BAD_ROW_MAP;
   if (ctas_per_sm < 1) return -22;
   if (n_max <= 0) return 0;
   const int64_t row_bytes = m->num_col * esz;
   if (row_bytes % 16 || (dst_ld * esz) % 16) return -9;
   if ((reinterpret_cast<uintptr_t>(dst_a) & 15) || (reinterpret_cast<uintptr_t>(dst_b) & 15)) return -9;
   PullDev a{};
-  a.m = to_dev(m, esz);
+  a.m = *m;
   a.ids = ids; a.n_ptr = n_ptr; a.n_max = n_max;
   a.dst_a = (unsigned char*)dst_a; a.dst_b = (unsigned char*)dst_b; a.dst_ld_bytes = dst_ld * esz;
   a.row_bytes = (int)row_bytes;
   rows_pull_kernel<<<mvb_num_sms() * ctas_per_sm, kSideThreads, 0, (cudaStream_t)stream>>>(a);
-  MVB_CUDA_CHECK(cudaGetLastError());
-  return 0;
-}
-
-// rows[ids[s]] += (cur[s] - old[s]) * scale for s in [0, n): AddDeltaParameter as one-sided red.add into the
-// owners' shards; all-zero 16-byte deltas are skipped.  Same count and grid conventions as mvb_rows_pull.
-extern "C" int mvb_rows_push_delta(const MvbRowMap* m, const int* ids, const int* n_ptr, int64_t n_max,
-                                   const float* cur, const float* old, int64_t ld, float scale, int ctas_per_sm,
-                                   void* stream) {
-  if (ctas_per_sm < 1) return -22;
-  if (n_max <= 0) return 0;
-  const int64_t row_bytes = m->num_col * 4;
-  if (row_bytes % 16 || (ld * 4) % 16) return -9;
-  if ((reinterpret_cast<uintptr_t>(cur) & 15) || (reinterpret_cast<uintptr_t>(old) & 15)) return -9;
-  PushDev a{};
-  a.m = to_dev(m, 4);
-  a.ids = ids; a.n_ptr = n_ptr; a.n_max = n_max;
-  a.cur = (const unsigned char*)cur; a.old = (const unsigned char*)old; a.ld_bytes = ld * 4;
-  a.row_bytes = (int)row_bytes; a.scale = scale;
-  rows_push_delta_kernel<<<mvb_num_sms() * ctas_per_sm, kSideThreads, 0, (cudaStream_t)stream>>>(a);
   MVB_CUDA_CHECK(cudaGetLastError());
   return 0;
 }

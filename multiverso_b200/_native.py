@@ -72,6 +72,9 @@ class RowMap(C.Structure):
                 ("rows_per_server", i64), ("shard_ptrs", VP8)]
 
 
+BAD_ROW_MAP = -70   # a row map without 1 <= nservers <= MAX_RANKS and rows_per_server >= 1
+
+
 class KV(C.Structure):
     _fields_ = [("vtype", C.c_int), ("nservers", C.c_int), ("capacity", i64), ("keys", VP8),
                 ("vals", VP8)]

@@ -12,6 +12,7 @@ from __future__ import annotations
 import torch
 
 from .. import _native as N
+from .topk import _rowmap_of
 
 
 def get_gemm_supported() -> bool:
@@ -54,11 +55,7 @@ def get_gemm(table, x: torch.Tensor, out: torch.Tensor = None) -> torch.Tensor:
     g = N.GetGemm()
     g.x, g.y, g.w_cache = x.data_ptr(), out.data_ptr(), None
     g.M, g.N, g.K = M, Nrows, K
-    g.wmap.num_row, g.wmap.num_col = Nrows, K
-    g.wmap.nservers = table.S
-    g.wmap.rows_per_server = table.rps
-    for s in range(table.S):
-        g.wmap.shard_ptrs[s] = table.shard_ptrs[s]
+    g.wmap = _rowmap_of(table, "get_gemm")[0]
     g.local_server = table.sid if table.S > 1 else 0
     N.cuda_lib().mvb_get_gemm_fused(g, N.stream_ptr())
     return out
@@ -81,8 +78,7 @@ def gemm_nt(x: torch.Tensor, w: torch.Tensor, out: torch.Tensor) -> torch.Tensor
     g = N.GetGemm()
     g.x, g.y, g.w_cache = x.data_ptr(), out.data_ptr(), None
     g.M, g.N, g.K = M, Nr, K
-    g.wmap.num_row, g.wmap.num_col, g.wmap.nservers, g.wmap.rows_per_server = Nr, K, 1, Nr
-    g.wmap.shard_ptrs[0] = w.data_ptr()
+    g.wmap = _rowmap_of(w, "gemm_nt")[0]
     g.local_server = 0
     N.cuda_lib().mvb_get_gemm_fused(g, N.stream_ptr())
     return out

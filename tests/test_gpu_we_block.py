@@ -129,29 +129,61 @@ def test_rows_pull_push(mv_device, rows, cols, k, ctas):
         N.cuda_lib().mvb_rows_pull(t._rowmap, 4, ids, None, k, full0, None, cols, 0, N.stream_ptr())
 
 
+def _get_add_rows(op, rm, full0, read_full, ids, cols):
+    """One of the int64-id row kernels (Get, stateless Add, fused AddDeltaParameter) on the rows ids."""
+    from multiverso_b200 import _native as N
+    lib, st, k = N.cuda_lib(), N.stream_ptr(), ids.numel()
+    ids = ids.long()
+    g = torch.Generator(device="cuda").manual_seed(11)
+    exp = full0.clone()
+    if op == "get_rows":
+        out = torch.full((k, cols), 7.0, device="cuda")
+        lib.mvb_get_rows(N.F32, rm, ids, k, out, cols, st)
+        torch.cuda.synchronize()
+        assert torch.equal(out, full0[ids])
+    elif op == "add_rows_red":
+        vals = torch.randn(k, cols, device="cuda", generator=g)
+        lib.mvb_add_rows_red(N.F32, rm, ids, k, vals, cols, -1.0, st)
+        exp[ids] -= vals
+    else:
+        old = torch.randn(k, cols, device="cuda", generator=g)
+        cur = old + torch.randn(k, cols, device="cuda", generator=g)
+        cur[::5] = old[::5]                                                # unchanged rows push nothing
+        lib.mvb_add_rows_delta(rm, ids, k, cur, old, cols, 0.5, st)
+        exp[ids] += (cur - old) * 0.5
+    torch.cuda.synchronize()
+    assert torch.allclose(read_full(), exp, rtol=0, atol=1e-6)
+
+
 def test_rows_pull_push_three_servers(mv_device):
-    """Owner arithmetic: three servers of 6000, 6000 and 8000 rows (the last takes the remainder), laid out
-    out of order in one local buffer with sentinel gaps between them, so a row read from or added to the wrong
-    server, or past its end, changes a value."""
+    """Owner arithmetic of every row kernel: three servers of 6000, 6000 and 8000 rows (the last takes the
+    remainder), laid out out of order in one local buffer with sentinel gaps between them, so a row read from or
+    added to the wrong server, or past its end, changes a value. Each kernel runs on a fresh copy of the layout:
+    row pull / delta push (int32 ids, device count), then mvb_get_rows, mvb_add_rows_red and mvb_add_rows_delta
+    (int64 ids)."""
     from multiverso_b200 import _native as N
     rows, cols, rps, gap = 20000, 300, 6000, 16
     lens = [rps, rps, rows - 2 * rps]
     starts = [lens[2] + gap, lens[2] + lens[0] + 2 * gap, 0]          # server 2 first, then 0, then 1
-    buf = torch.full((rows + 3 * gap, cols), 7.0, device="cuda")
-    shards = [buf[s0:s0 + n] for s0, n in zip(starts, lens)]
-    g = torch.Generator(device="cuda").manual_seed(3)
-    for sh in shards:
-        sh.copy_(torch.rand(sh.shape, device="cuda", generator=g) * 2 - 1)
-    gaps = torch.ones(buf.shape[0], dtype=torch.bool, device="cuda")
-    for s0, n in zip(starts, lens):
-        gaps[s0:s0 + n] = False
-    rm = N.RowMap()
-    rm.num_row, rm.num_col, rm.nservers, rm.rows_per_server = rows, cols, 3, rps
-    for s, sh in enumerate(shards):
-        rm.shard_ptrs[s] = sh.data_ptr()
-    full0 = torch.cat(shards)
     pick = torch.randperm(rows, generator=torch.Generator().manual_seed(7))[:5000]
     edges = torch.tensor([0, rps - 1, rps, 2 * rps - 1, 2 * rps, rows - 1])
     ids = torch.unique(torch.cat([pick, edges])).to(torch.int32).cuda()      # every owner, both ends of each
-    _pull_push(rm, full0, lambda: torch.cat(shards), ids, cols, 2)
-    assert bool((buf[gaps] == 7.0).all())
+    for op in ("pull_push", "get_rows", "add_rows_red", "add_rows_delta"):
+        buf = torch.full((rows + 3 * gap, cols), 7.0, device="cuda")
+        shards = [buf[s0:s0 + n] for s0, n in zip(starts, lens)]
+        g = torch.Generator(device="cuda").manual_seed(3)
+        for sh in shards:
+            sh.copy_(torch.rand(sh.shape, device="cuda", generator=g) * 2 - 1)
+        gaps = torch.ones(buf.shape[0], dtype=torch.bool, device="cuda")
+        for s0, n in zip(starts, lens):
+            gaps[s0:s0 + n] = False
+        rm = N.RowMap()
+        rm.num_row, rm.num_col, rm.nservers, rm.rows_per_server = rows, cols, 3, rps
+        for s, sh in enumerate(shards):
+            rm.shard_ptrs[s] = sh.data_ptr()
+        full0 = torch.cat(shards)
+        if op == "pull_push":
+            _pull_push(rm, full0, lambda: torch.cat(shards), ids, cols, 2)
+        else:
+            _get_add_rows(op, rm, full0, lambda: torch.cat(shards), ids, cols)
+        assert bool((buf[gaps] == 7.0).all()), op
