@@ -296,8 +296,7 @@ ArDev<T> to_dev(const MvbAllreduce* h) {
   a.epoch = h->epoch;
   a.err = h->err_flag;
   a.done_counter = h->done_counter;
-  double ts = h->timeout_s > 0 ? h->timeout_s : 60.0;
-  a.budget = (long long)(ts * 1.9e9);
+  a.budget = watchdog_cycles(h->timeout_s, 60.0);
   return a;
 }
 
@@ -305,20 +304,13 @@ template <typename T>
 int run(const MvbAllreduce* h, bool twoshot, cudaStream_t st) {
   ArDev<T> a = to_dev<T>(h);
   constexpr int VEC = 16 / sizeof(T);
-  int64_t work = h->n / VEC / (twoshot ? h->world : 1);
-  int64_t blocks = (work + 255) / 256;
-  int64_t cap = (int64_t)mvb_num_sms() * 4;
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
+  const int blocks = blocks_for(h->n / VEC / (twoshot ? h->world : 1), 256, 4);
   if (!twoshot) {
-    allreduce_oneshot_kernel<T><<<(int)blocks, 256, 0, st>>>(a);
+    allreduce_oneshot_kernel<T><<<blocks, 256, 0, st>>>(a);
   } else {
-    allreduce_twoshot_kernel<T><<<(int)blocks, 256, 0, st>>>(a);
-    int64_t b2 = (h->n / VEC + 255) / 256;
-    if (b2 > cap) b2 = cap;
-    if (b2 < 1) b2 = 1;
-    if (a.out == a.bufs[a.me]) b2 = 1;
-    allreduce_twoshot_finish<T><<<(int)b2, 256, 0, st>>>(a);
+    allreduce_twoshot_kernel<T><<<blocks, 256, 0, st>>>(a);
+    const int b2 = a.out == a.bufs[a.me] ? 1 : blocks_for(h->n / VEC, 256, 4);
+    allreduce_twoshot_finish<T><<<b2, 256, 0, st>>>(a);
   }
   MVB_CUDA_CHECK(cudaGetLastError());
   return 0;
@@ -337,16 +329,10 @@ int run_fused(const MvbAllreduce* h, const void* src, int64_t slot_off_bytes, cu
 }
 
 int dispatch(const MvbAllreduce* h, bool twoshot, void* stream) {
-  cudaStream_t st = (cudaStream_t)stream;
   if (h->world < 1 || h->world > MVB_MAX_RANKS) return -3;
-  switch (h->dtype) {
-    case MVB_F32: return run<float>(h, twoshot, st);
-    case MVB_F64: return run<double>(h, twoshot, st);
-    case MVB_I32: return run<int>(h, twoshot, st);
-    case MVB_I64: return run<long long>(h, twoshot, st);
-    case MVB_I8: return run<signed char>(h, twoshot, st);
-  }
-  return -1;
+  return with_dtype<float, double, int, long long, signed char>(h->dtype, [&](auto t) {
+    return run<typename decltype(t)::type>(h, twoshot, (cudaStream_t)stream);
+  });
 }
 
 }  // namespace
@@ -356,31 +342,18 @@ extern "C" int mvb_allreduce_nvls(const MvbAllreduce* h, void* multicast_ptr, vo
   if (h->dtype != MVB_F32 || multicast_ptr == nullptr) return -40;
   if (h->world < 2 || h->world > MVB_MAX_RANKS) return -3;
   ArDev<float> a = to_dev<float>(h);
-  int64_t work = h->n / 4 / h->world;
-  int64_t blocks = (work + 255) / 256;
-  int64_t cap = (int64_t)mvb_num_sms() * 2;
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
-  allreduce_nvls_kernel<<<(int)blocks, 256, 0, st>>>(a, (float*)multicast_ptr);
-  int64_t b2 = (h->n / 4 + 255) / 256;
-  if (b2 > cap * 2) b2 = cap * 2;
-  if (b2 < 1 || a.out == a.bufs[a.me]) b2 = 1;
-  allreduce_twoshot_finish<float><<<(int)b2, 256, 0, st>>>(a);
+  allreduce_nvls_kernel<<<blocks_for(h->n / 4 / h->world, 256, 2), 256, 0, st>>>(a, (float*)multicast_ptr);
+  const int b2 = a.out == a.bufs[a.me] ? 1 : blocks_for(h->n / 4, 256, 4);
+  allreduce_twoshot_finish<float><<<b2, 256, 0, st>>>(a);
   MVB_CUDA_CHECK(cudaGetLastError());
   return 0;
 }
 
 extern "C" int mvb_allreduce_fused(const MvbAllreduce* h, const void* src, int64_t slot_off_bytes, void* stream) {
-  cudaStream_t st = (cudaStream_t)stream;
   if (h->world < 1 || h->world > MVB_MAX_RANKS || (slot_off_bytes & 15)) return -3;
-  switch (h->dtype) {
-    case MVB_F32: return run_fused<float>(h, src, slot_off_bytes, st);
-    case MVB_F64: return run_fused<double>(h, src, slot_off_bytes, st);
-    case MVB_I32: return run_fused<int>(h, src, slot_off_bytes, st);
-    case MVB_I64: return run_fused<long long>(h, src, slot_off_bytes, st);
-    case MVB_I8: return run_fused<signed char>(h, src, slot_off_bytes, st);
-  }
-  return -1;
+  return with_dtype<float, double, int, long long, signed char>(h->dtype, [&](auto t) {
+    return run_fused<typename decltype(t)::type>(h, src, slot_off_bytes, (cudaStream_t)stream);
+  });
 }
 
 extern "C" int mvb_allreduce_oneshot(const MvbAllreduce* a, void* stream) {

@@ -55,41 +55,6 @@ MVB_DEVINL int prep_delta<int>(int g, float, float) {
   return g;
 }
 
-template <typename T, int VEC>
-struct Pack {
-  T v[VEC];
-};
-template <typename T, int VEC>
-MVB_DEVINL Pack<T, VEC> pk_load_nc(const T* p) {
-  Pack<T, VEC> r;
-  if constexpr (VEC == 1) {
-    r.v[0] = __ldg(p);
-  } else {
-    uint4 u = ld_nc_v4(p);
-    r = *reinterpret_cast<Pack<T, VEC>*>(&u);
-  }
-  return r;
-}
-template <typename T, int VEC>
-MVB_DEVINL Pack<T, VEC> pk_load(const T* p) {
-  Pack<T, VEC> r;
-  if constexpr (VEC == 1) {
-    r.v[0] = *p;
-  } else {
-    uint4 u = ld_v4(p);
-    r = *reinterpret_cast<Pack<T, VEC>*>(&u);
-  }
-  return r;
-}
-template <typename T, int VEC>
-MVB_DEVINL void pk_store(T* p, const Pack<T, VEC>& r) {
-  if constexpr (VEC == 1) {
-    *p = r.v[0];
-  } else {
-    st_v4(p, *reinterpret_cast<const uint4*>(&r));
-  }
-}
-
 // Fused Add -> Get: the freshly updated tile is pushed into EVERY rank's table replica while it
 // is still in registers -- one multimem.st (the NVSwitch replicates it) or a store per peer --
 // so the BSP step's Get degenerates to a flag wait (no second pass over NVLink).
@@ -183,29 +148,20 @@ add_dense_fused_kernel(const __grid_constant__ DenseAddDev<T> a) {
       if (w < a.W && ((mask >> w) & 1u)) g[w] = pk_load_nc<T, VEC>(a.delta[w] + a.shard_off + i);
     }
     Pack<T, VEC> d = pk_load<T, VEC>(a.shard + i);
-    Pack<T, VEC> s0, s1;
-#pragma unroll
-    for (int e = 0; e < VEC; ++e) s0.v[e] = s1.v[e] = (T)0;
-    if constexpr (U::kStates >= 1 && !U::kPerWorker) s0 = pk_load<T, VEC>(a.state0 + i);
+    // shared state is held across the workers' steps, per-worker state is worker w's slab during its step
+    Pack<T, VEC> s0{}, s1{};
+    if constexpr (!U::kPerWorker) state_load<U>(s0, s1, a.state0, a.state1, 0, a.state_stride, i);
 #pragma unroll
     for (int w = 0; w < MVB_MAX_RANKS; ++w) {
       if (w < a.W && ((mask >> w) & 1u)) {
-        if constexpr (U::kPerWorker) {
-          s0 = pk_load<T, VEC>(a.state0 + (int64_t)w * a.state_stride + i);
-          if constexpr (U::kStates >= 2)
-            s1 = pk_load<T, VEC>(a.state1 + (int64_t)w * a.state_stride + i);
-        }
+        if constexpr (U::kPerWorker) state_load<U>(s0, s1, a.state0, a.state1, w, a.state_stride, i);
 #pragma unroll
         for (int e = 0; e < VEC; ++e)
           U::Apply(d.v[e], prep_delta<T>(g[w].v[e], a.scale, a.clip), s0.v[e], s1.v[e], sopt[w]);
-        if constexpr (U::kPerWorker) {
-          pk_store<T, VEC>(a.state0 + (int64_t)w * a.state_stride + i, s0);
-          if constexpr (U::kStates >= 2)
-            pk_store<T, VEC>(a.state1 + (int64_t)w * a.state_stride + i, s1);
-        }
+        if constexpr (U::kPerWorker) state_store<U>(s0, s1, a.state0, a.state1, w, a.state_stride, i);
       }
     }
-    if constexpr (U::kStates >= 1 && !U::kPerWorker) pk_store<T, VEC>(a.state0 + i, s0);
+    if constexpr (!U::kPerWorker) state_store<U>(s0, s1, a.state0, a.state1, 0, a.state_stride, i);
     pk_store<T, VEC>(a.shard + i, d);
     if (a.has_replica) push_replica<T, VEC>(a, i, d);
   }
@@ -214,21 +170,15 @@ add_dense_fused_kernel(const __grid_constant__ DenseAddDev<T> a) {
     for (int64_t i = nvec * VEC + threadIdx.x; i < a.shard_len; i += blockDim.x) {
       T d = a.shard[i];
       T s0 = (T)0, s1 = (T)0;
-      if constexpr (U::kStates >= 1 && !U::kPerWorker) s0 = a.state0[i];
+      if constexpr (!U::kPerWorker) state_load<U>(s0, s1, a.state0, a.state1, 0, a.state_stride, i);
       for (int w = 0; w < a.W; ++w) {
         if (!((mask >> w) & 1u)) continue;
-        if constexpr (U::kPerWorker) {
-          s0 = a.state0[(int64_t)w * a.state_stride + i];
-          if constexpr (U::kStates >= 2) s1 = a.state1[(int64_t)w * a.state_stride + i];
-        }
+        if constexpr (U::kPerWorker) state_load<U>(s0, s1, a.state0, a.state1, w, a.state_stride, i);
         U::Apply(d, prep_delta<T>(__ldg(a.delta[w] + a.shard_off + i), a.scale, a.clip), s0, s1,
                  sopt[w]);
-        if constexpr (U::kPerWorker) {
-          a.state0[(int64_t)w * a.state_stride + i] = s0;
-          if constexpr (U::kStates >= 2) a.state1[(int64_t)w * a.state_stride + i] = s1;
-        }
+        if constexpr (U::kPerWorker) state_store<U>(s0, s1, a.state0, a.state1, w, a.state_stride, i);
       }
-      if constexpr (U::kStates >= 1 && !U::kPerWorker) a.state0[i] = s0;
+      if constexpr (!U::kPerWorker) state_store<U>(s0, s1, a.state0, a.state1, 0, a.state_stride, i);
       a.shard[i] = d;
       if (a.has_replica)
         for (int r = 0; r < a.world; ++r) a.replica[r][a.shard_off + i] = d;
@@ -302,35 +252,16 @@ int launch_add(const MvbDenseAdd* h, cudaStream_t st) {
   a.err = h->err_flag;
   a.fin_flag = h->fin_flag;
   a.done_counter = h->done_counter;
-  double ts = h->timeout_s > 0 ? h->timeout_s : 60.0;
-  a.budget = (long long)(ts * 1.9e9);
+  a.budget = watchdog_cycles(h->timeout_s, 60.0);
 
-  const int threads = 256;
   constexpr int VEC = VecOf<T>::N;
-  int64_t work = vec_ok ? (h->shard_len + VEC - 1) / VEC : h->shard_len;
-  int64_t blocks = (work + threads - 1) / threads;
-  int64_t cap = (int64_t)mvb_num_sms() * 4;
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
+  const int blocks = blocks_for(vec_ok ? (h->shard_len + VEC - 1) / VEC : h->shard_len, 256, 4);
   if (vec_ok)
-    add_dense_fused_kernel<UPD, T, VEC><<<(int)blocks, threads, 0, st>>>(a);
+    add_dense_fused_kernel<UPD, T, VEC><<<blocks, 256, 0, st>>>(a);
   else
-    add_dense_fused_kernel<UPD, T, 1><<<(int)blocks, threads, 0, st>>>(a);
+    add_dense_fused_kernel<UPD, T, 1><<<blocks, 256, 0, st>>>(a);
   MVB_CUDA_CHECK(cudaGetLastError());
   return 0;
-}
-
-template <typename T>
-int dispatch_add(const MvbDenseAdd* h, cudaStream_t st) {
-  switch (h->updater) {
-    case MVB_UPD_DEFAULT: return launch_add<MVB_UPD_DEFAULT, T>(h, st);
-    case MVB_UPD_SGD: return launch_add<MVB_UPD_SGD, T>(h, st);
-    case MVB_UPD_MOMENTUM: return launch_add<MVB_UPD_MOMENTUM, T>(h, st);
-    case MVB_UPD_ADAGRAD: return launch_add<MVB_UPD_ADAGRAD, T>(h, st);
-    case MVB_UPD_DCASGD: return launch_add<MVB_UPD_DCASGD, T>(h, st);
-    case MVB_UPD_DCASGDA: return launch_add<MVB_UPD_DCASGDA, T>(h, st);
-  }
-  return -2;
 }
 
 // ---------------------------------------------------------------------------
@@ -338,6 +269,21 @@ int dispatch_add(const MvbDenseAdd* h, cudaStream_t st) {
 // at (me + 1) so the 8 ranks hit 8 different sources at any instant and each
 // rank keeps loads in flight to every peer (NVSwitch: uniform bandwidth).
 // ---------------------------------------------------------------------------
+// this CTA's server segment s, its index among the CTAs dealt to s and their count
+struct SegCtas {
+  int s;
+  int64_t idx, count;
+};
+MVB_DEVINL SegCtas seg_ctas(int S, int me) {
+  const int grp = blockIdx.x % S;
+  return {(me + 1 + grp) % S, blockIdx.x / S, (gridDim.x - grp + S - 1) / S};
+}
+// a grid of at least `blocks` CTAs and a multiple of S, so that every segment gets the same number of CTAs
+static int seg_grid(int64_t blocks, int S) {
+  if (blocks < S) blocks = S;
+  return (int)((blocks + S - 1) / S * S);
+}
+
 template <typename T>
 struct DenseGetDev {
   T* out;
@@ -364,18 +310,14 @@ __global__ void __launch_bounds__(256) get_dense_kernel(const __grid_constant__ 
     }
     __syncthreads();
   }
-  const int groups = g.S;
-  const int grp = blockIdx.x % groups;
-  const int s = (g.me + 1 + grp) % groups;
-  const int64_t gidx = blockIdx.x / groups;
-  const int64_t gcount = (gridDim.x - grp + groups - 1) / groups;
-  const T* __restrict__ src = g.shard[s];
-  T* __restrict__ dst = g.out + g.off[s];
-  const int64_t len = g.len[s];
+  const SegCtas c = seg_ctas(g.S, g.me);
+  const T* __restrict__ src = g.shard[c.s];
+  T* __restrict__ dst = g.out + g.off[c.s];
+  const int64_t len = g.len[c.s];
   // `out` may be a view at any element offset: 16-byte accesses only where both ends are aligned
   const bool vec_ok = ((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst)) & 15) == 0;
-  const int64_t tid = gidx * blockDim.x + threadIdx.x;
-  const int64_t stride = gcount * blockDim.x;
+  const int64_t tid = c.idx * blockDim.x + threadIdx.x;
+  const int64_t stride = c.count * blockDim.x;
   if (vec_ok) {
     const int64_t nvec = len / VEC;
     int64_t v = tid;
@@ -398,7 +340,7 @@ __global__ void __launch_bounds__(256) get_dense_kernel(const __grid_constant__ 
 }
 
 // ---------------------------------------------------------------------------
-// K2, bulk-copy variant (EXPERIMENT, opt-in with MVB_GET_BULK=1; not measured yet).
+// K2, bulk-copy variant: the default for link-bound pulls (see launch_get; MVB_GET_BULK=0/1 overrides).
 // The register kernel above keeps 4 x 16 B per thread in flight; a link-bound pull wants megabytes
 // in flight per GPU. Here ONE thread per CTA drives a ring of kBulkStages x kBulkChunk bytes of
 // shared memory with the bulk-copy engine: cp.async.bulk global(peer) -> smem (mbarrier
@@ -423,15 +365,12 @@ __global__ void __launch_bounds__(32) get_dense_bulk_kernel(const __grid_constan
   if (threadIdx.x != 0) return;
   for (int i = 0; i < kBulkStages; ++i) mbar_init(&full[i], 1);
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  const int groups = g.S;
-  const int grp = blockIdx.x % groups;
-  const int s = (g.me + 1 + grp) % groups;
-  const int64_t gidx = blockIdx.x / groups;
-  const int64_t gcount = (gridDim.x - grp + groups - 1) / groups;
-  const char* src = reinterpret_cast<const char*>(g.shard[s]);
-  char* dst = reinterpret_cast<char*>(g.out + g.off[s]);
-  const int64_t bytes = g.len[s] * (int64_t)sizeof(T);
+  fence_proxy_async();
+  const SegCtas c = seg_ctas(g.S, g.me);
+  const int64_t gidx = c.idx, gcount = c.count;
+  const char* src = reinterpret_cast<const char*>(g.shard[c.s]);
+  char* dst = reinterpret_cast<char*>(g.out + g.off[c.s]);
+  const int64_t bytes = g.len[c.s] * (int64_t)sizeof(T);
   const int64_t body = bytes / 16 * 16;                          // bulk copies move multiples of 16 bytes
   const int64_t nchunks_total = (body + kBulkChunk - 1) / kBulkChunk;
   // chunks gidx, gidx + gcount, ... of this server's segment belong to this CTA
@@ -451,15 +390,15 @@ __global__ void __launch_bounds__(32) get_dense_bulk_kernel(const __grid_constan
     const int st = (int)(j % kBulkStages);
     mbar_wait(&full[st], (uint32_t)((j / kBulkStages) & 1));
     bulk_s2g(dst + chunk_off(j), ring + (size_t)st * kBulkChunk, chunk_len(j));
-    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+    bulk_commit();
     if (j + kBulkStages < mine) {
       // the stage is refilled only after the store has finished READING it; the other stages' loads
       // are still in flight meanwhile
-      asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+      bulk_wait_read<0>();
       load(j + kBulkStages);
     }
   }
-  asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");      // all stores performed before the kernel ends
+  bulk_wait_all();                                                // all stores performed before the kernel ends
   if (gidx == 0)                                                  // < 16 trailing bytes of the segment
     for (int64_t b = body; b < bytes; ++b) dst[b] = src[b];
 }
@@ -485,8 +424,7 @@ int launch_get(const MvbDenseGet* h, cudaStream_t st) {
   g.ch_done = h->ch_done;
   g.epoch = h->epoch;
   g.err = h->err_flag;
-  double ts = h->timeout_s > 0 ? h->timeout_s : 60.0;
-  g.budget = (long long)(ts * 1.9e9);
+  g.budget = watchdog_cycles(h->timeout_s, 60.0);
   // bulk-copy engine pull: measured at 8 GPUs (1M x 512 fp32) 2.76 ms vs 2.92 - 4.3 ms for the register
   // kernel and 2.81 ms for ncclAllGather; default for link-dominated pulls, MVB_GET_BULK=0/1 overrides
   static const int bulk_env = [] { const char* e = getenv("MVB_GET_BULK"); return e ? (atoi(e) != 0 ? 1 : 0) : -1; }();
@@ -503,22 +441,12 @@ int launch_get(const MvbDenseGet* h, cudaStream_t st) {
         MVB_CUDA_CHECK(cudaFuncSetAttribute(get_dense_bulk_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attr_set = true;
       }
-      int64_t blocks = mvb_num_sms();
-      if (blocks < h->nservers) blocks = h->nservers;
-      blocks = (blocks + h->nservers - 1) / h->nservers * h->nservers;
-      get_dense_bulk_kernel<T><<<(int)blocks, 32, smem, st>>>(g);
+      get_dense_bulk_kernel<T><<<seg_grid(mvb_num_sms(), h->nservers), 32, smem, st>>>(g);
       MVB_CUDA_CHECK(cudaGetLastError());
       return 0;
     }
   }
-  const int threads = 256;
-  int64_t blocks = (total / VecOf<T>::N / 4 + threads - 1) / threads;
-  int64_t cap = (int64_t)mvb_num_sms() * 8;
-  if (blocks > cap) blocks = cap;
-  if (blocks < h->nservers) blocks = h->nservers;
-  // keep the grid a multiple of the group count so segments get equal CTAs
-  blocks = (blocks + h->nservers - 1) / h->nservers * h->nservers;
-  get_dense_kernel<T><<<(int)blocks, threads, 0, st>>>(g);
+  get_dense_kernel<T><<<seg_grid(blocks_for(total / VecOf<T>::N / 4, 256, 8), h->nservers), 256, 0, st>>>(g);
   MVB_CUDA_CHECK(cudaGetLastError());
   return 0;
 }
@@ -533,43 +461,15 @@ updater_apply_kernel(T* __restrict__ data, const T* __restrict__ delta, T* __res
   using U = Updater<UPD, T>;
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    // one source: its state is slab 0 of s0p / s1p
     T d = data[i], s0 = (T)0, s1 = (T)0;
-    if constexpr (U::kStates >= 1) s0 = s0p[i];
-    if constexpr (U::kStates >= 2) s1 = s1p[i];
+    state_load<U>(s0, s1, s0p, s1p, 0, 0, i);
     U::Apply(d, prep_delta<T>(delta[i], scale, 0.f), s0, s1, opt);
-    if constexpr (U::kStates >= 1) s0p[i] = s0;
-    if constexpr (U::kStates >= 2) s1p[i] = s1;
+    state_store<U>(s0, s1, s0p, s1p, 0, 0, i);
     data[i] = d;
   }
 }
 
-template <typename T>
-int dispatch_apply(int upd, void* data, const void* delta, void* s0, void* s1, int64_t n,
-                   const MvbAddOpt* opt, float scale, cudaStream_t st) {
-  const int threads = 256;
-  int64_t blocks = (n + threads - 1) / threads;
-  int64_t cap = (int64_t)mvb_num_sms() * 8;
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
-#define MVB_LAUNCH_APPLY(U)                                                                   \
-  updater_apply_kernel<U, T><<<(int)blocks, threads, 0, st>>>((T*)data, (const T*)delta, (T*)s0, \
-                                                              (T*)s1, n, *opt, scale)
-  if constexpr (std::is_same<T, int>::value) {
-    MVB_LAUNCH_APPLY(MVB_UPD_DEFAULT);
-  } else
-  switch (upd) {
-    case MVB_UPD_DEFAULT: MVB_LAUNCH_APPLY(MVB_UPD_DEFAULT); break;
-    case MVB_UPD_SGD: MVB_LAUNCH_APPLY(MVB_UPD_SGD); break;
-    case MVB_UPD_MOMENTUM: MVB_LAUNCH_APPLY(MVB_UPD_MOMENTUM); break;
-    case MVB_UPD_ADAGRAD: MVB_LAUNCH_APPLY(MVB_UPD_ADAGRAD); break;
-    case MVB_UPD_DCASGD: MVB_LAUNCH_APPLY(MVB_UPD_DCASGD); break;
-    case MVB_UPD_DCASGDA: MVB_LAUNCH_APPLY(MVB_UPD_DCASGDA); break;
-    default: return -2;
-  }
-#undef MVB_LAUNCH_APPLY
-  MVB_CUDA_CHECK(cudaGetLastError());
-  return 0;
-}
 
 // ---------------------------------------------------------------------------
 // one-sided push (async PS): red.add into the owners' shards
@@ -584,13 +484,10 @@ struct PushDev {
 template <typename T>
 __global__ void __launch_bounds__(256)
 push_red_kernel(const T* __restrict__ delta, const __grid_constant__ PushDev p, float sign, int me) {
-  const int groups = p.S;
-  const int grp = blockIdx.x % groups;
-  const int s = (me + 1 + grp) % groups;
-  const int64_t gidx = blockIdx.x / groups;
-  const int64_t gcount = (gridDim.x - grp + groups - 1) / groups;
-  const int64_t tid = gidx * blockDim.x + threadIdx.x;
-  const int64_t stride = gcount * blockDim.x;
+  const SegCtas c = seg_ctas(p.S, me);
+  const int s = c.s;
+  const int64_t tid = c.idx * blockDim.x + threadIdx.x;
+  const int64_t stride = c.count * blockDim.x;
   const T* src = delta + p.off[s];
   T* dst = (T*)p.shard[s];
   const int64_t len = p.len[s];
@@ -630,53 +527,25 @@ template <int UPD, typename T>
 __global__ void __launch_bounds__(256)
 push_stateful_kernel(const T* __restrict__ delta, const __grid_constant__ PushStateDev p, MvbAddOpt opt, int me) {
   using U = Updater<UPD, T>;
-  const int groups = p.S;
-  const int grp = blockIdx.x % groups;
-  const int s = (me + 1 + grp) % groups;
-  const int64_t gidx = blockIdx.x / groups;
-  const int64_t gcount = (gridDim.x - grp + groups - 1) / groups;
-  const int64_t tid = gidx * blockDim.x + threadIdx.x;
-  const int64_t stride = gcount * blockDim.x;
+  const SegCtas c = seg_ctas(p.S, me);
+  const int s = c.s;
+  const int64_t tid = c.idx * blockDim.x + threadIdx.x;
+  const int64_t stride = c.count * blockDim.x;
   const T* src = delta + p.off[s];
   T* data = (T*)p.shard[s];
-  const int64_t woff = U::kPerWorker ? (int64_t)opt.worker_id * p.stride[s] : 0;
-  T* s0p = (T*)p.st0[s] + woff;
-  T* s1p = (T*)p.st1[s] + woff;
+  T* s0p = (T*)p.st0[s];
+  T* s1p = (T*)p.st1[s];
   const int64_t len = p.len[s];
   for (int64_t i = tid; i < len; i += stride) {
     const T d_old = data[i];
     T d = d_old, s0 = (T)0, s1 = (T)0;
-    if constexpr (U::kStates >= 1) s0 = s0p[i];
-    if constexpr (U::kStates >= 2) s1 = s1p[i];
+    state_load<U>(s0, s1, s0p, s1p, opt.worker_id, p.stride[s], i);
     U::Apply(d, src[i], s0, s1, opt);
-    if constexpr (U::kStates >= 1) s0p[i] = s0;
-    if constexpr (U::kStates >= 2) s1p[i] = s1;
+    state_store<U>(s0, s1, s0p, s1p, opt.worker_id, p.stride[s], i);
     // the step is applied ATOMICALLY (no lost updates when several workers push at once); only
     // the value DC-ASGD's compensation term saw may be stale, which is what it is built for
     red_add(data + i, (T)(d - d_old));
   }
-}
-
-template <typename T>
-int dispatch_push_stateful(int upd, const void* delta, const PushStateDev& p, const MvbAddOpt* opt, int me,
-                           int64_t total, cudaStream_t st) {
-  const int threads = 256;
-  int64_t blocks = (total + threads - 1) / threads;
-  int64_t cap = (int64_t)mvb_num_sms() * 8;
-  if (blocks > cap) blocks = cap;
-  if (blocks < p.S) blocks = p.S;
-  blocks = (blocks + p.S - 1) / p.S * p.S;
-#define MVB_PUSH_ST(U) push_stateful_kernel<U, T><<<(int)blocks, threads, 0, st>>>((const T*)delta, p, *opt, me)
-  switch (upd) {
-    case MVB_UPD_MOMENTUM: MVB_PUSH_ST(MVB_UPD_MOMENTUM); break;
-    case MVB_UPD_ADAGRAD: MVB_PUSH_ST(MVB_UPD_ADAGRAD); break;
-    case MVB_UPD_DCASGD: MVB_PUSH_ST(MVB_UPD_DCASGD); break;
-    case MVB_UPD_DCASGDA: MVB_PUSH_ST(MVB_UPD_DCASGDA); break;
-    default: return -2;
-  }
-#undef MVB_PUSH_ST
-  MVB_CUDA_CHECK(cudaGetLastError());
-  return 0;
 }
 
 }  // namespace
@@ -686,6 +555,7 @@ extern "C" int mvb_push_dense_stateful(int dtype, int updater, const void* delta
                                        void* const* state1_ptrs, const int64_t* shard_offs,
                                        const int64_t* shard_lens, const int64_t* state_strides,
                                        const MvbAddOpt* opt, int me, void* stream) {
+  if (nservers < 1 || nservers > MVB_MAX_RANKS) return -3;
   PushStateDev p{};
   p.S = nservers;
   int64_t total = 0;
@@ -698,52 +568,56 @@ extern "C" int mvb_push_dense_stateful(int dtype, int updater, const void* delta
     p.stride[s] = state_strides[s];
     total += shard_lens[s];
   }
-  cudaStream_t st = (cudaStream_t)stream;
-  switch (dtype) {
-    case MVB_F32: return dispatch_push_stateful<float>(updater, delta, p, opt, me, total, st);
-    case MVB_F64: return dispatch_push_stateful<double>(updater, delta, p, opt, me, total, st);
-  }
-  return -1;
+  return with_dtype<float, double>(dtype, [&](auto t) {
+    using T = typename decltype(t)::type;
+    return with_updater<T>(updater, [&](auto u) {
+      // the stateless updaters push with mvb_push_dense_red
+      if constexpr (Updater<decltype(u)::value, T>::kStates == 0) {
+        return -2;
+      } else {
+        push_stateful_kernel<decltype(u)::value, T><<<seg_grid(blocks_for(total, 256, 8), nservers), 256, 0,
+                                                      (cudaStream_t)stream>>>((const T*)delta, p, *opt, me);
+        MVB_CUDA_CHECK(cudaGetLastError());
+        return 0;
+      }
+    });
+  });
 }
 
 extern "C" int mvb_add_dense_fused(const MvbDenseAdd* a, void* stream) {
-  cudaStream_t st = (cudaStream_t)stream;
   if (a->nworkers < 1 || a->nworkers > MVB_MAX_RANKS) return -3;
-  switch (a->dtype) {
-    case MVB_F32: return dispatch_add<float>(a, st);
-    case MVB_F64: return dispatch_add<double>(a, st);
-    case MVB_I32: return launch_add<MVB_UPD_DEFAULT, int>(a, st);
-  }
-  return -1;
+  return with_dtype<float, double, int>(a->dtype, [&](auto t) {
+    using T = typename decltype(t)::type;
+    return with_updater<T>(a->updater,
+                           [&](auto u) { return launch_add<decltype(u)::value, T>(a, (cudaStream_t)stream); });
+  });
 }
 
 extern "C" int mvb_updater_apply(int dtype, int updater, void* data, const void* delta,
                                  void* state0, void* state1, int64_t n, const MvbAddOpt* opt,
                                  float scale, void* stream) {
-  cudaStream_t st = (cudaStream_t)stream;
-  switch (dtype) {
-    case MVB_F32: return dispatch_apply<float>(updater, data, delta, state0, state1, n, opt, scale, st);
-    case MVB_F64: return dispatch_apply<double>(updater, data, delta, state0, state1, n, opt, scale, st);
-    case MVB_I32: return dispatch_apply<int>(MVB_UPD_DEFAULT, data, delta, state0, state1, n, opt, 1.f, st);
-  }
-  return -1;
+  return with_dtype<float, double, int>(dtype, [&](auto t) {
+    using T = typename decltype(t)::type;
+    return with_updater<T>(updater, [&](auto u) {
+      updater_apply_kernel<decltype(u)::value, T><<<blocks_for(n, 256, 8), 256, 0, (cudaStream_t)stream>>>(
+          (T*)data, (const T*)delta, (T*)state0, (T*)state1, n, *opt, std::is_same<T, int>::value ? 1.f : scale);
+      MVB_CUDA_CHECK(cudaGetLastError());
+      return 0;
+    });
+  });
 }
 
 extern "C" int mvb_get_dense(const MvbDenseGet* g, void* stream) {
-  cudaStream_t st = (cudaStream_t)stream;
   if (g->nservers < 1 || g->nservers > MVB_MAX_RANKS) return -3;
-  switch (g->dtype) {
-    case MVB_F32: return launch_get<float>(g, st);
-    case MVB_F64: return launch_get<double>(g, st);
-    case MVB_I32: return launch_get<int>(g, st);
-  }
-  return -1;
+  return with_dtype<float, double, int>(g->dtype, [&](auto t) {
+    return launch_get<typename decltype(t)::type>(g, (cudaStream_t)stream);
+  });
 }
 
 extern "C" int mvb_push_dense_red(int dtype, const void* delta, int nservers,
                                   void* const* shard_ptrs, const int64_t* shard_offs,
                                   const int64_t* shard_lens, float sign, void* stream) {
-  cudaStream_t st = (cudaStream_t)stream;
+  if (nservers < 1 || nservers > MVB_MAX_RANKS) return -3;
   PushDev p{};
   p.S = nservers;
   int64_t total = 0;
@@ -753,19 +627,12 @@ extern "C" int mvb_push_dense_red(int dtype, const void* delta, int nservers,
     p.len[s] = shard_lens[s];
     total += shard_lens[s];
   }
-  const int threads = 256;
-  int64_t blocks = (total / 4 + threads - 1) / threads;
-  int64_t cap = (int64_t)mvb_num_sms() * 8;
-  if (blocks > cap) blocks = cap;
-  if (blocks < nservers) blocks = nservers;
-  blocks = (blocks + nservers - 1) / nservers * nservers;
-  int me = 0;  // segment rotation only; any value is correct
-  switch (dtype) {
-    case MVB_F32: push_red_kernel<float><<<(int)blocks, threads, 0, st>>>((const float*)delta, p, sign, me); break;
-    case MVB_F64: push_red_kernel<double><<<(int)blocks, threads, 0, st>>>((const double*)delta, p, sign, me); break;
-    case MVB_I32: push_red_kernel<int><<<(int)blocks, threads, 0, st>>>((const int*)delta, p, sign, me); break;
-    default: return -1;
-  }
-  MVB_CUDA_CHECK(cudaGetLastError());
-  return 0;
+  return with_dtype<float, double, int>(dtype, [&](auto t) {
+    using T = typename decltype(t)::type;
+    const int me = 0;  // segment rotation only; any value is correct
+    push_red_kernel<T><<<seg_grid(blocks_for(total / 4, 256, 8), nservers), 256, 0, (cudaStream_t)stream>>>(
+        (const T*)delta, p, sign, me);
+    MVB_CUDA_CHECK(cudaGetLastError());
+    return 0;
+  });
 }

@@ -189,32 +189,12 @@ __global__ void hash_dump_kernel(const long long* keys, const uint32_t* ready, i
   }
 }
 
-int blocks_for(int64_t n) {
-  int64_t b = (n + 255) / 256;
-  const int64_t cap = (int64_t)mvb_num_sms() * 8;
-  if (b > cap) b = cap;
-  if (b < 1) b = 1;
-  return (int)b;
-}
-
-long long budget_cycles(double timeout_s) {
-  static int khz = 0;
-  if (!khz) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&khz, cudaDevAttrClockRate, dev);
-    if (khz <= 0) khz = 1965000;
-  }
-  const double ts = timeout_s > 0 ? timeout_s : 120.0;
-  return (long long)(ts * 1e3 * khz);
-}
-
 }  // namespace
 
 extern "C" int mvb_hash_rows_init(void* keys, void* ready, void* count, int64_t slots, void* stream) {
   if (slots <= 0 || (slots & (slots - 1))) return -4;
   cudaStream_t st = (cudaStream_t)stream;
-  hash_init_kernel<<<blocks_for(slots), 256, 0, st>>>((long long*)keys, (uint32_t*)ready, slots);
+  hash_init_kernel<<<blocks_for(slots, 256, 8), 256, 0, st>>>((long long*)keys, (uint32_t*)ready, slots);
   MVB_CUDA_CHECK(cudaGetLastError());
   MVB_CUDA_CHECK(cudaMemsetAsync(count, 0, 8, st));
   return 0;
@@ -222,7 +202,8 @@ extern "C" int mvb_hash_rows_init(void* keys, void* ready, void* count, int64_t 
 
 extern "C" int mvb_hash_rows_lookup(const MvbHashLookup* a, void* stream) {
   if (a->n <= 0) return 0;
-  hash_lookup_kernel<<<blocks_for(a->n), 256, 0, (cudaStream_t)stream>>>(*a, budget_cycles(a->timeout_s));
+  hash_lookup_kernel<<<blocks_for(a->n, 256, 8), 256, 0, (cudaStream_t)stream>>>(*a,
+                                                                                 watchdog_cycles(a->timeout_s, 120.0));
   MVB_CUDA_CHECK(cudaGetLastError());
   return 0;
 }
@@ -238,7 +219,7 @@ extern "C" int mvb_hash_rows_dump(const MvbHashRows* h, int server, int64_t* out
   if (server < 0 || server >= h->nservers) return -1;
   cudaStream_t st = (cudaStream_t)stream;
   MVB_CUDA_CHECK(cudaMemsetAsync(out_count, 0, 8, st));
-  hash_dump_kernel<<<blocks_for(h->slots), 256, 0, st>>>((const long long*)h->keys[server],
+  hash_dump_kernel<<<blocks_for(h->slots, 256, 8), 256, 0, st>>>((const long long*)h->keys[server],
                                                           (const uint32_t*)h->ready[server], h->slots,
                                                           (int64_t)server * h->slots, out_keys, out_rows,
                                                           (unsigned long long*)out_count);

@@ -111,11 +111,6 @@ KeysDev to_dev(const MvbKeyMap* h) {
   }
   return m;
 }
-int blocks_for(int64_t n) {
-  int64_t b = (n + 255) / 256;
-  const int64_t cap = (int64_t)mvb_num_sms() * 8;
-  return (int)(b > cap ? cap : (b < 1 ? 1 : b));
-}
 
 }  // namespace
 
@@ -124,14 +119,14 @@ extern "C" int mvb_keys_add(const MvbKeyMap* m, const int64_t* keys, const float
   if (!row_split_ok(m->nservers, m->per_server)) return MVB_BAD_ROW_MAP;
   if (n <= 0) return 0;
   if (m->width < 1 || m->width > 16) return -8;
-  keys_add_kernel<<<blocks_for(n * m->width), 256, 0, (cudaStream_t)stream>>>(to_dev(m), (const long long*)keys, vals, n, sign);
+  keys_add_kernel<<<blocks_for(n * m->width, 256, 8), 256, 0, (cudaStream_t)stream>>>(to_dev(m), (const long long*)keys, vals, n, sign);
   MVB_CUDA_CHECK(cudaGetLastError());
   return 0;
 }
 extern "C" int mvb_keys_get(const MvbKeyMap* m, const int64_t* keys, float* out, int64_t n, void* stream) {
   if (!row_split_ok(m->nservers, m->per_server)) return MVB_BAD_ROW_MAP;
   if (n <= 0) return 0;
-  keys_get_kernel<<<blocks_for(n * m->width), 256, 0, (cudaStream_t)stream>>>(to_dev(m), (const long long*)keys, out, n);
+  keys_get_kernel<<<blocks_for(n * m->width, 256, 8), 256, 0, (cudaStream_t)stream>>>(to_dev(m), (const long long*)keys, out, n);
   MVB_CUDA_CHECK(cudaGetLastError());
   return 0;
 }
@@ -141,7 +136,7 @@ extern "C" int mvb_keys_collect(const MvbKeyMap* m, int64_t* out_keys, float* ou
   if (!row_split_ok(m->nservers, m->per_server)) return MVB_BAD_ROW_MAP;
   cudaStream_t st = (cudaStream_t)stream;
   MVB_CUDA_CHECK(cudaMemsetAsync(count, 0, 8, st));
-  keys_collect_kernel<<<blocks_for((m->size + 31) / 32 + m->nservers), 256, 0, st>>>(to_dev(m), (long long*)out_keys, out_vals,
+  keys_collect_kernel<<<blocks_for((m->size + 31) / 32 + m->nservers, 256, 8), 256, 0, st>>>(to_dev(m), (long long*)out_keys, out_vals,
                                                                                      (unsigned long long*)count, cap);
   MVB_CUDA_CHECK(cudaGetLastError());
   return 0;

@@ -142,75 +142,60 @@ KVDev to_dev(const MvbKV* h) {
   }
   return d;
 }
-int blocks_for(int64_t n) {
-  int64_t b = (n + 255) / 256;
-  int64_t cap = (int64_t)mvb_num_sms() * 8;
-  if (b > cap) b = cap;
-  if (b < 1) b = 1;
-  return (int)b;
-}
 
 }  // namespace
 
 extern "C" int mvb_kv_init(void* keys, int64_t capacity, void* stream) {
-  kv_init_kernel<<<blocks_for(capacity), 256, 0, (cudaStream_t)stream>>>((long long*)keys, capacity);
+  kv_init_kernel<<<blocks_for(capacity, 256, 8), 256, 0, (cudaStream_t)stream>>>((long long*)keys, capacity);
   MVB_CUDA_CHECK(cudaGetLastError());
   return 0;
 }
 extern "C" int mvb_kv_add(const MvbKV* kv, const int64_t* keys, const void* vals, int64_t n,
                           int* err_flag, void* stream) {
+  if (kv->nservers < 1 || kv->nservers > MVB_MAX_RANKS) return -3;
   if (n <= 0) return 0;
   if (kv->capacity & (kv->capacity - 1)) return -4;
-  KVDev d = to_dev(kv);
-  cudaStream_t st = (cudaStream_t)stream;
-  int b = blocks_for(n);
-  switch (kv->vtype) {
-    case MVB_F32: kv_add_kernel<float><<<b, 256, 0, st>>>(d, (const long long*)keys, (const float*)vals, n, err_flag); break;
-    case MVB_F64: kv_add_kernel<double><<<b, 256, 0, st>>>(d, (const long long*)keys, (const double*)vals, n, err_flag); break;
-    case MVB_I32: kv_add_kernel<int><<<b, 256, 0, st>>>(d, (const long long*)keys, (const int*)vals, n, err_flag); break;
-    case MVB_I64: kv_add_kernel<long long><<<b, 256, 0, st>>>(d, (const long long*)keys, (const long long*)vals, n, err_flag); break;
-    default: return -1;
-  }
-  MVB_CUDA_CHECK(cudaGetLastError());
-  return 0;
+  const KVDev d = to_dev(kv);
+  return with_dtype<float, double, int, long long>(kv->vtype, [&](auto t) {
+    using T = typename decltype(t)::type;
+    kv_add_kernel<T><<<blocks_for(n, 256, 8), 256, 0, (cudaStream_t)stream>>>(d, (const long long*)keys,
+                                                                               (const T*)vals, n, err_flag);
+    MVB_CUDA_CHECK(cudaGetLastError());
+    return 0;
+  });
 }
 extern "C" int mvb_kv_get(const MvbKV* kv, const int64_t* keys, void* out_vals, int64_t n,
                           void* stream) {
+  if (kv->nservers < 1 || kv->nservers > MVB_MAX_RANKS) return -3;
   if (n <= 0) return 0;
-  KVDev d = to_dev(kv);
-  cudaStream_t st = (cudaStream_t)stream;
-  int b = blocks_for(n);
-  switch (kv->vtype) {
-    case MVB_F32: kv_get_kernel<float><<<b, 256, 0, st>>>(d, (const long long*)keys, (float*)out_vals, n); break;
-    case MVB_F64: kv_get_kernel<double><<<b, 256, 0, st>>>(d, (const long long*)keys, (double*)out_vals, n); break;
-    case MVB_I32: kv_get_kernel<int><<<b, 256, 0, st>>>(d, (const long long*)keys, (int*)out_vals, n); break;
-    case MVB_I64: kv_get_kernel<long long><<<b, 256, 0, st>>>(d, (const long long*)keys, (long long*)out_vals, n); break;
-    default: return -1;
-  }
-  MVB_CUDA_CHECK(cudaGetLastError());
-  return 0;
+  const KVDev d = to_dev(kv);
+  return with_dtype<float, double, int, long long>(kv->vtype, [&](auto t) {
+    using T = typename decltype(t)::type;
+    kv_get_kernel<T><<<blocks_for(n, 256, 8), 256, 0, (cudaStream_t)stream>>>(d, (const long long*)keys,
+                                                                               (T*)out_vals, n);
+    MVB_CUDA_CHECK(cudaGetLastError());
+    return 0;
+  });
 }
 extern "C" int mvb_kv_dump(int vtype, const void* keys, const void* vals, int64_t capacity,
                            int64_t* out_keys, void* out_vals, int64_t* out_count, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
-  MVB_CUDA_CHECK(cudaMemsetAsync(out_count, 0, 8, st));
-  int b = blocks_for(capacity);
-  switch (vtype) {
-    case MVB_F32: kv_dump_kernel<float><<<b, 256, 0, st>>>((const long long*)keys, (const float*)vals, capacity, (long long*)out_keys, (float*)out_vals, (unsigned long long*)out_count); break;
-    case MVB_F64: kv_dump_kernel<double><<<b, 256, 0, st>>>((const long long*)keys, (const double*)vals, capacity, (long long*)out_keys, (double*)out_vals, (unsigned long long*)out_count); break;
-    case MVB_I32: kv_dump_kernel<int><<<b, 256, 0, st>>>((const long long*)keys, (const int*)vals, capacity, (long long*)out_keys, (int*)out_vals, (unsigned long long*)out_count); break;
-    case MVB_I64: kv_dump_kernel<long long><<<b, 256, 0, st>>>((const long long*)keys, (const long long*)vals, capacity, (long long*)out_keys, (long long*)out_vals, (unsigned long long*)out_count); break;
-    default: return -1;
-  }
-  MVB_CUDA_CHECK(cudaGetLastError());
-  return 0;
+  return with_dtype<float, double, int, long long>(vtype, [&](auto t) {
+    using T = typename decltype(t)::type;
+    MVB_CUDA_CHECK(cudaMemsetAsync(out_count, 0, 8, st));
+    kv_dump_kernel<T><<<blocks_for(capacity, 256, 8), 256, 0, st>>>((const long long*)keys, (const T*)vals, capacity,
+                                                                     (long long*)out_keys, (T*)out_vals,
+                                                                     (unsigned long long*)out_count);
+    MVB_CUDA_CHECK(cudaGetLastError());
+    return 0;
+  });
 }
 
 // Live keys of one shard (device count, zeroed here).
 extern "C" int mvb_kv_count(const void* keys, int64_t capacity, int64_t* out_count, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   MVB_CUDA_CHECK(cudaMemsetAsync(out_count, 0, 8, st));
-  kv_count_kernel<<<blocks_for(capacity), 256, 0, st>>>((const long long*)keys, capacity, (unsigned long long*)out_count);
+  kv_count_kernel<<<blocks_for(capacity, 256, 8), 256, 0, st>>>((const long long*)keys, capacity, (unsigned long long*)out_count);
   MVB_CUDA_CHECK(cudaGetLastError());
   return 0;
 }
@@ -218,15 +203,11 @@ extern "C" int mvb_kv_count(const void* keys, int64_t capacity, int64_t* out_cou
 extern "C" int mvb_kv_rehash(int vtype, const void* old_keys, const void* old_vals, int64_t old_cap, void* new_keys,
                              void* new_vals, int64_t new_cap, int* err_flag, void* stream) {
   if (new_cap & (new_cap - 1)) return -4;
-  cudaStream_t st = (cudaStream_t)stream;
-  const int b = blocks_for(old_cap);
-  switch (vtype) {
-    case MVB_F32: kv_rehash_kernel<float><<<b, 256, 0, st>>>((const long long*)old_keys, (const float*)old_vals, old_cap, (long long*)new_keys, (float*)new_vals, new_cap, err_flag); break;
-    case MVB_F64: kv_rehash_kernel<double><<<b, 256, 0, st>>>((const long long*)old_keys, (const double*)old_vals, old_cap, (long long*)new_keys, (double*)new_vals, new_cap, err_flag); break;
-    case MVB_I32: kv_rehash_kernel<int><<<b, 256, 0, st>>>((const long long*)old_keys, (const int*)old_vals, old_cap, (long long*)new_keys, (int*)new_vals, new_cap, err_flag); break;
-    case MVB_I64: kv_rehash_kernel<long long><<<b, 256, 0, st>>>((const long long*)old_keys, (const long long*)old_vals, old_cap, (long long*)new_keys, (long long*)new_vals, new_cap, err_flag); break;
-    default: return -1;
-  }
-  MVB_CUDA_CHECK(cudaGetLastError());
-  return 0;
+  return with_dtype<float, double, int, long long>(vtype, [&](auto t) {
+    using T = typename decltype(t)::type;
+    kv_rehash_kernel<T><<<blocks_for(old_cap, 256, 8), 256, 0, (cudaStream_t)stream>>>(
+        (const long long*)old_keys, (const T*)old_vals, old_cap, (long long*)new_keys, (T*)new_vals, new_cap, err_flag);
+    MVB_CUDA_CHECK(cudaGetLastError());
+    return 0;
+  });
 }

@@ -310,21 +310,12 @@ __global__ void axpy_kernel(float* __restrict__ y, const float* __restrict__ x, 
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) y[i] += alpha * x[i];
 }
 
-int ew_blocks(int64_t n) {
-  int64_t b = (n + 255) / 256;
-  int64_t cap = (int64_t)mvb_num_sms() * 8;
-  return (int)(b > cap ? cap : (b < 1 ? 1 : b));
-}
-
 }  // namespace
 
 extern "C" int mvb_lr_sparse_fwd_bwd(const MvbLrSparse* a, void* stream) {
   if (a->n <= 0) return 0;
   if (a->out > kMaxOut || a->out < 1) return -8;
-  int64_t blocks = (a->n + 3) / 4;
-  int64_t cap = (int64_t)mvb_num_sms() * 16;
-  if (blocks > cap) blocks = cap;
-  lr_sparse_fwd_kernel<<<(int)blocks, 128, 0, (cudaStream_t)stream>>>(*a);
+  lr_sparse_fwd_kernel<<<blocks_for(a->n * 32, 128, 16), 128, 0, (cudaStream_t)stream>>>(*a);
   MVB_CUDA_CHECK(cudaGetLastError());
   return 0;
 }
@@ -332,10 +323,7 @@ extern "C" int mvb_lr_dense_fwd_bwd(const MvbLrDense* a, void* stream) {
   if (a->n <= 0) return 0;
   if (a->out > kMaxOut || a->out < 1) return -8;
   cudaStream_t st = (cudaStream_t)stream;
-  int64_t blocks = (a->n + 3) / 4;
-  int64_t cap = (int64_t)mvb_num_sms() * 16;
-  if (blocks > cap) blocks = cap;
-  lr_dense_fwd_kernel<<<(int)blocks, 128, 0, st>>>(*a);
+  lr_dense_fwd_kernel<<<blocks_for(a->n * 32, 128, 16), 128, 0, st>>>(*a);
   if (a->compute_grad) {
     dim3 grid((unsigned)((a->dim + 127) / 128), (unsigned)((a->n + kSlab - 1) / kSlab));
     lr_dense_grad_kernel<<<grid, 128, 0, st>>>(*a);
@@ -345,19 +333,19 @@ extern "C" int mvb_lr_dense_fwd_bwd(const MvbLrDense* a, void* stream) {
 }
 extern "C" int mvb_ftrl_weights(const float* z, const float* n, float* w, int64_t len, float alpha,
                                 float beta, float l1, float l2, void* stream) {
-  ftrl_weights_kernel<<<ew_blocks(len), 256, 0, (cudaStream_t)stream>>>(z, n, w, len, alpha, beta, l1, l2);
+  ftrl_weights_kernel<<<blocks_for(len, 256, 8), 256, 0, (cudaStream_t)stream>>>(z, n, w, len, alpha, beta, l1, l2);
   MVB_CUDA_CHECK(cudaGetLastError());
   return 0;
 }
 extern "C" int mvb_ftrl_update(float* z, float* n, const float* w, const float* g, int64_t len,
                                float alpha, void* stream) {
-  ftrl_update_kernel<<<ew_blocks(len), 256, 0, (cudaStream_t)stream>>>(z, n, w, g, len, alpha);
+  ftrl_update_kernel<<<blocks_for(len, 256, 8), 256, 0, (cudaStream_t)stream>>>(z, n, w, g, len, alpha);
   MVB_CUDA_CHECK(cudaGetLastError());
   return 0;
 }
 extern "C" int mvb_regularize(float* grad, const float* w, int64_t len, int type, float coef,
                               void* stream) {
-  regularize_kernel<<<ew_blocks(len), 256, 0, (cudaStream_t)stream>>>(grad, w, len, type, coef);
+  regularize_kernel<<<blocks_for(len, 256, 8), 256, 0, (cudaStream_t)stream>>>(grad, w, len, type, coef);
   MVB_CUDA_CHECK(cudaGetLastError());
   return 0;
 }
@@ -370,10 +358,7 @@ extern "C" int mvb_lr_wide_epilogue(const float* logits, const float* labels, in
   if (out < 1 || n_pad < n) return -8;
   cudaStream_t st = (cudaStream_t)stream;
   MVB_CUDA_CHECK(cudaMemsetAsync(err_t, 0, (size_t)out * n_pad * sizeof(float), st));
-  int64_t blocks = (n + 3) / 4;
-  const int64_t cap = (int64_t)mvb_num_sms() * 16;
-  if (blocks > cap) blocks = cap;
-  lr_wide_epilogue_kernel<<<(int)blocks, 128, 0, st>>>(logits, labels, n, out, objective, 1.0f / (float)n, err_t,
+  lr_wide_epilogue_kernel<<<blocks_for(n * 32, 128, 16), 128, 0, st>>>(logits, labels, n, out, objective, 1.0f / (float)n, err_t,
                                                        n_pad, pred, loss_sum, correct);
   MVB_CUDA_CHECK(cudaGetLastError());
   return 0;
@@ -389,7 +374,7 @@ extern "C" int mvb_transpose_pad_f32(const float* in, int64_t rows, int64_t cols
 }
 extern "C" int mvb_axpy_f32(float* y, const float* x, int64_t n, float alpha, void* stream) {
   if (n <= 0) return 0;
-  axpy_kernel<<<ew_blocks(n), 256, 0, (cudaStream_t)stream>>>(y, x, n, alpha);
+  axpy_kernel<<<blocks_for(n, 256, 8), 256, 0, (cudaStream_t)stream>>>(y, x, n, alpha);
   MVB_CUDA_CHECK(cudaGetLastError());
   return 0;
 }
@@ -398,7 +383,7 @@ extern "C" int mvb_axpy_f32(float* y, const float* x, int64_t n, float alpha, vo
 extern "C" int mvb_ftrl_delta(const float* n, const float* w, const float* g, float* dz, float* dn, int64_t len,
                               float alpha, void* stream) {
   if (len <= 0) return 0;
-  ftrl_delta_kernel<<<ew_blocks(len), 256, 0, (cudaStream_t)stream>>>(n, w, g, dz, dn, len, alpha);
+  ftrl_delta_kernel<<<blocks_for(len, 256, 8), 256, 0, (cudaStream_t)stream>>>(n, w, g, dz, dn, len, alpha);
   MVB_CUDA_CHECK(cudaGetLastError());
   return 0;
 }

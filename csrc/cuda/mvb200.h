@@ -152,13 +152,15 @@ typedef struct MvbDenseGet {
 int mvb_get_dense(const MvbDenseGet* g, void* stream);
 
 /* One-sided async push: red.add of (sign * delta[shard range]) into every owner's
- * shard through the peer mapping. Stateless updaters only (default: +, sgd: -). */
+ * shard through the peer mapping. Stateless updaters only (default: +, sgd: -).
+ * Both one-sided pushes return -3 for nservers outside [1, MVB_MAX_RANKS], before any CUDA call. */
 int mvb_push_dense_red(int dtype, const void* delta, int nservers, void* const* shard_ptrs,
                        const int64_t* shard_offs, const int64_t* shard_lens, float sign,
                        void* stream);
 
 /* One-sided async push for STATEFUL updaters: remote read-modify-write of the owners' shard +
- * state slabs (state must be peer-mapped). Per-worker state is exact; data is Hogwild. */
+ * state slabs (state must be peer-mapped). Per-worker state is exact; data is Hogwild.
+ * f32 / f64 and the momentum, AdaGrad, DC-ASGD and DC-ASGD-A updaters only (-1 / -2 otherwise). */
 int mvb_push_dense_stateful(int dtype, int updater, const void* delta, int nservers,
                             void* const* shard_ptrs, void* const* state0_ptrs, void* const* state1_ptrs,
                             const int64_t* shard_offs, const int64_t* shard_lens,
@@ -219,6 +221,7 @@ int mvb_kv_init(void* keys, int64_t capacity, void* stream);
 int mvb_kv_count(const void* keys, int64_t capacity, int64_t* out_count, void* stream);
 int mvb_kv_rehash(int vtype, const void* old_keys, const void* old_vals, int64_t old_cap, void* new_keys,
                   void* new_vals, int64_t new_cap, int* err_flag, void* stream);
+/* mvb_kv_add and mvb_kv_get return -3 for nservers outside [1, MVB_MAX_RANKS], before any CUDA call */
 int mvb_kv_add(const MvbKV* kv, const int64_t* keys, const void* vals, int64_t n, int* err_flag,
                void* stream);
 int mvb_kv_get(const MvbKV* kv, const int64_t* keys, void* out_vals, int64_t n, void* stream);

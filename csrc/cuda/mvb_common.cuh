@@ -8,6 +8,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <type_traits>
 #include "mvb200.h"
 
 #define MVB_DEVINL __device__ __forceinline__
@@ -149,6 +150,42 @@ MVB_DEVINL void vec_store(T* p, const VecOf<T>& v) {
   st_v4(p, *reinterpret_cast<const uint4*>(&v));
 }
 
+// VEC elements of T: one element (VEC = 1) or a 16-byte vector, accessed with one load or store
+template <typename T, int VEC>
+struct Pack {
+  T v[VEC];
+};
+template <typename T, int VEC>
+MVB_DEVINL Pack<T, VEC> pk_load_nc(const T* p) {
+  Pack<T, VEC> r;
+  if constexpr (VEC == 1) {
+    r.v[0] = __ldg(p);
+  } else {
+    uint4 u = ld_nc_v4(p);
+    r = *reinterpret_cast<Pack<T, VEC>*>(&u);
+  }
+  return r;
+}
+template <typename T, int VEC>
+MVB_DEVINL Pack<T, VEC> pk_load(const T* p) {
+  Pack<T, VEC> r;
+  if constexpr (VEC == 1) {
+    r.v[0] = *p;
+  } else {
+    uint4 u = ld_v4(p);
+    r = *reinterpret_cast<Pack<T, VEC>*>(&u);
+  }
+  return r;
+}
+template <typename T, int VEC>
+MVB_DEVINL void pk_store(T* p, const Pack<T, VEC>& r) {
+  if constexpr (VEC == 1) {
+    *p = r.v[0];
+  } else {
+    st_v4(p, *reinterpret_cast<const uint4*>(&r));
+  }
+}
+
 MVB_DEVINL void red_add(float* p, float v) { red_add_f32(p, v); }
 MVB_DEVINL void red_add(double* p, double v) { red_add_f64(p, v); }
 MVB_DEVINL void red_add(int* p, int v) { red_add_s32(p, v); }
@@ -222,7 +259,34 @@ struct Updater<MVB_UPD_DCASGDA, T> {
     s0 = d;
   }
 };
-// int tables always use the plain add (reference: Updater<int>::GetUpdater).
+
+// Updater state of one element (T, or a float4 over float4 slabs) or of a pack of elements (Pack<T, VEC>). A state array holds
+// one slab shared by every worker or, for an updater with per-worker state, one slab per worker: worker w's
+// element i is at w * stride + i. state_load reads the updater's kStates values of element i of worker w's slab
+// before a run of Apply calls and state_store writes them back after it; a stateless updater touches no memory.
+template <typename T>
+MVB_DEVINL void state_ld(T& v, const T* p) { v = *p; }
+template <typename T, int VEC>
+MVB_DEVINL void state_ld(Pack<T, VEC>& v, const T* p) { v = pk_load<T, VEC>(p); }
+template <typename T>
+MVB_DEVINL void state_st(T* p, const T& v) { *p = v; }
+template <typename T, int VEC>
+MVB_DEVINL void state_st(T* p, const Pack<T, VEC>& v) { pk_store<T, VEC>(p, v); }
+
+template <class U>
+MVB_DEVINL int64_t state_at(int w, int64_t stride, int64_t i) {
+  return (U::kPerWorker ? (int64_t)w * stride : 0) + i;
+}
+template <class U, typename V, typename T>
+MVB_DEVINL void state_load(V& s0, V& s1, const T* st0, const T* st1, int w, int64_t stride, int64_t i) {
+  if constexpr (U::kStates >= 1) state_ld(s0, st0 + state_at<U>(w, stride, i));
+  if constexpr (U::kStates >= 2) state_ld(s1, st1 + state_at<U>(w, stride, i));
+}
+template <class U, typename V, typename T>
+MVB_DEVINL void state_store(const V& s0, const V& s1, T* st0, T* st1, int w, int64_t stride, int64_t i) {
+  if constexpr (U::kStates >= 1) state_st(st0 + state_at<U>(w, stride, i), s0);
+  if constexpr (U::kStates >= 2) state_st(st1 + state_at<U>(w, stride, i), s1);
+}
 
 // 64-bit finaliser of MurmurHash3: the counter-based RNG of the on-device samplers (a draw is a pure
 // function of its seed and index, so every rank and every run draws the same ids).
@@ -357,10 +421,65 @@ static inline int mvb_num_sms() {
   return sms;
 }
 
-// 256-thread CTAs for a grid-stride loop over `warps` items of a warp each, at most 8 CTAs per SM
-static inline int grid_for(int64_t warps) {
-  int64_t blocks = (warps * 32 + 255) / 256;
-  const int64_t cap = (int64_t)mvb_num_sms() * 8;
+// CTAs of `threads` threads for a grid-stride loop over n items of a thread each: enough to give every item a
+// thread, at least 1 and at most ctas_per_sm_cap per SM
+static inline int blocks_for(int64_t n, int threads, int ctas_per_sm_cap) {
+  int64_t blocks = (n + threads - 1) / threads;
+  const int64_t cap = (int64_t)mvb_num_sms() * ctas_per_sm_cap;
   if (blocks > cap) blocks = cap;
   return (int)(blocks < 1 ? 1 : blocks);
+}
+
+// 256-thread CTAs for a grid-stride loop over `warps` items of a warp each, at most 8 CTAs per SM
+static inline int grid_for(int64_t warps) { return blocks_for(warps * 32, 256, 8); }
+
+// clock64() cycles of a watchdog of timeout_s seconds (default_s when timeout_s <= 0) at the SM clock rate the
+// device reports
+static inline long long watchdog_cycles(double timeout_s, double default_s) {
+  static double hz = 0;
+  if (hz == 0) {
+    int dev = 0, khz = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&khz, cudaDevAttrClockRate, dev);
+    hz = khz > 0 ? khz * 1e3 : 1.9e9;
+  }
+  return (long long)((timeout_s > 0 ? timeout_s : default_s) * hz);
+}
+
+// Runtime codes to compile-time ones: f(std::integral_constant<int, UPD>{}) for an updater code, f(TypeTag<T>{})
+// for an element-type code of one of the types Ts an entry point accepts. Each returns what f returns, or -2 for
+// an unknown updater and -1 for an element type outside Ts. An int table always takes the plain add (reference:
+// Updater<int>::GetUpdater), whatever the code.
+template <typename T, typename F>
+static inline int with_updater(int upd, F&& f) {
+  using std::integral_constant;
+  if constexpr (std::is_same<T, int>::value) {
+    return f(integral_constant<int, MVB_UPD_DEFAULT>{});
+  } else {
+    switch (upd) {
+      case MVB_UPD_DEFAULT: return f(integral_constant<int, MVB_UPD_DEFAULT>{});
+      case MVB_UPD_SGD: return f(integral_constant<int, MVB_UPD_SGD>{});
+      case MVB_UPD_MOMENTUM: return f(integral_constant<int, MVB_UPD_MOMENTUM>{});
+      case MVB_UPD_ADAGRAD: return f(integral_constant<int, MVB_UPD_ADAGRAD>{});
+      case MVB_UPD_DCASGD: return f(integral_constant<int, MVB_UPD_DCASGD>{});
+      case MVB_UPD_DCASGDA: return f(integral_constant<int, MVB_UPD_DCASGDA>{});
+    }
+    return -2;
+  }
+}
+
+template <typename T>
+struct TypeTag { using type = T; };
+template <typename T> constexpr int kDtype = -1;
+template <> constexpr int kDtype<float> = MVB_F32;
+template <> constexpr int kDtype<double> = MVB_F64;
+template <> constexpr int kDtype<int> = MVB_I32;
+template <> constexpr int kDtype<long long> = MVB_I64;
+template <> constexpr int kDtype<signed char> = MVB_I8;
+
+template <typename... Ts, typename F>
+static inline int with_dtype(int dtype, F&& f) {
+  int rc = -1;
+  (void)((dtype == kDtype<Ts> ? (rc = f(TypeTag<Ts>{}), true) : false) || ...);
+  return rc;
 }

@@ -228,29 +228,27 @@ rowbox_apply_kernel(const __grid_constant__ BoxDev b, const __grid_constant__ Ap
   const int* ids = reinterpret_cast<const int*>(slot + kHdrBytes);
   const unsigned char* vals = slot + kHdrBytes + b.ids_bytes;
   const int lane = threadIdx.x & 31;
-  const int64_t woff = U::kPerWorker ? (int64_t)a.src * a.state_stride : 0;
   const int nvec = a.row_floats >> 2;
   for (int64_t i = warp_id(); i < count; i += num_warps()) {
     const int64_t r = (int64_t)__ldcg(ids + i);
     const int64_t base = (r - a.row_lo) * (int64_t)a.row_floats;
     if (r < a.row_lo || base < 0) continue;
     const float4* src = reinterpret_cast<const float4*>(vals + (size_t)i * b.ld_bytes);
+    float4* st0 = reinterpret_cast<float4*>(a.st0 + base);
+    float4* st1 = reinterpret_cast<float4*>(a.st1 + base);
+    const int64_t stride4 = a.state_stride >> 2;          // slabs of whole float4s: state_stride % 4 == 0
     for (int v = lane; v < nvec; v += 32) {
       const float4 g = __ldcg(src + v);
       float4* dp = reinterpret_cast<float4*>(a.shard + base) + v;
       float4 d = *dp;
       float4 s0 = make_float4(0, 0, 0, 0), s1 = make_float4(0, 0, 0, 0);
-      float4* s0p = nullptr;
-      float4* s1p = nullptr;
-      if constexpr (U::kStates >= 1) { s0p = reinterpret_cast<float4*>(a.st0 + woff + base) + v; s0 = *s0p; }
-      if constexpr (U::kStates >= 2) { s1p = reinterpret_cast<float4*>(a.st1 + woff + base) + v; s1 = *s1p; }
+      state_load<U>(s0, s1, st0, st1, a.src, stride4, v);
       U::Apply(d.x, g.x, s0.x, s1.x, opt);
       U::Apply(d.y, g.y, s0.y, s1.y, opt);
       U::Apply(d.z, g.z, s0.z, s1.z, opt);
       U::Apply(d.w, g.w, s0.w, s1.w, opt);
       *dp = d;
-      if constexpr (U::kStates >= 1) *s0p = s0;
-      if constexpr (U::kStates >= 2) *s1p = s1;
+      state_store<U>(s0, s1, st0, st1, a.src, stride4, v);
     }
   }
   // ---- completion: the last CTA records the epoch and acks the source ----
@@ -285,15 +283,9 @@ BoxDev to_dev(const MvbRowBox* h) {
   b.applied = h->applied;
   b.go = h->go;
   b.err = h->err_flag;
-  int dev = 0, khz = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&khz, cudaDevAttrClockRate, dev);
-  const double ts = h->timeout_s > 0 ? h->timeout_s : 120.0;
-  b.budget = (long long)(ts * 1e3 * (khz > 0 ? khz : 1965000));
+  b.budget = watchdog_cycles(h->timeout_s, 120.0);
   return b;
 }
-
-int grid_of(int ctas_per_sm) { return mvb_num_sms() * (ctas_per_sm > 0 ? ctas_per_sm : 1); }
 
 }  // namespace
 
@@ -318,9 +310,8 @@ static int push_common(const MvbRowBox* h, bool delta, const int* ids, const int
   a.src_ld_bytes = ld * 4; a.scale = scale; a.epoch = epoch;
   if (opt) a.opt = *opt;
   a.row_bytes = (int)(h->map.num_col * 4);
-  int grid = grid_of(ctas_per_sm);
-  const int64_t need = (n_max + 3) / 4;
-  if ((int64_t)grid > need) grid = (int)(need > 0 ? need : 1);
+  // a warp per row
+  const int grid = blocks_for(n_max * 32, kBoxThreads, ctas_per_sm > 0 ? ctas_per_sm : 1);
   if (delta) rowbox_push_kernel<true><<<grid, kBoxThreads, 0, st>>>(b, a);
   else rowbox_push_kernel<false><<<grid, kBoxThreads, 0, st>>>(b, a);
   MVB_CUDA_CHECK(cudaGetLastError());
@@ -360,17 +351,10 @@ extern "C" int mvb_rowbox_apply(const MvbRowBox* h, int updater, float* shard, f
   ApplyArgs a{};
   a.shard = shard; a.st0 = st0; a.st1 = st1; a.state_stride = state_stride; a.row_lo = row_lo;
   a.src = src; a.row_floats = (int)h->map.num_col;
-  const int grid = grid_of(ctas_per_sm);
-  cudaStream_t st = (cudaStream_t)stream;
-  switch (updater) {
-    case MVB_UPD_DEFAULT: rowbox_apply_kernel<MVB_UPD_DEFAULT><<<grid, kBoxThreads, 0, st>>>(b, a); break;
-    case MVB_UPD_SGD: rowbox_apply_kernel<MVB_UPD_SGD><<<grid, kBoxThreads, 0, st>>>(b, a); break;
-    case MVB_UPD_MOMENTUM: rowbox_apply_kernel<MVB_UPD_MOMENTUM><<<grid, kBoxThreads, 0, st>>>(b, a); break;
-    case MVB_UPD_ADAGRAD: rowbox_apply_kernel<MVB_UPD_ADAGRAD><<<grid, kBoxThreads, 0, st>>>(b, a); break;
-    case MVB_UPD_DCASGD: rowbox_apply_kernel<MVB_UPD_DCASGD><<<grid, kBoxThreads, 0, st>>>(b, a); break;
-    case MVB_UPD_DCASGDA: rowbox_apply_kernel<MVB_UPD_DCASGDA><<<grid, kBoxThreads, 0, st>>>(b, a); break;
-    default: return -2;
-  }
-  MVB_CUDA_CHECK(cudaGetLastError());
-  return 0;
+  return with_updater<float>(updater, [&](auto u) {
+    const int grid = mvb_num_sms() * (ctas_per_sm > 0 ? ctas_per_sm : 1);
+    rowbox_apply_kernel<decltype(u)::value><<<grid, kBoxThreads, 0, (cudaStream_t)stream>>>(b, a);
+    MVB_CUDA_CHECK(cudaGetLastError());
+    return 0;
+  });
 }

@@ -149,7 +149,6 @@ add_rows_owner_kernel(T* __restrict__ shard, T* __restrict__ st0, T* __restrict_
                       int64_t vals_ld, MvbAddOpt opt) {
   using U = Updater<UPD, T>;
   const int lane = threadIdx.x & 31;
-  const int64_t woff = U::kPerWorker ? (int64_t)opt.worker_id * state_stride : 0;
   for (int64_t i = warp_id(); i < k; i += num_warps()) {
     const int64_t r = ids[i];
     if (i > 0 && ids[i - 1] == r) continue;  // inside a run: applied by the run's first warp
@@ -159,11 +158,9 @@ add_rows_owner_kernel(T* __restrict__ shard, T* __restrict__ st0, T* __restrict_
     const int64_t base = (r - row_lo) * num_col;
     for (int64_t c = lane; c < num_col; c += 32) {
       T d = shard[base + c], s0 = (T)0, s1 = (T)0;
-      if constexpr (U::kStates >= 1) s0 = st0[woff + base + c];
-      if constexpr (U::kStates >= 2) s1 = st1[woff + base + c];
+      state_load<U>(s0, s1, st0, st1, opt.worker_id, state_stride, base + c);
       for (int64_t j = i; j < end; ++j) U::Apply(d, vals[j * vals_ld + c], s0, s1, opt);
-      if constexpr (U::kStates >= 1) st0[woff + base + c] = s0;
-      if constexpr (U::kStates >= 2) st1[woff + base + c] = s1;
+      state_store<U>(s0, s1, st0, st1, opt.worker_id, state_stride, base + c);
       shard[base + c] = d;
     }
   }
@@ -260,32 +257,6 @@ int add_rows_red_t(const MvbRowMap* m, const int64_t* ids, int64_t k, const void
   return 0;
 }
 
-template <typename T>
-int add_rows_owner_t(int upd, void* shard, void* s0, void* s1, int64_t lo, int64_t hi,
-                     int64_t cols, int64_t sstride, const int64_t* ids, int64_t k,
-                     const void* vals, int64_t vld, const MvbAddOpt* opt, cudaStream_t st) {
-  int grid = grid_for(k);
-#define MVB_ROWS_OWNER(U)                                                                  \
-  add_rows_owner_kernel<U, T><<<grid, 256, 0, st>>>((T*)shard, (T*)s0, (T*)s1, lo, hi, cols, \
-                                                    sstride, ids, k, (const T*)vals, vld, *opt)
-  if constexpr (std::is_same<T, int>::value) {
-    MVB_ROWS_OWNER(MVB_UPD_DEFAULT);
-  } else {
-    switch (upd) {
-      case MVB_UPD_DEFAULT: MVB_ROWS_OWNER(MVB_UPD_DEFAULT); break;
-      case MVB_UPD_SGD: MVB_ROWS_OWNER(MVB_UPD_SGD); break;
-      case MVB_UPD_MOMENTUM: MVB_ROWS_OWNER(MVB_UPD_MOMENTUM); break;
-      case MVB_UPD_ADAGRAD: MVB_ROWS_OWNER(MVB_UPD_ADAGRAD); break;
-      case MVB_UPD_DCASGD: MVB_ROWS_OWNER(MVB_UPD_DCASGD); break;
-      case MVB_UPD_DCASGDA: MVB_ROWS_OWNER(MVB_UPD_DCASGDA); break;
-      default: return -2;
-    }
-  }
-#undef MVB_ROWS_OWNER
-  MVB_CUDA_CHECK(cudaGetLastError());
-  return 0;
-}
-
 template <typename Id>
 int add_rows_delta_t(const MvbRowMap* m, const Id* ids, const int* n_ptr, int64_t n_max, const float* cur,
                      const float* old, int64_t ld, float scale, int64_t ctas, cudaStream_t st) {
@@ -305,32 +276,24 @@ extern "C" int mvb_get_rows(int dtype, const MvbRowMap* m, const int64_t* row_id
                             void* out, int64_t out_ld, void* stream) {
   if (!row_split_ok(m->nservers, m->rows_per_server)) return MVB_BAD_ROW_MAP;
   if (k <= 0) return 0;
-  cudaStream_t st = (cudaStream_t)stream;
-  switch (dtype) {
-    case MVB_F32: return get_rows_t<float>(m, row_ids, k, out, out_ld, st);
-    case MVB_F64: return get_rows_t<double>(m, row_ids, k, out, out_ld, st);
-    case MVB_I32: return get_rows_t<int>(m, row_ids, k, out, out_ld, st);
-  }
-  return -1;
+  return with_dtype<float, double, int>(dtype, [&](auto t) {
+    return get_rows_t<typename decltype(t)::type>(m, row_ids, k, out, out_ld, (cudaStream_t)stream);
+  });
 }
 extern "C" int mvb_add_rows_red(int dtype, const MvbRowMap* m, const int64_t* row_ids, int64_t k,
                                 const void* vals, int64_t vals_ld, float sign, void* stream) {
   if (!row_split_ok(m->nservers, m->rows_per_server)) return MVB_BAD_ROW_MAP;
   if (k <= 0) return 0;
-  cudaStream_t st = (cudaStream_t)stream;
-  switch (dtype) {
-    case MVB_F32: return add_rows_red_t<float>(m, row_ids, k, vals, vals_ld, sign, st);
-    case MVB_F64: return add_rows_red_t<double>(m, row_ids, k, vals, vals_ld, sign, st);
-    case MVB_I32: return add_rows_red_t<int>(m, row_ids, k, vals, vals_ld, sign, st);
-  }
-  return -1;
+  return with_dtype<float, double, int>(dtype, [&](auto t) {
+    return add_rows_red_t<typename decltype(t)::type>(m, row_ids, k, vals, vals_ld, sign, (cudaStream_t)stream);
+  });
 }
 extern "C" int mvb_add_rows_delta(const MvbRowMap* m, const int64_t* row_ids, int64_t k, const float* cur,
                                   const float* old, int64_t ld, float scale, void* stream) {
   if (!row_split_ok(m->nservers, m->rows_per_server)) return MVB_BAD_ROW_MAP;
   if (k <= 0) return 0;
   // a warp per row, at most 8 x 256 threads per SM
-  const int64_t ctas = std::min<int64_t>((k * 32 + kDeltaThreads - 1) / kDeltaThreads, (int64_t)mvb_num_sms() * 16);
+  const int ctas = blocks_for(k * 32, kDeltaThreads, 16);
   return add_rows_delta_t<int64_t>(m, row_ids, nullptr, k, cur, old, ld, scale, ctas, (cudaStream_t)stream);
 }
 // rows[ids[s]] += (cur[s] - old[s]) * scale for s in [0, n), n read on the device from n_ptr when given (clamped to
@@ -350,33 +313,26 @@ extern "C" int mvb_add_rows_owner(int dtype, int updater, void* shard, void* sta
                                   const void* vals, int64_t vals_ld, const MvbAddOpt* opt,
                                   void* stream) {
   if (k <= 0) return 0;
-  cudaStream_t st = (cudaStream_t)stream;
-  switch (dtype) {
-    case MVB_F32:
-      return add_rows_owner_t<float>(updater, shard, state0, state1, row_lo, row_hi, num_col,
-                                     state_stride, row_ids, k, vals, vals_ld, opt, st);
-    case MVB_F64:
-      return add_rows_owner_t<double>(updater, shard, state0, state1, row_lo, row_hi, num_col,
-                                      state_stride, row_ids, k, vals, vals_ld, opt, st);
-    case MVB_I32:
-      return add_rows_owner_t<int>(updater, shard, state0, state1, row_lo, row_hi, num_col,
-                                   state_stride, row_ids, k, vals, vals_ld, opt, st);
-  }
-  return -1;
+  return with_dtype<float, double, int>(dtype, [&](auto t) {
+    using T = typename decltype(t)::type;
+    return with_updater<T>(updater, [&](auto u) {
+      add_rows_owner_kernel<decltype(u)::value, T><<<grid_for(k), 256, 0, (cudaStream_t)stream>>>(
+          (T*)shard, (T*)state0, (T*)state1, row_lo, row_hi, num_col, state_stride, row_ids, k, (const T*)vals,
+          vals_ld, *opt);
+      MVB_CUDA_CHECK(cudaGetLastError());
+      return 0;
+    });
+  });
 }
 extern "C" int mvb_row_nonzero_mask(int dtype, const void* data, int64_t rows, int64_t cols,
                                     int64_t ld, uint8_t* mask, void* stream) {
   if (rows <= 0) return 0;
-  cudaStream_t st = (cudaStream_t)stream;
-  int grid = grid_for(rows);
-  switch (dtype) {
-    case MVB_F32: row_nonzero_kernel<float><<<grid, 256, 0, st>>>((const float*)data, rows, cols, ld, mask); break;
-    case MVB_F64: row_nonzero_kernel<double><<<grid, 256, 0, st>>>((const double*)data, rows, cols, ld, mask); break;
-    case MVB_I32: row_nonzero_kernel<int><<<grid, 256, 0, st>>>((const int*)data, rows, cols, ld, mask); break;
-    default: return -1;
-  }
-  MVB_CUDA_CHECK(cudaGetLastError());
-  return 0;
+  return with_dtype<float, double, int>(dtype, [&](auto t) {
+    using T = typename decltype(t)::type;
+    row_nonzero_kernel<T><<<grid_for(rows), 256, 0, (cudaStream_t)stream>>>((const T*)data, rows, cols, ld, mask);
+    MVB_CUDA_CHECK(cudaGetLastError());
+    return 0;
+  });
 }
 extern "C" int mvb_stale_mark(uint8_t* stale, int64_t rows, int nworkers, const int64_t* row_ids,
                               int64_t k, void* stream) {

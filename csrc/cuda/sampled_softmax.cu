@@ -146,18 +146,12 @@ int check_shapes(const MvbSampledSoftmax* a) {
   return 0;
 }
 
-int blocks_for(int64_t n, int threads) {
-  int64_t b = (n + threads - 1) / threads;
-  const int64_t cap = (int64_t)mvb_num_sms() * 8;
-  return (int)(b > cap ? cap : (b < 1 ? 1 : b));
-}
-
 }  // namespace
 
 extern "C" int mvb_ss_sample(const MvbSampledSoftmax* a, void* stream) {
   if (int rc = check_shapes(a)) return rc;
   if (!a->alias_prob || !a->alias_idx || !a->logq || !a->cand || !a->logq_c) return -61;
-  ss_sample_kernel<<<blocks_for(a->S, 256), 256, 0, (cudaStream_t)stream>>>(*a);
+  ss_sample_kernel<<<blocks_for(a->S, 256, 8), 256, 0, (cudaStream_t)stream>>>(*a);
   MVB_CUDA_CHECK(cudaGetLastError());
   return 0;
 }

@@ -157,12 +157,6 @@ extern "C" int mvb_event_destroy(void* event) {
 // ---------------------------------------------------------------------------
 // Signal pads. slot(channel, src) = pad[channel * MVB_MAX_RANKS + src].
 // ---------------------------------------------------------------------------
-static inline long long timeout_cycles(double s) {
-  // SM clock tops out at ~1.97 GHz; budget in cycles of clock64().
-  if (s <= 0) s = 60.0;
-  return (long long)(s * 1.9e9);
-}
-
 __global__ void signal_kernel(MvbPeers pads, int me, int world, int channel, uint64_t epoch) {
   int t = threadIdx.x;
   if (t < world) {
@@ -215,14 +209,14 @@ extern "C" int mvb_signal(void* const* pads, int me, int world, int channel, uin
 extern "C" int mvb_wait(void* const* pads, int me, int world, int channel, uint64_t epoch,
                         uint32_t src_mask, int* err_flag, double timeout_s, void* stream) {
   wait_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(to_peers(pads, world), me, world, channel, epoch,
-                                                  src_mask, err_flag, timeout_cycles(timeout_s));
+                                                  src_mask, err_flag, watchdog_cycles(timeout_s, 60.0));
   MVB_CUDA_CHECK(cudaGetLastError());
   return 0;
 }
 extern "C" int mvb_barrier(void* const* pads, int me, int world, int channel, uint64_t epoch,
                            int* err_flag, double timeout_s, void* stream) {
   barrier_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(to_peers(pads, world), me, world, channel,
-                                                     epoch, err_flag, timeout_cycles(timeout_s));
+                                                     epoch, err_flag, watchdog_cycles(timeout_s, 60.0));
   MVB_CUDA_CHECK(cudaGetLastError());
   return 0;
 }

@@ -532,3 +532,211 @@ def test_int64_tables_rejected(mv_device):
         mv.ArrayTable(8, "int64")
     with pytest.raises(FatalError, match="float32/float64/int32"):
         mv.MatrixTable(4, 4, "int64")
+
+
+# ------------------------------------------------------------------ GPU tier: updater kernels called directly
+_KSENT = -123.5           # sentinel of every buffer region a kernel must not write
+
+
+def _kopt(k, worker_id):
+    """The k-th AddOption of ``_OPTS`` for ``worker_id``, and its C struct."""
+    from multiverso_b200.tables.options import AddOption
+    from multiverso_b200.tables.device import _opt_struct
+    m, lr, rho, lam = _OPTS[k % len(_OPTS)]
+    o = AddOption(worker_id=worker_id, momentum=m, learning_rate=lr, rho=rho, lambda_=lam)
+    return o, _opt_struct(o)
+
+
+def _start_values(rng, n, dtype):
+    return (rng.choice([-1.0, 1.0], n) * rng.uniform(0.25, 1.0, n)).astype(dtype)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("scale", [1.0, 0.5])
+@pytest.mark.parametrize("dtype", ["float32", "float64", "int32"])
+@pytest.mark.parametrize("updater", STATEFUL)
+def test_updater_apply(mv_device, updater, dtype, scale):
+    """The stand-alone updater (``mvb_updater_apply``) over more elements than its grid covers at once: five
+    steps, the AddOption changing at every step, the delta scaled by ``scale``; values and the state slabs
+    (one shared slab each, whatever the updater) against the model. An int32 table always takes the plain
+    add, ignores ``scale`` and touches no state."""
+    from multiverso_b200 import _native as N
+    lib, st = N.cuda_lib(), N.stream_ptr()
+    n = 300_001
+    rng = np.random.default_rng(21)
+    is_int = dtype == "int32"
+    start = rng.integers(-1000, 1000, n).astype(dtype) if is_int else _start_values(rng, n, dtype)
+    data = torch.from_numpy(start).cuda()
+    nst = 0 if is_int else _STATES[updater][0]
+    states = [torch.zeros(n, dtype=getattr(torch, dtype), device="cuda") for _ in range(nst)]
+    model = ServerModel(start, 1, updater, dtype)
+    for k in range(5):
+        opt, copt = _kopt(k, 0)
+        d = _delta(rng, (n,), dtype)
+        lib.mvb_updater_apply(N.dtype_code(data.dtype), N.UPDATER_NAMES[updater], data, torch.from_numpy(d).cuda(),
+                              states[0] if nst >= 1 else None, states[1] if nst >= 2 else None, n, copt, scale, st)
+        model.add(d if is_int else d * scale, opt)
+    torch.cuda.synchronize()
+    what = f"updater_apply {updater} {dtype} scale={scale}"
+    _assert_close(data.cpu().numpy(), model.data.reshape(-1), (np.abs(model.data) + model.mag).reshape(-1),
+                  model.nupd.reshape(-1), dtype, f"{what} values")
+    for i in range(nst):
+        _assert_close(states[i].cpu().numpy(), model.state[i][0].reshape(-1), model.state_scale(i).reshape(-1),
+                      model.nupd.reshape(-1), dtype, f"{what} state{i}")
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("worker_id", [0, 2])
+@pytest.mark.parametrize("nservers", [1, 3])
+@pytest.mark.parametrize("dtype", ["float32", "float64"])
+@pytest.mark.parametrize("updater", STATEFUL)
+def test_push_dense_stateful(mv_device, updater, dtype, nservers, worker_id):
+    """The one-sided stateful push (``mvb_push_dense_stateful``) of worker ``worker_id`` into ``nservers``
+    servers, emulated as slices of one device buffer laid out out of order with sentinel gaps; each server's
+    state is a slab of three workers (one shared slab for momentum) at a padded stride. Three pushes; values
+    and the worker's state slab against the model, every other word of the buffers bitwise unchanged."""
+    from multiverso_b200 import _native as N
+    import ctypes as C
+    lib, st = N.cuda_lib(), N.stream_ptr()
+    n, gap, W = 10007, 16, 3
+    lens = [n] if nservers == 1 else [3000, 3000, n - 6000]
+    offs = np.concatenate([[0], np.cumsum(lens)[:-1]]).tolist()
+    order = list(range(nservers))[::-1]                       # the last server first in the buffers
+    nst, per_worker = _STATES[updater]
+    nslab = W if per_worker else 1
+    strides = [(ln + 3) // 4 * 4 + 8 for ln in lens]          # padding between a server's worker slabs
+    tdt = getattr(torch, dtype)
+    data_at, state_at, pos, spos = {}, {}, gap, gap
+    for s in order:
+        data_at[s], state_at[s] = pos, spos
+        pos += lens[s] + gap
+        spos += strides[s] * nslab + gap
+    rng = np.random.default_rng(nservers * 10 + worker_id)
+    start = _start_values(rng, n, dtype)
+    data = torch.full((pos,), _KSENT, dtype=tdt, device="cuda")
+    states = [torch.full((spos,), _KSENT, dtype=tdt, device="cuda") for _ in range(nst)]
+    slab = worker_id if per_worker else 0
+    for s in range(nservers):
+        data[data_at[s]:data_at[s] + lens[s]] = torch.from_numpy(start[offs[s]:offs[s] + lens[s]]).cuda()
+        for t in states:
+            o = state_at[s] + slab * strides[s]
+            t[o:o + lens[s]] = 0
+    data0, states0 = data.clone(), [t.clone() for t in states]
+    esz = data.element_size()
+    sp = (C.c_void_p * nservers)(*[data.data_ptr() + data_at[s] * esz for s in range(nservers)])
+    s0 = (C.c_void_p * nservers)(*[(states[0].data_ptr() + state_at[s] * esz) if nst >= 1 else 0
+                                   for s in range(nservers)])
+    s1 = (C.c_void_p * nservers)(*[(states[1].data_ptr() + state_at[s] * esz) if nst >= 2 else 0
+                                   for s in range(nservers)])
+    so, sl = (C.c_int64 * nservers)(*offs), (C.c_int64 * nservers)(*lens)
+    ss = (C.c_int64 * nservers)(*strides)
+    model = ServerModel(start, 1, updater, dtype, workers=W)
+    for k in range(3):
+        opt, copt = _kopt(k, worker_id)
+        d = _delta(rng, (n,), dtype)
+        lib.mvb_push_dense_stateful(N.dtype_code(tdt), N.UPDATER_NAMES[updater], torch.from_numpy(d).cuda(), nservers,
+                                    sp, s0, s1, so, sl, ss, copt, 1, st)
+        model.add(d, opt)
+    torch.cuda.synchronize()
+    what = f"push_dense_stateful {updater} {dtype} S={nservers} worker {worker_id}"
+    got = torch.cat([data[data_at[s]:data_at[s] + lens[s]] for s in range(nservers)]).cpu().numpy()
+    _assert_close(got, model.data.reshape(-1), (np.abs(model.data) + model.mag).reshape(-1),
+                  model.nupd.reshape(-1), dtype, f"{what} values")
+    written = torch.zeros(pos, dtype=torch.bool, device="cuda")
+    for s in range(nservers):
+        written[data_at[s]:data_at[s] + lens[s]] = True
+    assert torch.equal(data[~written], data0[~written]), f"{what}: data written outside the shards"
+    mw = worker_id if per_worker else 0
+    for i, t in enumerate(states):
+        got = torch.cat([t[state_at[s] + slab * strides[s]:][:lens[s]] for s in range(nservers)]).cpu().numpy()
+        _assert_close(got, model.state[i][mw].reshape(-1), model.state_scale(i, mw).reshape(-1),
+                      model.nupd.reshape(-1), dtype, f"{what} state{i}")
+        mine = torch.zeros(spos, dtype=torch.bool, device="cuda")
+        for s in range(nservers):
+            mine[state_at[s] + slab * strides[s]:][:lens[s]] = True
+        assert torch.equal(t[~mine], states0[i][~mine]), f"{what}: state{i} written outside worker's slab"
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("dtype", ["float32", "float64"])
+@pytest.mark.parametrize("updater", STATEFUL)
+def test_fused_add_three_workers(mv_device, updater, dtype):
+    """The fused whole-table Add (``mvb_add_dense_fused``, no signal pads) with three workers' deltas on one
+    device: the owner applies worker 0, 1, 2 in that order, each with its own AddOption and, for the per-worker
+    updaters, its own state slab. 4099 elements: the 16-byte path and the scalar tail. Values and every
+    worker's state against the model; the padding between the state slabs stays untouched."""
+    from multiverso_b200 import _native as N
+    lib, st = N.cuda_lib(), N.stream_ptr()
+    n, W = 4099, 3
+    nst, per_worker = _STATES[updater]
+    stride = (n + 3) // 4 * 4 + 8
+    tdt = getattr(torch, dtype)
+    rng = np.random.default_rng(31)
+    start = _start_values(rng, n, dtype)
+    shard = torch.from_numpy(start).cuda()
+    states = [torch.full((stride * (W if per_worker else 1),), _KSENT, dtype=tdt, device="cuda")
+              for _ in range(nst)]
+    for t in states:
+        t.view(-1, stride)[:, :n] = 0
+    model = ServerModel(start, 1, updater, dtype, workers=W)
+    a = N.DenseAdd()
+    a.dtype, a.updater = N.dtype_code(tdt), N.UPDATER_NAMES[updater]
+    a.shard = shard.data_ptr()
+    a.state0 = states[0].data_ptr() if nst >= 1 else None
+    a.state1 = states[1].data_ptr() if nst >= 2 else None
+    a.shard_len, a.shard_off, a.state_stride = n, 0, stride
+    a.nworkers, a.worker_mask, a.world = W, (1 << W) - 1, 1
+    a.scale, a.clip, a.my_worker = 0.5, 0.0, 0
+    for k in range(2):
+        deltas = [torch.from_numpy(_delta(rng, (n,), dtype)).cuda() for _ in range(W)]
+        for w in range(W):
+            opt, a.opts[w] = _kopt(k * W + w, w)
+            a.delta_ptrs[w] = deltas[w].data_ptr()
+            model.add(deltas[w].cpu().numpy() * 0.5, opt)
+        lib.mvb_add_dense_fused(a, st)
+        torch.cuda.synchronize()
+    what = f"fused Add {updater} {dtype} W={W}"
+    _assert_close(shard.cpu().numpy(), model.data.reshape(-1), (np.abs(model.data) + model.mag).reshape(-1),
+                  model.nupd.reshape(-1), dtype, f"{what} values")
+    for i, t in enumerate(states):
+        slabs = t.view(-1, stride)
+        for w in range(slabs.shape[0]):
+            _assert_close(slabs[w, :n].cpu().numpy(), model.state[i][w].reshape(-1),
+                          model.state_scale(i, w).reshape(-1), model.nupd.reshape(-1), dtype,
+                          f"{what} state{i}[worker {w}]")
+        assert bool((slabs[:, n:] == _KSENT).all()), f"{what}: state{i} padding written"
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("updater", STATEFUL)
+def test_row_mailbox_apply(mv_device, updater):
+    """Row Adds through the row mailbox of a one-process fp32 MatrixTable (``push_vals`` then
+    ``drain(wait=True)``, ``mvb_rowbox_apply`` on the owner), held to the model. With one rank the push waits
+    only for acks of its own earlier drains and the drain only for the push's doorbell; one push per drain, and
+    the push has completed (device synchronise) before the drain polls, so nothing waits on work not yet run.
+    Rows never named stay bitwise unchanged in the shard and in the state."""
+    from multiverso_b200.runtime import Runtime
+    mv = mv_device
+    rows, cols = 300, 68
+    rng = np.random.default_rng(41)
+    t, model = _make_table(mv, "matrix", (rows, cols), "float32", updater)
+    start = model.data.copy()
+    mb = t.enable_row_mailbox()
+    named = set()
+    for k in range(4):
+        ids = np.sort(rng.choice(rows, 90, replace=False)).astype(np.int32)
+        v = _delta(rng, (ids.size, cols), "float32")
+        opt, _ = _kopt(k, 0)
+        mb.push_vals(torch.from_numpy(ids).cuda(), torch.from_numpy(v).cuda(), opt)
+        torch.cuda.synchronize()
+        mb.drain(wait=True)
+        mb.drain_stream.synchronize()
+        model.add_rows(ids.astype(np.int64), v, opt)
+        named.update(ids.tolist())
+    Runtime.get().check_watchdog()
+    what = f"row mailbox {updater}"
+    _check_model(t, model, "float32", what)
+    untouched = np.setdiff1d(np.arange(rows), sorted(named))
+    assert np.array_equal(t.get().cpu().numpy().reshape(rows, cols)[untouched], start[untouched])
+    for i in range(len(model.state)):
+        assert not _device_state(t, i).reshape(rows, cols)[untouched].any(), f"{what}: state{i} of an unnamed row"
