@@ -12,6 +12,7 @@
 //  K2  get_dense        -- Worker::Get for whole tables (all-gather by pull).
 //  K9  updater_apply    -- stand-alone updater (NCCL comparator path, local adds).
 //      push_dense_red   -- one-sided async push with red.global.add.v4.f32.
+//      push_rowwise     -- one-sided async push of a row-state updater (row-wise AdaGrad).
 #include <type_traits>
 #include "mvb_common.cuh"
 
@@ -42,6 +43,7 @@ struct DenseAddDev {
   int* fin_flag;
   unsigned int* done_counter;
   long long budget;
+  int64_t num_col;       // row length (row-state updaters)
 };
 
 template <typename T>
@@ -72,6 +74,55 @@ MVB_DEVINL void push_replica(const A& a, int64_t i, const Pack<T, VEC>& d) {
       if constexpr (VEC == 1) a.replica[r][a.shard_off + i] = d.v[0];
       else st_na_v4(a.replica[r] + a.shard_off + i, *reinterpret_cast<const uint4*>(&d));
     }
+}
+
+// The fused Add of a row-state updater: one warp per local row of num_col elements. Pass A sums the squares of
+// every contributing worker's delta row, then each worker's factor and accumulator are formed (row_factor). Pass B
+// loads d once, applies the workers in worker order, each with its own factor and AddOption, and stores d once.
+// A worker's factor depends only on its own delta and accumulator, so this equals applying the workers one after
+// the other; each delta element is read twice.
+template <class U, typename T, int VEC>
+MVB_DEVINL void add_rows_fused(const DenseAddDev<T>& a, unsigned int mask, const MvbAddOpt* sopt) {
+  const int lane = threadIdx.x & 31;
+  const int64_t C = a.num_col, rows = a.shard_len / C, nv = C / VEC;
+  for (int64_t r = warp_id(); r < rows; r += num_warps()) {
+    const int64_t base = r * C;
+    T part[MVB_MAX_RANKS], f[MVB_MAX_RANKS];
+#pragma unroll
+    for (int w = 0; w < MVB_MAX_RANKS; ++w) part[w] = f[w] = (T)0;
+    for (int64_t v = lane; v < nv; v += 32) {
+#pragma unroll
+      for (int w = 0; w < MVB_MAX_RANKS; ++w) {
+        if (w < a.W && ((mask >> w) & 1u)) {
+          const Pack<T, VEC> g = pk_load_nc<T, VEC>(a.delta[w] + a.shard_off + base + v * VEC);
+#pragma unroll
+          for (int e = 0; e < VEC; ++e) part[w] += U::Square(prep_delta<T>(g.v[e], a.scale, a.clip), sopt[w]);
+        }
+      }
+    }
+#pragma unroll
+    for (int w = 0; w < MVB_MAX_RANKS; ++w) {
+      if (w < a.W && ((mask >> w) & 1u)) {
+        T* hp = a.state0 + state_at<U>(w, a.state_stride, r);
+        T h = *hp;
+        f[w] = row_factor<U>(part[w], h, hp, C, sopt[w]);
+      }
+    }
+    for (int64_t v = lane; v < nv; v += 32) {
+      const int64_t i = base + v * VEC;
+      Pack<T, VEC> d = pk_load<T, VEC>(a.shard + i);
+#pragma unroll
+      for (int w = 0; w < MVB_MAX_RANKS; ++w) {
+        if (w < a.W && ((mask >> w) & 1u)) {
+          const Pack<T, VEC> g = pk_load_nc<T, VEC>(a.delta[w] + a.shard_off + i);
+#pragma unroll
+          for (int e = 0; e < VEC; ++e) U::Step(d.v[e], prep_delta<T>(g.v[e], a.scale, a.clip), f[w], sopt[w]);
+        }
+      }
+      pk_store<T, VEC>(a.shard + i, d);
+      if (a.has_replica) push_replica<T, VEC>(a, i, d);
+    }
+  }
 }
 
 template <int UPD, typename T, int VEC>
@@ -122,66 +173,70 @@ add_dense_fused_kernel(const __grid_constant__ DenseAddDev<T> a) {
   const unsigned int mask = smask;
   if (a.fin_flag && blockIdx.x == 0 && threadIdx.x == 0 && mask == 0) *a.fin_flag = 1;
 
-  const int64_t nvec = a.shard_len / VEC;
-  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  for (int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; v < nvec; v += stride) {
-    const int64_t i = v * VEC;
-    if constexpr (std::is_same<T, float>::value && VEC == 4 && (UPD == MVB_UPD_DEFAULT || UPD == MVB_UPD_SGD)) {
-      if (a.delta_mc != nullptr) {
-        // NVLS: one multimem.ld_reduce returns the sum over every worker's staging buffer,
-        // reduced inside the NVSwitch (ingress = 1/W of the P2P pull); linear updaters only.
-        float4 sum = multimem_ld_reduce_add_v4_f32(a.delta_mc + a.shard_off + i);
-        Pack<T, VEC> d = pk_load<T, VEC>(a.shard + i);
-        T z0 = 0, z1 = 0;
-        U::Apply(d.v[0], prep_delta<T>(sum.x, a.scale, a.clip), z0, z1, sopt[0]);
-        U::Apply(d.v[1], prep_delta<T>(sum.y, a.scale, a.clip), z0, z1, sopt[0]);
-        U::Apply(d.v[2], prep_delta<T>(sum.z, a.scale, a.clip), z0, z1, sopt[0]);
-        U::Apply(d.v[3], prep_delta<T>(sum.w, a.scale, a.clip), z0, z1, sopt[0]);
-        pk_store<T, VEC>(a.shard + i, d);
-        if (a.has_replica) push_replica<T, VEC>(a, i, d);
-        continue;
+  if constexpr (U::kRowState) {
+    add_rows_fused<U, T, VEC>(a, mask, sopt);
+  } else {
+    const int64_t nvec = a.shard_len / VEC;
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; v < nvec; v += stride) {
+      const int64_t i = v * VEC;
+      if constexpr (std::is_same<T, float>::value && VEC == 4 && (UPD == MVB_UPD_DEFAULT || UPD == MVB_UPD_SGD)) {
+        if (a.delta_mc != nullptr) {
+          // NVLS: one multimem.ld_reduce returns the sum over every worker's staging buffer,
+          // reduced inside the NVSwitch (ingress = 1/W of the P2P pull); linear updaters only.
+          float4 sum = multimem_ld_reduce_add_v4_f32(a.delta_mc + a.shard_off + i);
+          Pack<T, VEC> d = pk_load<T, VEC>(a.shard + i);
+          T z0 = 0, z1 = 0;
+          U::Apply(d.v[0], prep_delta<T>(sum.x, a.scale, a.clip), z0, z1, sopt[0]);
+          U::Apply(d.v[1], prep_delta<T>(sum.y, a.scale, a.clip), z0, z1, sopt[0]);
+          U::Apply(d.v[2], prep_delta<T>(sum.z, a.scale, a.clip), z0, z1, sopt[0]);
+          U::Apply(d.v[3], prep_delta<T>(sum.w, a.scale, a.clip), z0, z1, sopt[0]);
+          pk_store<T, VEC>(a.shard + i, d);
+          if (a.has_replica) push_replica<T, VEC>(a, i, d);
+          continue;
+        }
       }
-    }
-    Pack<T, VEC> g[MVB_MAX_RANKS];
+      Pack<T, VEC> g[MVB_MAX_RANKS];
 #pragma unroll
-    for (int w = 0; w < MVB_MAX_RANKS; ++w) {
-      if (w < a.W && ((mask >> w) & 1u)) g[w] = pk_load_nc<T, VEC>(a.delta[w] + a.shard_off + i);
-    }
-    Pack<T, VEC> d = pk_load<T, VEC>(a.shard + i);
-    // shared state is held across the workers' steps, per-worker state is worker w's slab during its step
-    Pack<T, VEC> s0{}, s1{};
-    if constexpr (!U::kPerWorker) state_load<U>(s0, s1, a.state0, a.state1, 0, a.state_stride, i);
-#pragma unroll
-    for (int w = 0; w < MVB_MAX_RANKS; ++w) {
-      if (w < a.W && ((mask >> w) & 1u)) {
-        if constexpr (U::kPerWorker) state_load<U>(s0, s1, a.state0, a.state1, w, a.state_stride, i);
-#pragma unroll
-        for (int e = 0; e < VEC; ++e)
-          U::Apply(d.v[e], prep_delta<T>(g[w].v[e], a.scale, a.clip), s0.v[e], s1.v[e], sopt[w]);
-        if constexpr (U::kPerWorker) state_store<U>(s0, s1, a.state0, a.state1, w, a.state_stride, i);
+      for (int w = 0; w < MVB_MAX_RANKS; ++w) {
+        if (w < a.W && ((mask >> w) & 1u)) g[w] = pk_load_nc<T, VEC>(a.delta[w] + a.shard_off + i);
       }
-    }
-    if constexpr (!U::kPerWorker) state_store<U>(s0, s1, a.state0, a.state1, 0, a.state_stride, i);
-    pk_store<T, VEC>(a.shard + i, d);
-    if (a.has_replica) push_replica<T, VEC>(a, i, d);
-  }
-  // scalar tail (shard_len % VEC) handled by the first threads of block 0
-  if (VEC > 1 && blockIdx.x == 0) {
-    for (int64_t i = nvec * VEC + threadIdx.x; i < a.shard_len; i += blockDim.x) {
-      T d = a.shard[i];
-      T s0 = (T)0, s1 = (T)0;
+      Pack<T, VEC> d = pk_load<T, VEC>(a.shard + i);
+      // shared state is held across the workers' steps, per-worker state is worker w's slab during its step
+      Pack<T, VEC> s0{}, s1{};
       if constexpr (!U::kPerWorker) state_load<U>(s0, s1, a.state0, a.state1, 0, a.state_stride, i);
-      for (int w = 0; w < a.W; ++w) {
-        if (!((mask >> w) & 1u)) continue;
-        if constexpr (U::kPerWorker) state_load<U>(s0, s1, a.state0, a.state1, w, a.state_stride, i);
-        U::Apply(d, prep_delta<T>(__ldg(a.delta[w] + a.shard_off + i), a.scale, a.clip), s0, s1,
-                 sopt[w]);
-        if constexpr (U::kPerWorker) state_store<U>(s0, s1, a.state0, a.state1, w, a.state_stride, i);
+#pragma unroll
+      for (int w = 0; w < MVB_MAX_RANKS; ++w) {
+        if (w < a.W && ((mask >> w) & 1u)) {
+          if constexpr (U::kPerWorker) state_load<U>(s0, s1, a.state0, a.state1, w, a.state_stride, i);
+#pragma unroll
+          for (int e = 0; e < VEC; ++e)
+            U::Apply(d.v[e], prep_delta<T>(g[w].v[e], a.scale, a.clip), s0.v[e], s1.v[e], sopt[w]);
+          if constexpr (U::kPerWorker) state_store<U>(s0, s1, a.state0, a.state1, w, a.state_stride, i);
+        }
       }
       if constexpr (!U::kPerWorker) state_store<U>(s0, s1, a.state0, a.state1, 0, a.state_stride, i);
-      a.shard[i] = d;
-      if (a.has_replica)
-        for (int r = 0; r < a.world; ++r) a.replica[r][a.shard_off + i] = d;
+      pk_store<T, VEC>(a.shard + i, d);
+      if (a.has_replica) push_replica<T, VEC>(a, i, d);
+    }
+    // scalar tail (shard_len % VEC) handled by the first threads of block 0
+    if (VEC > 1 && blockIdx.x == 0) {
+      for (int64_t i = nvec * VEC + threadIdx.x; i < a.shard_len; i += blockDim.x) {
+        T d = a.shard[i];
+        T s0 = (T)0, s1 = (T)0;
+        if constexpr (!U::kPerWorker) state_load<U>(s0, s1, a.state0, a.state1, 0, a.state_stride, i);
+        for (int w = 0; w < a.W; ++w) {
+          if (!((mask >> w) & 1u)) continue;
+          if constexpr (U::kPerWorker) state_load<U>(s0, s1, a.state0, a.state1, w, a.state_stride, i);
+          U::Apply(d, prep_delta<T>(__ldg(a.delta[w] + a.shard_off + i), a.scale, a.clip), s0, s1,
+                   sopt[w]);
+          if constexpr (U::kPerWorker) state_store<U>(s0, s1, a.state0, a.state1, w, a.state_stride, i);
+        }
+        if constexpr (!U::kPerWorker) state_store<U>(s0, s1, a.state0, a.state1, 0, a.state_stride, i);
+        a.shard[i] = d;
+        if (a.has_replica)
+          for (int r = 0; r < a.world; ++r) a.replica[r][a.shard_off + i] = d;
+      }
     }
   }
 
@@ -221,8 +276,13 @@ int launch_add(const MvbDenseAdd* h, cudaStream_t st) {
   a.state_stride = h->state_stride;
   a.W = h->nworkers;
   a.mask = h->worker_mask;
-  bool vec_ok = aligned16<T>(h->shard) && aligned16<T>(h->state0) && aligned16<T>(h->state1) &&
-                (h->state_stride % VecOf<T>::N == 0) && (h->shard_off % VecOf<T>::N == 0);
+  // 16-byte accesses of the shard and the staging buffers; the element-wise updaters also index their state by
+  // element, a row-state updater needs whole vectors in every row instead
+  bool vec_ok = aligned16<T>(h->shard) && (h->shard_off % VecOf<T>::N == 0);
+  if constexpr (Updater<UPD, T>::kRowState)
+    vec_ok = vec_ok && (h->num_col % VecOf<T>::N == 0);
+  else
+    vec_ok = vec_ok && aligned16<T>(h->state0) && aligned16<T>(h->state1) && (h->state_stride % VecOf<T>::N == 0);
   for (int w = 0; w < MVB_MAX_RANKS; ++w) {
     a.delta[w] = w < h->nworkers ? (const T*)h->delta_ptrs[w] : nullptr;
     a.opts[w] = h->opts[w];
@@ -253,9 +313,12 @@ int launch_add(const MvbDenseAdd* h, cudaStream_t st) {
   a.fin_flag = h->fin_flag;
   a.done_counter = h->done_counter;
   a.budget = watchdog_cycles(h->timeout_s, 60.0);
+  a.num_col = h->num_col;
 
   constexpr int VEC = VecOf<T>::N;
-  const int blocks = blocks_for(vec_ok ? (h->shard_len + VEC - 1) / VEC : h->shard_len, 256, 4);
+  // a thread per element or vector, or a warp per row
+  const int blocks = Updater<UPD, T>::kRowState ? grid_for(h->shard_len / h->num_col)
+                                                : blocks_for(vec_ok ? (h->shard_len + VEC - 1) / VEC : h->shard_len, 256, 4);
   if (vec_ok)
     add_dense_fused_kernel<UPD, T, VEC><<<blocks, 256, 0, st>>>(a);
   else
@@ -548,7 +611,74 @@ push_stateful_kernel(const T* __restrict__ delta, const __grid_constant__ PushSt
   }
 }
 
+// The one-sided push of a row-state updater: one warp per row of the worker's delta reduces the row, updates the
+// worker's accumulator of that row at the owner and red.adds the step into the owner's row. The step depends on
+// the worker's delta and accumulator only, never on the row's value, so concurrent pushes of other workers only
+// reorder the additions.
+template <int UPD, typename T>
+__global__ void __launch_bounds__(256)
+push_rowwise_kernel(const T* __restrict__ delta, const __grid_constant__ PushStateDev p, int64_t C, MvbAddOpt opt,
+                    int me) {
+  using U = Updater<UPD, T>;
+  const SegCtas c = seg_ctas(p.S, me);
+  const int s = c.s;
+  const int lane = threadIdx.x & 31;
+  const int64_t wid = c.idx * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int64_t nw = c.count * (blockDim.x >> 5);
+  const T* src = delta + p.off[s];
+  T* data = (T*)p.shard[s];
+  T* hs = (T*)p.st0[s];
+  const int64_t rows = p.len[s] / C;
+  for (int64_t r = wid; r < rows; r += nw) {
+    const T* g = src + r * C;
+    T part = (T)0;
+    for (int64_t j = lane; j < C; j += 32) part += U::Square(g[j], opt);
+    T* hp = hs + state_at<U>(opt.worker_id, p.stride[s], r);
+    T h = *hp;
+    const T f = row_factor<U>(part, h, hp, C, opt);
+    for (int64_t j = lane; j < C; j += 32) {
+      T step = (T)0;
+      U::Step(step, g[j], f, opt);
+      red_add(data + r * C + j, step);
+    }
+  }
+}
+
 }  // namespace
+
+extern "C" int mvb_push_dense_rowwise(int dtype, int updater, const void* delta, int nservers, void* const* shard_ptrs,
+                                      void* const* state_ptrs, const int64_t* shard_offs, const int64_t* shard_lens,
+                                      const int64_t* state_strides, int64_t num_col, const MvbAddOpt* opt, int me,
+                                      void* stream) {
+  if (nservers < 1 || nservers > MVB_MAX_RANKS) return -3;
+  PushStateDev p{};
+  p.S = nservers;
+  int64_t rows = 0;
+  bool geometry_ok = num_col >= 1;
+  for (int s = 0; s < nservers && geometry_ok; ++s) {
+    p.shard[s] = shard_ptrs[s];
+    p.st0[s] = state_ptrs[s];
+    p.off[s] = shard_offs[s];
+    p.len[s] = shard_lens[s];
+    p.stride[s] = state_strides[s];
+    geometry_ok = shard_lens[s] % num_col == 0 && state_strides[s] >= shard_lens[s] / num_col;
+    rows += shard_lens[s] / num_col;
+  }
+  return with_dtype<float, double>(dtype, [&](auto t) {
+    using T = typename decltype(t)::type;
+    return with_updater<T>(updater, [&](auto u) {
+      if constexpr (!Updater<decltype(u)::value, T>::kRowState) {
+        return -2;
+      } else {
+        if (!geometry_ok) return (int)MVB_BAD_ROW_MAP;
+        push_rowwise_kernel<decltype(u)::value, T><<<seg_grid(grid_for(rows), nservers), 256, 0,
+                                                     (cudaStream_t)stream>>>((const T*)delta, p, num_col, *opt, me);
+        MVB_CUDA_CHECK(cudaGetLastError());
+        return 0;
+      }
+    });
+  });
+}
 
 extern "C" int mvb_push_dense_stateful(int dtype, int updater, const void* delta, int nservers,
                                        void* const* shard_ptrs, void* const* state0_ptrs,
@@ -571,8 +701,8 @@ extern "C" int mvb_push_dense_stateful(int dtype, int updater, const void* delta
   return with_dtype<float, double>(dtype, [&](auto t) {
     using T = typename decltype(t)::type;
     return with_updater<T>(updater, [&](auto u) {
-      // the stateless updaters push with mvb_push_dense_red
-      if constexpr (Updater<decltype(u)::value, T>::kStates == 0) {
+      // the stateless updaters push with mvb_push_dense_red, the row-state ones with mvb_push_dense_rowwise
+      if constexpr (Updater<decltype(u)::value, T>::kStates == 0 || Updater<decltype(u)::value, T>::kRowState) {
         return -2;
       } else {
         push_stateful_kernel<decltype(u)::value, T><<<seg_grid(blocks_for(total, 256, 8), nservers), 256, 0,
@@ -588,8 +718,13 @@ extern "C" int mvb_add_dense_fused(const MvbDenseAdd* a, void* stream) {
   if (a->nworkers < 1 || a->nworkers > MVB_MAX_RANKS) return -3;
   return with_dtype<float, double, int>(a->dtype, [&](auto t) {
     using T = typename decltype(t)::type;
-    return with_updater<T>(a->updater,
-                           [&](auto u) { return launch_add<decltype(u)::value, T>(a, (cudaStream_t)stream); });
+    return with_updater<T>(a->updater, [&](auto u) {
+      if constexpr (Updater<decltype(u)::value, T>::kRowState) {
+        if (a->num_col < 1 || a->shard_len % a->num_col != 0 || a->state_stride < a->shard_len / a->num_col)
+          return (int)MVB_BAD_ROW_MAP;
+      }
+      return launch_add<decltype(u)::value, T>(a, (cudaStream_t)stream);
+    });
   });
 }
 
@@ -599,10 +734,15 @@ extern "C" int mvb_updater_apply(int dtype, int updater, void* data, const void*
   return with_dtype<float, double, int>(dtype, [&](auto t) {
     using T = typename decltype(t)::type;
     return with_updater<T>(updater, [&](auto u) {
-      updater_apply_kernel<decltype(u)::value, T><<<blocks_for(n, 256, 8), 256, 0, (cudaStream_t)stream>>>(
-          (T*)data, (const T*)delta, (T*)state0, (T*)state1, n, *opt, std::is_same<T, int>::value ? 1.f : scale);
-      MVB_CUDA_CHECK(cudaGetLastError());
-      return 0;
+      // one source and no row geometry: the row-state updaters are served by the row-shaped kernels only
+      if constexpr (Updater<decltype(u)::value, T>::kRowState) {
+        return -2;
+      } else {
+        updater_apply_kernel<decltype(u)::value, T><<<blocks_for(n, 256, 8), 256, 0, (cudaStream_t)stream>>>(
+            (T*)data, (const T*)delta, (T*)state0, (T*)state1, n, *opt, std::is_same<T, int>::value ? 1.f : scale);
+        MVB_CUDA_CHECK(cudaGetLastError());
+        return 0;
+      }
     });
   });
 }

@@ -19,14 +19,20 @@ extern "C" {
 
 /* element types */
 enum { MVB_F32 = 0, MVB_F64 = 1, MVB_I32 = 2, MVB_I64 = 3, MVB_I8 = 4 };
-/* updaters (reference: -updater_type default|sgd|momentum_sgd|adagrad|dcasgd|dcasgda) */
+/* updaters (reference: -updater_type default|sgd|momentum_sgd|adagrad|dcasgd|dcasgda, plus rowwise_adagrad).
+ * rowwise_adagrad is AdaGrad with one accumulator per (worker, table row): h += mean_j (g_j / lr)^2 over the
+ * row's C columns, d_j -= rho * rsqrt(h + 1e-6) * g_j / lr. Its state slab is indexed by local row, not by
+ * element, so the entry points that update whole rows take the row length (MvbDenseAdd.num_col,
+ * mvb_push_dense_rowwise); mvb_updater_apply and mvb_push_dense_stateful have none and return -2 for it.
+ * Code 6 is left unassigned: it is the "unknown updater" of the dispatch tests. */
 enum {
   MVB_UPD_DEFAULT = 0,
   MVB_UPD_SGD = 1,
   MVB_UPD_MOMENTUM = 2,
   MVB_UPD_ADAGRAD = 3,
   MVB_UPD_DCASGD = 4,
-  MVB_UPD_DCASGDA = 5
+  MVB_UPD_DCASGDA = 5,
+  MVB_UPD_ROWWISE_ADAGRAD = 7
 };
 
 /* Same 20-byte layout as the reference AddOption (updater.h:13-69):
@@ -123,11 +129,16 @@ typedef struct MvbDenseAdd {
      NULL boxes: opts[] are used as given (single process / identical options).                       */
   void* opt_box[MVB_MAX_RANKS];
   int my_worker;          /* this rank's worker id (-1: not a worker)  */
+  /* row length of the table; read by row-state updaters only (rowwise_adagrad), which need num_col >= 1,
+     shard_len % num_col == 0 and state_stride >= shard_len / num_col, else MVB_BAD_ROW_MAP before any
+     CUDA call. Their state slabs hold one element per local row. */
+  int64_t num_col;
 } MvbDenseAdd;
 int mvb_add_dense_fused(const MvbDenseAdd* a, void* stream);
 
 /* Local (single-source) updater apply: the stand-alone K9 kernel used by the
- * NCCL comparator path and by row-wise / whole adds with one worker. */
+ * NCCL comparator path and by row-wise / whole adds with one worker. Element-wise updaters only
+ * (-2 for rowwise_adagrad, which needs rows). */
 int mvb_updater_apply(int dtype, int updater, void* data, const void* delta, void* state0,
                       void* state1, int64_t n, const MvbAddOpt* opt, float scale, void* stream);
 
@@ -165,6 +176,16 @@ int mvb_push_dense_stateful(int dtype, int updater, const void* delta, int nserv
                             void* const* shard_ptrs, void* const* state0_ptrs, void* const* state1_ptrs,
                             const int64_t* shard_offs, const int64_t* shard_lens,
                             const int64_t* state_strides, const MvbAddOpt* opt, int me, void* stream);
+/* The same push for row-state updaters (rowwise_adagrad): one warp per row of num_col elements reduces the
+ * worker's delta row, read-modify-writes the worker's accumulator of that row at the owner (state_ptrs[s] +
+ * opt->worker_id * state_strides[s] + local row) and red.adds the step into the owner's row. Returns -3 for
+ * nservers outside [1, MVB_MAX_RANKS], -1 for element types other than f32 / f64, -2 for updaters without row
+ * state and MVB_BAD_ROW_MAP when num_col < 1, a shard_lens[s] is not a multiple of num_col or a
+ * state_strides[s] is below shard_lens[s] / num_col; all before any CUDA call. */
+int mvb_push_dense_rowwise(int dtype, int updater, const void* delta, int nservers, void* const* shard_ptrs,
+                           void* const* state_ptrs, const int64_t* shard_offs, const int64_t* shard_lens,
+                           const int64_t* state_strides, int64_t num_col, const MvbAddOpt* opt, int me,
+                           void* stream);
 
 /* ---- row-sparse Get / Add (K3, K4, K10) ------------------------------------ */
 /* Server min(r / rows_per_server, nservers - 1) holds row r, at local index r - server * rows_per_server.
@@ -191,7 +212,8 @@ int mvb_add_rows_delta(const MvbRowMap* m, const int64_t* row_ids, int64_t k, co
 /* Stateful row add applied by the OWNER on its local shard for rows in its range:
  * ids/vals may be another rank's (peer-mapped) staging.  A repeated row is updated once per
  * occurrence, in list order, when its occurrences are adjacent (sort the request stably by id);
- * occurrences that are not adjacent race. */
+ * occurrences that are not adjacent race. rowwise_adagrad indexes its state slab by local row
+ * (state_stride >= row_hi - row_lo). */
 int mvb_add_rows_owner(int dtype, int updater, void* shard, void* state0, void* state1,
                        int64_t row_lo, int64_t row_hi, int64_t num_col, int64_t state_stride,
                        const int64_t* row_ids, int64_t k, const void* vals, int64_t vals_ld,
@@ -397,6 +419,7 @@ int mvb_rowbox_push_vals(const MvbRowBox* b, const int* ids, const int* n_ptr, i
                          const float* vals, int64_t ld, float scale, uint64_t epoch, const MvbAddOpt* opt,
                          int ctas_per_sm, void* stream);
 int mvb_rowbox_poll(const MvbRowBox* b, int src, int wait, void* stream);
+/* state_stride: elements per source slab; rowwise_adagrad indexes its slab by local row */
 int mvb_rowbox_apply(const MvbRowBox* b, int updater, float* shard, float* st0, float* st1,
                      int64_t state_stride, int64_t row_lo, int src, int ctas_per_sm, void* stream);
 

@@ -197,6 +197,7 @@ MVB_DEVINL void red_add(int* p, int v) { red_add_s32(p, v); }
 //   adagrad  : s0 = G^2 history                (per worker)
 //   dcasgd   : s0 = shadow copy                (per worker)
 //   dcasgda  : s0 = shadow copy, s1 = mean sq  (per worker)
+//   rowwise_adagrad : s0 = G^2 history of a ROW (per worker, one element per local row)
 // Semantics follow the reference accessors (Q1/Q3); AdaGrad implements the
 // *intended* rule (Q2: the reference copies the history by value and subtracts
 // squares, so its history never persists).
@@ -208,18 +209,21 @@ template <typename T>
 struct Updater<MVB_UPD_DEFAULT, T> {
   static constexpr int kStates = 0;
   static constexpr bool kPerWorker = false;
+  static constexpr bool kRowState = false;
   MVB_DEVINL static void Apply(T& d, T g, T&, T&, const MvbAddOpt&) { d += g; }
 };
 template <typename T>
 struct Updater<MVB_UPD_SGD, T> {
   static constexpr int kStates = 0;
   static constexpr bool kPerWorker = false;
+  static constexpr bool kRowState = false;
   MVB_DEVINL static void Apply(T& d, T g, T&, T&, const MvbAddOpt&) { d -= g; }
 };
 template <typename T>
 struct Updater<MVB_UPD_MOMENTUM, T> {
   static constexpr int kStates = 1;
   static constexpr bool kPerWorker = false;
+  static constexpr bool kRowState = false;
   MVB_DEVINL static void Apply(T& d, T g, T& s0, T&, const MvbAddOpt& o) {
     s0 = (T)o.momentum * s0 + (T)(1.0f - o.momentum) * g;
     d -= s0;
@@ -229,6 +233,7 @@ template <typename T>
 struct Updater<MVB_UPD_ADAGRAD, T> {
   static constexpr int kStates = 1;
   static constexpr bool kPerWorker = true;
+  static constexpr bool kRowState = false;
   MVB_DEVINL static void Apply(T& d, T g, T& s0, T&, const MvbAddOpt& o) {
     T gn = g / (T)o.lr;
     s0 += gn * gn;
@@ -241,6 +246,7 @@ template <typename T>
 struct Updater<MVB_UPD_DCASGD, T> {
   static constexpr int kStates = 1;
   static constexpr bool kPerWorker = true;
+  static constexpr bool kRowState = false;
   MVB_DEVINL static void Apply(T& d, T g, T& s0, T&, const MvbAddOpt& o) {
     T gn = g / (T)o.lr;
     d -= (T)o.lr * (gn + (T)o.lambda * gn * gn * (d - s0));
@@ -251,6 +257,7 @@ template <typename T>
 struct Updater<MVB_UPD_DCASGDA, T> {
   static constexpr int kStates = 2;
   static constexpr bool kPerWorker = true;
+  static constexpr bool kRowState = false;
   MVB_DEVINL static void Apply(T& d, T g, T& s0, T& s1, const MvbAddOpt& o) {
     T gn = g / (T)o.lr;
     s1 = (T)o.momentum * s1 + (T)(1.0f - o.momentum) * gn * gn;
@@ -258,6 +265,27 @@ struct Updater<MVB_UPD_DCASGDA, T> {
                              gn * (d - s0));
     s0 = d;
   }
+};
+
+// Row-wise AdaGrad (kRowState): one accumulator per (worker, row) instead of per element. Worker w's step on a
+// row of C elements g_j is  h += (1/C) sum_j (g_j/lr)^2,  d_j -= rho * rsqrt(h + 1e-6) * g_j/lr  (AdaGrad at C = 1),
+// split into the per-element square, the accumulate-and-factor step (once per row, see row_factor) and the
+// per-element apply. Kernels serve it with a row-shaped body (a warp per row) instead of Apply.
+template <typename T>
+struct Updater<MVB_UPD_ROWWISE_ADAGRAD, T> {
+  static constexpr int kStates = 1;
+  static constexpr bool kPerWorker = true;
+  static constexpr bool kRowState = true;
+  MVB_DEVINL static T Square(T g, const MvbAddOpt& o) {
+    const T gn = g / (T)o.lr;
+    return gn * gn;
+  }
+  // h takes the row's mean square; returns the row's factor rho / sqrt(h + 1e-6)
+  MVB_DEVINL static T Factor(T& h, T sum, int64_t C, const MvbAddOpt& o) {
+    h += sum / (T)C;
+    return (T)o.rho * Updater<MVB_UPD_ADAGRAD, T>::rsqrt_t(h + (T)1e-6);
+  }
+  MVB_DEVINL static void Step(T& d, T g, T f, const MvbAddOpt& o) { d -= f * (g / (T)o.lr); }
 };
 
 // Updater state of one element (T, or a float4 over float4 slabs) or of a pack of elements (Pack<T, VEC>). A state array holds
@@ -344,6 +372,22 @@ MVB_DEVINL float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
+}
+MVB_DEVINL double warp_sum(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+// A row-state updater's step on one row, for the whole warp: `part` is the lane's share of the row's sum of
+// U::Square, h the worker's accumulator of the row (the same value in every lane) and hp where it lives. The
+// butterfly sum gives every lane the same total, so every lane updates h alike and returns the same factor;
+// lane 0 stores h. Call it with the whole warp.
+template <class U, typename T>
+MVB_DEVINL T row_factor(T part, T& h, T* hp, int64_t C, const MvbAddOpt& o) {
+  const T f = U::Factor(h, warp_sum(part), C, o);
+  if ((threadIdx.x & 31) == 0) *hp = h;
+  return f;
 }
 
 // word2vec's logistic: sigmoid and -log(sigmoid(x)) = log(1 + exp(-x))
@@ -463,6 +507,7 @@ static inline int with_updater(int upd, F&& f) {
       case MVB_UPD_ADAGRAD: return f(integral_constant<int, MVB_UPD_ADAGRAD>{});
       case MVB_UPD_DCASGD: return f(integral_constant<int, MVB_UPD_DCASGD>{});
       case MVB_UPD_DCASGDA: return f(integral_constant<int, MVB_UPD_DCASGDA>{});
+      case MVB_UPD_ROWWISE_ADAGRAD: return f(integral_constant<int, MVB_UPD_ROWWISE_ADAGRAD>{});
     }
     return -2;
   }

@@ -229,26 +229,58 @@ rowbox_apply_kernel(const __grid_constant__ BoxDev b, const __grid_constant__ Ap
   const unsigned char* vals = slot + kHdrBytes + b.ids_bytes;
   const int lane = threadIdx.x & 31;
   const int nvec = a.row_floats >> 2;
-  for (int64_t i = warp_id(); i < count; i += num_warps()) {
-    const int64_t r = (int64_t)__ldcg(ids + i);
-    const int64_t base = (r - a.row_lo) * (int64_t)a.row_floats;
-    if (r < a.row_lo || base < 0) continue;
-    const float4* src = reinterpret_cast<const float4*>(vals + (size_t)i * b.ld_bytes);
-    float4* st0 = reinterpret_cast<float4*>(a.st0 + base);
-    float4* st1 = reinterpret_cast<float4*>(a.st1 + base);
-    const int64_t stride4 = a.state_stride >> 2;          // slabs of whole float4s: state_stride % 4 == 0
-    for (int v = lane; v < nvec; v += 32) {
-      const float4 g = __ldcg(src + v);
-      float4* dp = reinterpret_cast<float4*>(a.shard + base) + v;
-      float4 d = *dp;
-      float4 s0 = make_float4(0, 0, 0, 0), s1 = make_float4(0, 0, 0, 0);
-      state_load<U>(s0, s1, st0, st1, a.src, stride4, v);
-      U::Apply(d.x, g.x, s0.x, s1.x, opt);
-      U::Apply(d.y, g.y, s0.y, s1.y, opt);
-      U::Apply(d.z, g.z, s0.z, s1.z, opt);
-      U::Apply(d.w, g.w, s0.w, s1.w, opt);
-      *dp = d;
-      state_store<U>(s0, s1, st0, st1, a.src, stride4, v);
+  if constexpr (U::kRowState) {
+    // a row-state updater: the row's square sum, then its factor and the source's accumulator of the row (indexed
+    // by local row), then the apply
+    for (int64_t i = warp_id(); i < count; i += num_warps()) {
+      const int64_t r = (int64_t)__ldcg(ids + i);
+      const int64_t base = (r - a.row_lo) * (int64_t)a.row_floats;
+      if (r < a.row_lo || base < 0) continue;
+      const float4* src = reinterpret_cast<const float4*>(vals + (size_t)i * b.ld_bytes);
+      float part = 0.f;
+      for (int v = lane; v < nvec; v += 32) {
+        const float4 g = __ldcg(src + v);
+        part += U::Square(g.x, opt);
+        part += U::Square(g.y, opt);
+        part += U::Square(g.z, opt);
+        part += U::Square(g.w, opt);
+      }
+      float* hp = a.st0 + state_at<U>(a.src, a.state_stride, r - a.row_lo);
+      float h = *hp;
+      const float f = row_factor<U>(part, h, hp, a.row_floats, opt);
+      for (int v = lane; v < nvec; v += 32) {
+        const float4 g = __ldcg(src + v);
+        float4* dp = reinterpret_cast<float4*>(a.shard + base) + v;
+        float4 d = *dp;
+        U::Step(d.x, g.x, f, opt);
+        U::Step(d.y, g.y, f, opt);
+        U::Step(d.z, g.z, f, opt);
+        U::Step(d.w, g.w, f, opt);
+        *dp = d;
+      }
+    }
+  } else {
+    for (int64_t i = warp_id(); i < count; i += num_warps()) {
+      const int64_t r = (int64_t)__ldcg(ids + i);
+      const int64_t base = (r - a.row_lo) * (int64_t)a.row_floats;
+      if (r < a.row_lo || base < 0) continue;
+      const float4* src = reinterpret_cast<const float4*>(vals + (size_t)i * b.ld_bytes);
+      float4* st0 = reinterpret_cast<float4*>(a.st0 + base);
+      float4* st1 = reinterpret_cast<float4*>(a.st1 + base);
+      const int64_t stride4 = a.state_stride >> 2;          // slabs of whole float4s: state_stride % 4 == 0
+      for (int v = lane; v < nvec; v += 32) {
+        const float4 g = __ldcg(src + v);
+        float4* dp = reinterpret_cast<float4*>(a.shard + base) + v;
+        float4 d = *dp;
+        float4 s0 = make_float4(0, 0, 0, 0), s1 = make_float4(0, 0, 0, 0);
+        state_load<U>(s0, s1, st0, st1, a.src, stride4, v);
+        U::Apply(d.x, g.x, s0.x, s1.x, opt);
+        U::Apply(d.y, g.y, s0.y, s1.y, opt);
+        U::Apply(d.z, g.z, s0.z, s1.z, opt);
+        U::Apply(d.w, g.w, s0.w, s1.w, opt);
+        *dp = d;
+        state_store<U>(s0, s1, st0, st1, a.src, stride4, v);
+      }
     }
   }
   // ---- completion: the last CTA records the epoch and acks the source ----

@@ -156,12 +156,39 @@ add_rows_owner_kernel(T* __restrict__ shard, T* __restrict__ st0, T* __restrict_
     int64_t end = i + 1;
     while (end < k && ids[end] == r) ++end;
     const int64_t base = (r - row_lo) * num_col;
-    for (int64_t c = lane; c < num_col; c += 32) {
-      T d = shard[base + c], s0 = (T)0, s1 = (T)0;
-      state_load<U>(s0, s1, st0, st1, opt.worker_id, state_stride, base + c);
-      for (int64_t j = i; j < end; ++j) U::Apply(d, vals[j * vals_ld + c], s0, s1, opt);
-      state_store<U>(s0, s1, st0, st1, opt.worker_id, state_stride, base + c);
-      shard[base + c] = d;
+    if constexpr (U::kRowState) {
+      // the row's accumulator (indexed by local row) stays in registers over the run; the run goes in chunks of
+      // up to 32 occurrences: first their factors in list order (occurrence j sees h after the occurrences
+      // before it; lane j keeps the chunk's j-th factor), then one pass over the row applies the chunk
+      T* hp = st0 + state_at<U>(opt.worker_id, state_stride, r - row_lo);
+      T h = *hp;
+      for (int64_t j0 = i; j0 < end; j0 += 32) {
+        const int n = (int)(end - j0 < 32 ? end - j0 : 32);
+        T mine = (T)0;
+        for (int j = 0; j < n; ++j) {
+          T part = (T)0;
+          for (int64_t c = lane; c < num_col; c += 32) part += U::Square(vals[(j0 + j) * vals_ld + c], opt);
+          const T f = row_factor<U>(part, h, hp, num_col, opt);
+          if (lane == j) mine = f;
+        }
+        for (int64_t c0 = 0; c0 < num_col; c0 += 32) {
+          const int64_t c = c0 + lane;
+          T d = c < num_col ? shard[base + c] : (T)0;
+          for (int j = 0; j < n; ++j) {
+            const T f = __shfl_sync(0xffffffffu, mine, j);
+            if (c < num_col) U::Step(d, vals[(j0 + j) * vals_ld + c], f, opt);
+          }
+          if (c < num_col) shard[base + c] = d;
+        }
+      }
+    } else {
+      for (int64_t c = lane; c < num_col; c += 32) {
+        T d = shard[base + c], s0 = (T)0, s1 = (T)0;
+        state_load<U>(s0, s1, st0, st1, opt.worker_id, state_stride, base + c);
+        for (int64_t j = i; j < end; ++j) U::Apply(d, vals[j * vals_ld + c], s0, s1, opt);
+        state_store<U>(s0, s1, st0, st1, opt.worker_id, state_stride, base + c);
+        shard[base + c] = d;
+      }
     }
   }
 }

@@ -260,7 +260,7 @@ void MatrixServerTable<T>::Init(integer_t num_row, integer_t num_col) {
   row_offset_ = part.row_begin[server_id_];
   my_num_row_ = part.row_begin[server_id_ + 1] - row_offset_;
   storage_.assign(static_cast<size_t>(my_num_row_ * num_col_), T(0));
-  updater_ = Updater<T>::GetUpdater(storage_.size());
+  updater_ = Updater<T>::GetUpdater(storage_.size(), static_cast<size_t>(num_col_));
   Log::Debug("server %d created MatrixTable shard: rows [%lld, %lld) x %lld", server_id_,
              (long long)row_offset_, (long long)(row_offset_ + my_num_row_), (long long)num_col);
 }

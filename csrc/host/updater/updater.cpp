@@ -6,6 +6,7 @@
 #include "multiverso/updater/dcasgd_updater.h"
 #include "multiverso/updater/dcasgda_updater.h"
 #include "multiverso/updater/momentum_updater.h"
+#include "multiverso/updater/rowwise_adagrad_updater.h"
 #include "multiverso/updater/sgd_updater.h"
 #include "multiverso/util/configure.h"
 #include "multiverso/util/log.h"
@@ -34,18 +35,19 @@ void Updater<T>::Access(size_t num_element, T* data, T* blob_data, size_t offset
 
 // Gradient-based updaters only make sense for floating-point tables.
 template <>
-Updater<int>* Updater<int>::GetUpdater(size_t) { return new Updater<int>(); }
+Updater<int>* Updater<int>::GetUpdater(size_t, size_t) { return new Updater<int>(); }
 template <>
-Updater<long long>* Updater<long long>::GetUpdater(size_t) { return new Updater<long long>(); }
+Updater<long long>* Updater<long long>::GetUpdater(size_t, size_t) { return new Updater<long long>(); }
 
 template <typename T>
-Updater<T>* Updater<T>::GetUpdater(size_t size) {
+Updater<T>* Updater<T>::GetUpdater(size_t size, size_t num_col) {
   const std::string type = MV_CONFIG(updater_type);
   if (type == "sgd") return new SGDUpdater<T>(size);
   if (type == "adagrad") return new AdaGradUpdater<T>(size);
   if (type == "momentum_sgd") return new MomentumUpdater<T>(size);
   if (type == "dcasgd") return new DCASGDUpdater<T>(size);
   if (type == "dcasgda") return new DCASGDAUpdater<T>(size);
+  if (type == "rowwise_adagrad") return new RowwiseAdaGradUpdater<T>(size, num_col);
   if (type != "default") Log::Error("unknown updater_type '%s', using default", type.c_str());
   return new Updater<T>();
 }

@@ -21,9 +21,11 @@ EPOCH_FIN = 1 << 62
 
 F32, F64, I32, I64, I8 = 0, 1, 2, 3, 4
 UPD_DEFAULT, UPD_SGD, UPD_MOMENTUM, UPD_ADAGRAD, UPD_DCASGD, UPD_DCASGDA = range(6)
+UPD_ROWWISE_ADAGRAD = 7          # 6 is unassigned
 UPDATER_NAMES = {
     "default": UPD_DEFAULT, "sgd": UPD_SGD, "momentum_sgd": UPD_MOMENTUM,
     "adagrad": UPD_ADAGRAD, "dcasgd": UPD_DCASGD, "dcasgda": UPD_DCASGDA,
+    "rowwise_adagrad": UPD_ROWWISE_ADAGRAD,
 }
 
 _LIBDIR = Path(__file__).resolve().parent / "_lib"
@@ -54,7 +56,7 @@ class DenseAdd(C.Structure):
         ("clip", C.c_float), ("pads", C.POINTER(vp)), ("me", C.c_int), ("world", C.c_int),
         ("ch_ready", C.c_int), ("ch_done", C.c_int), ("epoch", C.c_uint64), ("worker_rank", I32x8),
         ("is_worker", C.c_int), ("err_flag", vp), ("fin_flag", vp), ("done_counter", vp),
-        ("timeout_s", C.c_double), ("opt_box", VP8), ("my_worker", C.c_int),
+        ("timeout_s", C.c_double), ("opt_box", VP8), ("my_worker", C.c_int), ("num_col", i64),
     ]
 
 
@@ -262,6 +264,8 @@ _CUDA_FUNCS = {
     "mvb_push_dense_red": _status(i32, Ptr, i32, vpp, i64p, i64p, f32, Ptr),
     "mvb_push_dense_stateful": _status(i32, i32, Ptr, i32, vpp, vpp, vpp, i64p, i64p, i64p, C.POINTER(AddOpt), i32,
                                        Ptr),
+    "mvb_push_dense_rowwise": _status(i32, i32, Ptr, i32, vpp, vpp, i64p, i64p, i64p, i64, C.POINTER(AddOpt), i32,
+                                      Ptr),
     "mvb_get_rows": _status(i32, C.POINTER(RowMap), Ptr, i64, Ptr, i64, Ptr),
     "mvb_add_rows_red": _status(i32, C.POINTER(RowMap), Ptr, i64, Ptr, i64, f32, Ptr),
     "mvb_add_rows_delta": _status(C.POINTER(RowMap), Ptr, i64, Ptr, Ptr, i64, f32, Ptr),

@@ -122,17 +122,21 @@ class DenseDeviceTable(_AsyncOps):
         # server s's shard as seen from here (indexed by server id)
         self.shard_ptrs = [self.shard_buf.ptrs[rt.server_id_to_rank(s)] for s in range(S)] \
             if rt.num_servers() else [self.shard_buf.local_ptr]
-        nst, per_worker = {"default": (0, False), "sgd": (0, False), "momentum_sgd": (1, False),
-                           "adagrad": (1, True), "dcasgd": (1, True),
-                           "dcasgda": (2, True)}[name]
-        self.n_states, self.state_per_worker = nst, per_worker
-        self.state_stride = (self.my_len + 3) // 4 * 4
+        # (state slabs, one slab per worker, state element per row rather than per element)
+        nst, per_worker, per_row = {"default": (0, False, False), "sgd": (0, False, False),
+                                    "momentum_sgd": (1, False, False), "adagrad": (1, True, False),
+                                    "dcasgd": (1, True, False), "dcasgda": (2, True, False),
+                                    "rowwise_adagrad": (1, True, True)}[name]
+        self.n_states, self.state_per_worker, self.state_per_row = nst, per_worker, per_row
+        # a slab holds one element per shard element, or per shard row; slabs start at multiples of 4 elements
+        gran = self.num_col if per_row else 1
+        self.state_stride = (self.my_len // gran + 3) // 4 * 4
         slab = self.state_stride * (W if per_worker else 1)
         # state slabs are symmetric (peer-mapped) too: the async one-sided push of a stateful
         # updater updates the owner's state remotely
         self._state_bufs = [rt.alloc_symm(max(slab, 1) * self.esz) for _ in range(nst)]
         self.state = [b.tensor(self.dtype, max(slab, 1)) for b in self._state_bufs]
-        self.state_strides = [(l + 3) // 4 * 4 for l in self.lens]
+        self.state_strides = [(l // gran + 3) // 4 * 4 for l in self.lens]
         # collective path resources (lazy)
         self._stage: List = []
         self._stage_idx = 0
@@ -250,8 +254,12 @@ class DenseDeviceTable(_AsyncOps):
                     ss = (C.c_int64 * self.S)(*self.state_strides)
                     ao = _opt_struct(opt)
                     ao.worker_id = max(rt.worker_id(), 0)
-                    lib.mvb_push_dense_stateful(self.dcode, self.updater, src, self.S, sp, s0, s1, so, sl, ss, ao,
-                                                rt.rank, N.stream_ptr())
+                    if self.state_per_row:
+                        lib.mvb_push_dense_rowwise(self.dcode, self.updater, src, self.S, sp, s0, so, sl, ss,
+                                                   self.num_col, ao, rt.rank, N.stream_ptr())
+                    else:
+                        lib.mvb_push_dense_stateful(self.dcode, self.updater, src, self.S, sp, s0, s1, so, sl, ss, ao,
+                                                    rt.rank, N.stream_ptr())
                 self._keep = src
             if rt.is_worker():
                 self._note_add()
@@ -287,6 +295,7 @@ class DenseDeviceTable(_AsyncOps):
         a.state0 = self.state[0].data_ptr() if self.n_states >= 1 else None
         a.state1 = self.state[1].data_ptr() if self.n_states >= 2 else None
         a.shard_len, a.shard_off, a.state_stride = self.my_len, self.my_off, self.state_stride
+        a.num_col = self.num_col
         nw = len(delta_ptrs)
         a.nworkers = nw
         a.worker_mask = (1 << nw) - 1
