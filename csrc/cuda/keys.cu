@@ -72,12 +72,14 @@ keys_collect_kernel(const __grid_constant__ KeysDev m, long long* __restrict__ o
   const int64_t words = (m.size + 31) / 32 + m.S;            // upper bound; words are per shard
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < words; t += stride) {
-    // word t of the concatenated per-shard bitmaps: shard o has ceil(len_o / 32) words
+    // word t of the concatenated per-shard bitmaps: shard o has ceil(len_o / 32) words, and when size < S the
+    // shards from `size` on hold no keys and have no bitmap words
     int64_t w = t;
     int o = 0;
     int64_t len = 0;
     for (; o < m.S; ++o) {
-      len = (o == m.S - 1) ? m.size - (int64_t)o * m.per : m.per;
+      const int64_t lo = min((int64_t)o * m.per, m.size);
+      len = (o == m.S - 1 ? m.size : min((int64_t)(o + 1) * m.per, m.size)) - lo;
       const int64_t nw = (len + 31) / 32;
       if (w < nw) break;
       w -= nw;
@@ -117,14 +119,15 @@ KeysDev to_dev(const MvbKeyMap* h) {
 extern "C" int mvb_keys_add(const MvbKeyMap* m, const int64_t* keys, const float* vals, int64_t n, float sign,
                             void* stream) {
   if (!row_split_ok(m->nservers, m->per_server)) return MVB_BAD_ROW_MAP;
-  if (n <= 0) return 0;
   if (m->width < 1 || m->width > 16) return -8;
+  if (n <= 0) return 0;
   keys_add_kernel<<<blocks_for(n * m->width, 256, 8), 256, 0, (cudaStream_t)stream>>>(to_dev(m), (const long long*)keys, vals, n, sign);
   MVB_CUDA_CHECK(cudaGetLastError());
   return 0;
 }
 extern "C" int mvb_keys_get(const MvbKeyMap* m, const int64_t* keys, float* out, int64_t n, void* stream) {
   if (!row_split_ok(m->nservers, m->per_server)) return MVB_BAD_ROW_MAP;
+  if (m->width < 1 || m->width > 16) return -8;
   if (n <= 0) return 0;
   keys_get_kernel<<<blocks_for(n * m->width, 256, 8), 256, 0, (cudaStream_t)stream>>>(to_dev(m), (const long long*)keys, out, n);
   MVB_CUDA_CHECK(cudaGetLastError());
@@ -134,6 +137,7 @@ extern "C" int mvb_keys_get(const MvbKeyMap* m, const int64_t* keys, float* out,
 extern "C" int mvb_keys_collect(const MvbKeyMap* m, int64_t* out_keys, float* out_vals, int64_t* count, int64_t cap,
                                 void* stream) {
   if (!row_split_ok(m->nservers, m->per_server)) return MVB_BAD_ROW_MAP;
+  if (m->width < 1 || m->width > 16) return -8;
   cudaStream_t st = (cudaStream_t)stream;
   MVB_CUDA_CHECK(cudaMemsetAsync(count, 0, 8, st));
   keys_collect_kernel<<<blocks_for((m->size + 31) / 32 + m->nservers, 256, 8), 256, 0, st>>>(to_dev(m), (long long*)out_keys, out_vals,

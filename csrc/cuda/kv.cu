@@ -6,6 +6,10 @@
 // missing keys.  Here every server shard is an open-addressing table in HBM
 // (int64 keys, linear probing); remote shards are reached with system-scope CAS /
 // atomic adds through the peer mapping, so Add/Get are single one-sided kernels.
+//
+// INT64_MIN marks an empty slot, so it cannot be a key: Add skips it and sets error 5003 (the rule of the hash
+// index, hash_rows.cu), Get returns 0 for it without probing. A CAS of an empty slot from "empty" to INT64_MIN
+// would succeed without claiming it, and the value added there would then belong to the next key in that slot.
 #include "mvb_common.cuh"
 
 namespace {
@@ -44,6 +48,10 @@ __global__ void kv_add_kernel(const __grid_constant__ KVDev kv, const long long*
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
     const long long key = keys[i];
+    if (key == kEmpty) {
+      if (err) atomicExch(err, 5003);   // reserved key
+      continue;
+    }
     const int o = owner_of(key, kv.S);
     long long* tk = kv.keys[o];
     V* tv = reinterpret_cast<V*>(kv.vals[o]);
@@ -73,6 +81,10 @@ __global__ void kv_get_kernel(const __grid_constant__ KVDev kv, const long long*
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
     const long long key = keys[i];
+    if (key == kEmpty) {                 // reserved key: never stored
+      out[i] = (V)0;
+      continue;
+    }
     const int o = owner_of(key, kv.S);
     const long long* tk = kv.keys[o];
     const V* tv = reinterpret_cast<const V*>(kv.vals[o]);
@@ -153,8 +165,8 @@ extern "C" int mvb_kv_init(void* keys, int64_t capacity, void* stream) {
 extern "C" int mvb_kv_add(const MvbKV* kv, const int64_t* keys, const void* vals, int64_t n,
                           int* err_flag, void* stream) {
   if (kv->nservers < 1 || kv->nservers > MVB_MAX_RANKS) return -3;
+  if (kv->capacity < 1 || (kv->capacity & (kv->capacity - 1))) return -4;
   if (n <= 0) return 0;
-  if (kv->capacity & (kv->capacity - 1)) return -4;
   const KVDev d = to_dev(kv);
   return with_dtype<float, double, int, long long>(kv->vtype, [&](auto t) {
     using T = typename decltype(t)::type;
@@ -167,6 +179,7 @@ extern "C" int mvb_kv_add(const MvbKV* kv, const int64_t* keys, const void* vals
 extern "C" int mvb_kv_get(const MvbKV* kv, const int64_t* keys, void* out_vals, int64_t n,
                           void* stream) {
   if (kv->nservers < 1 || kv->nservers > MVB_MAX_RANKS) return -3;
+  if (kv->capacity < 1 || (kv->capacity & (kv->capacity - 1))) return -4;
   if (n <= 0) return 0;
   const KVDev d = to_dev(kv);
   return with_dtype<float, double, int, long long>(kv->vtype, [&](auto t) {
@@ -202,7 +215,7 @@ extern "C" int mvb_kv_count(const void* keys, int64_t capacity, int64_t* out_cou
 // Re-insert every live (key, value) of a shard into a new, initialised, larger LOCAL table (growth).
 extern "C" int mvb_kv_rehash(int vtype, const void* old_keys, const void* old_vals, int64_t old_cap, void* new_keys,
                              void* new_vals, int64_t new_cap, int* err_flag, void* stream) {
-  if (new_cap & (new_cap - 1)) return -4;
+  if (new_cap < 1 || (new_cap & (new_cap - 1))) return -4;
   return with_dtype<float, double, int, long long>(vtype, [&](auto t) {
     using T = typename decltype(t)::type;
     kv_rehash_kernel<T><<<blocks_for(old_cap, 256, 8), 256, 0, (cudaStream_t)stream>>>(

@@ -243,7 +243,10 @@ int mvb_kv_init(void* keys, int64_t capacity, void* stream);
 int mvb_kv_count(const void* keys, int64_t capacity, int64_t* out_count, void* stream);
 int mvb_kv_rehash(int vtype, const void* old_keys, const void* old_vals, int64_t old_cap, void* new_keys,
                   void* new_vals, int64_t new_cap, int* err_flag, void* stream);
-/* mvb_kv_add and mvb_kv_get return -3 for nservers outside [1, MVB_MAX_RANKS], before any CUDA call */
+/* mvb_kv_add and mvb_kv_get return -3 for nservers outside [1, MVB_MAX_RANKS] and -4 for a capacity that is not
+ * a power of two >= 1 (mvb_kv_rehash: -4 for such a new_cap), before any CUDA call. INT64_MIN is not a key:
+ * mvb_kv_add skips it and sets *err_flag = 5003, mvb_kv_get returns 0 for it. A key with no free slot on its
+ * probe chain sets *err_flag = 5001 (5002 in mvb_kv_rehash). */
 int mvb_kv_add(const MvbKV* kv, const int64_t* keys, const void* vals, int64_t n, int* err_flag,
                void* stream);
 int mvb_kv_get(const MvbKV* kv, const int64_t* keys, void* out_vals, int64_t n, void* stream);
@@ -383,6 +386,7 @@ typedef struct MvbKeyMap {
   void* shard_ptrs[MVB_MAX_RANKS];     /* server s: [keys of s x width] fp32, peer mapped      */
   void* touched_ptrs[MVB_MAX_RANKS];   /* server s: touched bitmap uint32[ceil(keys of s / 32)] */
 } MvbKeyMap;
+/* all three return -8 for a width outside [1, 16] before any CUDA call */
 int mvb_keys_add(const MvbKeyMap* m, const int64_t* keys, const float* vals, int64_t n, float sign, void* stream);
 int mvb_keys_get(const MvbKeyMap* m, const int64_t* keys, float* out, int64_t n, void* stream);
 int mvb_keys_collect(const MvbKeyMap* m, int64_t* out_keys, float* out_vals, int64_t* count, int64_t cap,

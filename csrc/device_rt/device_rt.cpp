@@ -234,6 +234,9 @@ void CheckWatchdog() {
   CopyToHost(&code, c.err_flag, sizeof code);
   if (code == 0) return;
   MVB_CHECK(mvb_memset_async(c.err_flag, 0, sizeof(int), nullptr));
+  if (code == 5003)
+    Log::Fatal("KVTable: key INT64_MIN is reserved for empty slots (code 5003: kv-bad-key); the other keys of the "
+               "batch were added\n");
   static const char* kWhat[] = {"?", "wait", "barrier", "add-ready", "get-done", "kv-full", "allreduce"};
   const int kind = code / 1000;
   Log::Fatal("device watchdog: wait on peer timed out (code %d: %s, peer index %d)\n", code,

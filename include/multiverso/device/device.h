@@ -224,12 +224,14 @@ class MatrixTable : public DenseTable<T> {
 };
 
 // KVTable<int64, V>: hash-partitioned (key mod servers) open-addressing tables in HBM, remote
-// shards through system-scope atomics. V in {float, double, int, int64_t}.
+// shards through system-scope atomics. V in {float, double, int, int64_t}. The capacity is fixed.
 template <typename V>
 class KVTable : public Serializable {
  public:
   explicit KVTable(int64_t capacity = 0);   // 0: -kv_capacity
   ~KVTable() override;
+  // Fatal "kv-full" if a key finds no free slot, and "kv-bad-key" for INT64_MIN (it marks empty slots and is
+  // skipped; the other keys are added).
   void Add(const int64_t* device_keys, const V* device_vals, int64_t n, CudaStream stream = nullptr);
   void Get(const int64_t* device_keys, V* device_out, int64_t n, CudaStream stream = nullptr);
   // Convenience for host-side scalars (word counts and the like).

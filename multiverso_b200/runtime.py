@@ -465,6 +465,9 @@ class Runtime:
         code = int(self.err_flag.item())
         if code:
             self.err_flag.zero_()
+            if code == 5003:
+                Log.fatal("KVTable: key INT64_MIN is reserved for empty slots (code 5003: kv-bad-key); the other "
+                          "keys of the batch were added")
             Log.fatal("device watchdog: wait on peer timed out (code %d: %s, peer index %d)", code,
                       {1: "wait", 2: "barrier", 3: "add-ready", 4: "get-done", 5: "kv-full",
                        6: "allreduce"}.get(code // 1000, "?"), code % 1000)

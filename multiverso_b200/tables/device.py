@@ -970,7 +970,10 @@ class KVDeviceTable(_AsyncOps):
     ``reserve``) the ranks agree on the fullest shard's load factor and, above 1/2, every owner re-inserts its
     shard into a table of twice (or more) the capacity in a freshly allocated symmetric slab; the old slab is
     released in two phases.  Between two collective points a shard therefore accepts at least as many new keys as it
-    already holds slots in use ("kv-full" is reported by the watchdog if even that is exceeded).
+    already holds slots in use ("kv-full" is reported by the watchdog if even that is exceeded). In a single process
+    ``add`` grows the table before a batch that could take it above 1/2, so one batch of any size fits.
+    INT64_MIN marks empty slots and is not a key: ``add`` skips it (the batch's other keys are added) and flags
+    "kv-bad-key", which the next watchdog check raises; ``get`` returns 0 for it.
     ``add`` / ``get`` are asynchronous device operations (no stream synchronisation, no D2H per call): ``get``
     returns a device tensor; the worker-side cache ``raw()`` (kv_table.h:30) is refreshed lazily from the batches
     that were pulled."""
@@ -1067,11 +1070,15 @@ class KVDeviceTable(_AsyncOps):
         k = self._keys([keys] if scalar else keys)
         v = torch.as_tensor([vals] if scalar else vals).to(self.vdtype).to(self.rt.device).contiguous().view(-1)
         assert k.numel() == v.numel()
+        n = k.numel()
+        if self.rt.size == 1 and self._added_ub + n > self.MAX_LOAD * self.capacity:
+            # single process: every point is a collective point, so grow for this batch's distinct keys before it
+            # runs (reserve synchronises anyway)
+            n = int(torch.unique(k).numel())
+            self.reserve(self.live_keys() + n)
         lib.mvb_kv_add(self._kv, k, v, k.numel(), self.rt.err_flag, N.stream_ptr())
         self._keep_add = (k, v)
-        self._added_ub += k.numel()
-        if self.rt.size == 1 and self._added_ub > self.MAX_LOAD * self.capacity:
-            self.reserve()                       # single process: every point is a collective point
+        self._added_ub += n
 
     def get(self, keys):
         """Batched lookup; returns a device tensor (a Python scalar for a scalar key)."""

@@ -1,7 +1,9 @@
 """The kernel library's argument codes, checked without a GPU: -2 for an unknown updater, -1 for an element type an
-entry point does not serve, and -3 for a server count outside [1, MVB_MAX_RANKS] where an entry point copies one
-pointer per server into a fixed array of MVB_MAX_RANKS. Every other argument is well formed, the pointers are dummies
-that must never be dereferenced, and a CUDA call on a machine without a device would return a different code.
+entry point does not serve, -3 for a server count outside [1, MVB_MAX_RANKS] where an entry point copies one
+pointer per server into a fixed array of MVB_MAX_RANKS, -4 for a KV capacity that is not a power of two >= 1 (the
+probe chains wrap with capacity - 1 as a mask), and -8 for a key-table width outside [1, 16]. Every other argument is
+well formed, the pointers are dummies that must never be dereferenced, and a CUDA call on a machine without a device
+would return a different code.
 
 The calls run in a child process that sees no CUDA device (CUDA_VISIBLE_DEVICES=""), also where a GPU is present: an
 argument check that stopped working then returns a CUDA error instead of launching a kernel on a dummy pointer."""
@@ -90,9 +92,9 @@ def _row_nonzero(lib, dtype):
     return lib.mvb_row_nonzero_mask(dtype, DUMMY, 4, 4, 4, DUMMY, None)
 
 
-def _kv(dtype, S=1):
+def _kv(dtype, S=1, cap=16):
     kv = N.KV()
-    kv.vtype, kv.nservers, kv.capacity = dtype, S, 16
+    kv.vtype, kv.nservers, kv.capacity = dtype, S, cap
     for s in range(N.MAX_RANKS):
         kv.keys[s] = kv.vals[s] = DUMMY
     return kv
@@ -104,6 +106,27 @@ def _kv_add(lib, dtype, S=1):
 
 def _kv_get(lib, dtype, S=1):
     return lib.mvb_kv_get(_kv(dtype, S), DUMMY, DUMMY, 1, None)
+
+
+def _kv_capacity(fn, cap):
+    def call(lib):
+        if fn == "mvb_kv_rehash":
+            return lib.mvb_kv_rehash(N.F32, DUMMY, DUMMY, 16, DUMMY, DUMMY, cap, DUMMY, None)
+        return getattr(lib, fn)(_kv(N.F32, 1, cap), DUMMY, DUMMY, *((1, DUMMY) if fn == "mvb_kv_add" else (1,)), None)
+    return call
+
+
+def _keys_width(fn, width):
+    def call(lib):
+        m = N.KeyMap()
+        m.size, m.per_server, m.nservers, m.width = 16, 16, 1, width
+        m.shard_ptrs[0] = m.touched_ptrs[0] = DUMMY
+        if fn == "mvb_keys_add":
+            return lib.mvb_keys_add(m, DUMMY, DUMMY, 1, 1.0, None)
+        if fn == "mvb_keys_get":
+            return lib.mvb_keys_get(m, DUMMY, DUMMY, 1, None)
+        return lib.mvb_keys_collect(m, DUMMY, DUMMY, DUMMY, 1, None)
+    return call
 
 
 def _kv_dump(lib, dtype):
@@ -161,6 +184,12 @@ def _cases():
     for fn, call in SERVER_ENTRIES.items():
         for S in (0, N.MAX_RANKS + 1):
             c[f"servers/{fn}/{S}"] = (call, (S,))
+    for fn in ("mvb_kv_add", "mvb_kv_get", "mvb_kv_rehash"):
+        for cap in (0, -16, 3, 48):
+            c[f"capacity/{fn}/{cap}"] = (_kv_capacity(fn, cap), ())
+    for fn in ("mvb_keys_add", "mvb_keys_get", "mvb_keys_collect"):
+        for width in (0, -1, 17):
+            c[f"width/{fn}/{width}"] = (_keys_width(fn, width), ())
     return c
 
 
@@ -209,6 +238,16 @@ def test_stateful_push_rejects_stateless_updaters(codes, case):
 @pytest.mark.parametrize("case", _ids("servers/"))
 def test_server_count_is_checked(codes, case):
     assert codes[case] == -3
+
+
+@pytest.mark.parametrize("case", _ids("capacity/"))
+def test_kv_capacity_is_checked(codes, case):
+    assert codes[case] == -4
+
+
+@pytest.mark.parametrize("case", _ids("width/"))
+def test_key_table_width_is_checked(codes, case):
+    assert codes[case] == -8
 
 
 if __name__ == "__main__":
