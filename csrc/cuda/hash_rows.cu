@@ -15,11 +15,23 @@
 // Every other thread that meets the key (in this launch or on another rank) waits for ready[j] with an acquire
 // spin under the clock64 watchdog of spin_wait_ge, so no row is returned before its initial value is visible.
 // The counter only ever holds keys that got a row: a CAS comes before the count, so the thousands of lanes that
-// race for a Zipf head key at first touch never over-count. Slots are never freed, so the updater state rows of
-// a new key are still zero from allocation.
+// race for a Zipf head key at first touch never over-count. A slot is only freed by an eviction, which leaves it
+// with zero updater state, so the updater state rows of a new key are zero.
 //
 // Lanes of a warp that carry the same (table, key) are merged with __match_any_sync: one lane probes and the
 // row is broadcast, so a Zipf head repeated thousands of times costs one probe per warp.
+//
+// Access clock (a descriptor with last_seen): an inserting lookup stamps every key it resolves. The claimer stores
+// last_seen[j] = clock before its release of ready[j]; a lookup that finds the key raises last_seen[j] to its
+// clock with atomicMax_system, after a plain load shows it older, so a Zipf head costs about one atomic per clock
+// value rather than one per warp. Stamps of ranks at different clocks combine by max.
+//
+// Eviction (mvb_hash_rows_mark, mvb_hash_rows_evict) runs between barriers, with no lookup in flight. Marking sets
+// ready[j] = 3 for the listed keys; the rebuild of a server then removes marked, refused and idle slots with the
+// textbook in-place rehash of linear probing, one warp per cluster of non-empty slots (see mvb200.h). A cluster
+// starts after an empty slot, so a survivor's probe from its home stays inside the part of the cluster already
+// walked: survivors only move back toward their homes, never onto a slot not yet walked, and no copy of the shard
+// or the state is needed.
 #include "mvb_common.cuh"
 
 namespace {
@@ -35,7 +47,8 @@ MVB_DEVINL void st_release_sys_u32(uint32_t* p, uint32_t v) {
   asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
 
-constexpr uint32_t kReady = 1, kRefused = 2;   // ready[j]: 0 while the claimer initialises the row
+// ready[j]: 0 while the claimer initialises the row (or for an empty slot); kMarked only during an eviction
+constexpr uint32_t kReady = 1, kRefused = 2, kMarked = 3;
 
 // ready[j] once it is set (kReady / kRefused), or 0 after `budget` cycles (the backoff of spin_wait_ge)
 MVB_DEVINL uint32_t wait_ready(const uint32_t* p, long long budget) {
@@ -108,6 +121,7 @@ MVB_DEVINL int64_t translate(const MvbHashRows& h, int t, long long key, int ins
                                  init_col(h, key, c + 3));
           st_v4(row + c, *reinterpret_cast<uint4*>(&v));
         }
+        if (h.last_seen[s]) reinterpret_cast<long long*>(h.last_seen[s])[j] = *h.clock;
         fence_sys();
         st_release_sys_u32(rdy, kReady);
         return (int64_t)s * P + (int64_t)j;
@@ -122,6 +136,11 @@ MVB_DEVINL int64_t translate(const MvbHashRows& h, int t, long long key, int ins
       if (r != kReady) {
         set_status(status, MVB_HASH_TIMEOUT, t, s);
         return zero_row;
+      }
+      if (insert && h.last_seen[s]) {
+        long long* ls = reinterpret_cast<long long*>(h.last_seen[s]) + j;
+        const long long now = *h.clock;
+        if (*reinterpret_cast<volatile long long*>(ls) < now) atomicMax_system(ls, now);
       }
       return (int64_t)s * P + (int64_t)j;
     }
@@ -189,6 +208,218 @@ __global__ void hash_dump_kernel(const long long* keys, const uint32_t* ready, i
   }
 }
 
+// ---- eviction ---------------------------------------------------------------------------------------------------
+
+__global__ void hash_mark_kernel(const __grid_constant__ MvbHashRows h, const int64_t* keys, int64_t n) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  const uint64_t mask = (uint64_t)h.slots - 1;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    const long long key = keys[i];
+    if (key == kEmpty) continue;
+    const int s = owner_of(key, h.nservers);
+    const long long* ks = reinterpret_cast<const long long*>(h.keys[s]);
+    volatile uint32_t* ready = reinterpret_cast<volatile uint32_t*>(h.ready[s]);
+    uint64_t j = mix64((uint64_t)key) & mask;
+    for (int64_t probe = 0; probe < h.slots; ++probe, j = (j + 1) & mask) {
+      const long long cur = ks[j];
+      if (cur == kEmpty) break;
+      if (cur == key) {
+        if (ready[j] == kReady) ready[j] = kMarked;   // a refused slot is a victim anyway, and holds no live key
+        break;
+      }
+    }
+  }
+}
+
+// One server's index and the payload that moves with a slot: its row, its state rows, its last_seen.
+struct EvictArgs {
+  long long* keys;
+  uint32_t* ready;
+  long long* ls;            // or nullptr
+  float* rows;              // local row j = slot j, num_col floats
+  int64_t num_col;
+  float* st[2];             // state arrays, or nullptr
+  int n_slabs;
+  int64_t stride, srow;     // elements between slabs; elements per state row
+  int64_t P;
+  long long older_than;     // INT64_MIN: no age rule
+  int64_t* counts;          // {live keys removed, survivors moved}
+  long long* work;          // {clusters, first victim, cluster starts...}
+};
+
+MVB_DEVINL void copy_f32(float* dst, const float* src, int64_t n, int lane) {
+  if ((n & 3) == 0) {
+    for (int64_t c = (int64_t)lane * 4; c < n; c += 128) st_v4(dst + c, ld_v4(src + c));
+  } else {
+    for (int64_t c = lane; c < n; c += 32) dst[c] = src[c];
+  }
+}
+MVB_DEVINL void zero_f32(float* dst, int64_t n, int lane) {
+  if ((n & 3) == 0) {
+    for (int64_t c = (int64_t)lane * 4; c < n; c += 128) st_v4(dst + c, make_uint4(0, 0, 0, 0));
+  } else {
+    for (int64_t c = lane; c < n; c += 32) dst[c] = 0.f;
+  }
+}
+
+// Empty slot j: zero state rows and last_seen, the empty key (the row keeps whatever it holds). Whole warp.
+MVB_DEVINL void clear_slot(const EvictArgs& e, int64_t j, int lane) {
+  for (int a = 0; a < 2; ++a)
+    if (e.st[a])
+      for (int k = 0; k < e.n_slabs; ++k) zero_f32(e.st[a] + k * e.stride + j * e.srow, e.srow, lane);
+  if (lane == 0) {
+    e.keys[j] = kEmpty;
+    e.ready[j] = 0;
+    if (e.ls) e.ls[j] = 0;
+  }
+  __syncwarp();
+}
+
+// Slot `from` moves to the empty slot `to`, then `from` is cleared. Whole warp.
+MVB_DEVINL void move_slot(const EvictArgs& e, int64_t to, int64_t from, int lane) {
+  copy_f32(e.rows + to * e.num_col, e.rows + from * e.num_col, e.num_col, lane);
+  for (int a = 0; a < 2; ++a)
+    if (e.st[a])
+      for (int k = 0; k < e.n_slabs; ++k) {
+        float* slab = e.st[a] + k * e.stride;
+        copy_f32(slab + to * e.srow, slab + from * e.srow, e.srow, lane);
+      }
+  if (lane == 0) {
+    e.keys[to] = e.keys[from];
+    e.ready[to] = e.ready[from];
+    if (e.ls) e.ls[to] = e.ls[from];
+  }
+  __syncwarp();
+  clear_slot(e, from, lane);
+}
+
+// Pass 1, before any slot changes: idle live keys become marked; live victims are counted (and leave the server's
+// count); every cluster start (a non-empty slot after an empty one) is listed; the lowest victim slot is kept for
+// an index without an empty slot.
+__global__ void hash_evict_scan_kernel(const EvictArgs e, unsigned long long* count) {
+  const int lane = threadIdx.x & 31;
+  const uint64_t mask = (uint64_t)e.P - 1;
+  const int64_t n32 = (e.P + 31) & ~(int64_t)31;
+  int64_t removed = 0;
+  for (int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n32; j += (int64_t)gridDim.x * blockDim.x) {
+    bool live_victim = false, victim = false, start = false;
+    if (j < e.P) {
+      const long long k = e.keys[j];
+      if (k != kEmpty) {
+        uint32_t r = e.ready[j];
+        if (r == kReady && e.ls && e.ls[j] < e.older_than) {
+          r = kMarked;
+          e.ready[j] = kMarked;
+        }
+        victim = r != kReady;
+        live_victim = r == kMarked;
+        start = e.keys[(j - 1) & mask] == kEmpty;
+      }
+    }
+    const unsigned vb = __ballot_sync(0xffffffffu, live_victim), sb = __ballot_sync(0xffffffffu, start);
+    removed += __popc(vb);
+    const unsigned first = __reduce_min_sync(0xffffffffu, victim ? (unsigned)j : 0xffffffffu);
+    long long base = 0;
+    if (lane == 0) {
+      if (first != 0xffffffffu) atomicMin(reinterpret_cast<unsigned long long*>(e.work + 1), first);
+      if (sb) base = (long long)atomicAdd(reinterpret_cast<unsigned long long*>(e.work), (unsigned long long)__popc(sb));
+    }
+    base = __shfl_sync(0xffffffffu, base, 0);
+    if (start) e.work[2 + base + __popc(sb & ((1u << lane) - 1))] = j;
+  }
+  if (lane == 0 && removed) {
+    atomicAdd(reinterpret_cast<unsigned long long*>(e.counts), (unsigned long long)removed);
+    atomicAdd(count, (unsigned long long)-removed);
+  }
+}
+
+// An index without an empty slot has no cluster to cut. Its lowest victim v is deleted by backward shifting
+// (Knuth's Algorithm R for linear probing): walking on from the hole, an entry whose home is not cyclically in
+// (hole, j] moves into the hole, which then moves to j. The walk ends at the first empty slot, which is the last
+// hole; the rest of the index is then one cluster starting after it. One warp.
+__global__ void hash_evict_unwrap_kernel(const EvictArgs e) {
+  const int lane = threadIdx.x & 31;
+  if (e.work[0] != 0 || (unsigned long long)e.work[1] >= (unsigned long long)e.P) return;   // clusters, or no victim
+  const uint64_t mask = (uint64_t)e.P - 1;
+  const int64_t v = e.work[1];
+  clear_slot(e, v, lane);
+  int64_t hole = v, j = v;
+  long long moved = 0;
+  while (true) {
+    j = (j + 1) & mask;
+    const long long k = e.keys[j];
+    if (k == kEmpty) break;
+    const int64_t home = (int64_t)(mix64((uint64_t)k) & mask);
+    const bool stays = hole <= j ? (hole < home && home <= j) : (hole < home || home <= j);
+    if (!stays) {
+      moved += e.ready[j] == kReady;
+      move_slot(e, hole, j, lane);
+      hole = j;
+    }
+  }
+  if (lane == 0) {
+    e.work[0] = 1;
+    e.work[2] = (hole + 1) & mask;
+    if (moved) atomicAdd(reinterpret_cast<unsigned long long*>(e.counts + 1), (unsigned long long)moved);
+  }
+}
+
+// Pass 2: a warp walks each cluster from its first slot to the empty slot after it. Slots ahead of the walk are
+// still as pass 1 saw them (moves only go backwards), so the walk ends where the old cluster did. Until the first
+// victim every survivor stays, so the walk skips 32 slots per ballot; after it, each survivor probes from its home
+// with ballots over 32 slots for the first empty slot before its own and moves there.
+__global__ void __launch_bounds__(256) hash_evict_walk_kernel(const EvictArgs e) {
+  const int lane = threadIdx.x & 31;
+  const uint64_t mask = (uint64_t)e.P - 1;
+  long long moved = 0;
+  const long long nclusters = *reinterpret_cast<volatile long long*>(e.work);
+  for (long long c = warp_id(); c < nclusters; c += num_warps()) {
+    uint64_t x = (uint64_t)e.work[2 + c];
+    // survivors before the cluster's first victim keep their slots
+    bool done = false;
+    while (true) {
+      const uint64_t j = (x + lane) & mask;
+      const long long k = e.keys[j];
+      const uint32_t r = e.ready[j];
+      const unsigned eb = __ballot_sync(0xffffffffu, k == kEmpty);
+      unsigned vb = __ballot_sync(0xffffffffu, k != kEmpty && r != kReady);
+      if (eb) vb &= (1u << (__ffs(eb) - 1)) - 1;     // the cluster ends at its first empty slot
+      if (vb) {
+        x += __ffs(vb) - 1;
+        break;
+      }
+      if (eb) {
+        done = true;
+        break;
+      }
+      x += 32;
+    }
+    if (done) continue;
+    for (;; ++x) {
+      const uint64_t j = x & mask;
+      const long long k = e.keys[j];
+      if (k == kEmpty) break;
+      if (e.ready[j] != kReady) {
+        clear_slot(e, (int64_t)j, lane);
+        continue;
+      }
+      const uint64_t home = mix64((uint64_t)k) & mask;
+      const uint64_t dist = (j - home) & mask;               // the old chain home .. j has no empty slot
+      for (uint64_t d0 = 0; d0 < dist; d0 += 32) {
+        const uint64_t d = d0 + lane;
+        const bool free = d < dist && e.keys[(home + d) & mask] == kEmpty;
+        const unsigned fb = __ballot_sync(0xffffffffu, free);
+        if (fb) {
+          move_slot(e, (int64_t)((home + d0 + __ffs(fb) - 1) & mask), (int64_t)j, lane);
+          ++moved;
+          break;
+        }
+      }
+    }
+  }
+  if (lane == 0 && moved) atomicAdd(reinterpret_cast<unsigned long long*>(e.counts + 1), (unsigned long long)moved);
+}
+
 }  // namespace
 
 extern "C" int mvb_hash_rows_init(void* keys, void* ready, void* count, int64_t slots, void* stream) {
@@ -223,6 +454,48 @@ extern "C" int mvb_hash_rows_dump(const MvbHashRows* h, int server, int64_t* out
                                                           (const uint32_t*)h->ready[server], h->slots,
                                                           (int64_t)server * h->slots, out_keys, out_rows,
                                                           (unsigned long long*)out_count);
+  MVB_CUDA_CHECK(cudaGetLastError());
+  return 0;
+}
+
+static int check_index(const MvbHashRows* h) {
+  if (h->nservers < 1 || h->nservers > MVB_MAX_RANKS) return -3;
+  if (h->slots < 2 || h->slots > (int64_t(1) << 31) || (h->slots & (h->slots - 1))) return -4;
+  return 0;
+}
+
+extern "C" int mvb_hash_rows_mark(const MvbHashRows* h, const int64_t* keys, int64_t n, void* stream) {
+  if (int rc = check_index(h)) return rc;
+  if (n <= 0) return 0;
+  hash_mark_kernel<<<blocks_for(n, 256, 8), 256, 0, (cudaStream_t)stream>>>(*h, keys, n);
+  MVB_CUDA_CHECK(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int mvb_hash_rows_evict(const MvbHashRows* h, int server, int64_t older_than, void* state0, void* state1,
+                                   int n_slabs, int64_t state_stride, int64_t state_row, int64_t* counts,
+                                   int64_t* work, void* stream) {
+  if (int rc = check_index(h)) return rc;
+  if (server < 0 || server >= h->nservers) return -1;
+  const MvbRowMap& m = h->map;
+  if (!row_split_ok(m.nservers, m.rows_per_server) || m.nservers != h->nservers || m.rows_per_server < h->slots ||
+      m.num_col < 4 || m.num_col % 4)
+    return MVB_BAD_ROW_MAP;
+  if (older_than != INT64_MIN && !h->last_seen[server]) return -5;
+  if ((state0 || state1) && (n_slabs < 1 || state_row < 1 || (n_slabs > 1 && state_stride < h->slots * state_row)))
+    return -6;
+  cudaStream_t st = (cudaStream_t)stream;
+  const EvictArgs e{(long long*)h->keys[server], (uint32_t*)h->ready[server], (long long*)h->last_seen[server],
+                    (float*)m.shard_ptrs[server], m.num_col, {(float*)state0, (float*)state1}, n_slabs,
+                    state_stride, state_row, h->slots, (long long)older_than, counts, (long long*)work};
+  MVB_CUDA_CHECK(cudaMemsetAsync(counts, 0, 16, st));
+  MVB_CUDA_CHECK(cudaMemsetAsync(work, 0, 8, st));              // no cluster yet
+  MVB_CUDA_CHECK(cudaMemsetAsync(work + 1, 0xff, 8, st));       // no victim yet
+  hash_evict_scan_kernel<<<blocks_for(h->slots, 256, 8), 256, 0, st>>>(e, (unsigned long long*)h->count[server]);
+  MVB_CUDA_CHECK(cudaGetLastError());
+  hash_evict_unwrap_kernel<<<1, 32, 0, st>>>(e);
+  MVB_CUDA_CHECK(cudaGetLastError());
+  hash_evict_walk_kernel<<<grid_for(h->slots / 2), 256, 0, st>>>(e);
   MVB_CUDA_CHECK(cudaGetLastError());
   return 0;
 }

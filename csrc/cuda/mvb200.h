@@ -271,6 +271,10 @@ typedef struct MvbHashRows {
   int init;                        /* MVB_HASH_INIT_CONST: init_value; UNIFORM: lo + u (hi - lo), u from the key */
   float init_value, lo, hi;
   uint64_t seed;
+  /* access clock (optional): a lookup that inserts stamps each key it finds or inserts with
+     last_seen[j] = max(last_seen[j], *clock); lookups that do not insert stamp nothing                    */
+  void* last_seen[MVB_MAX_RANKS];  /* int64[P] per server, symmetric, or NULL: not tracked (clock unused)   */
+  const int64_t* clock;            /* device int64 of the calling rank; needed when last_seen is set        */
 } MvbHashRows;
 typedef struct MvbHashLookup {
   const MvbHashRows* tables;       /* device [T] index descriptors                                          */
@@ -296,6 +300,29 @@ int mvb_hash_rows_count(const MvbHashRows* h, int64_t* out, void* stream);
 /* (key, row) of every live slot (ready == 1) of server `server`, in no particular order; *out_count on the device */
 int mvb_hash_rows_dump(const MvbHashRows* h, int server, int64_t* out_keys, int64_t* out_rows, int64_t* out_count,
                        void* stream);
+/* Eviction. Both calls need every lookup of the index to have completed on every rank (run them between barriers).
+ * mvb_hash_rows_mark: a translation without insert of keys[0, n) that sets ready[j] = 3 ("marked") at the owner of
+ * every live key found (peer stores included). Missing keys and INT64_MIN are ignored.
+ * mvb_hash_rows_evict: rebuilds server `server`'s index in place (run by the rank holding it). It removes the marked
+ * and refused slots and, unless older_than is INT64_MIN, the live keys with last_seen < older_than. The survivors
+ * are placed by the in-place rehash: the index is cut into clusters (maximal runs of non-empty slots, wrapping
+ * P - 1 -> 0), each walked from its first slot; a victim is cleared, a survivor moves to the first empty slot
+ * probing from its home, or stays. A survivor carries its row (num_col floats), its updater state rows and
+ * last_seen. The state is nst = (state0 != NULL) + (state1 != NULL) arrays of n_slabs fp32 slabs state_stride
+ * elements apart, slot j owning elements [j state_row, (j + 1) state_row) of each slab. Every slot left empty
+ * holds zero state and last_seen 0; its row is left as it was. An index without an empty slot first loses its
+ * lowest victim slot by a sequential backward-shift deletion (one warp), then is walked as one cluster. The zero row
+ * is never touched. counts: device int64[2] out, {live keys removed, survivors moved}; the server's count drops by
+ * counts[0]. work: device int64[slots / 2 + 2] scratch.
+ * Returns, before any CUDA call: -3 for nservers outside [1, MVB_MAX_RANKS], -1 for a server outside
+ * [0, nservers), -4 for slots not a power of two in [2, 2^31], MVB_BAD_ROW_MAP for a map that fails the row map
+ * rule, disagrees with nservers, has rows_per_server < slots or num_col not a positive multiple of 4, -5 for
+ * older_than != INT64_MIN without last_seen[server], -6 for a state description with n_slabs < 1, state_row < 1
+ * or n_slabs > 1 and state_stride < slots * state_row. mvb_hash_rows_mark returns -3 and -4 alike. */
+int mvb_hash_rows_mark(const MvbHashRows* h, const int64_t* keys, int64_t n, void* stream);
+int mvb_hash_rows_evict(const MvbHashRows* h, int server, int64_t older_than, void* state0, void* state1,
+                        int n_slabs, int64_t state_stride, int64_t state_row, int64_t* counts, int64_t* work,
+                        void* stream);
 
 /* ---- all-reduce (K6) --------------------------------------------------------- */
 /* One-shot P2P: every rank reads all peers' symmetric buffers and reduces locally

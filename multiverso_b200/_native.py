@@ -89,7 +89,7 @@ HASH_FULL, HASH_TIMEOUT, HASH_BAD_KEY = 1, 2, 3
 class HashRows(C.Structure):
     _fields_ = [("nservers", C.c_int), ("slots", i64), ("keys", VP8), ("ready", VP8), ("count", VP8),
                 ("map", RowMap), ("init", C.c_int), ("init_value", C.c_float), ("lo", C.c_float),
-                ("hi", C.c_float), ("seed", C.c_uint64)]
+                ("hi", C.c_float), ("seed", C.c_uint64), ("last_seen", VP8), ("clock", vp)]
 
 
 class HashLookup(C.Structure):
@@ -284,6 +284,8 @@ _CUDA_FUNCS = {
     "mvb_hash_rows_lookup": _status(C.POINTER(HashLookup), Ptr),
     "mvb_hash_rows_count": _status(C.POINTER(HashRows), Ptr, Ptr),
     "mvb_hash_rows_dump": _status(C.POINTER(HashRows), i32, Ptr, Ptr, Ptr, Ptr),
+    "mvb_hash_rows_mark": _status(C.POINTER(HashRows), Ptr, i64, Ptr),
+    "mvb_hash_rows_evict": _status(C.POINTER(HashRows), i32, i64, Ptr, Ptr, i32, i64, i64, Ptr, Ptr, Ptr),
     "mvb_allreduce_oneshot": _status(C.POINTER(Allreduce), Ptr),
     "mvb_allreduce_twoshot": _status(C.POINTER(Allreduce), Ptr),
     "mvb_allreduce_fused": _status(C.POINTER(Allreduce), Ptr, i64, Ptr),

@@ -812,10 +812,17 @@ class HashMatrixTable(MatrixDeviceTable):
 
     A key's initial row depends on the key only: ``init_value`` (default 0) in every column, or, with
     ``min_value`` and ``max_value``, ``lo + u (hi - lo)`` with ``u`` drawn from ``(key, seed, column)``. Which slot
-    (row id) a key gets depends on the order in which keys arrive, which may depend on timing; nothing else does."""
+    (row id) a key gets depends on the order in which keys arrive, which may depend on timing; nothing else does.
+
+    ``track_access=True`` keeps a last-seen stamp per key: every lookup that inserts (a training forward of
+    ``PSEmbedding`` / ``PSEmbeddingCollection``, ``lookup(insert=True)``, ``add``) raises the stamp of each key it
+    touches to this rank's ``clock``, a user-defined int64 time (a step, an hour, ...). Reads (``get``,
+    ``lookup(insert=False)``, eval-mode layers) stamp nothing. ``evict`` removes idle keys (``older_than``) or listed
+    keys and frees their slots, so a table of fixed capacity can serve a stream of new ids. It costs one int64 per
+    slot and an atomic per key and clock value."""
 
     def __init__(self, capacity: int, num_col: int, dtype="float32", updater: Optional[str] = None,
-                 init_value=None, min_value=None, max_value=None, seed: int = 1):
+                 init_value=None, min_value=None, max_value=None, seed: int = 1, track_access: bool = False):
         rt = Runtime.get()
         if not rt.started:
             Log.fatal("MV_Init must be called before creating tables")
@@ -851,6 +858,21 @@ class HashMatrixTable(MatrixDeviceTable):
         else:
             h.init, h.init_value = N.HASH_INIT_CONST, float(init_value or 0.0)
         h.seed = int(seed) & ((1 << 64) - 1)
+        self.track_access = bool(track_access)
+        self._ls_buf = None
+        if self.track_access:
+            # P stamps per server plus one word that stays 0: the stamp of the zero row for last_seen()
+            self._ls_buf = rt.alloc_symm((P + 1) * 8)
+            self._ls_buf.tensor(torch.int64, P + 1).zero_()
+            self._clock = torch.zeros(1, dtype=torch.int64, device=rt.device)
+            self._clock_value = 0
+            self._ls_map = N.RowMap()
+            self._ls_map.num_row, self._ls_map.num_col = self.num_row, 2
+            self._ls_map.nservers, self._ls_map.rows_per_server = self.S, self.rps
+            for s in range(self.S):
+                r = rt.server_id_to_rank(s) if rt.num_servers() else rt.rank
+                h.last_seen[s] = self._ls_map.shard_ptrs[s] = self._ls_buf.ptrs[r]
+            h.clock = self._clock.data_ptr()
         self._hash = h
         self._d_hash = torch.frombuffer(bytearray(h), dtype=torch.uint8).to(rt.device)
         self.zero_row = self.S * P
@@ -912,6 +934,74 @@ class HashMatrixTable(MatrixDeviceTable):
         raise TypeError("HashMatrixTable: the whole-table add is not offered (its layout is the slot layout); "
                         "use add(keys, values)")
 
+    # ---- access clock and eviction ----------------------------------------------------------
+    def _need_tracking(self, what: str) -> None:
+        if not self.track_access:
+            raise ValueError(f"HashMatrixTable #{self.table_id}: {what} needs track_access=True")
+
+    @property
+    def clock(self) -> int:
+        """This rank's access clock: inserting lookups stamp the keys they touch with it (default 0)."""
+        self._need_tracking("the access clock")
+        return self._clock_value
+
+    @clock.setter
+    def clock(self, value: int) -> None:
+        self._need_tracking("the access clock")
+        value = int(value)
+        if not INT64_MIN <= value < -INT64_MIN:
+            raise ValueError(f"HashMatrixTable #{self.table_id}: clock {value} is not an int64")
+        self._clock.fill_(value)          # in stream order: lookups enqueued before still read the old value
+        self._clock_value = value
+
+    def last_seen(self, keys) -> torch.Tensor:
+        """int64 stamp of each key (the largest clock of an inserting lookup that touched it), -1 for a missing key."""
+        self._need_tracking("last_seen")
+        rows = self.lookup(keys, insert=False)
+        out = torch.empty(rows.numel(), 2, dtype=torch.int32, device=self.rt.device)
+        if rows.numel():
+            N.cuda_lib().mvb_get_rows(N.I32, self._ls_map, rows, rows.numel(), out, 2, N.stream_ptr())
+        return torch.where(rows == self.zero_row, -1, out.view(torch.int64).view(-1))
+
+    def evict(self, older_than: Optional[int] = None, keys=None) -> int:
+        """Collective (every rank calls it at the same point): remove the keys with ``last_seen < older_than`` (the
+        same value on every rank; needs ``track_access``), the ``keys`` given on any rank (missing keys and
+        INT64_MIN are ignored) and the slots refused at the capacity limit, and free their slots. Returns the
+        number of keys removed over all servers.
+
+        Survivors keep their values, updater state and stamp bit for bit, but may move to another slot: row ids that
+        ``lookup`` returned before are stale afterwards. A removed key reads zeros, and when it comes back it is
+        inserted like a new key (initial row from the key, zero updater state). ``PSEmbedding`` and
+        ``PSEmbeddingCollection`` translate keys on every call and keep working. Each server rebuilds its index in
+        place (csrc/cuda/hash_rows.cu) with a scratch of ``(slots // 2 + 2) * 8`` bytes."""
+        rt, lib = self.rt, N.cuda_lib()
+        if older_than is not None:
+            self._need_tracking("evict(older_than=...)")
+            older_than = int(older_than)
+            if not INT64_MIN < older_than < -INT64_MIN:
+                raise ValueError(f"HashMatrixTable #{self.table_id}: older_than {older_than} is not an int64 above "
+                                 "INT64_MIN")
+        if len(set(rt.all_gather_object(older_than))) != 1:
+            raise ValueError(f"HashMatrixTable #{self.table_id}: evict(older_than=...) differs between ranks")
+        k = self._key_tensor(keys) if keys is not None else torch.empty(0, dtype=torch.int64, device=rt.device)
+        for handle in list(self._events):         # this table's outstanding async ops
+            self.wait(handle)
+        rt.barrier()                              # every lookup and push has landed (row mailboxes drained)
+        if k.numel():
+            lib.mvb_hash_rows_mark(self._hash, k, k.numel(), N.stream_ptr())
+        rt.barrier()
+        removed = 0
+        if self.sid >= 0:
+            counts = torch.empty(2, dtype=torch.int64, device=rt.device)
+            work = torch.empty(self.slots // 2 + 2, dtype=torch.int64, device=rt.device)
+            lib.mvb_hash_rows_evict(self._hash, self.sid, INT64_MIN if older_than is None else older_than,
+                                    self._sp(0), self._sp(1), self.W if self.state_per_worker else 1,
+                                    self.state_stride, 1 if self.state_per_row else self.num_col, counts, work,
+                                    N.stream_ptr())
+            removed = int(counts[0].item())
+        rt.barrier()
+        return sum(rt.all_gather_object(removed))
+
     def num_keys(self) -> int:
         """Keys held over all servers (reads the device)."""
         out = torch.empty(1, dtype=torch.int64, device=self.rt.device)
@@ -935,12 +1025,15 @@ class HashMatrixTable(MatrixDeviceTable):
         return keys, self.get_rows(rows[order])
 
     def store(self, stream) -> None:
-        """This rank's shard and updater state (the slot layout), then its server's keys. A table of the same
-        capacity, width and number of servers loads it back with every key in its slot."""
+        """This rank's shard and updater state (the slot layout), then its server's keys, then, with
+        ``track_access``, their last-seen stamps. A table of the same capacity, width, number of servers and
+        ``track_access`` loads it back with every key in its slot. The clock is not stored."""
         super().store(stream)
         torch.cuda.current_stream().synchronize()
         stream.write(self._keys_buf.tensor(torch.int64, self.slots).cpu().numpy().tobytes())
         stream.write(self._ready_buf.tensor(torch.int32, self.slots).cpu().numpy().tobytes())
+        if self.track_access:
+            stream.write(self._ls_buf.tensor(torch.int64, self.slots).cpu().numpy().tobytes())
 
     def load(self, stream) -> None:
         import numpy as np
@@ -954,11 +1047,18 @@ class HashMatrixTable(MatrixDeviceTable):
         self._keys_buf.tensor(torch.int64, self.slots).copy_(keys)
         self._ready_buf.tensor(torch.int32, self.slots).copy_(ready)
         self._count_buf.tensor(torch.int64, 1).fill_(int((ready == 1).sum()))     # refused slots hold no row
+        if self.track_access:
+            raw = stream.read(self.slots * 8)
+            if len(raw) != self.slots * 8:
+                raise ValueError(f"HashMatrixTable #{self.table_id}: the stream holds no last-seen stamps of "
+                                 f"{self.slots} slots (stored without track_access?)")
+            ls = torch.from_numpy(np.frombuffer(raw, dtype=np.int64).copy()).to(self.rt.device)
+            self._ls_buf.tensor(torch.int64, self.slots).copy_(ls)
         torch.cuda.synchronize()
 
     def free(self) -> None:
         super().free()
-        for b in (self._keys_buf, self._ready_buf, self._count_buf):
+        for b in (self._keys_buf, self._ready_buf, self._count_buf) + ((self._ls_buf,) if self.track_access else ()):
             self.rt.release_symm(b)
 
 
