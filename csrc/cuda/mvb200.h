@@ -390,7 +390,9 @@ typedef struct MvbSgns {
   const float* scale_in;
   const float* scale_out;
   const int* neg_pool_size_ptr;  /* optional: pool size read on the DEVICE (mvb_we_prepare counts[2]);
-                                    deterministic and window kernels, overrides neg_pool_size          */
+                                    deterministic and window kernels, overrides neg_pool_size.  An input
+                                    that routes elsewhere (K >= 8, CBOW, HS, AdaGrad, register-kernel
+                                    shapes) makes mvb_sgns_train return -23 before any CUDA call       */
   /* direct mode (nservers > 1, window kernel only): train IN the row-sharded tables over NVLink -- rows
      are loaded from and reduced into their owners' shards (owner = id / rows_per_server, last server takes the
      remainder) through the peer mappings; no block cache, no maps (Hogwild across GPUs)                 */
@@ -403,7 +405,8 @@ int mvb_sgns_train(const MvbSgns* a, void* stream);
 int mvb_sgns_train_win(const MvbSgns* a, void* stream);   /* window-batched TMA pipeline      */
 int mvb_sgns_train_det(const MvbSgns* a, void* stream);   /* deterministic waves (default)    */
 int mvb_sgns_last_launches(void);   /* kernel launches of the last mvb_sgns_train call */
-int mvb_sgns_win_inflight(int dim, int negative, int window);  /* centre positions in flight */
+int mvb_sgns_win_inflight(int dim, int negative, int window);  /* centre positions in flight; 0 outside
+                                                                  1 <= negative <= 7                     */
 /* ---- key-addressed shards for application-defined tables (keys.cu): the device-side extension point ---- */
 typedef struct MvbKeyMap {
   int64_t size;                        /* keys 0 .. size-1                                   */

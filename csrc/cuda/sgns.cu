@@ -395,6 +395,7 @@ extern "C" int mvb_sgns_last_launches(void) { return mvb_sgns_launches; }
 //   skip-gram + NS, register-row shapes  otherwise the window kernel (hogwild = 1) where it covers the input,
 //                                        else the register kernel
 //   anything else                        the generic kernel
+// -23: neg_pool_size_ptr is set and the input reaches the register or generic kernel, which cannot honour it.
 extern "C" int mvb_sgns_train(const MvbSgns* h, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   mvb_sgns_launches = 1;
@@ -411,16 +412,19 @@ extern "C" int mvb_sgns_train(const MvbSgns* h, void* stream) {
     if (!declined(rc)) return rc;
     mvb_sgns_launches = 1;
   }
-  SgnsDev d = to_dev(h);
   const bool fast = sg_ns && (h->dim % 4 == 0) && (h->ld % 4 == 0) && h->dim <= 512 && h->window <= 15 &&
                     ((reinterpret_cast<uintptr_t>(h->w_in) & 15) == 0) &&
                     ((reinterpret_cast<uintptr_t>(h->w_out) & 15) == 0);
+  if (fast && h->hogwild) {
+    const int rc = mvb_sgns_train_win(h, stream);
+    if (!declined(rc)) return rc;
+  }
+  // the register and generic kernels draw from neg_pool_size entries: a pool size that only the device knows
+  // would be ignored, and in a device-prepared block neg_pool_size is the pool's capacity
+  if (h->neg_pool_size_ptr) return -23;
+  SgnsDev d = to_dev(h);
   const int sms = mvb_num_sms();
   if (fast) {
-    if (h->hogwild) {
-      const int rc = mvb_sgns_train_win(h, stream);
-      if (!declined(rc)) return rc;
-    }
     const int nvec = h->dim / 4;
     const int vpl = (nvec + 31) / 32;
     // persistent-style grid: 4 CTAs of 4 warps per SM, warps stride over positions

@@ -1108,8 +1108,10 @@ sgns_det_apply(const __grid_constant__ DetDev a) {
 }  // namespace
 
 // Centre positions the window-batched kernel keeps in flight on this device (every consumer warp owns
-// a double-buffered stage): the staleness window the hot-row step cap is computed from.
+// a double-buffered stage): the staleness window the hot-row step cap is computed from.  0 for a K the kernel does
+// not take (K >= 8 runs on the register kernel, which applies no step scales).
 extern "C" int mvb_sgns_win_inflight(int dim, int negative, int window) {
+  if (negative < 1 || negative > kKO - 1) return 0;
   int dev = 0, max_smem = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);

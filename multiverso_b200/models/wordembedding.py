@@ -328,8 +328,10 @@ class WordEmbedding:
     # ------------------------------------------------------------------ device-side block protocol
     def _dev_block_ok(self) -> bool:
         o = self.opt
+        # the pool size of a device-prepared block is only known on the device, and only the deterministic and
+        # window kernels read it there (dim <= 512, window <= 15)
         return (not o.hs and not o.cbow and not o.use_adagrad and o.negative_num >= 1 and o.negative_num <= 7
-                and self.D % 4 == 0)
+                and self.D % 4 == 0 and self.D <= 512 and o.window_size <= 15)
 
     def _block_buffers(self, slot: int, n_tokens: int) -> dict:
         """Fixed-capacity buffers of one in-flight block: nothing is allocated or sized on the host per

@@ -91,6 +91,38 @@ def _sgns_direct(lib, fn, S, rps):
     return getattr(lib, fn)(h, None)
 
 
+def _sgns_pool_size_ptr(lib, fn, case):
+    """A device pool size (neg_pool_size_ptr) on an input that routes to the register or the generic kernel,
+    which draw from neg_pool_size entries: refused with -23 before any CUDA call."""
+    h = N.Sgns()
+    h.tokens, h.n_tokens, h.dim, h.ld, h.window, h.negative, h.lr, h.vocab = DUMMY, 64, 64, 64, 5, 5, 0.025, 16
+    h.w_in = h.w_out = DUMMY
+    h.neg_pool, h.neg_pool_size, h.neg_pool_size_ptr = DUMMY, 16, DUMMY
+    if case == "k8":
+        h.negative = 8
+    elif case == "k8_hogwild":
+        h.negative, h.hogwild = 8, 1
+    elif case == "cbow":
+        h.cbow = 1
+    elif case == "adagrad":
+        h.use_adagrad, h.g2_in, h.g2_out = 1, DUMMY, DUMMY
+    elif case == "hogwild_dim_37":
+        h.dim = h.ld = 37
+        h.hogwild = 1
+    elif case == "hogwild_misaligned":
+        h.w_in, h.hogwild = DUMMY + 4, 1
+    return getattr(lib, fn)(h, None)
+
+
+POOL_PTR_CASES = ["k8", "k8_hogwild", "cbow", "adagrad", "hogwild_dim_37", "hogwild_misaligned"]
+
+
+@pytest.mark.parametrize("case", POOL_PTR_CASES)
+def test_device_pool_size_is_refused_where_the_kernel_ignores_it(case):
+    with pytest.raises(N.NativeError, match=r"^mvb_sgns_train failed rc=-23:"):
+        _sgns_pool_size_ptr(N.cuda_lib(), "mvb_sgns_train", case)
+
+
 # (entry point, caller, its map code)
 ENTRIES = [(fn, _rows, N.BAD_ROW_MAP) for fn in
            ("mvb_get_rows", "mvb_add_rows_red", "mvb_add_rows_delta", "mvb_rows_pull", "mvb_rows_push_delta")]
