@@ -13,6 +13,7 @@
 //  K9  updater_apply    -- stand-alone updater (NCCL comparator path, local adds).
 //      push_dense_red   -- one-sided async push with red.global.add.v4.f32.
 //      push_rowwise     -- one-sided async push of a row-state updater (row-wise AdaGrad).
+//      push_adam        -- one-sided async push of Adam (element moments, a step count per row).
 #include <type_traits>
 #include "mvb_common.cuh"
 
@@ -116,9 +117,60 @@ MVB_DEVINL void add_rows_fused(const DenseAddDev<T>& a, unsigned int mask, const
         if (w < a.W && ((mask >> w) & 1u)) {
           const Pack<T, VEC> g = pk_load_nc<T, VEC>(a.delta[w] + a.shard_off + i);
 #pragma unroll
-          for (int e = 0; e < VEC; ++e) U::Step(d.v[e], prep_delta<T>(g.v[e], a.scale, a.clip), f[w], sopt[w]);
+          for (int e = 0; e < VEC; ++e) {
+            T none = (T)0;
+            U::Step(d.v[e], prep_delta<T>(g.v[e], a.scale, a.clip), f[w], none, none, sopt[w]);
+          }
         }
       }
+      pk_store<T, VEC>(a.shard + i, d);
+      if (a.has_replica) push_replica<T, VEC>(a, i, d);
+    }
+  }
+}
+
+// Lanes per row of a row-stepped body without a row reduction: the power of two that covers the row's nv vectors,
+// up to a warp, so a 1-D table (one element per row) runs a thread per row and a row of 32 or more vectors a warp.
+__host__ __device__ __forceinline__ int lanes_per_row(int64_t nv) {
+  int g = 1;
+  while (g < 32 && g < nv) g <<= 1;
+  return g;
+}
+
+// The fused Add of a row-stepped updater with element slabs (adam): a group of lanes_per_row lanes per local row.
+// Every lane of the group reads the row's step count and forms each contributing worker's factors itself (one
+// step per worker, in worker order; the same values in every lane), and the group's first lane stores the count.
+// Then each vector of the row loads d, m and v once, applies the workers in worker order and stores them once.
+template <class U, typename T, int VEC>
+MVB_DEVINL void add_rows_stepped(const DenseAddDev<T>& a, unsigned int mask, const MvbAddOpt* sopt) {
+  const int64_t C = a.num_col, rows = a.shard_len / C, nv = C / VEC;
+  const int G = lanes_per_row(nv);
+  const int q = threadIdx.x & (G - 1);
+  const int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x, nthreads = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t r = tid / G; r < rows; r += nthreads / G) {
+    const int64_t base = r * C;
+    T* tp = row_state_at<U>(a.state0, a.state1, 0, a.state_stride, r);
+    T t = *tp;
+    typename U::RowF f[MVB_MAX_RANKS];
+#pragma unroll
+    for (int w = 0; w < MVB_MAX_RANKS; ++w)
+      if (w < a.W && ((mask >> w) & 1u)) f[w] = U::Factor(t, (T)0, C, sopt[w]);
+    if (q == 0) *tp = t;
+    for (int64_t v = q; v < nv; v += G) {
+      const int64_t i = base + v * VEC;
+      Pack<T, VEC> d = pk_load<T, VEC>(a.shard + i);
+      Pack<T, VEC> s0{}, s1{};
+      row_elem_load<U>(s0, s1, a.state0, a.state1, 0, a.state_stride, i);
+#pragma unroll
+      for (int w = 0; w < MVB_MAX_RANKS; ++w) {
+        if (w < a.W && ((mask >> w) & 1u)) {
+          const Pack<T, VEC> g = pk_load_nc<T, VEC>(a.delta[w] + a.shard_off + i);
+#pragma unroll
+          for (int e = 0; e < VEC; ++e)
+            U::Step(d.v[e], prep_delta<T>(g.v[e], a.scale, a.clip), f[w], s0.v[e], s1.v[e], sopt[w]);
+        }
+      }
+      row_elem_store<U>(s0, s1, a.state0, a.state1, 0, a.state_stride, i);
       pk_store<T, VEC>(a.shard + i, d);
       if (a.has_replica) push_replica<T, VEC>(a, i, d);
     }
@@ -173,8 +225,10 @@ add_dense_fused_kernel(const __grid_constant__ DenseAddDev<T> a) {
   const unsigned int mask = smask;
   if (a.fin_flag && blockIdx.x == 0 && threadIdx.x == 0 && mask == 0) *a.fin_flag = 1;
 
-  if constexpr (U::kRowState) {
+  if constexpr (U::kRowState && U::kRowSum) {
     add_rows_fused<U, T, VEC>(a, mask, sopt);
+  } else if constexpr (U::kRowState) {
+    add_rows_stepped<U, T, VEC>(a, mask, sopt);
   } else {
     const int64_t nvec = a.shard_len / VEC;
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
@@ -281,7 +335,7 @@ int launch_add(const MvbDenseAdd* h, cudaStream_t st) {
   bool vec_ok = aligned16<T>(h->shard) && (h->shard_off % VecOf<T>::N == 0);
   if constexpr (Updater<UPD, T>::kRowState)
     vec_ok = vec_ok && (h->num_col % VecOf<T>::N == 0);
-  else
+  if constexpr (!Updater<UPD, T>::kRowState || Updater<UPD, T>::kElemState)
     vec_ok = vec_ok && aligned16<T>(h->state0) && aligned16<T>(h->state1) && (h->state_stride % VecOf<T>::N == 0);
   for (int w = 0; w < MVB_MAX_RANKS; ++w) {
     a.delta[w] = w < h->nworkers ? (const T*)h->delta_ptrs[w] : nullptr;
@@ -316,9 +370,15 @@ int launch_add(const MvbDenseAdd* h, cudaStream_t st) {
   a.num_col = h->num_col;
 
   constexpr int VEC = VecOf<T>::N;
-  // a thread per element or vector, or a warp per row
-  const int blocks = Updater<UPD, T>::kRowState ? grid_for(h->shard_len / h->num_col)
-                                                : blocks_for(vec_ok ? (h->shard_len + VEC - 1) / VEC : h->shard_len, 256, 4);
+  // a thread per element or vector, a warp per row, or (adam) lanes_per_row lanes per row
+  int blocks;
+  if constexpr (Updater<UPD, T>::kRowState && !Updater<UPD, T>::kRowSum) {
+    const int64_t rows = h->shard_len / h->num_col;
+    blocks = blocks_for(rows * lanes_per_row(vec_ok ? h->num_col / VEC : h->num_col), 256, 8);
+  } else {
+    blocks = Updater<UPD, T>::kRowState ? grid_for(h->shard_len / h->num_col)
+                                        : blocks_for(vec_ok ? (h->shard_len + VEC - 1) / VEC : h->shard_len, 256, 4);
+  }
   if (vec_ok)
     add_dense_fused_kernel<UPD, T, VEC><<<blocks, 256, 0, st>>>(a);
   else
@@ -637,9 +697,68 @@ push_rowwise_kernel(const T* __restrict__ delta, const __grid_constant__ PushSta
     T h = *hp;
     const T f = row_factor<U>(part, h, hp, C, opt);
     for (int64_t j = lane; j < C; j += 32) {
-      T step = (T)0;
-      U::Step(step, g[j], f, opt);
+      T step = (T)0, none = (T)0;
+      U::Step(step, g[j], f, none, none, opt);
       red_add(data + r * C + j, step);
+    }
+  }
+}
+
+// Adam's step count of one row at its owner, counted atomically: concurrent pushes of other workers each count
+// their own step. Returns the count after this step.
+template <class U>
+MVB_DEVINL float count_step_atomic(float* tp) {
+  unsigned int* p = reinterpret_cast<unsigned int*>(tp);
+  unsigned int old = *reinterpret_cast<volatile unsigned int*>(p), seen;
+  do {
+    seen = old;
+    old = atomicCAS(p, seen, __float_as_uint(U::Count(__uint_as_float(seen))));
+  } while (old != seen);
+  return U::Count(__uint_as_float(seen));
+}
+template <class U>
+MVB_DEVINL double count_step_atomic(double* tp) {
+  unsigned long long* p = reinterpret_cast<unsigned long long*>(tp);
+  unsigned long long old = *reinterpret_cast<volatile unsigned long long*>(p), seen;
+  do {
+    seen = old;
+    old = atomicCAS(p, seen, (unsigned long long)__double_as_longlong(U::Count(__longlong_as_double((long long)seen))));
+  } while (old != seen);
+  return U::Count(__longlong_as_double((long long)seen));
+}
+
+// The one-sided push of adam: lanes_per_row lanes per row of the worker's delta. The group's first lane counts the
+// row's step at the owner atomically and passes the count to its group, which forms the factors and steps the
+// owner's m and v (read-modify-write, Hogwild across concurrent pushers, as momentum_sgd's push) and red.adds the
+// step into the owner's row.
+template <int UPD, typename T>
+__global__ void __launch_bounds__(256)
+push_adam_kernel(const T* __restrict__ delta, const __grid_constant__ PushStateDev p, int64_t C, MvbAddOpt opt,
+                 int me) {
+  using U = Updater<UPD, T>;
+  const SegCtas c = seg_ctas(p.S, me);
+  const int s = c.s;
+  const int G = lanes_per_row(C);
+  const int lane = threadIdx.x & 31, q = lane & (G - 1);
+  const unsigned gmask = G == 32 ? 0xffffffffu : ((1u << G) - 1) << (lane & ~(G - 1));
+  const int64_t tid = c.idx * blockDim.x + threadIdx.x, nthreads = c.count * blockDim.x;
+  const T* src = delta + p.off[s];
+  T* data = (T*)p.shard[s];
+  T* m = (T*)p.st0[s];
+  T* v = (T*)p.st1[s];
+  const int64_t rows = p.len[s] / C;
+  for (int64_t r = tid / G; r < rows; r += nthreads / G) {
+    T t = (T)0;
+    if (q == 0) t = count_step_atomic<U>(row_state_at<U>(m, v, 0, p.stride[s], r));
+    t = __shfl_sync(gmask, t, lane & ~(G - 1));
+    const typename U::RowF f = U::Bias(t, opt);
+    for (int64_t j = q; j < C; j += G) {
+      const int64_t i = r * C + j;
+      T step = (T)0, m0 = m[i], v0 = v[i];
+      U::Step(step, src[i], f, m0, v0, opt);
+      m[i] = m0;
+      v[i] = v0;
+      red_add(data + i, step);
     }
   }
 }
@@ -667,12 +786,48 @@ extern "C" int mvb_push_dense_rowwise(int dtype, int updater, const void* delta,
   return with_dtype<float, double>(dtype, [&](auto t) {
     using T = typename decltype(t)::type;
     return with_updater<T>(updater, [&](auto u) {
-      if constexpr (!Updater<decltype(u)::value, T>::kRowState) {
+      if constexpr (!Updater<decltype(u)::value, T>::kRowState || Updater<decltype(u)::value, T>::kElemState) {
         return -2;
       } else {
         if (!geometry_ok) return (int)MVB_BAD_ROW_MAP;
         push_rowwise_kernel<decltype(u)::value, T><<<seg_grid(grid_for(rows), nservers), 256, 0,
                                                      (cudaStream_t)stream>>>((const T*)delta, p, num_col, *opt, me);
+        MVB_CUDA_CHECK(cudaGetLastError());
+        return 0;
+      }
+    });
+  });
+}
+
+extern "C" int mvb_push_dense_adam(int dtype, int updater, const void* delta, int nservers, void* const* shard_ptrs,
+                                   void* const* state0_ptrs, void* const* state1_ptrs, const int64_t* shard_offs,
+                                   const int64_t* shard_lens, const int64_t* state_strides, int64_t num_col,
+                                   const MvbAddOpt* opt, int me, void* stream) {
+  if (nservers < 1 || nservers > MVB_MAX_RANKS) return -3;
+  PushStateDev p{};
+  p.S = nservers;
+  int64_t rows = 0;
+  bool geometry_ok = num_col >= 1;
+  for (int s = 0; s < nservers && geometry_ok; ++s) {
+    p.shard[s] = shard_ptrs[s];
+    p.st0[s] = state0_ptrs[s];
+    p.st1[s] = state1_ptrs[s];
+    p.off[s] = shard_offs[s];
+    p.len[s] = shard_lens[s];
+    p.stride[s] = state_strides[s];
+    geometry_ok = shard_lens[s] % num_col == 0 && state_strides[s] >= shard_lens[s];
+    rows += shard_lens[s] / num_col;
+  }
+  return with_dtype<float, double>(dtype, [&](auto t) {
+    using T = typename decltype(t)::type;
+    return with_updater<T>(updater, [&](auto u) {
+      if constexpr (!Updater<decltype(u)::value, T>::kElemState) {
+        return -2;
+      } else {
+        if (!geometry_ok) return (int)MVB_BAD_ROW_MAP;
+        push_adam_kernel<decltype(u)::value, T><<<seg_grid(blocks_for(rows * lanes_per_row(num_col), 256, 8),
+                                                           nservers), 256, 0, (cudaStream_t)stream>>>(
+            (const T*)delta, p, num_col, *opt, me);
         MVB_CUDA_CHECK(cudaGetLastError());
         return 0;
       }
@@ -720,7 +875,8 @@ extern "C" int mvb_add_dense_fused(const MvbDenseAdd* a, void* stream) {
     using T = typename decltype(t)::type;
     return with_updater<T>(a->updater, [&](auto u) {
       if constexpr (Updater<decltype(u)::value, T>::kRowState) {
-        if (a->num_col < 1 || a->shard_len % a->num_col != 0 || a->state_stride < a->shard_len / a->num_col)
+        if (a->num_col < 1 || a->shard_len % a->num_col != 0 ||
+            !row_state_fits<Updater<decltype(u)::value, T>>(a->state_stride, a->shard_len, a->num_col))
           return (int)MVB_BAD_ROW_MAP;
       }
       return launch_add<decltype(u)::value, T>(a, (cudaStream_t)stream);

@@ -245,6 +245,8 @@ struct EvictArgs {
   long long older_than;     // INT64_MIN: no age rule
   int64_t* counts;          // {live keys removed, survivors moved}
   long long* work;          // {clusters, first victim, cluster starts...}
+  float* st2;               // a state slab with its own row length (adam's step counts), or nullptr
+  int64_t srow2;
 };
 
 MVB_DEVINL void copy_f32(float* dst, const float* src, int64_t n, int lane) {
@@ -267,6 +269,7 @@ MVB_DEVINL void clear_slot(const EvictArgs& e, int64_t j, int lane) {
   for (int a = 0; a < 2; ++a)
     if (e.st[a])
       for (int k = 0; k < e.n_slabs; ++k) zero_f32(e.st[a] + k * e.stride + j * e.srow, e.srow, lane);
+  if (e.st2) zero_f32(e.st2 + j * e.srow2, e.srow2, lane);
   if (lane == 0) {
     e.keys[j] = kEmpty;
     e.ready[j] = 0;
@@ -284,6 +287,7 @@ MVB_DEVINL void move_slot(const EvictArgs& e, int64_t to, int64_t from, int lane
         float* slab = e.st[a] + k * e.stride;
         copy_f32(slab + to * e.srow, slab + from * e.srow, e.srow, lane);
       }
+  if (e.st2) copy_f32(e.st2 + to * e.srow2, e.st2 + from * e.srow2, e.srow2, lane);
   if (lane == 0) {
     e.keys[to] = e.keys[from];
     e.ready[to] = e.ready[from];
@@ -368,7 +372,8 @@ __global__ void hash_evict_unwrap_kernel(const EvictArgs e) {
 // still as pass 1 saw them (moves only go backwards), so the walk ends where the old cluster did. Until the first
 // victim every survivor stays, so the walk skips 32 slots per ballot; after it, each survivor probes from its home
 // with ballots over 32 slots for the first empty slot before its own and moves there.
-__global__ void __launch_bounds__(256) hash_evict_walk_kernel(const EvictArgs e) {
+// (256, 1): without the minimum the compiler holds the walk to 64 registers and spills
+__global__ void __launch_bounds__(256, 1) hash_evict_walk_kernel(const EvictArgs e) {
   const int lane = threadIdx.x & 31;
   const uint64_t mask = (uint64_t)e.P - 1;
   long long moved = 0;
@@ -475,6 +480,14 @@ extern "C" int mvb_hash_rows_mark(const MvbHashRows* h, const int64_t* keys, int
 extern "C" int mvb_hash_rows_evict(const MvbHashRows* h, int server, int64_t older_than, void* state0, void* state1,
                                    int n_slabs, int64_t state_stride, int64_t state_row, int64_t* counts,
                                    int64_t* work, void* stream) {
+  return mvb_hash_rows_evict_ex(h, server, older_than, state0, state1, n_slabs, state_stride, state_row, counts, work,
+                                stream, nullptr, 0);
+}
+
+extern "C" int mvb_hash_rows_evict_ex(const MvbHashRows* h, int server, int64_t older_than, void* state0,
+                                      void* state1, int n_slabs, int64_t state_stride, int64_t state_row,
+                                      int64_t* counts, int64_t* work, void* stream, void* state2,
+                                      int64_t state2_row) {
   if (int rc = check_index(h)) return rc;
   if (server < 0 || server >= h->nservers) return -1;
   const MvbRowMap& m = h->map;
@@ -484,10 +497,12 @@ extern "C" int mvb_hash_rows_evict(const MvbHashRows* h, int server, int64_t old
   if (older_than != INT64_MIN && !h->last_seen[server]) return -5;
   if ((state0 || state1) && (n_slabs < 1 || state_row < 1 || (n_slabs > 1 && state_stride < h->slots * state_row)))
     return -6;
+  if (state2 && state2_row < 1) return -6;
   cudaStream_t st = (cudaStream_t)stream;
   const EvictArgs e{(long long*)h->keys[server], (uint32_t*)h->ready[server], (long long*)h->last_seen[server],
                     (float*)m.shard_ptrs[server], m.num_col, {(float*)state0, (float*)state1}, n_slabs,
-                    state_stride, state_row, h->slots, (long long)older_than, counts, (long long*)work};
+                    state_stride, state_row, h->slots, (long long)older_than, counts, (long long*)work,
+                    (float*)state2, state2_row};
   MVB_CUDA_CHECK(cudaMemsetAsync(counts, 0, 16, st));
   MVB_CUDA_CHECK(cudaMemsetAsync(work, 0, 8, st));              // no cluster yet
   MVB_CUDA_CHECK(cudaMemsetAsync(work + 1, 0xff, 8, st));       // no victim yet

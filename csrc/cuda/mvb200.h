@@ -19,11 +19,20 @@ extern "C" {
 
 /* element types */
 enum { MVB_F32 = 0, MVB_F64 = 1, MVB_I32 = 2, MVB_I64 = 3, MVB_I8 = 4 };
-/* updaters (reference: -updater_type default|sgd|momentum_sgd|adagrad|dcasgd|dcasgda, plus rowwise_adagrad).
+/* updaters (reference: -updater_type default|sgd|momentum_sgd|adagrad|dcasgd|dcasgda, plus rowwise_adagrad and
+ * adam).
  * rowwise_adagrad is AdaGrad with one accumulator per (worker, table row): h += mean_j (g_j / lr)^2 over the
  * row's C columns, d_j -= rho * rsqrt(h + 1e-6) * g_j / lr. Its state slab is indexed by local row, not by
  * element, so the entry points that update whole rows take the row length (MvbDenseAdd.num_col,
  * mvb_push_dense_rowwise); mvb_updater_apply and mvb_push_dense_stateful have none and return -2 for it.
+ * adam is Adam with per-element moments m, v and one step count t per table row, all shared by every worker. One
+ * worker's delta row is one step: t += 1 (it stops at 2^24), then per element g = delta / lr,
+ * m = b1 m + (1 - b1) g, v = b2 v + (1 - b2) g^2, d -= rho / (1 - b1^t) * m / (sqrt(v) / sqrt(1 - b2^t) + eps),
+ * with b1 = momentum, b2 = 0.999 and eps = 1e-8 (torch.optim.Adam's step). Its state geometry: m is state0 and v
+ * state1, indexed by element (state_stride >= the shard's elements), and t of local row r is state1[state_stride
+ * + r], after v's slab; a shard of R rows x C needs 2 round4(R C) + round4(R) elements. Like rowwise_adagrad it
+ * needs the row length (mvb_push_dense_adam for the one-sided push) and mvb_updater_apply and
+ * mvb_push_dense_stateful return -2 for it. Integer tables keep the plain add.
  * Code 6 is left unassigned: it is the "unknown updater" of the dispatch tests. */
 enum {
   MVB_UPD_DEFAULT = 0,
@@ -32,7 +41,8 @@ enum {
   MVB_UPD_ADAGRAD = 3,
   MVB_UPD_DCASGD = 4,
   MVB_UPD_DCASGDA = 5,
-  MVB_UPD_ROWWISE_ADAGRAD = 7
+  MVB_UPD_ROWWISE_ADAGRAD = 7,
+  MVB_UPD_ADAM = 8
 };
 
 /* Same 20-byte layout as the reference AddOption (updater.h:13-69):
@@ -129,16 +139,17 @@ typedef struct MvbDenseAdd {
      NULL boxes: opts[] are used as given (single process / identical options).                       */
   void* opt_box[MVB_MAX_RANKS];
   int my_worker;          /* this rank's worker id (-1: not a worker)  */
-  /* row length of the table; read by row-state updaters only (rowwise_adagrad), which need num_col >= 1,
-     shard_len % num_col == 0 and state_stride >= shard_len / num_col, else MVB_BAD_ROW_MAP before any
-     CUDA call. Their state slabs hold one element per local row. */
+  /* row length of the table; read by row-state updaters only (rowwise_adagrad, adam), which need num_col >= 1,
+     shard_len % num_col == 0 and state_stride >= shard_len / num_col (rowwise_adagrad: its slabs hold one
+     element per local row) or state_stride >= shard_len (adam: element slabs, then the step counts), else
+     MVB_BAD_ROW_MAP before any CUDA call. */
   int64_t num_col;
 } MvbDenseAdd;
 int mvb_add_dense_fused(const MvbDenseAdd* a, void* stream);
 
 /* Local (single-source) updater apply: the stand-alone K9 kernel used by the
  * NCCL comparator path and by row-wise / whole adds with one worker. Element-wise updaters only
- * (-2 for rowwise_adagrad, which needs rows). */
+ * (-2 for rowwise_adagrad and adam, which need rows). */
 int mvb_updater_apply(int dtype, int updater, void* data, const void* delta, void* state0,
                       void* state1, int64_t n, const MvbAddOpt* opt, float scale, void* stream);
 
@@ -186,6 +197,17 @@ int mvb_push_dense_rowwise(int dtype, int updater, const void* delta, int nserve
                            void* const* state_ptrs, const int64_t* shard_offs, const int64_t* shard_lens,
                            const int64_t* state_strides, int64_t num_col, const MvbAddOpt* opt, int me,
                            void* stream);
+/* The same push for adam: per row of num_col elements, the owner's step count of the row (state1_ptrs[s] +
+ * state_strides[s] + local row) is counted atomically, so concurrent pushers each count their step; the owner's
+ * m (state0_ptrs[s]) and v (state1_ptrs[s]) elements are read-modify-written (Hogwild across concurrent pushers,
+ * exact for one) and the step is red.added into the owner's row. A row of C elements runs on the power of two
+ * lanes >= C up to a warp. Returns -3 for nservers outside [1, MVB_MAX_RANKS], -1 for element types other than
+ * f32 / f64, -2 for updaters other than adam and MVB_BAD_ROW_MAP when num_col < 1, a shard_lens[s] is not a
+ * multiple of num_col or a state_strides[s] is below shard_lens[s]; all before any CUDA call. */
+int mvb_push_dense_adam(int dtype, int updater, const void* delta, int nservers, void* const* shard_ptrs,
+                        void* const* state0_ptrs, void* const* state1_ptrs, const int64_t* shard_offs,
+                        const int64_t* shard_lens, const int64_t* state_strides, int64_t num_col,
+                        const MvbAddOpt* opt, int me, void* stream);
 
 /* ---- row-sparse Get / Add (K3, K4, K10) ------------------------------------ */
 /* Server min(r / rows_per_server, nservers - 1) holds row r, at local index r - server * rows_per_server.
@@ -213,7 +235,9 @@ int mvb_add_rows_delta(const MvbRowMap* m, const int64_t* row_ids, int64_t k, co
  * ids/vals may be another rank's (peer-mapped) staging.  A repeated row is updated once per
  * occurrence, in list order, when its occurrences are adjacent (sort the request stably by id);
  * occurrences that are not adjacent race. rowwise_adagrad indexes its state slab by local row
- * (state_stride >= row_hi - row_lo). */
+ * (state_stride >= row_hi - row_lo). adam indexes m and v by element and keeps the step counts after v's slab
+ * (state_stride >= (row_hi - row_lo) * num_col, else MVB_BAD_ROW_MAP before any CUDA call); a repeated row
+ * counts one step per occurrence. */
 int mvb_add_rows_owner(int dtype, int updater, void* shard, void* state0, void* state1,
                        int64_t row_lo, int64_t row_hi, int64_t num_col, int64_t state_stride,
                        const int64_t* row_ids, int64_t k, const void* vals, int64_t vals_ld,
@@ -318,11 +342,18 @@ int mvb_hash_rows_dump(const MvbHashRows* h, int server, int64_t* out_keys, int6
  * [0, nservers), -4 for slots not a power of two in [2, 2^31], MVB_BAD_ROW_MAP for a map that fails the row map
  * rule, disagrees with nservers, has rows_per_server < slots or num_col not a positive multiple of 4, -5 for
  * older_than != INT64_MIN without last_seen[server], -6 for a state description with n_slabs < 1, state_row < 1
- * or n_slabs > 1 and state_stride < slots * state_row. mvb_hash_rows_mark returns -3 and -4 alike. */
+ * or n_slabs > 1 and state_stride < slots * state_row. mvb_hash_rows_mark returns -3 and -4 alike.
+ * mvb_hash_rows_evict_ex also moves and clears a third state slab with its own row length: slot j owns elements
+ * [j state2_row, (j + 1) state2_row) of state2 (adam's step counts: state2 = v's array + state_stride,
+ * state2_row = 1). It returns -6 for state2 != NULL with state2_row < 1; with state2 NULL it is
+ * mvb_hash_rows_evict. */
 int mvb_hash_rows_mark(const MvbHashRows* h, const int64_t* keys, int64_t n, void* stream);
 int mvb_hash_rows_evict(const MvbHashRows* h, int server, int64_t older_than, void* state0, void* state1,
                         int n_slabs, int64_t state_stride, int64_t state_row, int64_t* counts, int64_t* work,
                         void* stream);
+int mvb_hash_rows_evict_ex(const MvbHashRows* h, int server, int64_t older_than, void* state0, void* state1,
+                           int n_slabs, int64_t state_stride, int64_t state_row, int64_t* counts, int64_t* work,
+                           void* stream, void* state2, int64_t state2_row);
 
 /* ---- all-reduce (K6) --------------------------------------------------------- */
 /* One-shot P2P: every rank reads all peers' symmetric buffers and reduces locally
@@ -453,7 +484,8 @@ int mvb_rowbox_push_vals(const MvbRowBox* b, const int* ids, const int* n_ptr, i
                          const float* vals, int64_t ld, float scale, uint64_t epoch, const MvbAddOpt* opt,
                          int ctas_per_sm, void* stream);
 int mvb_rowbox_poll(const MvbRowBox* b, int src, int wait, void* stream);
-/* state_stride: elements per source slab; rowwise_adagrad indexes its slab by local row */
+/* state_stride: elements per source slab; rowwise_adagrad indexes its slab by local row; adam's m and v are
+ * element slabs, its step counts follow v's slab (st1 + state_stride + local row) */
 int mvb_rowbox_apply(const MvbRowBox* b, int updater, float* shard, float* st0, float* st1,
                      int64_t state_stride, int64_t row_lo, int src, int ctas_per_sm, void* stream);
 

@@ -198,6 +198,7 @@ MVB_DEVINL void red_add(int* p, int v) { red_add_s32(p, v); }
 //   dcasgd   : s0 = shadow copy                (per worker)
 //   dcasgda  : s0 = shadow copy, s1 = mean sq  (per worker)
 //   rowwise_adagrad : s0 = G^2 history of a ROW (per worker, one element per local row)
+//   adam     : s0 = m, s1 = v (shared), and a step count t per ROW after v's slab (see row_state_at)
 // Semantics follow the reference accessors (Q1/Q3); AdaGrad implements the
 // *intended* rule (Q2: the reference copies the history by value and subtracts
 // squares, so its history never persists).
@@ -210,6 +211,7 @@ struct Updater<MVB_UPD_DEFAULT, T> {
   static constexpr int kStates = 0;
   static constexpr bool kPerWorker = false;
   static constexpr bool kRowState = false;
+  static constexpr bool kRowSum = false, kElemState = false;
   MVB_DEVINL static void Apply(T& d, T g, T&, T&, const MvbAddOpt&) { d += g; }
 };
 template <typename T>
@@ -217,6 +219,7 @@ struct Updater<MVB_UPD_SGD, T> {
   static constexpr int kStates = 0;
   static constexpr bool kPerWorker = false;
   static constexpr bool kRowState = false;
+  static constexpr bool kRowSum = false, kElemState = false;
   MVB_DEVINL static void Apply(T& d, T g, T&, T&, const MvbAddOpt&) { d -= g; }
 };
 template <typename T>
@@ -224,6 +227,7 @@ struct Updater<MVB_UPD_MOMENTUM, T> {
   static constexpr int kStates = 1;
   static constexpr bool kPerWorker = false;
   static constexpr bool kRowState = false;
+  static constexpr bool kRowSum = false, kElemState = false;
   MVB_DEVINL static void Apply(T& d, T g, T& s0, T&, const MvbAddOpt& o) {
     s0 = (T)o.momentum * s0 + (T)(1.0f - o.momentum) * g;
     d -= s0;
@@ -234,6 +238,7 @@ struct Updater<MVB_UPD_ADAGRAD, T> {
   static constexpr int kStates = 1;
   static constexpr bool kPerWorker = true;
   static constexpr bool kRowState = false;
+  static constexpr bool kRowSum = false, kElemState = false;
   MVB_DEVINL static void Apply(T& d, T g, T& s0, T&, const MvbAddOpt& o) {
     T gn = g / (T)o.lr;
     s0 += gn * gn;
@@ -247,6 +252,7 @@ struct Updater<MVB_UPD_DCASGD, T> {
   static constexpr int kStates = 1;
   static constexpr bool kPerWorker = true;
   static constexpr bool kRowState = false;
+  static constexpr bool kRowSum = false, kElemState = false;
   MVB_DEVINL static void Apply(T& d, T g, T& s0, T&, const MvbAddOpt& o) {
     T gn = g / (T)o.lr;
     d -= (T)o.lr * (gn + (T)o.lambda * gn * gn * (d - s0));
@@ -258,6 +264,7 @@ struct Updater<MVB_UPD_DCASGDA, T> {
   static constexpr int kStates = 2;
   static constexpr bool kPerWorker = true;
   static constexpr bool kRowState = false;
+  static constexpr bool kRowSum = false, kElemState = false;
   MVB_DEVINL static void Apply(T& d, T g, T& s0, T& s1, const MvbAddOpt& o) {
     T gn = g / (T)o.lr;
     s1 = (T)o.momentum * s1 + (T)(1.0f - o.momentum) * gn * gn;
@@ -276,6 +283,9 @@ struct Updater<MVB_UPD_ROWWISE_ADAGRAD, T> {
   static constexpr int kStates = 1;
   static constexpr bool kPerWorker = true;
   static constexpr bool kRowState = true;
+  static constexpr bool kRowSum = true;      // the row step reduces the row (U::Square)
+  static constexpr bool kElemState = false;  // no per-element slabs besides the row state
+  using RowF = T;
   MVB_DEVINL static T Square(T g, const MvbAddOpt& o) {
     const T gn = g / (T)o.lr;
     return gn * gn;
@@ -285,7 +295,48 @@ struct Updater<MVB_UPD_ROWWISE_ADAGRAD, T> {
     h += sum / (T)C;
     return (T)o.rho * Updater<MVB_UPD_ADAGRAD, T>::rsqrt_t(h + (T)1e-6);
   }
-  MVB_DEVINL static void Step(T& d, T g, T f, const MvbAddOpt& o) { d -= f * (g / (T)o.lr); }
+  MVB_DEVINL static void Step(T& d, T g, T f, T&, T&, const MvbAddOpt& o) { d -= f * (g / (T)o.lr); }
+  MVB_DEVINL static T Shfl(T f, int src) { return __shfl_sync(0xffffffffu, f, src); }
+};
+
+// Adam (kRowState with element slabs): m (s0) and v (s1) per element and a step count t per row, all shared by
+// every worker. One worker's delta row is one step: t += 1 (it stops at 2^24, where both bias factors are 1), then
+// per element  g = delta/lr,  m = b1 m + (1 - b1) g,  v = b2 v + (1 - b2) g^2,
+// d -= rho / (1 - b1^t) * m / (sqrt(v) / sqrt(1 - b2^t) + eps)  -- torch.optim.Adam's step in its operation order,
+// with b1 = o.momentum, b2 = 0.999 and eps = 1e-8. The bias factors are formed once per row in fp64 (Factor), the
+// moments and the apply per element (Step). No row reduction.
+template <typename T>
+struct Updater<MVB_UPD_ADAM, T> {
+  static constexpr int kStates = 2;
+  static constexpr bool kPerWorker = false;
+  static constexpr bool kRowState = true;
+  static constexpr bool kRowSum = false;
+  static constexpr bool kElemState = true;
+  struct RowF {
+    T step, bc2;  // rho / (1 - b1^t), sqrt(1 - b2^t)
+  };
+  MVB_DEVINL static T Square(T, const MvbAddOpt&) { return (T)0; }
+  MVB_DEVINL static T Count(T t) { return t < (T)16777216 ? t + (T)1 : t; }
+  // the row's factors at step count t
+  MVB_DEVINL static RowF Bias(T t, const MvbAddOpt& o) {
+    const double td = (double)t;
+    const double bc1 = 1.0 - pow((double)o.momentum, td), bc2 = 1.0 - pow(0.999, td);
+    return {(T)((double)o.rho / bc1), (T)sqrt(bc2)};
+  }
+  // t counts the step; returns the step's factors
+  MVB_DEVINL static RowF Factor(T& t, T, int64_t, const MvbAddOpt& o) {
+    t = Count(t);
+    return Bias(t, o);
+  }
+  MVB_DEVINL static void Step(T& d, T g, const RowF& f, T& m, T& v, const MvbAddOpt& o) {
+    const T gn = g / (T)o.lr;
+    m = (T)o.momentum * m + (T)(1.0f - o.momentum) * gn;
+    v = (T)0.999 * v + (T)(1.0 - 0.999) * gn * gn;
+    d -= f.step * (m / (sqrt(v) / f.bc2 + (T)1e-8));
+  }
+  MVB_DEVINL static RowF Shfl(const RowF& f, int src) {
+    return {__shfl_sync(0xffffffffu, f.step, src), __shfl_sync(0xffffffffu, f.bc2, src)};
+  }
 };
 
 // Updater state of one element (T, or a float4 over float4 slabs) or of a pack of elements (Pack<T, VEC>). A state array holds
@@ -314,6 +365,29 @@ template <class U, typename V, typename T>
 MVB_DEVINL void state_store(const V& s0, const V& s1, T* st0, T* st1, int w, int64_t stride, int64_t i) {
   if constexpr (U::kStates >= 1) state_st(st0 + state_at<U>(w, stride, i), s0);
   if constexpr (U::kStates >= 2) state_st(st1 + state_at<U>(w, stride, i), s1);
+}
+
+// The state of a row-state updater (kRowState). Its row value (rowwise_adagrad's accumulator, adam's step count)
+// of local row r: rowwise_adagrad keeps it in worker w's slab of st0, indexed by row; adam after v's element slab,
+// at st1 + stride + r. Its element slabs (adam's m and v) follow state_load's layout; rowwise_adagrad has none, so
+// row_elem_load / row_elem_store touch no memory for it.
+template <class U, typename T>
+MVB_DEVINL T* row_state_at(T* st0, T* st1, int w, int64_t stride, int64_t r) {
+  if constexpr (U::kElemState) return st1 + stride + r;
+  else return st0 + state_at<U>(w, stride, r);
+}
+template <class U, typename V, typename T>
+MVB_DEVINL void row_elem_load(V& s0, V& s1, const T* st0, const T* st1, int w, int64_t stride, int64_t i) {
+  if constexpr (U::kElemState) state_load<U>(s0, s1, st0, st1, w, stride, i);
+}
+template <class U, typename V, typename T>
+MVB_DEVINL void row_elem_store(const V& s0, const V& s1, T* st0, T* st1, int w, int64_t stride, int64_t i) {
+  if constexpr (U::kElemState) state_store<U>(s0, s1, st0, st1, w, stride, i);
+}
+// the smallest state stride of a row-state updater for a shard of len elements in rows of C
+template <class U>
+static inline bool row_state_fits(int64_t stride, int64_t len, int64_t C) {
+  return stride >= (U::kElemState ? len : len / C);
 }
 
 // 64-bit finaliser of MurmurHash3: the counter-based RNG of the on-device samplers (a draw is a pure
@@ -382,10 +456,13 @@ MVB_DEVINL double warp_sum(double v) {
 // A row-state updater's step on one row, for the whole warp: `part` is the lane's share of the row's sum of
 // U::Square, h the worker's accumulator of the row (the same value in every lane) and hp where it lives. The
 // butterfly sum gives every lane the same total, so every lane updates h alike and returns the same factor;
-// lane 0 stores h. Call it with the whole warp.
+// lane 0 stores h. Call it with the whole warp. An updater without a row sum (adam: h is the step count) ignores
+// `part`.
 template <class U, typename T>
-MVB_DEVINL T row_factor(T part, T& h, T* hp, int64_t C, const MvbAddOpt& o) {
-  const T f = U::Factor(h, warp_sum(part), C, o);
+MVB_DEVINL typename U::RowF row_factor(T part, T& h, T* hp, int64_t C, const MvbAddOpt& o) {
+  T sum = part;
+  if constexpr (U::kRowSum) sum = warp_sum(part);
+  const typename U::RowF f = U::Factor(h, sum, C, o);
   if ((threadIdx.x & 31) == 0) *hp = h;
   return f;
 }
@@ -508,6 +585,7 @@ static inline int with_updater(int upd, F&& f) {
       case MVB_UPD_DCASGD: return f(integral_constant<int, MVB_UPD_DCASGD>{});
       case MVB_UPD_DCASGDA: return f(integral_constant<int, MVB_UPD_DCASGDA>{});
       case MVB_UPD_ROWWISE_ADAGRAD: return f(integral_constant<int, MVB_UPD_ROWWISE_ADAGRAD>{});
+      case MVB_UPD_ADAM: return f(integral_constant<int, MVB_UPD_ADAM>{});
     }
     return -2;
   }

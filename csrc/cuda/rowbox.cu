@@ -230,33 +230,41 @@ rowbox_apply_kernel(const __grid_constant__ BoxDev b, const __grid_constant__ Ap
   const int lane = threadIdx.x & 31;
   const int nvec = a.row_floats >> 2;
   if constexpr (U::kRowState) {
-    // a row-state updater: the row's square sum, then its factor and the source's accumulator of the row (indexed
-    // by local row), then the apply
+    // a row-state updater: the row's square sum (rowwise_adagrad), then its factor and the row state (the source's
+    // accumulator, or adam's step count; see row_state_at), then the apply with the element state (adam's m, v)
     for (int64_t i = warp_id(); i < count; i += num_warps()) {
       const int64_t r = (int64_t)__ldcg(ids + i);
       const int64_t base = (r - a.row_lo) * (int64_t)a.row_floats;
       if (r < a.row_lo || base < 0) continue;
       const float4* src = reinterpret_cast<const float4*>(vals + (size_t)i * b.ld_bytes);
       float part = 0.f;
-      for (int v = lane; v < nvec; v += 32) {
-        const float4 g = __ldcg(src + v);
-        part += U::Square(g.x, opt);
-        part += U::Square(g.y, opt);
-        part += U::Square(g.z, opt);
-        part += U::Square(g.w, opt);
+      if constexpr (U::kRowSum) {
+        for (int v = lane; v < nvec; v += 32) {
+          const float4 g = __ldcg(src + v);
+          part += U::Square(g.x, opt);
+          part += U::Square(g.y, opt);
+          part += U::Square(g.z, opt);
+          part += U::Square(g.w, opt);
+        }
       }
-      float* hp = a.st0 + state_at<U>(a.src, a.state_stride, r - a.row_lo);
+      float* hp = row_state_at<U>(a.st0, a.st1, a.src, a.state_stride, r - a.row_lo);
       float h = *hp;
-      const float f = row_factor<U>(part, h, hp, a.row_floats, opt);
+      const typename U::RowF f = row_factor<U>(part, h, hp, a.row_floats, opt);
+      float4* st0 = reinterpret_cast<float4*>(a.st0 + base);
+      float4* st1 = reinterpret_cast<float4*>(a.st1 + base);
+      const int64_t stride4 = a.state_stride >> 2;
       for (int v = lane; v < nvec; v += 32) {
         const float4 g = __ldcg(src + v);
         float4* dp = reinterpret_cast<float4*>(a.shard + base) + v;
         float4 d = *dp;
-        U::Step(d.x, g.x, f, opt);
-        U::Step(d.y, g.y, f, opt);
-        U::Step(d.z, g.z, f, opt);
-        U::Step(d.w, g.w, f, opt);
+        float4 s0 = make_float4(0, 0, 0, 0), s1 = make_float4(0, 0, 0, 0);
+        row_elem_load<U>(s0, s1, st0, st1, a.src, stride4, v);
+        U::Step(d.x, g.x, f, s0.x, s1.x, opt);
+        U::Step(d.y, g.y, f, s0.y, s1.y, opt);
+        U::Step(d.z, g.z, f, s0.z, s1.z, opt);
+        U::Step(d.w, g.w, f, s0.w, s1.w, opt);
         *dp = d;
+        row_elem_store<U>(s0, s1, st0, st1, a.src, stride4, v);
       }
     }
   } else {

@@ -157,28 +157,34 @@ add_rows_owner_kernel(T* __restrict__ shard, T* __restrict__ st0, T* __restrict_
     while (end < k && ids[end] == r) ++end;
     const int64_t base = (r - row_lo) * num_col;
     if constexpr (U::kRowState) {
-      // the row's accumulator (indexed by local row) stays in registers over the run; the run goes in chunks of
-      // up to 32 occurrences: first their factors in list order (occurrence j sees h after the occurrences
-      // before it; lane j keeps the chunk's j-th factor), then one pass over the row applies the chunk
-      T* hp = st0 + state_at<U>(opt.worker_id, state_stride, r - row_lo);
+      // the row's state (rowwise_adagrad's accumulator, adam's step count; see row_state_at) stays in registers
+      // over the run; the run goes in chunks of up to 32 occurrences: first their factors in list order (occurrence
+      // j sees the row state after the occurrences before it; lane j keeps the chunk's j-th factor), then one pass
+      // over the row applies the chunk, with the element state (adam's m, v) in registers over the chunk
+      T* hp = row_state_at<U>(st0, st1, opt.worker_id, state_stride, r - row_lo);
       T h = *hp;
       for (int64_t j0 = i; j0 < end; j0 += 32) {
         const int n = (int)(end - j0 < 32 ? end - j0 : 32);
-        T mine = (T)0;
+        typename U::RowF mine{};
         for (int j = 0; j < n; ++j) {
           T part = (T)0;
-          for (int64_t c = lane; c < num_col; c += 32) part += U::Square(vals[(j0 + j) * vals_ld + c], opt);
-          const T f = row_factor<U>(part, h, hp, num_col, opt);
+          if constexpr (U::kRowSum)
+            for (int64_t c = lane; c < num_col; c += 32) part += U::Square(vals[(j0 + j) * vals_ld + c], opt);
+          const typename U::RowF f = row_factor<U>(part, h, hp, num_col, opt);
           if (lane == j) mine = f;
         }
         for (int64_t c0 = 0; c0 < num_col; c0 += 32) {
           const int64_t c = c0 + lane;
-          T d = c < num_col ? shard[base + c] : (T)0;
+          T d = c < num_col ? shard[base + c] : (T)0, s0 = (T)0, s1 = (T)0;
+          if (c < num_col) row_elem_load<U>(s0, s1, st0, st1, opt.worker_id, state_stride, base + c);
           for (int j = 0; j < n; ++j) {
-            const T f = __shfl_sync(0xffffffffu, mine, j);
-            if (c < num_col) U::Step(d, vals[(j0 + j) * vals_ld + c], f, opt);
+            const typename U::RowF f = U::Shfl(mine, j);
+            if (c < num_col) U::Step(d, vals[(j0 + j) * vals_ld + c], f, s0, s1, opt);
           }
-          if (c < num_col) shard[base + c] = d;
+          if (c < num_col) {
+            row_elem_store<U>(s0, s1, st0, st1, opt.worker_id, state_stride, base + c);
+            shard[base + c] = d;
+          }
         }
       }
     } else {
@@ -343,6 +349,10 @@ extern "C" int mvb_add_rows_owner(int dtype, int updater, void* shard, void* sta
   return with_dtype<float, double, int>(dtype, [&](auto t) {
     using T = typename decltype(t)::type;
     return with_updater<T>(updater, [&](auto u) {
+      if constexpr (Updater<decltype(u)::value, T>::kElemState) {
+        // adam: m and v are element slabs, the step counts follow v's slab
+        if (num_col < 1 || state_stride < (row_hi - row_lo) * num_col) return (int)MVB_BAD_ROW_MAP;
+      }
       add_rows_owner_kernel<decltype(u)::value, T><<<grid_for(k), 256, 0, (cudaStream_t)stream>>>(
           (T*)shard, (T*)state0, (T*)state1, row_lo, row_hi, num_col, state_stride, row_ids, k, (const T*)vals,
           vals_ld, *opt);

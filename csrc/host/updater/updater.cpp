@@ -3,6 +3,7 @@
 #include "multiverso/updater/updater.h"
 #include <string>
 #include "multiverso/updater/adagrad_updater.h"
+#include "multiverso/updater/adam_updater.h"
 #include "multiverso/updater/dcasgd_updater.h"
 #include "multiverso/updater/dcasgda_updater.h"
 #include "multiverso/updater/momentum_updater.h"
@@ -48,6 +49,7 @@ Updater<T>* Updater<T>::GetUpdater(size_t size, size_t num_col) {
   if (type == "dcasgd") return new DCASGDUpdater<T>(size);
   if (type == "dcasgda") return new DCASGDAUpdater<T>(size);
   if (type == "rowwise_adagrad") return new RowwiseAdaGradUpdater<T>(size, num_col);
+  if (type == "adam") return new AdamUpdater<T>(size, num_col);
   if (type != "default") Log::Error("unknown updater_type '%s', using default", type.c_str());
   return new Updater<T>();
 }

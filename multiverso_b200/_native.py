@@ -22,10 +22,11 @@ EPOCH_FIN = 1 << 62
 F32, F64, I32, I64, I8 = 0, 1, 2, 3, 4
 UPD_DEFAULT, UPD_SGD, UPD_MOMENTUM, UPD_ADAGRAD, UPD_DCASGD, UPD_DCASGDA = range(6)
 UPD_ROWWISE_ADAGRAD = 7          # 6 is unassigned
+UPD_ADAM = 8
 UPDATER_NAMES = {
     "default": UPD_DEFAULT, "sgd": UPD_SGD, "momentum_sgd": UPD_MOMENTUM,
     "adagrad": UPD_ADAGRAD, "dcasgd": UPD_DCASGD, "dcasgda": UPD_DCASGDA,
-    "rowwise_adagrad": UPD_ROWWISE_ADAGRAD,
+    "rowwise_adagrad": UPD_ROWWISE_ADAGRAD, "adam": UPD_ADAM,
 }
 
 _LIBDIR = Path(__file__).resolve().parent / "_lib"
@@ -266,6 +267,8 @@ _CUDA_FUNCS = {
                                        Ptr),
     "mvb_push_dense_rowwise": _status(i32, i32, Ptr, i32, vpp, vpp, i64p, i64p, i64p, i64, C.POINTER(AddOpt), i32,
                                       Ptr),
+    "mvb_push_dense_adam": _status(i32, i32, Ptr, i32, vpp, vpp, vpp, i64p, i64p, i64p, i64, C.POINTER(AddOpt), i32,
+                                   Ptr),
     "mvb_get_rows": _status(i32, C.POINTER(RowMap), Ptr, i64, Ptr, i64, Ptr),
     "mvb_add_rows_red": _status(i32, C.POINTER(RowMap), Ptr, i64, Ptr, i64, f32, Ptr),
     "mvb_add_rows_delta": _status(C.POINTER(RowMap), Ptr, i64, Ptr, Ptr, i64, f32, Ptr),
@@ -286,6 +289,8 @@ _CUDA_FUNCS = {
     "mvb_hash_rows_dump": _status(C.POINTER(HashRows), i32, Ptr, Ptr, Ptr, Ptr),
     "mvb_hash_rows_mark": _status(C.POINTER(HashRows), Ptr, i64, Ptr),
     "mvb_hash_rows_evict": _status(C.POINTER(HashRows), i32, i64, Ptr, Ptr, i32, i64, i64, Ptr, Ptr, Ptr),
+    "mvb_hash_rows_evict_ex": _status(C.POINTER(HashRows), i32, i64, Ptr, Ptr, i32, i64, i64, Ptr, Ptr, Ptr, Ptr,
+                                      i64),
     "mvb_allreduce_oneshot": _status(C.POINTER(Allreduce), Ptr),
     "mvb_allreduce_twoshot": _status(C.POINTER(Allreduce), Ptr),
     "mvb_allreduce_fused": _status(C.POINTER(Allreduce), Ptr, i64, Ptr),

@@ -15,7 +15,7 @@ from typing import List, Optional
 import numpy as np
 
 from . import _native as N
-from .tables.options import AddOption, GetOption
+from .tables.options import AddOption, GetOption, check_add_option
 from .utils import FLAGS, Log
 
 _DT = {"float32": (0, np.float32), "float": (0, np.float32), "float64": (1, np.float64),
@@ -115,8 +115,12 @@ def net_finalize() -> None:
     _lib().MV_NetFinalizeC()
 
 
-def _opt_bytes(option: Optional[AddOption]):
-    return (option or AddOption()).pack()
+def _opt_bytes(option: Optional[AddOption], npdt=None):
+    """The 20-byte AddOption of an Add; a float table checks it against the servers' updater (-updater_type)."""
+    opt = option or AddOption()
+    if npdt is not None and np.issubdtype(npdt, np.floating):
+        check_add_option(str(FLAGS.get("updater_type")), opt)
+    return opt.pack()
 
 
 def _as_np(data, npdt) -> np.ndarray:
@@ -180,7 +184,7 @@ class HostArrayTable(_HostTable):
         arr = _as_np(data, self.npdt).reshape(-1)
         assert arr.size == self.size
         _lib().MV_AddArrayTable64(self.handle, self.code, arr.ctypes.data_as(C.c_void_p),
-                                  C.c_int64(self.size), _opt_bytes(option), 0 if sync else 1)
+                                  C.c_int64(self.size), _opt_bytes(option, self.npdt), 0 if sync else 1)
 
     def add_async(self, data, option: Optional[AddOption] = None):
         self.add(data, option, sync=False)
@@ -237,7 +241,7 @@ class HostMatrixTable(_HostTable):
         arr = _as_np(data, self.npdt).reshape(-1)
         assert arr.size == self.size
         _lib().MV_AddMatrixTable64(self.handle, self.code, arr.ctypes.data_as(C.c_void_p),
-                                   C.c_int64(self.size), None, C.c_int64(0), _opt_bytes(option),
+                                   C.c_int64(self.size), None, C.c_int64(0), _opt_bytes(option, self.npdt),
                                    0 if sync else 1)
 
     def add_rows(self, row_ids, values, option: Optional[AddOption] = None, sync: bool = True) -> None:
@@ -246,7 +250,7 @@ class HostMatrixTable(_HostTable):
         assert arr.size == ids.size * self.num_col
         _lib().MV_AddMatrixTable64(self.handle, self.code, arr.ctypes.data_as(C.c_void_p),
                                    C.c_int64(arr.size), ids.ctypes.data_as(C.c_void_p),
-                                   C.c_int64(ids.size), _opt_bytes(option), 0 if sync else 1)
+                                   C.c_int64(ids.size), _opt_bytes(option, self.npdt), 0 if sync else 1)
 
     def add_row(self, row_id: int, values, option: Optional[AddOption] = None) -> None:
         self.add_rows([row_id], values, option)

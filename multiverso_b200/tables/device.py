@@ -28,7 +28,7 @@ import torch
 from .. import _native as N
 from ..runtime import Runtime
 from ..utils import FLAGS, Log, monitor
-from .options import AddOption, GetOption
+from .options import AddOption, GetOption, check_add_option
 
 _DT = {"float32": torch.float32, "float": torch.float32, "float64": torch.float64,
        "double": torch.float64, "int32": torch.int32, "int": torch.int32, "int64": torch.int64}
@@ -122,20 +122,26 @@ class DenseDeviceTable(_AsyncOps):
         # server s's shard as seen from here (indexed by server id)
         self.shard_ptrs = [self.shard_buf.ptrs[rt.server_id_to_rank(s)] for s in range(S)] \
             if rt.num_servers() else [self.shard_buf.local_ptr]
-        # (state slabs, one slab per worker, state element per row rather than per element)
-        nst, per_worker, per_row = {"default": (0, False, False), "sgd": (0, False, False),
-                                    "momentum_sgd": (1, False, False), "adagrad": (1, True, False),
-                                    "dcasgd": (1, True, False), "dcasgda": (2, True, False),
-                                    "rowwise_adagrad": (1, True, True)}[name]
+        # (state slabs, one slab per worker, state element per row rather than per element, a step count per row)
+        nst, per_worker, per_row, row_count = {
+            "default": (0, False, False, False), "sgd": (0, False, False, False),
+            "momentum_sgd": (1, False, False, False), "adagrad": (1, True, False, False),
+            "dcasgd": (1, True, False, False), "dcasgda": (2, True, False, False),
+            "rowwise_adagrad": (1, True, True, False), "adam": (2, False, False, True)}[name]
         self.n_states, self.state_per_worker, self.state_per_row = nst, per_worker, per_row
         # a slab holds one element per shard element, or per shard row; slabs start at multiples of 4 elements
         gran = self.num_col if per_row else 1
         self.state_stride = (self.my_len // gran + 3) // 4 * 4
         slab = self.state_stride * (W if per_worker else 1)
+        # adam's step counts (one per shard row) follow v's slab in the last state array, at state_stride
+        self.state_row_count = (self.my_len // self.num_col + 3) // 4 * 4 if row_count else 0
+        sizes = [slab] * nst
+        if row_count:
+            sizes[-1] += self.state_row_count
         # state slabs are symmetric (peer-mapped) too: the async one-sided push of a stateful
         # updater updates the owner's state remotely
-        self._state_bufs = [rt.alloc_symm(max(slab, 1) * self.esz) for _ in range(nst)]
-        self.state = [b.tensor(self.dtype, max(slab, 1)) for b in self._state_bufs]
+        self._state_bufs = [rt.alloc_symm(max(n, 1) * self.esz) for n in sizes]
+        self.state = [b.tensor(self.dtype, max(n, 1)) for b, n in zip(self._state_bufs, sizes)]
         self.state_strides = [(l // gran + 3) // 4 * 4 for l in self.lens]
         # collective path resources (lazy)
         self._stage: List = []
@@ -216,6 +222,7 @@ class DenseDeviceTable(_AsyncOps):
     def add_async(self, delta=None, option: Optional[AddOption] = None, staged: bool = False) -> int:
         rt, lib = self.rt, N.cuda_lib()
         opt = option or AddOption()
+        check_add_option(self.updater_name, opt)
         nbytes = self.size * self.esz
         with monitor("WORKER_TABLE_ADD", cuda=True, nbytes=nbytes):
             if rt.size == 1:
@@ -254,7 +261,10 @@ class DenseDeviceTable(_AsyncOps):
                     ss = (C.c_int64 * self.S)(*self.state_strides)
                     ao = _opt_struct(opt)
                     ao.worker_id = max(rt.worker_id(), 0)
-                    if self.state_per_row:
+                    if self.updater == N.UPD_ADAM:
+                        lib.mvb_push_dense_adam(self.dcode, self.updater, src, self.S, sp, s0, s1, so, sl, ss,
+                                                self.num_col, ao, rt.rank, N.stream_ptr())
+                    elif self.state_per_row:
                         lib.mvb_push_dense_rowwise(self.dcode, self.updater, src, self.S, sp, s0, so, sl, ss,
                                                    self.num_col, ao, rt.rank, N.stream_ptr())
                     else:
@@ -512,6 +522,7 @@ class RowMailbox:
 
     def push_vals(self, ids32: torch.Tensor, vals: torch.Tensor, option: Optional[AddOption] = None,
                   scale: float = 1.0, ctas_per_sm: int = 1) -> None:
+        check_add_option(self.t.updater_name, option or AddOption())
         self.epoch += 1
         ao = _opt_struct(option or AddOption())
         N.cuda_lib().mvb_rowbox_push_vals(self.c, ids32, None, ids32.numel(), vals, vals.stride(0), scale, self.epoch,
@@ -652,6 +663,7 @@ class MatrixDeviceTable(DenseDeviceTable):
             vals = vals.to(rt.device, non_blocking=True)
         vals = vals.contiguous().view(k, self.num_col)
         opt = option or AddOption()
+        check_add_option(self.updater_name, opt)
         with monitor("WORKER_TABLE_ADD_ROWS", cuda=True, nbytes=k * self.num_col * self.esz):
             if self.updater in (N.UPD_DEFAULT, N.UPD_SGD):
                 sign = -1.0 if self.updater == N.UPD_SGD else 1.0
@@ -994,10 +1006,16 @@ class HashMatrixTable(MatrixDeviceTable):
         if self.sid >= 0:
             counts = torch.empty(2, dtype=torch.int64, device=rt.device)
             work = torch.empty(self.slots // 2 + 2, dtype=torch.int64, device=rt.device)
-            lib.mvb_hash_rows_evict(self._hash, self.sid, INT64_MIN if older_than is None else older_than,
-                                    self._sp(0), self._sp(1), self.W if self.state_per_worker else 1,
-                                    self.state_stride, 1 if self.state_per_row else self.num_col, counts, work,
-                                    N.stream_ptr())
+            older = INT64_MIN if older_than is None else older_than
+            if self.state_row_count:
+                # adam: m and v rows of num_col elements, and the step count (one element per slot) after v's slab
+                lib.mvb_hash_rows_evict_ex(self._hash, self.sid, older, self._sp(0), self._sp(1), 1,
+                                           self.state_stride, self.num_col, counts, work, N.stream_ptr(),
+                                           self.state[1][self.state_stride:], 1)
+            else:
+                lib.mvb_hash_rows_evict(self._hash, self.sid, older, self._sp(0), self._sp(1),
+                                        self.W if self.state_per_worker else 1, self.state_stride,
+                                        1 if self.state_per_row else self.num_col, counts, work, N.stream_ptr())
             removed = int(counts[0].item())
         rt.barrier()
         return sum(rt.all_gather_object(removed))

@@ -45,6 +45,22 @@ class AddOption:
                 f"{self.lambda_}")
 
 
+def _f32(x: float) -> float:
+    return struct.unpack("<f", struct.pack("<f", x))[0]
+
+
+def check_add_option(updater: str, opt: AddOption) -> None:
+    """Raises ValueError for an AddOption the updater cannot step with, as the fp32 values it travels as: adam needs
+    beta1 (``momentum``) in [0, 1), ``learning_rate > 0`` (it recovers the gradient as delta / learning_rate) and
+    ``rho >= 0`` (the step size)."""
+    if updater != "adam":
+        return
+    b1, lr, rho = _f32(opt.momentum), _f32(opt.learning_rate), _f32(opt.rho)
+    if not (0.0 <= b1 < 1.0 and lr > 0.0 and rho >= 0.0):
+        raise ValueError(f"adam needs 0 <= momentum (beta1) < 1, learning_rate > 0 and rho >= 0 as fp32, got "
+                         f"momentum={opt.momentum}, learning_rate={opt.learning_rate}, rho={opt.rho}")
+
+
 class GetOption:
     __slots__ = ("worker_id",)
 
