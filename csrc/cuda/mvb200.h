@@ -464,7 +464,7 @@ int mvb_stale_on_get(void* const* version_ptrs, int nservers, unsigned long long
 typedef struct MvbRowBox {
   MvbRowMap map;             /* the table's shards (fp32, num_col % 4 == 0, every rank worker + server)   */
   int me;                    /* my rank == worker id == server id                                     */
-  int64_t cap;               /* rows per (owner, source) slot (>= rows of the largest shard)           */
+  int64_t cap;               /* entries per (owner, source) slot: the rows of the largest shard         */
   int64_t slot_bytes;        /* mvb_rowbox_slot_bytes(cap, num_col)                                    */
   void* box[MVB_MAX_RANKS];  /* rank r's mailbox slab: nservers x mvb_rowbox_slots() slots, peer mapped */
   void* ack[MVB_MAX_RANKS];  /* rank r's ack array uint64[nservers], peer mapped                       */
@@ -475,6 +475,9 @@ typedef struct MvbRowBox {
   int* err_flag;
   double timeout_s;
 } MvbRowBox;
+/* A push's ids (the first *n_ptr, or n_max) are ascending; a repeated id is applied once per entry, in list order;
+ * ids outside [0, num_row) are ignored; at most `cap` entries may fall to one owner (more set err_flag to 3100 + owner
+ * and the excess is dropped), so a list with repeats longer than `cap` goes in several pushes. */
 int64_t mvb_rowbox_slot_bytes(int64_t cap, int64_t num_col);
 int mvb_rowbox_slots(void);            /* slots per (owner, source) pair (double-buffered: 2) */
 int mvb_rowbox_push_delta(const MvbRowBox* b, const int* ids, const int* n_ptr, int64_t n_max,

@@ -17,15 +17,16 @@
 //          Before touching a slot the kernel waits for the owner's ack of its previous push (a flag
 //          in the SOURCE's memory, written by the owner), so a slot is never overwritten unread.
 //   apply  (owner, its own stream) per source: acquire the doorbell (spin with watchdog, or -- poll
-//          mode -- return immediately when nothing new arrived), then warp-per-row plain
-//          read-modify-write of the shard through the Updater functor with the SOURCE's AddOption:
-//          every (worker,row) is applied exactly once, stateful updaters included; the last CTA bumps
-//          the device-side `applied` counter and acks.
+//          mode -- return immediately when nothing new arrived), then a plain read-modify-write of the
+//          shard through the Updater functor with the SOURCE's AddOption, one warp per run of equal ids:
+//          every entry is applied exactly once and a repeated row once per entry, in list order; ids
+//          outside the owner's rows are skipped. The last CTA bumps the device-side `applied` counter
+//          and acks.
 //
 // No atomics on the data path (co-scheduled under K7 the red.add push ran at ~90 GB/s, the plain-store
 // gather at ~800 GB/s), no host barrier, no all_gather_object; workers may push different numbers
-// of times -- the owner drains whatever has arrived.  The kernels use no shared memory and <= 40
-// registers so they co-reside with the persistent K7 CTAs on every SM.
+// of times -- the owner drains whatever has arrived.  The kernels use a few bytes of shared memory and
+// <= 56 registers so they co-reside with the persistent K7 CTAs on every SM.
 #include "mvb_common.cuh"
 
 namespace {
@@ -64,15 +65,17 @@ MVB_DEVINL unsigned char* slot_of(const BoxDev& b, int owner, int source, uint64
   return b.box[owner] + ((size_t)source * kSlots + (size_t)(epoch & 1)) * b.slot_bytes;
 }
 
-// seg[o] = first position of the sorted id list that belongs to owner o
+// seg[o] = first position of the sorted id list that belongs to owner o; seg[S] = first id >= num_row. Ids outside
+// [0, num_row) lie before seg[0] or after seg[S] and count toward no owner; an owner whose first row lies past
+// num_row (fewer rows than servers) gets an empty segment.
 __global__ void rowbox_seg_kernel(const __grid_constant__ BoxDev b, const int* __restrict__ ids,
                                   const int* __restrict__ n_ptr, int64_t n_max) {
   int64_t n = n_ptr ? (int64_t)*n_ptr : n_max;
   if (n > n_max) n = n_max;
   const int o = threadIdx.x;
   if (o > b.S) return;
-  if (o == b.S) { b.seg[o] = (int)n; return; }
-  const int64_t key = server_rows(b.map, o).lo;    // first row of owner o
+  const int64_t first = o == b.S ? b.map.num_row : server_rows(b.map, o).lo;
+  const int64_t key = first < b.map.num_row ? first : b.map.num_row;
   int64_t lo = 0, hi = n;
   while (lo < hi) {
     const int64_t mid = (lo + hi) >> 1;
@@ -168,7 +171,8 @@ rowbox_push_kernel(const __grid_constant__ BoxDev b, const __grid_constant__ Pus
   if (threadIdx.x < b.S) {
     const int o = threadIdx.x;
     BoxHdr* h = reinterpret_cast<BoxHdr*>(slot_of(b, o, b.me, a.epoch));
-    h->count = b.seg[o + 1] - b.seg[o];
+    const int count = b.seg[o + 1] - b.seg[o];
+    h->count = count < b.cap ? count : (int)b.cap;    // an overflowing push (error 3100 + o) never reads past the slot
     h->opt = a.opt;
     fence_sys();
     st_release_sys_u64(&h->seq, a.epoch);
@@ -227,66 +231,75 @@ rowbox_apply_kernel(const __grid_constant__ BoxDev b, const __grid_constant__ Ap
   opt.worker_id = a.src;
   const int* ids = reinterpret_cast<const int*>(slot + kHdrBytes);
   const unsigned char* vals = slot + kHdrBytes + b.ids_bytes;
+  const int64_t row_hi = min(server_rows(b.map, b.me).hi, b.map.num_row);
   const int lane = threadIdx.x & 31;
   const int nvec = a.row_floats >> 2;
-  if constexpr (U::kRowState) {
-    // a row-state updater: the row's square sum (rowwise_adagrad), then its factor and the row state (the source's
-    // accumulator, or adam's step count; see row_state_at), then the apply with the element state (adam's m, v)
-    for (int64_t i = warp_id(); i < count; i += num_warps()) {
-      const int64_t r = (int64_t)__ldcg(ids + i);
-      const int64_t base = (r - a.row_lo) * (int64_t)a.row_floats;
-      if (r < a.row_lo || base < 0) continue;
-      const float4* src = reinterpret_cast<const float4*>(vals + (size_t)i * b.ld_bytes);
-      float part = 0.f;
-      if constexpr (U::kRowSum) {
-        for (int v = lane; v < nvec; v += 32) {
-          const float4 g = __ldcg(src + v);
-          part += U::Square(g.x, opt);
-          part += U::Square(g.y, opt);
-          part += U::Square(g.z, opt);
-          part += U::Square(g.w, opt);
-        }
-      }
+  const int64_t stride4 = a.state_stride >> 2;          // slabs of whole float4s: state_stride % 4 == 0
+  // The slot holds the source's sorted list, so a repeated row is a run of equal ids: the warp that meets the run's
+  // first entry applies the whole run in slot order (the list order of the push), as add_rows_owner_kernel does.
+  for (int i = (int)warp_id(); i < count; i += (int)num_warps()) {
+    const int id = __ldcg(ids + i);
+    if (i > 0 && __ldcg(ids + i - 1) == id) continue;       // inside a run: applied by the run's first warp
+    const int64_t r = id;
+    if (r < a.row_lo || r >= row_hi) continue;
+    const int64_t base = (r - a.row_lo) * (int64_t)a.row_floats;
+    const int gld = (int)(b.ld_bytes >> 4);              // float4s per slot row
+    if constexpr (U::kRowState) {
+      // a row-state updater: the row state (the source's accumulator, or adam's step count; see row_state_at) stays
+      // in registers over the run; each entry takes its factor (its row's square sum for rowwise_adagrad) from the
+      // state the entries before it left, then one pass over the row applies it with the element state (adam's m,
+      // v). add_rows_owner_kernel batches the factors of 32 entries per pass; that does not fit these kernels'
+      // register budget, and the result is the same step by step.
       float* hp = row_state_at<U>(a.st0, a.st1, a.src, a.state_stride, r - a.row_lo);
       float h = *hp;
-      const typename U::RowF f = row_factor<U>(part, h, hp, a.row_floats, opt);
+      float4* row = reinterpret_cast<float4*>(a.shard + base);
       float4* st0 = reinterpret_cast<float4*>(a.st0 + base);
       float4* st1 = reinterpret_cast<float4*>(a.st1 + base);
-      const int64_t stride4 = a.state_stride >> 2;
-      for (int v = lane; v < nvec; v += 32) {
-        const float4 g = __ldcg(src + v);
-        float4* dp = reinterpret_cast<float4*>(a.shard + base) + v;
-        float4 d = *dp;
-        float4 s0 = make_float4(0, 0, 0, 0), s1 = make_float4(0, 0, 0, 0);
-        row_elem_load<U>(s0, s1, st0, st1, a.src, stride4, v);
-        U::Step(d.x, g.x, f, s0.x, s1.x, opt);
-        U::Step(d.y, g.y, f, s0.y, s1.y, opt);
-        U::Step(d.z, g.z, f, s0.z, s1.z, opt);
-        U::Step(d.w, g.w, f, s0.w, s1.w, opt);
-        *dp = d;
-        row_elem_store<U>(s0, s1, st0, st1, a.src, stride4, v);
+#pragma unroll 1
+      for (int j = i; j < count && __ldcg(ids + j) == id; ++j) {
+        const float4* src = reinterpret_cast<const float4*>(vals + (size_t)j * b.ld_bytes);
+        float part = 0.f;
+        if constexpr (U::kRowSum) {
+          for (int v = lane; v < nvec; v += 32) {
+            const float4 g = __ldcg(src + v);
+            part += U::Square(g.x, opt);
+            part += U::Square(g.y, opt);
+            part += U::Square(g.z, opt);
+            part += U::Square(g.w, opt);
+          }
+        }
+        const typename U::RowF f = row_factor<U>(part, h, hp, a.row_floats, opt);
+        for (int v = lane; v < nvec; v += 32) {
+          const float4 g = __ldcg(src + v);
+          float4 d = row[v];
+          float4 s0 = make_float4(0, 0, 0, 0), s1 = make_float4(0, 0, 0, 0);
+          row_elem_load<U>(s0, s1, st0, st1, a.src, stride4, v);
+          U::Step(d.x, g.x, f, s0.x, s1.x, opt);
+          U::Step(d.y, g.y, f, s0.y, s1.y, opt);
+          U::Step(d.z, g.z, f, s0.z, s1.z, opt);
+          U::Step(d.w, g.w, f, s0.w, s1.w, opt);
+          row[v] = d;
+          row_elem_store<U>(s0, s1, st0, st1, a.src, stride4, v);
+        }
       }
-    }
-  } else {
-    for (int64_t i = warp_id(); i < count; i += num_warps()) {
-      const int64_t r = (int64_t)__ldcg(ids + i);
-      const int64_t base = (r - a.row_lo) * (int64_t)a.row_floats;
-      if (r < a.row_lo || base < 0) continue;
-      const float4* src = reinterpret_cast<const float4*>(vals + (size_t)i * b.ld_bytes);
+    } else {
+      const float4* g0 = reinterpret_cast<const float4*>(vals + (size_t)i * b.ld_bytes);
+      float4* row = reinterpret_cast<float4*>(a.shard + base);
       float4* st0 = reinterpret_cast<float4*>(a.st0 + base);
       float4* st1 = reinterpret_cast<float4*>(a.st1 + base);
-      const int64_t stride4 = a.state_stride >> 2;          // slabs of whole float4s: state_stride % 4 == 0
       for (int v = lane; v < nvec; v += 32) {
-        const float4 g = __ldcg(src + v);
-        float4* dp = reinterpret_cast<float4*>(a.shard + base) + v;
-        float4 d = *dp;
+        float4 d = row[v];
         float4 s0 = make_float4(0, 0, 0, 0), s1 = make_float4(0, 0, 0, 0);
         state_load<U>(s0, s1, st0, st1, a.src, stride4, v);
-        U::Apply(d.x, g.x, s0.x, s1.x, opt);
-        U::Apply(d.y, g.y, s0.y, s1.y, opt);
-        U::Apply(d.z, g.z, s0.z, s1.z, opt);
-        U::Apply(d.w, g.w, s0.w, s1.w, opt);
-        *dp = d;
+#pragma unroll 1
+        for (int j = i; j < count && __ldcg(ids + j) == id; ++j) {
+          const float4 g = __ldcg(g0 + (j - i) * gld + v);
+          U::Apply(d.x, g.x, s0.x, s1.x, opt);
+          U::Apply(d.y, g.y, s0.y, s1.y, opt);
+          U::Apply(d.z, g.z, s0.z, s1.z, opt);
+          U::Apply(d.w, g.w, s0.w, s1.w, opt);
+        }
+        row[v] = d;
         state_store<U>(s0, s1, st0, st1, a.src, stride4, v);
       }
     }

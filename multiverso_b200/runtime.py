@@ -468,6 +468,9 @@ class Runtime:
             if code == 5003:
                 Log.fatal("KVTable: key INT64_MIN is reserved for empty slots (code 5003: kv-bad-key); the other "
                           "keys of the batch were added")
+            if code // 100 == 31:
+                Log.fatal("row mailbox overflow (code %d): a push named more rows of owner %d than a mailbox slot "
+                          "holds; those rows were dropped", code, code % 100)
             Log.fatal("device watchdog: wait on peer timed out (code %d: %s, peer index %d)", code,
                       {1: "wait", 2: "barrier", 3: "add-ready", 4: "get-done", 5: "kv-full",
                        6: "allreduce"}.get(code // 1000, "?"), code % 1000)

@@ -482,7 +482,7 @@ class RowMailbox:
         self.nslots = lib.mvb_rowbox_slots()
         self.box = rt.alloc_symm(S * self.nslots * self.slot_bytes)
         self.ack = rt.alloc_symm(8 * N.MAX_RANKS)
-        self.box.tensor(torch.uint8)[:].view(S * self.nslots, self.slot_bytes)[:, :128].zero_()   # headers: seq = 0
+        self.box.tensor(torch.uint8)[:S * self.nslots * self.slot_bytes].zero_()   # seq = 0, and no stale rows
         self.ack.tensor(torch.int64).zero_()
         dev = rt.device
         self.seg = torch.zeros(S + 1, dtype=torch.int32, device=dev)
@@ -699,13 +699,23 @@ class MatrixDeviceTable(DenseDeviceTable):
         rt, lib = self.rt, N.cuda_lib()
         k = ids.numel()
         if self._mailbox is not None:
-            # device-side path: sort by row id (the owner segments are contiguous ranges of the sorted
-            # list), one-sided push into the owners' mailboxes, then serve my own mailboxes
-            order = torch.argsort(ids)
-            ids32 = ids[order].to(torch.int32)
-            self._mailbox.push_vals(ids32, vals[order].contiguous(), opt)
-            self._keep_push = (ids32,)
-            self._mailbox.drain(wait=False)
+            # device-side path: ids outside the table become -1 (an id >= 2^31 must not wrap to a row in the int32
+            # list), then a stable sort makes each owner's entries one contiguous range and keeps the entries of a
+            # repeated row in list order; one-sided pushes into the owners' mailboxes, then serve my own mailboxes
+            ids = torch.where((ids >= 0) & (ids < self.num_row), ids, -1)
+            ids, order = torch.sort(ids, stable=True)
+            ids32, vals = ids.to(torch.int32), vals[order]
+            # a slot holds `cap` entries per source, so a longer list goes in pushes of at most `cap` entries, in
+            # order. The push of chunk c waits on the device for every owner's ack of chunk c - 2, and this rank's
+            # own ack comes only from its own drain: wait() serves this rank's mailboxes until chunk c's push has
+            # completed, so chunk c - 2 (complete before chunk c starts, same stream) is drained before it is needed
+            cap = self._mailbox.cap
+            for c0 in range(0, k, cap):
+                if c0:
+                    self.wait(self._record())
+                self._mailbox.push_vals(ids32[c0:c0 + cap], vals[c0:c0 + cap], opt)
+                self._mailbox.drain(wait=False)
+            self._keep_push = (ids32, vals)
             return
         # a repeated row is applied once per occurrence, in list order (MatrixServerTable::ProcessAdd): the
         # owner kernel walks each run of equal ids on one warp, so make the runs adjacent without reordering
