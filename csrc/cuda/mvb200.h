@@ -640,6 +640,33 @@ typedef struct MvbFullSoftmax {
 int64_t mvb_full_softmax_scratch_bytes(int64_t M, int k, int64_t n_rows);
 int mvb_full_softmax(const MvbFullSoftmax* a, void* stream);
 
+/* Backward of the full softmax over all num_row rows of the table (full_softmax_bwd.cu): with the forward's lse,
+ * the upstream gradient g of loss = lse - z_label and G_bn = g_b (exp(z_bn - lse_b) - [labels_b = n]),
+ *   dq = G W            ([M x dim] at pitch lddq, or NULL: not computed)
+ *   dw = scale G^T Q    ([num_row x dim] at pitch lddw, every row written whole, or NULL: not computed)
+ * recomputing the tf32 logits tile by tile; the [M x num_row] logits are never written. dw is bitwise the same for
+ * every sharding of the table; dq agrees across shardings within the tf32 bound. M == 0 zeroes dw. The caller
+ * validates labels (in [0, num_row)). Errors, all before any CUDA call: MVB_BAD_ROW_MAP, -42 pitches (ldq, num_col),
+ * -43 dim, -44 num_row, -45 M or scratch, -46 outputs or inputs missing, -47 output pitches below dim. */
+typedef struct MvbFullSoftmaxBwd {
+  const float* q;            /* [M x ldq] fp32, ldq % 4 == 0, columns >= dim unused             */
+  int64_t M, ldq;
+  int64_t dim;               /* columns used (<= wmap.num_col)                                  */
+  MvbRowMap wmap;            /* the table's shards, row pitch wmap.num_col (% 4 == 0)           */
+  const int64_t* labels;     /* [M]                                                             */
+  const float* lse;          /* [M] the forward's log-partition                                 */
+  const float* g;            /* [M] dL/dloss                                                    */
+  float* dq;                 /* [M x lddq] out or NULL                                          */
+  int64_t lddq;
+  float* dw;                 /* [num_row x lddw] out or NULL, columns >= dim untouched          */
+  int64_t lddw;
+  float scale;               /* dw multiplier                                                   */
+  void* scratch;             /* device, mvb_full_softmax_bwd_scratch_bytes(M, dim, num_row, dq != NULL, dw != NULL) */
+  int64_t scratch_bytes;
+} MvbFullSoftmaxBwd;
+int64_t mvb_full_softmax_bwd_scratch_bytes(int64_t M, int64_t dim, int64_t n_rows, int with_dq, int with_dw);
+int mvb_full_softmax_bwd(const MvbFullSoftmaxBwd* a, void* stream);
+
 /* ---- embedding bag over a row-sharded fp32 MatrixTable (emb_bag.cu) ---------------------------- */
 /* Bag b holds the lookups [offsets[b], offsets[b + 1]) (the last bag ends at L); its output row is the sum
  * (mean: the sum over the bag length) of psw_j * W[ids_j, :dim]; an empty bag gives zeros. Rows are read

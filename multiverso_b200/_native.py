@@ -172,6 +172,12 @@ class FullSoftmax(C.Structure):
                 ("scratch", vp), ("scratch_bytes", i64)]
 
 
+class FullSoftmaxBwd(C.Structure):
+    _fields_ = [("q", vp), ("M", i64), ("ldq", i64), ("dim", i64), ("wmap", RowMap), ("labels", vp), ("lse", vp),
+                ("g", vp), ("dq", vp), ("lddq", i64), ("dw", vp), ("lddw", i64), ("scale", C.c_float),
+                ("scratch", vp), ("scratch_bytes", i64)]
+
+
 EMB_PUSH, EMB_COMPACT = 0, 1
 
 
@@ -333,6 +339,8 @@ _CUDA_FUNCS = {
     "mvb_topk_cosine": _status(C.POINTER(TopkCos), Ptr),
     "mvb_full_softmax_scratch_bytes": _unchecked(i64, i64, i32, i64),
     "mvb_full_softmax": _status(C.POINTER(FullSoftmax), Ptr),
+    "mvb_full_softmax_bwd_scratch_bytes": _unchecked(i64, i64, i64, i64, i32, i32),
+    "mvb_full_softmax_bwd": _status(C.POINTER(FullSoftmaxBwd), Ptr),
     "mvb_embedding_bag_scratch_bytes": _unchecked(i64, i64, i64),
     "mvb_embedding_bag_fwd": _status(C.POINTER(EmbBag), Ptr),
     "mvb_embedding_bag_bwd": _status(C.POINTER(EmbBag), Ptr),

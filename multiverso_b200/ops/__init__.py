@@ -1,6 +1,7 @@
 from .embedding import PSEmbedding, embedding_bag, embedding_bag_reference
 from .embedding_collection import EmbeddingBagConfig, PSEmbeddingCollection
-from .full_softmax import FullSoftmaxResult, full_softmax, full_softmax_reference, topk_dot
+from .full_softmax import (FullSoftmaxResult, PSFullSoftmax, full_softmax, full_softmax_grad_reference,
+                           full_softmax_reference, topk_dot)
 from .get_gemm import gemm_nt, get_gemm, get_gemm_supported
 from .ps_linear import PSLinear, ps_linear
 from .sampled_softmax import PSSampledSoftmax
@@ -9,4 +10,5 @@ from .topk import TOPK_MAX, topk_cosine, topk_cosine_reference
 __all__ = ["get_gemm", "get_gemm_supported", "ps_linear", "PSLinear", "topk_cosine", "topk_cosine_reference",
            "TOPK_MAX", "embedding_bag", "embedding_bag_reference", "PSEmbedding",
            "EmbeddingBagConfig", "PSEmbeddingCollection", "gemm_nt", "PSSampledSoftmax",
-           "full_softmax", "full_softmax_reference", "topk_dot", "FullSoftmaxResult"]
+           "full_softmax", "full_softmax_reference", "topk_dot", "FullSoftmaxResult",
+           "PSFullSoftmax", "full_softmax_grad_reference"]

@@ -196,3 +196,204 @@ def topk_dot(table, queries, k: int, rows: Optional[int] = None) -> Tuple[torch.
     k = _check_k(k, 1, "topk_dot")
     r = _call(table, queries, None, k, rows, False, "queries", "topk_dot")
     return r.scores, r.ids
+
+
+# ------------------------------------------------------------------------------------------------ training
+_WHAT = "PSFullSoftmax"
+
+
+def _lse64(w: torch.Tensor, x64: torch.Tensor, row_chunk: int) -> torch.Tensor:
+    lse = torch.full((x64.shape[0],), float("-inf"), dtype=torch.float64)
+    for lo in range(0, w.shape[0] if x64.shape[0] else 0, row_chunk):
+        z = x64 @ w[lo:lo + row_chunk, :x64.shape[1]].to(torch.float64).t()
+        lse = torch.logaddexp(lse, torch.logsumexp(z, 1))
+    return lse
+
+
+def full_softmax_grad_reference(weights, hidden, labels, g, row_chunk: int = 65536):
+    """The exact full-softmax cross-entropy and its gradients in fp64, chunked over the rows of ``weights``
+    [N, d] so that no [B, N] buffer is formed: returns ``(loss, dX, dW)`` for ``hidden`` [B, d], ``labels`` [B]
+    and upstream gradient ``g`` [B], with ``dX = g (P W - W_y)`` and ``dW = (g (P - Y))^T X``."""
+    w = torch.as_tensor(weights).cpu()
+    x64 = torch.as_tensor(hidden).detach().cpu().to(torch.float64)
+    y = torch.as_tensor(labels).cpu().to(torch.int64)
+    g64 = torch.as_tensor(g).detach().cpu().to(torch.float64)
+    B, d = x64.shape
+    lse = _lse64(w, x64, row_chunk)
+    loss = lse - (x64 * w[y, :d].to(torch.float64)).sum(1)
+    dx = torch.zeros(B, d, dtype=torch.float64)
+    dw = torch.zeros(w.shape[0], d, dtype=torch.float64)
+    for lo in range(0, w.shape[0] if B else 0, row_chunk):
+        wc = w[lo:lo + row_chunk, :d].to(torch.float64)
+        p = torch.exp(x64 @ wc.t() - lse[:, None]) * g64[:, None]
+        dx += p @ wc
+        dw[lo:lo + wc.shape[0]] = p.t() @ x64
+    dx -= g64[:, None] * w[y, :d].to(torch.float64)
+    dw.index_add_(0, y, -g64[:, None] * x64)
+    return loss, dx, dw
+
+
+class PSFullSoftmax(torch.nn.Module):
+    """Output layer trained with the exact softmax over every row of a MatrixTable::
+
+        fsm = mv.ops.PSFullSoftmax(table, push_scale=lr, option=None)
+        loss = fsm(hidden, labels)        # [B] exact cross-entropy, hidden [B, num_col] fp32
+        loss.mean().backward()            # dL/dhidden to autograd; one dense Add of push_scale * dL/dW
+        r = fsm.evaluate(hidden, labels, k=10)   # = full_softmax(table, hidden, labels, k)
+
+    The forward is :func:`full_softmax` (lse and loss, one host read for the label check) and saves hidden, the
+    labels and lse. With ``G_bn = g_b (p_bn - [y_b = n])``, ``p_bn = exp(z_bn - lse_b)`` and ``g_b`` the upstream
+    gradient of ``loss_b``, the backward computes ``dL/dhidden = G W`` (only when hidden requires grad) and
+    ``dL/dW = G^T hidden`` for every row, written times ``push_scale`` into the table's ``staging()`` buffer and
+    pushed as one dense ``add_async(staged=True)`` through the table's updater (``push_scale=None``: neither the
+    dW pass nor the Add runs). On the device both products run in ``csrc/cuda/full_softmax_bwd.cu``, which
+    recomputes the tf32 logits tile by tile and never writes the [B, N] logits or their gradient; the backward
+    makes no host read.
+
+    Every backward issues exactly one Add, also for an empty batch (a zero gradient): a dense Add is collective
+    under BSP with several workers. With momentum or adam every row takes a step, as with any dense Add.
+
+    The backward reads the table again: an Add that lands between a call's forward and its backward changes the
+    recomputed logits. In one process, or under BSP, that happens only if the caller adds; in async mode it is
+    ordinary staleness.
+
+    Numerics on the device: with ``T = 2^-10`` (tf32 truncation of each operand), ``|x_b|`` and ``|w_n|`` the
+    largest row norms, every logit is within ``e_z = 2 T |x| |w| + 1e-6`` of fp64, so ``|p - p_fp64| <= p (2 e_z +
+    e_lse)`` with ``e_lse = |lse - lse_fp64|`` (the forward's bound); G then enters a second tf32 product. With
+    ``f_b = 1.1 (2 e_z + e_lse + 2 T)`` (1.1 covers exp(e) - 1 <= 1.1 e for small e) and ``U = 2^-24`` for the
+    fp32 accumulation of the products over the N classes (dX) and the B queries (dW), per element,
+
+        |dX_bj - dX_fp64| <= |g_b| ((f_b + N U) sum_n p_bn |w_nj| + (2 T + N U) |w_{y_b, j}|) + 1e-6
+        |dW_nj - dW_fp64| <= |scale| (sum_b |g_b| ((f_b + B U) p_bn + (2 T + B U) [y_b = n]) |x_bj| + 1e-6)
+
+    and ``sum_n p_bn |w_nj| <= max_n |w_nj|``. The bound is checked against fp64 up to N = 1,000,003. dW is bitwise the same for every sharding of the table and every run;
+    dX is bitwise repeatable and within its bound across shardings.
+
+    Refused before anything runs: HashMatrixTable, ``is_sparse`` tables (their staged Adds do not mark rows
+    stale), non-fp32 tables, a row pitch that is not a multiple of 4, hidden whose width is not ``num_col`` and
+    CPU hidden with a device table. On the host backend the same formula runs in fp64, chunked over rows
+    (:func:`full_softmax_grad_reference`), and the gradient goes out as one ``table.add``.
+    """
+
+    def __init__(self, table, push_scale: Optional[float] = 1.0, option=None):
+        super().__init__()
+        from ..tables.device import HashMatrixTable
+        from .embedding import _device_of, _dtype_of
+        if isinstance(table, torch.Tensor):
+            raise TypeError(f"{_WHAT}: the weight must be a MatrixTable (a tensor has no updater to push to)")
+        if isinstance(table, HashMatrixTable):
+            raise TypeError(f"{_WHAT}: a HashMatrixTable has no dense Add over all rows; use a MatrixTable")
+        if getattr(table, "is_sparse", False):
+            raise ValueError(f"{_WHAT}: is_sparse tables are not supported (a staged Add does not mark rows stale)")
+        if _dtype_of(table) != torch.float32:
+            raise TypeError(f"{_WHAT}: the table must be float32, got {_dtype_of(table)}")
+        self.table, self.push_scale, self.option = table, push_scale, option
+        self.num_classes, self.in_features = int(table.num_row), int(table.num_col)
+        self._device = _device_of(table)
+        if self._device is not None:
+            self._rm = _rowmap_of(table, _WHAT)[0]
+            if self._rm.num_col % 4 != 0:
+                raise ValueError(f"{_WHAT}: the table's row pitch ({self._rm.num_col} floats) must be a multiple of "
+                                 "4 (16-byte TMA rows)")
+        # hidden may not require grad: the anchor makes autograd run the backward, and so the push
+        self.anchor = torch.nn.Parameter(torch.zeros(0))
+
+    def _check(self, hidden, labels):
+        h = hidden
+        if not isinstance(h, torch.Tensor) or h.dim() != 2 or h.dtype != torch.float32:
+            raise TypeError(f"{_WHAT}: hidden must be a 2-D float32 tensor, got "
+                            f"{getattr(h, 'dtype', type(h).__name__)} {tuple(getattr(h, 'shape', ()))}")
+        if h.shape[1] != self.in_features:
+            raise ValueError(f"{_WHAT}: hidden has {h.shape[1]} columns, the table rows {self.in_features}")
+        if self._device is not None and not h.is_cuda:
+            raise ValueError(f"{_WHAT}: the table is on the GPU, hidden must be too")
+        return _check_labels(labels, h.shape[0], self.num_classes, self._device or "cpu", _WHAT)
+
+    def forward(self, hidden: torch.Tensor, labels) -> torch.Tensor:
+        y = self._check(hidden, labels)
+        if self._device is None:
+            return _FullSoftmaxHostFn.apply(self.anchor, hidden, y, self)
+        return _FullSoftmaxFn.apply(self.anchor, hidden, y, self)
+
+    def evaluate(self, hidden: torch.Tensor, labels, k: int = 0) -> FullSoftmaxResult:
+        """:func:`full_softmax` over the table: ``lse``, ``loss`` and for ``k > 0`` the top-k classes. Nothing is
+        pushed."""
+        h = torch.as_tensor(hidden)
+        if self._device is not None and not h.is_cuda:
+            raise ValueError(f"{_WHAT}: the table is on the GPU, hidden must be too")
+        return full_softmax(self.table, h, labels, k)
+
+    def extra_repr(self) -> str:
+        return (f"{self.in_features}, {self.num_classes}, push_scale={self.push_scale}, "
+                f"weight=MatrixTable#{getattr(self.table, 'table_id', '?')}")
+
+
+def full_softmax_bwd(rm: N.RowMap, q: torch.Tensor, d: int, y: torch.Tensor, lse: torch.Tensor, g: torch.Tensor,
+                     dq: Optional[torch.Tensor], dw: Optional[torch.Tensor], scale: float) -> None:
+    """One ``mvb_full_softmax_bwd`` call: ``q`` [B, ldq] fp32 (ldq % 4 == 0), ``dq`` [B, >= d] and / or ``dw``
+    [num_row, >= d] written (see ``csrc/cuda/mvb200.h``); arguments already checked."""
+    lib = N.cuda_lib()
+    B = q.shape[0]
+    nbytes = lib.mvb_full_softmax_bwd_scratch_bytes(B, d, rm.num_row, dq is not None, dw is not None)
+    scratch = torch.empty(max(nbytes, 16), dtype=torch.uint8, device=q.device)
+    a = N.FullSoftmaxBwd()
+    a.q, a.M, a.ldq, a.dim, a.wmap = q.data_ptr(), B, q.shape[1], d, rm
+    a.labels, a.lse, a.g = y.data_ptr(), lse.data_ptr(), g.data_ptr()
+    if dq is not None:
+        a.dq, a.lddq = dq.data_ptr(), dq.stride(0)
+    if dw is not None:
+        a.dw, a.lddw, a.scale = dw.data_ptr(), dw.stride(0), float(scale)
+    a.scratch, a.scratch_bytes = scratch.data_ptr(), scratch.numel()
+    lib.mvb_full_softmax_bwd(a, N.stream_ptr())
+
+
+class _FullSoftmaxFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, anchor, hidden, y, fsm):
+        x = hidden.detach()
+        r = _device(fsm._rm, fsm.in_features, x, y, 0, fsm.num_classes, True)
+        ctx.fsm = fsm
+        ctx.save_for_backward(padded_queries(x) if x.shape[0] else x.contiguous(), y, r.lse)
+        return r.loss
+
+    @staticmethod
+    def backward(ctx, grad):
+        q, y, lse = ctx.saved_tensors
+        fsm = ctx.fsm
+        B, d = q.shape[0], fsm.in_features
+        want_dx = ctx.needs_input_grad[1]
+        dq = torch.empty(B, d, dtype=torch.float32, device=q.device) if want_dx else None
+        dw = None
+        if fsm.push_scale is not None:
+            dw = fsm.table.staging().view(fsm.num_classes, fsm.table.num_col)
+        if dq is not None or dw is not None:
+            g = grad.to(torch.float32).contiguous()
+            full_softmax_bwd(fsm._rm, q, d, y, lse, g, dq, dw, 0.0 if dw is None else fsm.push_scale)
+        if dw is not None:
+            fsm.table.add_async(None, fsm.option, staged=True)
+        return torch.zeros_like(fsm.anchor), dq, None, None
+
+
+class _FullSoftmaxHostFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, anchor, hidden, y, fsm):
+        w = torch.as_tensor(fsm.table.get()).view(fsm.num_classes, fsm.in_features)
+        x64 = hidden.detach().cpu().to(torch.float64)
+        loss = _lse64(w, x64, 65536) - (x64 * w[y].to(torch.float64)).sum(1)
+        ctx.fsm = fsm
+        ctx.save_for_backward(hidden.detach(), y)
+        return loss.to(torch.float32).to(hidden.device)
+
+    @staticmethod
+    def backward(ctx, grad):
+        x, y = ctx.saved_tensors
+        fsm = ctx.fsm
+        want_dx = ctx.needs_input_grad[1]
+        dx = None
+        if want_dx or fsm.push_scale is not None:
+            w = torch.as_tensor(fsm.table.get()).view(fsm.num_classes, fsm.in_features)
+            _, dx64, dw64 = full_softmax_grad_reference(w, x, y, grad)
+            dx = dx64.to(torch.float32).to(x.device) if want_dx else None
+            if fsm.push_scale is not None:
+                fsm.table.add((dw64 * float(fsm.push_scale)).to(torch.float32).reshape(-1).numpy(), fsm.option)
+        return torch.zeros_like(fsm.anchor), dx, None, None
