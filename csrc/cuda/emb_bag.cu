@@ -9,6 +9,8 @@
 //            runs that cross chunk boundaries in chunk order. Every unique id gets exactly one epilogue:
 //              push     red.add.v4.f32 of scale * g into the owner's row (default / sgd updaters)
 //              compact  grads[u] = scale * g, uniq[u] = id, u = rank of the id among the unique ids
+//            with push_rows > 0, ids >= push_rows (the zero row of a hash table with admission) get none and are
+//            not counted; they sort last, so every other id's rank, chunk and summation order stay as they were.
 //  psw_grad  dpsw_j = s_bag * <dout[bag(j)], W[ids_j, :dim]>, one warp per lookup.
 // The algorithms live in emb_bag.cuh, shared with the collection (emb_bag_coll.cu); the kernels here are the
 // grid-stride loops over bags, chunks and lookups of one table.
@@ -49,10 +51,10 @@ MVB_DEVINL EmbChunk chunk_of(int64_t c, int64_t L) {
 }
 
 __global__ void __launch_bounds__(256)
-emb_bwd_count_kernel(const int64_t* __restrict__ sid, int64_t L, int64_t* __restrict__ cnt) {
+emb_bwd_count_kernel(const int64_t* __restrict__ sid, int64_t L, int64_t bound, int64_t* __restrict__ cnt) {
   for (int64_t c = warp_id(); c * EMB_CHUNK < L; c += num_warps()) {
     const EmbChunk k = chunk_of(c, L);
-    const int64_t n = emb_count_runs(sid, k.c0, k.c1);
+    const int64_t n = emb_count_runs(sid, k.c0, k.c1, bound);
     if ((threadIdx.x & 31) == 0) cnt[c] = n;
   }
 }
@@ -64,11 +66,12 @@ emb_bwd_scan_kernel(int64_t* __restrict__ cnt, int64_t n, int64_t* __restrict__ 
   if (threadIdx.x == 1023 && total_out) *total_out = total;
 }
 
-// the epilogue of unique id u of the table
+// the epilogue of unique id u of the table; rows >= push_rows get none
 template <int VPL>
 struct BwdEpilogue {
   const MvbEmbBag& a;
   MVB_DEVINL void operator()(int64_t id, int64_t u, int v0, const float4* g) const {
+    if (id >= emb_push_bound(0, a.push_rows)) return;
     emb_epilogue<VPL>(a.epilogue == MVB_EMB_PUSH, a.wmap, id, a.grads, u * a.ldg, a.uniq, u, (int)a.dim, a.scale, v0,
                       g);
   }
@@ -152,7 +155,7 @@ extern "C" int mvb_embedding_bag_bwd(const MvbEmbBag* a, void* stream) {
   const BwdScratch s = scratch_of(*a);
   const int64_t nch = n_chunks(a->L);
   const int grid = grid_for(nch);
-  emb_bwd_count_kernel<<<grid, 256, 0, st>>>(a->ids, a->L, s.base);
+  emb_bwd_count_kernel<<<grid, 256, 0, st>>>(a->ids, a->L, emb_push_bound(0, a->push_rows), s.base);
   MVB_CUDA_CHECK(cudaGetLastError());
   emb_bwd_scan_kernel<<<1, 1024, 0, st>>>(s.base, nch, a->n_unique);
   MVB_CUDA_CHECK(cudaGetLastError());

@@ -11,13 +11,13 @@
 //                Group g sums the lookups g, g + NG, g + 2 NG, ... of its bag in order and the groups are combined
 //                by a fixed butterfly, so the summation order depends only on positions within the bag and on dim.
 //  backward      the lookups arrive sorted by (key, position), cut into chunks of EMB_CHUNK within each segment:
-//    count       emb_count_runs: the run starts (unique keys) of one chunk
+//    count       emb_count_runs: the run starts (unique keys) of one chunk, leaving out rows that are not pushed
 //    scan        emb_block_scan: exclusive scan of the per-chunk counts, one 1024-thread CTA
 //    run-sum     emb_run_sum: sums psw_j * s_bag * dout[bag(j)] over each run of equal keys of one chunk in
 //                ascending position. A run inside the chunk goes straight to the epilogue; the pieces of a run
 //                that crosses chunk boundaries go to scratch
 //    merge       emb_merge_run: sums those pieces in chunk order, by the warp of the chunk the run starts in
-//    epilogue    emb_epilogue: every unique key gets exactly one
+//    epilogue    emb_epilogue: every unique key below the table's push bound gets exactly one
 //                  push     red.add.v4.f32 of scale * g into the owner's row (default / sgd updaters)
 //                  compact  grads[u] = scale * g, uniq[u] = id, u = rank of the id among the unique ids
 //  psw grad      emb_psw_dot: s_bag * <dout[bag(j)], W[ids_j, :dim]> of one lookup.
@@ -173,15 +173,21 @@ struct EmbChunk {
   int64_t s0, s1, cb, c, c0, c1;
 };
 
-// the run starts among the sorted positions [c0, c1), on every lane
-MVB_DEVINL int64_t emb_count_runs(const int64_t* __restrict__ sid, int64_t c0, int64_t c1) {
+// the starts of runs of keys below `bound` among the sorted positions [c0, c1), on every lane. Keys >= bound (rows
+// that are not pushed) sort after all others, so leaving them out changes no other run's rank
+MVB_DEVINL int64_t emb_count_runs(const int64_t* __restrict__ sid, int64_t c0, int64_t c1, int64_t bound) {
   const int lane = threadIdx.x & 31;
   int64_t n = 0;
   for (int64_t i0 = c0; i0 < c1; i0 += 32) {
     const int64_t i = i0 + lane;
-    n += __popc(__ballot_sync(FULL, i < c1 && run_start(sid, i)));
+    n += __popc(__ballot_sync(FULL, i < c1 && run_start(sid, i) && sid[i] < bound));
   }
   return n;
+}
+
+// the first key not pushed of a table whose pushed rows are [0, push_rows) (push_rows <= 0: every row is)
+__host__ __device__ __forceinline__ int64_t emb_push_bound(int64_t key_base, int64_t push_rows) {
+  return push_rows > 0 ? key_base + push_rows : INT64_MAX;
 }
 
 // in place: cnt[0..n) -> exclusive scan, cnt[n] = total; returns the total. One CTA of 1024 threads.

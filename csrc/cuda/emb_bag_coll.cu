@@ -13,6 +13,7 @@
 //            lookups and equals one mvb_embedding_bag_bwd over its features' bags stacked in feature order.
 //              push     red.add.v4.f32 of scale * g into the owner's row (default / sgd tables)
 //              compact  table t's grads[u] = scale * g, uniq[u] = id, u = rank among t's unique ids
+//            a table's rows >= its push_rows get no epilogue and are not counted (see emb_bag.cu)
 //  psw_grad  dpsw_j = s_bag * <dout[bag(j), feature columns], W_table[ids_j, :dim]>, one warp per lookup.
 // The algorithms live in emb_bag.cuh and are the ones emb_bag.cu runs; the kernels here find each bag's table and
 // output columns and each chunk's table segment, and pass them on.
@@ -103,7 +104,8 @@ emb_coll_count_kernel(const __grid_constant__ MvbEmbColl a, CollScratch s, int64
     if (c < nc) {
       int t;
       const EmbChunk k = chunk_of(a, s, c, t);
-      n = emb_count_runs(a.skeys, k.c0, k.c1);
+      const MvbEmbTable* tb = a.tables + t;
+      n = emb_count_runs(a.skeys, k.c0, k.c1, emb_push_bound(tb->key_base, tb->push_rows));
     }
     if ((threadIdx.x & 31) == 0) s.base[c] = n;
   }
@@ -128,13 +130,15 @@ emb_coll_scan_kernel(const __grid_constant__ MvbEmbColl a, CollScratch s, int64_
   }
 }
 
-// the epilogue of unique key u of table t; its compact rows start at info[4 t + 2] of grads, info[4 t + 3] of uniq
+// the epilogue of unique key u of table t; its compact rows start at info[4 t + 2] of grads, info[4 t + 3] of uniq.
+// Rows >= the table's push_rows get none
 template <int VPL>
 struct CollEpilogue {
   const MvbEmbColl& a;
   const MvbEmbTable* tb;
   int t;
   MVB_DEVINL void operator()(int64_t key, int64_t u, int v0, const float4* g) const {
+    if (key >= emb_push_bound(tb->key_base, tb->push_rows)) return;
     const bool push = tb->epilogue == MVB_EMB_PUSH;
     if (!push && (!a.grads || !a.uniq)) return;      // no compact destination: nothing to write
     const int64_t* in = a.info + 4 * t;

@@ -26,6 +26,17 @@
 // clock with atomicMax_system, after a plain load shows it older, so a Zipf head costs about one atomic per clock
 // value rather than one per warp. Stamps of ranks at different clocks combine by max.
 //
+// Admission (a descriptor with admit_after >= 2): a count-min sketch per server, 4 rows of W uint32 counters and a
+// uint64 total, next to keys / ready / count. An inserting call runs hash_count_keys_kernel first: with the same grid
+// and lane merge as the lookup, the leader of each group of equal (table, key) probes read-only and, when the key
+// holds no slot, adds the group's size to the key's 4 counters and to the total at the owner. The translation then
+// claims an empty slot for such a key only when its estimate (the minimum of its counters) reaches admit_after; a
+// key below it reads the zero row and leaves no trace. Counting a whole call before admitting any of it makes the
+// outcome per call: on one rank every occurrence of a key sees the same estimate. The counter of row r is
+// (hash64(key + (r + 1) golden) >> 32) & (W - 1): the high half of a hash of a shifted key, unrelated to the probe
+// home (the low bits of mix64(key)) and to the owner (key mod S). mvb_hash_rows_age then halves (TinyLFU's reset)
+// every server whose total reached W / 2.
+//
 // Eviction (mvb_hash_rows_mark, mvb_hash_rows_evict) runs between barriers, with no lookup in flight. Marking sets
 // ready[j] = 3 for the listed keys; the rebuild of a server then removes marked, refused and idle slots with the
 // textbook in-place rehash of linear probing, one warp per cluster of non-empty slots (see mvb200.h). A cluster
@@ -78,6 +89,34 @@ MVB_DEVINL float init_col(const MvbHashRows& h, long long key, int64_t c) {
   return __fadd_rn(h.lo, __fmul_rn(u, __fsub_rn(h.hi, h.lo)));
 }
 
+// ---- admission ----------------------------------------------------------------------------------------------------
+MVB_DEVINL uint32_t* sketch_cell(const MvbHashRows& h, int s, long long key, int r) {
+  const uint64_t W = (uint64_t)h.width;
+  const uint64_t c = (hash64((uint64_t)key + (uint64_t)(r + 1) * 0x9E3779B97F4A7C15ull) >> 32) & (W - 1);
+  return reinterpret_cast<uint32_t*>(h.sketch[s]) + (uint64_t)r * W + c;
+}
+
+MVB_DEVINL bool admitted(const MvbHashRows& h, int s, long long key) {
+  if (h.admit_after < 2) return true;
+  uint32_t e = 0xffffffffu;
+#pragma unroll
+  for (int r = 0; r < 4; ++r) e = min(e, *reinterpret_cast<volatile uint32_t*>(sketch_cell(h, s, key, r)));
+  return e >= (uint32_t)h.admit_after;
+}
+
+// whether `key` holds a slot (ready, being initialised or refused) at its owner: a probe that claims nothing
+MVB_DEVINL bool holds_slot(const MvbHashRows& h, long long key) {
+  const long long* keys = reinterpret_cast<const long long*>(h.keys[owner_of(key, h.nservers)]);
+  const uint64_t mask = (uint64_t)h.slots - 1;
+  uint64_t j = mix64((uint64_t)key) & mask;
+  for (int64_t probe = 0; probe < h.slots; ++probe, j = (j + 1) & mask) {
+    const long long cur = *reinterpret_cast<const volatile long long*>(keys + j);
+    if (cur == key) return true;
+    if (cur == kEmpty) return false;
+  }
+  return false;
+}
+
 // The row of `key` in index `h` (descriptor `t`); the zero row when it is missing and not inserted.
 MVB_DEVINL int64_t translate(const MvbHashRows& h, int t, long long key, int insert, int64_t* status,
                              long long budget) {
@@ -98,7 +137,7 @@ MVB_DEVINL int64_t translate(const MvbHashRows& h, int t, long long key, int ins
   for (int64_t probe = 0; probe < P; ++probe, j = (j + 1) & mask) {
     long long cur = *reinterpret_cast<volatile long long*>(keys + j);
     if (cur == kEmpty) {
-      if (!insert) return zero_row;
+      if (!insert || !admitted(h, s, key)) return zero_row;        // not admitted yet: missing, not an error
       if (*reinterpret_cast<volatile unsigned long long*>(count) >= limit) {   // full: take no slot
         set_status(status, MVB_HASH_FULL, t, s);
         return zero_row;
@@ -145,8 +184,44 @@ MVB_DEVINL int64_t translate(const MvbHashRows& h, int t, long long key, int ins
       return (int64_t)s * P + (int64_t)j;
     }
   }
-  if (insert) set_status(status, MVB_HASH_FULL, t, s);   // a whole chain without an empty slot
+  if (insert && admitted(h, s, key)) set_status(status, MVB_HASH_FULL, t, s);   // a whole chain without an empty slot
   return zero_row;
+}
+
+// the descriptor of lookup i (-1: a row id copied unchanged), -2 past the end
+MVB_DEVINL int table_of(const MvbHashLookup& a, int64_t i) {
+  if (i >= a.n) return -2;
+  if (!a.seg_end) return 0;
+  int lo = 0, hi = a.G - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (i < a.seg_end[mid]) hi = mid; else lo = mid + 1;
+  }
+  return a.seg_table[lo];
+}
+
+MVB_DEVINL int effective_insert(const MvbHashLookup& a) {
+  return a.insert && (a.insert_ok == nullptr || *a.insert_ok != 0);
+}
+
+// the count pass of an inserting call: the grid and lane groups of hash_lookup_kernel
+__global__ void __launch_bounds__(256) hash_count_keys_kernel(const __grid_constant__ MvbHashLookup a) {
+  if (!effective_insert(a)) return;
+  const int lane = threadIdx.x & 31;
+  for (int64_t base = warp_id() * 32; base < a.n; base += num_warps() * 32) {
+    const int64_t i = base + lane;
+    const int t = table_of(a, i);
+    const long long key = t != -2 ? (long long)a.keys[i] : 0;
+    const unsigned same = __match_any_sync(0xffffffffu, key) & __match_any_sync(0xffffffffu, t);
+    if (t < 0 || lane != __ffs(same) - 1 || key == kEmpty) continue;
+    const MvbHashRows& h = a.tables[t];
+    if (h.admit_after < 2 || holds_slot(h, key)) continue;
+    const int s = owner_of(key, h.nservers);
+    const unsigned n = __popc(same);
+#pragma unroll
+    for (int r = 0; r < 4; ++r) atomicAdd_system(sketch_cell(h, s, key, r), n);
+    atomicAdd_system(reinterpret_cast<unsigned long long*>(h.total[s]), (unsigned long long)n);
+  }
 }
 
 __global__ void __launch_bounds__(256) hash_lookup_kernel(const __grid_constant__ MvbHashLookup a,
@@ -154,23 +229,12 @@ __global__ void __launch_bounds__(256) hash_lookup_kernel(const __grid_constant_
   const int lane = threadIdx.x & 31;
   const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
-  const int insert = a.insert && (a.insert_ok == nullptr || *a.insert_ok != 0);
+  const int insert = effective_insert(a);
   for (int64_t base = warp * 32; base < a.n; base += nwarps * 32) {
     const int64_t i = base + lane;
     const bool valid = i < a.n;
     const long long key = valid ? (long long)a.keys[i] : 0;
-    int t = -2;
-    if (valid) {
-      t = 0;
-      if (a.seg_end) {
-        int lo = 0, hi = a.G - 1;
-        while (lo < hi) {
-          const int mid = (lo + hi) >> 1;
-          if (i < a.seg_end[mid]) hi = mid; else lo = mid + 1;
-        }
-        t = a.seg_table[lo];
-      }
-    }
+    const int t = table_of(a, i);
     const unsigned same = __match_any_sync(0xffffffffu, key) & __match_any_sync(0xffffffffu, t);
     const int leader = __ffs(same) - 1;
     int64_t row = 0;
@@ -178,6 +242,46 @@ __global__ void __launch_bounds__(256) hash_lookup_kernel(const __grid_constant_
       row = t < 0 ? (int64_t)key : translate(a.tables[t], t, key, insert, a.status, budget);
     row = __shfl_sync(0xffffffffu, row, leader);
     if (valid) a.rows[i] = row;
+  }
+}
+
+// Aging, part 1: thread s elects itself to shift server s (a CAS of the total from what it read to the shifted value)
+// and leaves the shift, 0 when the total is below W / 2 or another caller won, in age[s]
+__global__ void hash_age_elect_kernel(const __grid_constant__ MvbHashRows h) {
+  const int s = threadIdx.x;
+  if (s >= h.nservers) return;
+  unsigned long long* tot = reinterpret_cast<unsigned long long*>(h.total[s]);
+  const unsigned long long R = (unsigned long long)h.width >> 1;
+  unsigned k = 0;
+  unsigned long long old = *reinterpret_cast<volatile unsigned long long*>(tot);
+  while (old >= R) {
+    unsigned kk = 1;
+    while ((old >> kk) >= R) ++kk;
+    const unsigned long long seen = atomicCAS_system(tot, old, old >> kk);
+    if (seen == old) {
+      k = kk;
+      break;
+    }
+    old = seen;                                       // a count landed in between: decide again
+  }
+  reinterpret_cast<uint32_t*>(h.age)[s] = k;
+}
+
+// Aging, part 2: the elected servers' counters shifted by CAS, so a concurrent count is shifted or kept, never lost
+__global__ void __launch_bounds__(256) hash_age_shift_kernel(const __grid_constant__ MvbHashRows h) {
+  const int64_t n = 4 * h.width, stride = (int64_t)gridDim.x * blockDim.x;
+  for (int s = 0; s < h.nservers; ++s) {
+    const uint32_t k = reinterpret_cast<const uint32_t*>(h.age)[s];
+    if (!k) continue;
+    uint32_t* c = reinterpret_cast<uint32_t*>(h.sketch[s]);
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+      uint32_t old = *reinterpret_cast<volatile uint32_t*>(c + i);
+      while (old) {
+        const uint32_t seen = atomicCAS_system(c + i, old, k < 32 ? old >> k : 0u);
+        if (seen == old) break;
+        old = seen;
+      }
+    }
   }
 }
 
@@ -438,6 +542,10 @@ extern "C" int mvb_hash_rows_init(void* keys, void* ready, void* count, int64_t 
 
 extern "C" int mvb_hash_rows_lookup(const MvbHashLookup* a, void* stream) {
   if (a->n <= 0) return 0;
+  if (a->admit) {
+    hash_count_keys_kernel<<<blocks_for(a->n, 256, 8), 256, 0, (cudaStream_t)stream>>>(*a);
+    MVB_CUDA_CHECK(cudaGetLastError());
+  }
   hash_lookup_kernel<<<blocks_for(a->n, 256, 8), 256, 0, (cudaStream_t)stream>>>(*a,
                                                                                  watchdog_cycles(a->timeout_s, 120.0));
   MVB_CUDA_CHECK(cudaGetLastError());
@@ -466,6 +574,21 @@ extern "C" int mvb_hash_rows_dump(const MvbHashRows* h, int server, int64_t* out
 static int check_index(const MvbHashRows* h) {
   if (h->nservers < 1 || h->nservers > MVB_MAX_RANKS) return -3;
   if (h->slots < 2 || h->slots > (int64_t(1) << 31) || (h->slots & (h->slots - 1))) return -4;
+  return 0;
+}
+
+extern "C" int mvb_hash_rows_age(const MvbHashRows* h, void* stream) {
+  if (int rc = check_index(h)) return rc;
+  if (h->admit_after < 2) return -7;
+  if (h->width < 2 || h->width > (int64_t(1) << 31) || (h->width & (h->width - 1))) return -8;
+  if (!h->age) return -9;
+  for (int s = 0; s < h->nservers; ++s)
+    if (!h->sketch[s] || !h->total[s]) return -9;
+  cudaStream_t st = (cudaStream_t)stream;
+  hash_age_elect_kernel<<<1, MVB_MAX_RANKS, 0, st>>>(*h);
+  MVB_CUDA_CHECK(cudaGetLastError());
+  hash_age_shift_kernel<<<blocks_for(4 * h->width, 256, 4), 256, 0, st>>>(*h);
+  MVB_CUDA_CHECK(cudaGetLastError());
   return 0;
 }
 

@@ -299,6 +299,14 @@ typedef struct MvbHashRows {
      last_seen[j] = max(last_seen[j], *clock); lookups that do not insert stamp nothing                    */
   void* last_seen[MVB_MAX_RANKS];  /* int64[P] per server, symmetric, or NULL: not tracked (clock unused)   */
   const int64_t* clock;            /* device int64 of the calling rank; needed when last_seen is set        */
+  /* count-based admission (optional; admit_after < 2, as in a zeroed descriptor, is off): an inserting lookup
+     gives a missing key a slot only once the key's count-min estimate at its owner is >= admit_after        */
+  void* sketch[MVB_MAX_RANKS];     /* uint32[4 width] per server, symmetric: row r's counters at r width    */
+  void* total[MVB_MAX_RANKS];      /* uint64 per server, symmetric: occurrences counted since the last aging */
+  void* age;                       /* device uint32[MVB_MAX_RANKS] of the calling rank: mvb_hash_rows_age's
+                                      scratch                                                               */
+  int64_t width;                   /* W counters per sketch row, a power of two in [2, 2^31]; aging at W / 2 */
+  int admit_after;                 /* n                                                                     */
 } MvbHashRows;
 typedef struct MvbHashLookup {
   const MvbHashRows* tables;       /* device [T] index descriptors                                          */
@@ -315,10 +323,28 @@ typedef struct MvbHashLookup {
   int64_t* rows;                   /* [n] out                                                               */
   int64_t* status;                 /* device int64, 0 on entry; the first error as kind << 40 | table << 8 | server */
   double timeout_s;                /* watchdog of the wait for a slot another thread is initialising        */
+  int admit;                       /* 1: some descriptor of the call has admission on: a count pass runs
+                                      before the translation; 0: it is not launched                         */
 } MvbHashLookup;
 /* empty keys, zero ready flags and counter of one server's index */
 int mvb_hash_rows_init(void* keys, void* ready, void* count, int64_t slots, void* stream);
+/* Admission. With a->admit set and the lookup inserting (insert and *insert_ok != 0), a count pass runs first:
+ * every occurrence of a key of a descriptor with admission on that holds no slot at its owner (no key in its probe
+ * chain: ready, being initialised or refused keys hold one) adds 1 to its 4 counters
+ * sketch[s][r W + ((hash64(key + (r + 1) 0x9E3779B97F4A7C15) >> 32) & (W - 1))], r = 0..3, and to total[s]
+ * (system-scope atomics, peers included). The translation then gives such a key a slot only when its estimate, the
+ * minimum of its 4 counters, is >= admit_after; otherwise it reads the zero row, sets no status and takes nothing.
+ * All occurrences of a call are counted before any is admitted, so on one rank every occurrence of a key in a call
+ * gets the same row. Counts of other ranks landing during the translation can admit a key in the middle of a call:
+ * an occurrence may then read the zero row in the call in which another occurrence got the slot. */
 int mvb_hash_rows_lookup(const MvbHashLookup* a, void* stream);
+/* Aging step of an index with admission (run after each inserting lookup): every server whose total is >= W / 2
+ * has its total and all its counters shifted right by the smallest k that takes the total below W / 2. One CAS on
+ * the total elects the one caller that shifts a server, and each counter is shifted by a CAS loop, so a count
+ * landing concurrently is never lost (it is shifted or kept whole). Returns, before any CUDA call, -3 / -4 as
+ * mvb_hash_rows_mark, -7 for admit_after < 2, -8 for a width not a power of two in [2, 2^31], -9 for a NULL age,
+ * sketch[s] or total[s] (s < nservers). */
+int mvb_hash_rows_age(const MvbHashRows* h, void* stream);
 /* *out = live keys over all servers of the (host) descriptor */
 int mvb_hash_rows_count(const MvbHashRows* h, int64_t* out, void* stream);
 /* (key, row) of every live slot (ready == 1) of server `server`, in no particular order; *out_count on the device */
@@ -697,6 +723,9 @@ typedef struct MvbEmbBag {
   float* dpsw;               /* psw grad: [L]                                                           */
   void* scratch;             /* backward: mvb_embedding_bag_scratch_bytes(L, dim) bytes of device memory */
   int64_t scratch_bytes;
+  int64_t push_rows;         /* backward: > 0: lookups of rows >= push_rows contribute nothing (no epilogue,
+                                not in n_unique); <= 0: every row. Those rows sort last, so no other row's
+                                rank or chunk boundary moves                                             */
 } MvbEmbBag;
 int mvb_embedding_bag_fwd(const MvbEmbBag* a, void* stream);
 int64_t mvb_embedding_bag_scratch_bytes(int64_t L, int64_t dim);
@@ -722,6 +751,8 @@ typedef struct MvbEmbTable {
   int epilogue;              /* MVB_EMB_PUSH, MVB_EMB_COMPACT or MVB_EMB_NO_PUSH                         */
   float scale;               /* the pushed value is scale * g                                            */
   int64_t ldg;               /* compact: row pitch of the table's gradient, % 4 == 0, >= round4(dim)     */
+  int64_t push_rows;         /* > 0: lookups of rows >= push_rows contribute nothing to the backward (as in
+                                MvbEmbBag); <= 0: every row                                              */
 } MvbEmbTable;
 typedef struct MvbEmbFeature {
   int table;                 /* index into the table descriptors                                         */

@@ -90,12 +90,14 @@ HASH_FULL, HASH_TIMEOUT, HASH_BAD_KEY = 1, 2, 3
 class HashRows(C.Structure):
     _fields_ = [("nservers", C.c_int), ("slots", i64), ("keys", VP8), ("ready", VP8), ("count", VP8),
                 ("map", RowMap), ("init", C.c_int), ("init_value", C.c_float), ("lo", C.c_float),
-                ("hi", C.c_float), ("seed", C.c_uint64), ("last_seen", VP8), ("clock", vp)]
+                ("hi", C.c_float), ("seed", C.c_uint64), ("last_seen", VP8), ("clock", vp), ("sketch", VP8),
+                ("total", VP8), ("age", vp), ("width", i64), ("admit_after", C.c_int)]
 
 
 class HashLookup(C.Structure):
     _fields_ = [("tables", vp), ("keys", vp), ("n", i64), ("seg_end", vp), ("seg_table", vp), ("G", C.c_int),
-                ("insert", C.c_int), ("insert_ok", vp), ("rows", vp), ("status", vp), ("timeout_s", C.c_double)]
+                ("insert", C.c_int), ("insert_ok", vp), ("rows", vp), ("status", vp), ("timeout_s", C.c_double),
+                ("admit", C.c_int)]
 
 
 class Allreduce(C.Structure):
@@ -185,7 +187,8 @@ class EmbBag(C.Structure):
     _fields_ = [("wmap", RowMap), ("dim", i64), ("ids", vp), ("L", i64), ("offsets", vp), ("B", i64),
                 ("psw", vp), ("mean", C.c_int), ("out", vp), ("ldo", i64), ("dout", vp), ("ldd", i64),
                 ("perm", vp), ("epilogue", C.c_int), ("scale", C.c_float), ("grads", vp), ("ldg", i64),
-                ("uniq", vp), ("n_unique", vp), ("dpsw", vp), ("scratch", vp), ("scratch_bytes", i64)]
+                ("uniq", vp), ("n_unique", vp), ("dpsw", vp), ("scratch", vp), ("scratch_bytes", i64),
+                ("push_rows", i64)]
 
 
 EMB_NO_PUSH = 2
@@ -193,7 +196,7 @@ EMB_NO_PUSH = 2
 
 class EmbTable(C.Structure):
     _fields_ = [("wmap", RowMap), ("dim", i64), ("key_base", i64), ("mean", C.c_int), ("epilogue", C.c_int),
-                ("scale", C.c_float), ("ldg", i64)]
+                ("scale", C.c_float), ("ldg", i64), ("push_rows", i64)]
 
 
 class EmbFeature(C.Structure):
@@ -291,6 +294,7 @@ _CUDA_FUNCS = {
     "mvb_kv_dump": _status(i32, Ptr, Ptr, i64, Ptr, Ptr, Ptr, Ptr),
     "mvb_hash_rows_init": _status(Ptr, Ptr, Ptr, i64, Ptr),
     "mvb_hash_rows_lookup": _status(C.POINTER(HashLookup), Ptr),
+    "mvb_hash_rows_age": _status(C.POINTER(HashRows), Ptr),
     "mvb_hash_rows_count": _status(C.POINTER(HashRows), Ptr, Ptr),
     "mvb_hash_rows_dump": _status(C.POINTER(HashRows), i32, Ptr, Ptr, Ptr, Ptr),
     "mvb_hash_rows_mark": _status(C.POINTER(HashRows), Ptr, i64, Ptr),

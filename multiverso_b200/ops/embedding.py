@@ -24,7 +24,9 @@ coalesced gradient times ``push_scale``:
 Over a :class:`~multiverso_b200.tables.device.HashMatrixTable` the ids are int64 keys: one ``mvb_hash_rows_lookup``
 translates them to rows before the input checks (its status word is read in the checks' one host read), then the
 same kernels run on the rows. ``PSEmbedding`` in training mode inserts missing keys; in eval mode, and in
-``embedding_bag``, they read the zero row, and a backward after such a forward raises.
+``embedding_bag``, they read the zero row, and a backward after such a forward raises. Over a table with
+``admit_after``, keys not admitted yet read the zero row in training mode too, and the backward pushes nothing for
+them (the zero row stays zero).
 
 On the host backend the same calls run :func:`embedding_bag_reference` over ``get_rows`` of the unique ids, and the
 backward pushes the gradient coalesced in torch with ``add_rows``: the same semantics.
@@ -151,6 +153,12 @@ def _args(rm: N.RowMap, dim: int, ids: torch.Tensor, offsets: torch.Tensor, psw:
     return a
 
 
+def _push_rows(table) -> int:
+    """The backward's row bound: keys a table with admission has not admitted read the zero row, its last row,
+    which is never pushed (0: every row is)."""
+    return table.zero_row if isinstance(table, HashMatrixTable) and table.admit_after > 1 else 0
+
+
 def _fwd_device(rm, dim, ids, offsets, psw, mode) -> torch.Tensor:
     ldo = (dim + 3) // 4 * 4
     out = torch.empty(offsets.numel(), ldo, dtype=torch.float32, device=ids.device)
@@ -194,6 +202,7 @@ def _push_device(table, rm, dim, ids, offsets, psw, mode, dout, push_scale: floa
     a = _args(rm, dim, sid, offsets, psw, mode)
     a.dout, a.ldd, a.perm = d.data_ptr(), ldd, perm.data_ptr()
     a.scratch, a.scratch_bytes = scratch.data_ptr(), nbytes
+    a.push_rows = _push_rows(table)
     st = N.stream_ptr()
     fused = table.updater in (N.UPD_DEFAULT, N.UPD_SGD) and not table.is_sparse
     with monitor("WORKER_TABLE_EMBEDDING_BAG_GRAD", cuda=True, nbytes=L * dim * 4):

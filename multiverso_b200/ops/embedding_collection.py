@@ -29,6 +29,8 @@ not ``is_sparse``); otherwise it reads the unique-row counts of all compact tabl
 A config may name a ``HashMatrixTable``: its features' ids are then int64 keys, translated to rows by one launch per
 call that covers every hash feature (dense features' ids pass through unchanged), before the input checks and inside
 their one host read. In training mode missing keys are inserted; in eval mode they add zeros and a backward raises.
+Keys that a table with ``admit_after`` has not admitted yet add zeros in training mode too, and the backward pushes
+nothing for them.
 
 On the host backend the same module runs ``get_rows`` of the unique ids of each table over all of its features,
 torch's ``embedding_bag`` per feature, and in the backward one coalesced ``add_rows`` per table: the same semantics.
@@ -45,7 +47,7 @@ from .. import _native as N
 from ..tables.device import HashMatrixTable, raise_hash_status
 from ..tables.options import AddOption
 from ..utils import monitor
-from .embedding import MODES, _INT, _device_of, _dtype_of, _host_rows
+from .embedding import MODES, _INT, _device_of, _dtype_of, _host_rows, _push_rows
 from .topk import _rowmap_of
 
 MAX_DIM = 512
@@ -156,6 +158,7 @@ class PSEmbeddingCollection(torch.nn.Module):
                 raise ValueError(f"{_WHAT}: config {t}: table dims must be in [1, {MAX_DIM}], got {dim}")
             d = tabs[t]
             d.wmap, d.dim, d.key_base, d.mean = rm, dim, key_base, int(c.mode == "mean")
+            d.push_rows = _push_rows(c.table)
             key_base += nrow
             if c.push_scale is None:
                 d.epilogue = N.EMB_NO_PUSH
@@ -244,7 +247,7 @@ class PSEmbeddingCollection(torch.nn.Module):
                 if lengths.numel():
                     ok &= (lengths.view(-1).min().view(1) >= 0).to(torch.int64)
             self._hash[0].lookup_call(ids, rows, status, self.training, seg_end, self._seg_table, self._d_hash,
-                                      insert_ok=ok)
+                                      insert_ok=ok, hash_tables=self._hash)
         else:
             status.zero_()
         return rows, status

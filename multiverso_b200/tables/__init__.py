@@ -43,14 +43,16 @@ def KVTable(key_dtype="int64", val_dtype="float32", capacity=None):
 
 
 def HashMatrixTable(capacity, num_col, dtype="float32", updater=None, init_value=None, min_value=None,
-                    max_value=None, seed=1, track_access=False):
+                    max_value=None, seed=1, track_access=False, admit_after=1):
     """fp32 rows keyed by any int64, allocated on first lookup (device backend only; see
     :class:`multiverso_b200.tables.device.HashMatrixTable`)."""
+    from .device import check_admit_after
+    check_admit_after(admit_after)
     if not _device():
         raise NotImplementedError("HashMatrixTable needs the device backend (a CUDA device): its index is a GPU "
                                   "hash table; the host backend has no counterpart")
     from .device import HashMatrixTable as _Hash
-    return _Hash(capacity, num_col, dtype, updater, init_value, min_value, max_value, seed, track_access)
+    return _Hash(capacity, num_col, dtype, updater, init_value, min_value, max_value, seed, track_access, admit_after)
 
 
 def create_table(option):

@@ -819,6 +819,14 @@ def raise_hash_status(code: int, tables: Sequence["HashMatrixTable"]) -> None:
     raise RuntimeError(f"HashMatrixTable #{tid}: lookup status {code:#x}")
 
 
+def check_admit_after(admit_after) -> None:
+    """``admit_after`` of a HashMatrixTable: an int in [1, 2^31) (TypeError / ValueError otherwise)."""
+    if isinstance(admit_after, bool) or not isinstance(admit_after, int):
+        raise TypeError(f"HashMatrixTable: admit_after must be an int, got {type(admit_after).__name__}")
+    if not 1 <= admit_after < 1 << 31:
+        raise ValueError(f"HashMatrixTable: admit_after must be in [1, 2^31), got {admit_after}")
+
+
 class HashMatrixTable(MatrixDeviceTable):
     """Rows keyed by any int64 (but INT64_MIN), one row per distinct key, allocated on first lookup.
 
@@ -841,10 +849,26 @@ class HashMatrixTable(MatrixDeviceTable):
     touches to this rank's ``clock``, a user-defined int64 time (a step, an hour, ...). Reads (``get``,
     ``lookup(insert=False)``, eval-mode layers) stamp nothing. ``evict`` removes idle keys (``older_than``) or listed
     keys and frees their slots, so a table of fixed capacity can serve a stream of new ids. It costs one int64 per
-    slot and an atomic per key and clock value."""
+    slot and an atomic per key and clock value.
+
+    ``admit_after=n >= 2`` turns on count-based admission: an inserting lookup gives a missing key a slot only once
+    the key's estimated count reaches ``n``. Until then the key behaves as a missing key does in eval mode: it reads
+    the zero row, takes no slot, initial row, updater state or stamp, and is not an error; ``PSEmbedding`` and
+    ``PSEmbeddingCollection`` push nothing for it, ``add`` drops its values. Every occurrence of a missing key in an
+    inserting call (a training forward, ``lookup(insert=True)``, ``add``) counts once; keys holding a slot and
+    lookups that do not insert count nothing. A call counts all its occurrences before it admits any, so a key at
+    ``n - 2`` seen twice in a batch is admitted in that batch, and on one rank every occurrence of a key in a call
+    gets the same row. While other ranks count concurrently, an occurrence may read zeros (and push nothing) in the
+    call in which another occurrence of the same key is admitted. The count is a count-min sketch per server
+    (4 rows of ``slots`` uint32 counters, 16 bytes per slot, in symmetric memory): it never under-counts, so no key
+    is admitted below ``n``; a key never seen before reads at least 1 too many with probability below 2.5 %. Every
+    server halves its counters once ``slots / 2`` occurrences have been counted there since the last halving, so
+    counts of keys that stopped arriving fade. ``admit_after=1`` (the default) is the table without admission."""
 
     def __init__(self, capacity: int, num_col: int, dtype="float32", updater: Optional[str] = None,
-                 init_value=None, min_value=None, max_value=None, seed: int = 1, track_access: bool = False):
+                 init_value=None, min_value=None, max_value=None, seed: int = 1, track_access: bool = False,
+                 admit_after: int = 1):
+        check_admit_after(admit_after)
         rt = Runtime.get()
         if not rt.started:
             Log.fatal("MV_Init must be called before creating tables")
@@ -895,6 +919,18 @@ class HashMatrixTable(MatrixDeviceTable):
                 r = rt.server_id_to_rank(s) if rt.num_servers() else rt.rank
                 h.last_seen[s] = self._ls_map.shard_ptrs[s] = self._ls_buf.ptrs[r]
             h.clock = self._clock.data_ptr()
+        self.admit_after = admit_after
+        self._sketch_buf = None
+        if admit_after > 1:
+            # per server: 4 rows of W = P uint32 counters, then the uint64 total; the aging step's scratch is local
+            self._sketch_buf = rt.alloc_symm(16 * P + 8)
+            self._sketch_buf.tensor(torch.uint8).zero_()
+            self._age = torch.zeros(N.MAX_RANKS, dtype=torch.int32, device=rt.device)
+            for s in range(self.S):
+                r = rt.server_id_to_rank(s) if rt.num_servers() else rt.rank
+                h.sketch[s] = self._sketch_buf.ptrs[r]
+                h.total[s] = self._sketch_buf.ptrs[r] + 16 * P
+            h.age, h.width, h.admit_after = self._age.data_ptr(), P, admit_after
         self._hash = h
         self._d_hash = torch.frombuffer(bytearray(h), dtype=torch.uint8).to(rt.device)
         self.zero_row = self.S * P
@@ -910,11 +946,14 @@ class HashMatrixTable(MatrixDeviceTable):
 
     def lookup_call(self, keys: torch.Tensor, rows: torch.Tensor, status: torch.Tensor, insert: bool,
                     seg_end: Optional[torch.Tensor] = None, seg_table: Optional[torch.Tensor] = None,
-                    tables: Optional[torch.Tensor] = None, insert_ok: Optional[torch.Tensor] = None) -> None:
+                    tables: Optional[torch.Tensor] = None, insert_ok: Optional[torch.Tensor] = None,
+                    hash_tables: Optional[Sequence["HashMatrixTable"]] = None) -> None:
         """Launch one translation of int64 device ``keys`` into ``rows`` (no host read). ``status`` (device int64,
         zeroed here) receives the first error; ``raise_hash_status`` interprets it. ``seg_end`` / ``seg_table`` /
-        ``tables``: several indexes in one launch (see ``MvbHashLookup``). ``insert_ok``: device int64; when it
-        holds 0 nothing is inserted."""
+        ``tables``: several indexes in one launch (see ``MvbHashLookup``), ``hash_tables`` the tables of ``tables``
+        in order (default: this table). ``insert_ok``: device int64; when it holds 0 nothing is inserted (nor
+        counted). An inserting call over tables with admission counts its keys before the translation and runs each
+        such table's aging step after it."""
         a = N.HashLookup()
         a.tables = (self._d_hash if tables is None else tables).data_ptr()
         a.keys, a.n, a.rows, a.status = keys.data_ptr(), keys.numel(), rows.data_ptr(), status.data_ptr()
@@ -922,13 +961,20 @@ class HashMatrixTable(MatrixDeviceTable):
         a.G = 0 if seg_end is None else seg_end.numel()
         a.insert, a.insert_ok = int(bool(insert)), N.ptr(insert_ok)
         a.timeout_s = float(FLAGS.get("barrier_timeout_s"))
+        admitting = [t for t in (hash_tables or [self]) if t.admit_after > 1] if insert else []
+        a.admit = int(bool(admitting))
         status.zero_()
+        lib, st = N.cuda_lib(), N.stream_ptr()
         with monitor("WORKER_TABLE_HASH_LOOKUP", cuda=True):
-            N.cuda_lib().mvb_hash_rows_lookup(a, N.stream_ptr())
+            lib.mvb_hash_rows_lookup(a, st)
+            for t in admitting:
+                if keys.numel():
+                    lib.mvb_hash_rows_age(t._hash, st)
 
     def lookup(self, keys, insert: bool = True) -> torch.Tensor:
-        """int64 rows of ``keys`` (device tensor). ``insert``: a missing key gets a row, initialised; otherwise it
-        reads the zero row. INT64_MIN raises ValueError before anything is inserted."""
+        """int64 rows of ``keys`` (device tensor). ``insert``: a missing key gets a row, initialised (with
+        ``admit_after``: once admitted); otherwise it reads the zero row. INT64_MIN raises ValueError before anything
+        is inserted."""
         k = self._key_tensor(keys)
         rows = torch.empty_like(k)
         if k.numel():
@@ -945,8 +991,13 @@ class HashMatrixTable(MatrixDeviceTable):
         return self.get_rows(self.lookup(keys, insert=False), out)
 
     def add(self, keys, values, option: Optional[AddOption] = None) -> None:
-        """Insert the missing keys, then ``add_rows`` of their rows (the table's updater, ``option``)."""
-        self.add_rows(self.lookup(keys, insert=True), values, option)
+        """Insert the missing keys, then ``add_rows`` of their rows (the table's updater, ``option``). With
+        ``admit_after``, the values of keys not admitted are dropped."""
+        rows = self.lookup(keys, insert=True)
+        if self.admit_after > 1:
+            keep = rows != self.zero_row
+            rows, values = rows[keep], self._as_device(values).view(-1, self.num_col)[keep]
+        self.add_rows(rows, values, option)
 
     def get_async(self, *args, **kwargs):
         raise TypeError("HashMatrixTable: the whole-table get is not offered (its layout is the slot layout); "
@@ -1052,16 +1103,23 @@ class HashMatrixTable(MatrixDeviceTable):
         keys, order = torch.sort(keys)
         return keys, self.get_rows(rows[order])
 
+    _ADMIT_TAG = b"MVBADMIT"
+
     def store(self, stream) -> None:
         """This rank's shard and updater state (the slot layout), then its server's keys, then, with
-        ``track_access``, their last-seen stamps. A table of the same capacity, width, number of servers and
-        ``track_access`` loads it back with every key in its slot. The clock is not stored."""
+        ``track_access``, their last-seen stamps, then, with ``admit_after``, a tag, ``admit_after`` and its
+        server's sketch and total. A table of the same capacity, width, number of servers, ``track_access`` and
+        ``admit_after`` loads it back with every key in its slot, and then counts and admits as this one would. The
+        clock is not stored."""
         super().store(stream)
         torch.cuda.current_stream().synchronize()
         stream.write(self._keys_buf.tensor(torch.int64, self.slots).cpu().numpy().tobytes())
         stream.write(self._ready_buf.tensor(torch.int32, self.slots).cpu().numpy().tobytes())
         if self.track_access:
             stream.write(self._ls_buf.tensor(torch.int64, self.slots).cpu().numpy().tobytes())
+        if self.admit_after > 1:
+            stream.write(self._ADMIT_TAG + int(self.admit_after).to_bytes(8, "little"))
+            stream.write(self._sketch_buf.tensor(torch.uint8).cpu().numpy().tobytes())
 
     def load(self, stream) -> None:
         import numpy as np
@@ -1082,12 +1140,41 @@ class HashMatrixTable(MatrixDeviceTable):
                                  f"{self.slots} slots (stored without track_access?)")
             ls = torch.from_numpy(np.frombuffer(raw, dtype=np.int64).copy()).to(self.rt.device)
             self._ls_buf.tensor(torch.int64, self.slots).copy_(ls)
+        self._load_sketch(stream)
         torch.cuda.synchronize()
+
+    def _load_sketch(self, stream) -> None:
+        """The admission part of a stream: required with ``admit_after``, refused without it (a seekable stream is
+        peeked at and left where it was)."""
+        tid = self.table_id
+        if self.admit_after == 1:
+            if hasattr(stream, "seekable") and stream.seekable():
+                at = stream.tell()
+                tag = stream.read(len(self._ADMIT_TAG))
+                stream.seek(at)
+                if tag == self._ADMIT_TAG:
+                    raise ValueError(f"HashMatrixTable #{tid}: the stream was stored with admit_after >= 2; this "
+                                     "table has admission off")
+            return
+        head = stream.read(16)
+        if len(head) != 16 or head[:8] != self._ADMIT_TAG:
+            raise ValueError(f"HashMatrixTable #{tid}: the stream holds no admission sketch (stored with "
+                             f"admit_after=1?); this table has admit_after={self.admit_after}")
+        stored = int.from_bytes(head[8:], "little")
+        if stored != self.admit_after:
+            raise ValueError(f"HashMatrixTable #{tid}: the stream was stored with admit_after={stored}; this table "
+                             f"has admit_after={self.admit_after}")
+        n = 16 * self.slots + 8
+        raw = stream.read(n)
+        if len(raw) != n:
+            raise ValueError(f"HashMatrixTable #{tid}: the stream holds no sketch of {self.slots} counters per row")
+        self._sketch_buf.tensor(torch.uint8).copy_(torch.frombuffer(bytearray(raw), dtype=torch.uint8))
 
     def free(self) -> None:
         super().free()
-        for b in (self._keys_buf, self._ready_buf, self._count_buf) + ((self._ls_buf,) if self.track_access else ()):
-            self.rt.release_symm(b)
+        for b in (self._keys_buf, self._ready_buf, self._count_buf, self._ls_buf, self._sketch_buf):
+            if b is not None:
+                self.rt.release_symm(b)
 
 
 class KVDeviceTable(_AsyncOps):
