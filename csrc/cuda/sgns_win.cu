@@ -1017,45 +1017,58 @@ sgns_det_kernel(const __grid_constant__ DetDev a) {
     }
   }
 
-  // ---- phase 2: output-row deltas sum_c g_ck * in_c in registers, one row of REDs per (centre, k) -----------
+  // ---- phase 2: output-row deltas sum_c g_ck * in_c, two output rows at a time in registers (O is dead).  A row
+  // this (centre, k) alone reads is loaded before its sums start, so its loads are in flight during the sums, and
+  // is written in place: the row as the wave found it (nothing else reads or writes it in this wave) plus the one
+  // term its fixed-point sum would hold; zero terms leave the element untouched, as in the apply.  Every other row
+  // leaves as one row of REDs.  Each element's FMA chain runs over the contexts in mask order whatever the
+  // grouping of the rows, so the grouping changes no bit. ------------------------------------------------------
+  static_assert(KO % 2 == 0, "phase 2 takes the output rows in pairs");
   if (ctx) {
+#pragma unroll 1
+    for (int k0 = 0; k0 < KO; k0 += 2) {
+      if (!((used >> k0) & 3u)) continue;
+      float x[2][NJ], acc[2][NJ];
 #pragma unroll
-    for (int k = 0; k < KO; ++k)
+      for (int j = 0; j < 2; ++j) {
+        if ((owned >> (k0 + j)) & 1u) {
+          const float* row = a.w_out + (int64_t)orid[c * KO + k0 + j] * a.ld;
 #pragma unroll
-      for (int u = 0; u < NJ; ++u) O[k][u] = 0.f;
-    for (uint32_t m = ctx; m; m &= m - 1) {
-      const int t = __ffs(m) - 1;
-      float h[NJ];
-      det_load(h, hrow + (size_t)(c + W + t - hw) * dim, dim, lane, true);
-#pragma unroll
-      for (int k = 0; k < KO; ++k) {
-        const float gk = gs[t * KO + k] * osc[c * KO + k];
-#pragma unroll
-        for (int u = 0; u < NJ; ++u) O[k][u] = __fmaf_rn(gk, h[u], O[k][u]);
-      }
-    }
-#pragma unroll
-    for (int k = 0; k < KO; ++k) {
-      const int sl = __shfl_sync(0xffffffffu, oslot, k);
-      if (!((used >> k) & 1u)) continue;
-      if ((owned >> k) & 1u) {
-        // the row as the wave found it (nothing else reads or writes it in this wave) plus the one term its
-        // fixed-point sum would hold; zero terms leave the element untouched, as in the apply
-        float* row = a.w_out + (int64_t)orid[c * KO + k] * a.ld;
-        float x[NJ];
-#pragma unroll
-        for (int u = 0; u < NJ; ++u) x[u] = lane + 32 * u < dim ? row[lane + 32 * u] : 0.f;
-#pragma unroll
-        for (int u = 0; u < NJ; ++u) {
-          const long long v = __float2ll_rn(O[k][u] * kFixScale);
-          if (lane + 32 * u < dim && v != 0) row[lane + 32 * u] = det_fix_add(x[u], v);
+          for (int u = 0; u < NJ - 1; ++u) x[j][u] = row[lane + 32 * u];   // NJ = ceil(dim / 32)
+          x[j][NJ - 1] = lane + 32 * (NJ - 1) < dim ? row[lane + 32 * (NJ - 1)] : 0.f;
         }
-        continue;
-      }
-      unsigned long long* dst = a.acc + (int64_t)sl * dim;
 #pragma unroll
-      for (int u = 0; u < NJ; ++u)
-        if (lane + 32 * u < dim) atomicAdd(dst + lane + 32 * u, (unsigned long long)__float2ll_rn(O[k][u] * kFixScale));
+        for (int u = 0; u < NJ; ++u) acc[j][u] = 0.f;
+      }
+      for (uint32_t m = ctx; m; m &= m - 1) {
+        const int t = __ffs(m) - 1;
+        float h[NJ];
+        det_load(h, hrow + (size_t)(c + W + t - hw) * dim, dim, lane, true);
+#pragma unroll
+        for (int j = 0; j < 2; ++j) {
+          const float gk = gs[t * KO + k0 + j] * osc[c * KO + k0 + j];
+#pragma unroll
+          for (int u = 0; u < NJ; ++u) acc[j][u] = __fmaf_rn(gk, h[u], acc[j][u]);
+        }
+      }
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {
+        const int k = k0 + j;
+        if (!((used >> k) & 1u)) continue;
+        if ((owned >> k) & 1u) {
+          float* row = a.w_out + (int64_t)orid[c * KO + k] * a.ld;
+#pragma unroll
+          for (int u = 0; u < NJ; ++u) {
+            const long long v = __float2ll_rn(acc[j][u] * kFixScale);
+            if (lane + 32 * u < dim && v != 0) row[lane + 32 * u] = det_fix_add(x[j][u], v);
+          }
+          continue;
+        }
+        unsigned long long* dst = a.acc + (int64_t)__shfl_sync(0xffffffffu, oslot, k) * dim;
+#pragma unroll
+        for (int u = 0; u < NJ; ++u)
+          if (lane + 32 * u < dim) atomicAdd(dst + lane + 32 * u, (unsigned long long)__float2ll_rn(acc[j][u] * kFixScale));
+      }
     }
   }
   if (lane == 0) {
