@@ -1,4 +1,4 @@
-"""adagrad, rowwise_adagrad and adam: row Adds, an embedding-collection training step and whole-table Adds.
+"""adagrad, rowwise_adagrad, adam and ftrl: row Adds, an embedding-collection training step and whole-table Adds.
 
     python bench/adam.py [--iters 20] [--out FILE]
 
@@ -17,8 +17,9 @@ Times are CUDA-event times over ``--iters`` calls after three warm-up calls, the
 names the card and its power limit, read in the same run. Words moved per element of a whole-table Add: adagrad
 reads the delta, the row and its state and writes both (5); rowwise_adagrad reads the delta twice and the row and
 writes the row (4, plus one accumulator read and write per row); adam reads the delta, the row, m and v and writes
-the last three (7, plus one step count read and write per row). The AddOption is lr 0.05, rho 0.1, momentum 0.9
-(adam's beta1; the other updaters ignore it).
+the last three (7, plus one step count read and write per row); ftrl reads the delta, the row, z and n and writes
+the last three (7). The AddOption is lr 0.05, rho 0.1, momentum 0.9 and lambda 0.1 (adam's beta1 is momentum; ftrl's
+alpha, lambda1 and lambda2 are rho, lambda and momentum; the other updaters ignore what they do not use).
 """
 import argparse
 import json
@@ -29,8 +30,9 @@ import sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 
-UPDATERS = ["adagrad", "rowwise_adagrad", "adam"]
-WORDS = {"adagrad": 5, "rowwise_adagrad": 4, "adam": 7}
+UPDATERS = ["adagrad", "rowwise_adagrad", "adam", "ftrl"]
+WORDS = {"adagrad": 5, "rowwise_adagrad": 4, "adam": 7, "ftrl": 7}
+ROW_STATE = ("rowwise_adagrad", "adam")        # one state word per row, read and written
 
 
 def gpu_info():
@@ -73,7 +75,7 @@ def main():
     mv.init()
     card = gpu_info()
     g = torch.Generator(device="cuda").manual_seed(1)
-    opt = mv.AddOption(learning_rate=0.05, rho=0.1, momentum=0.9)
+    opt = mv.AddOption(learning_rate=0.05, rho=0.1, momentum=0.9, lambda_=0.1)
     lines = []
 
     def state_bytes(*tables):
@@ -130,7 +132,7 @@ def main():
     for upd in UPDATERS:
         t = mv.ArrayTable(n, "float32", updater=upd)
         ms = timed(lambda: t.add(d, opt), a.iters)
-        gb = n * 4 * (WORDS[upd] + (2 if upd != "adagrad" else 0)) / 1e9
+        gb = n * 4 * (WORDS[upd] + (2 if upd in ROW_STATE else 0)) / 1e9
         emit({"bench": "whole_add_1d", "updater": upd, "size": n, "ms": round(ms, 4),
               "gbps_counted": round(gb / (ms / 1e3), 1), "state_bytes": state_bytes(t)})
         t.free()

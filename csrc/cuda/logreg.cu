@@ -170,13 +170,8 @@ lr_dense_grad_kernel(MvbLrDense a) {
 __global__ void ftrl_weights_kernel(const float* z, const float* n, float* w, int64_t len,
                                     float alpha, float beta, float l1, float l2) {
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < len; i += stride) {
-    float zi = z[i];
-    float sgn = zi < 0.f ? -1.f : 1.f;
-    float out = 0.f;
-    if (sgn * zi > l1) out = (sgn * l1 - zi) / ((beta + sqrtf(n[i])) / alpha + l2);
-    w[i] = out;
-  }
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < len; i += stride)
+    w[i] = ftrl_weight<float>(z[i], [&] { return n[i]; }, alpha, beta, l1, l2);
 }
 __global__ void ftrl_update_kernel(float* z, float* n, const float* w, const float* g, int64_t len,
                                    float alpha) {

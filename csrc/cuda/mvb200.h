@@ -19,8 +19,8 @@ extern "C" {
 
 /* element types */
 enum { MVB_F32 = 0, MVB_F64 = 1, MVB_I32 = 2, MVB_I64 = 3, MVB_I8 = 4 };
-/* updaters (reference: -updater_type default|sgd|momentum_sgd|adagrad|dcasgd|dcasgda, plus rowwise_adagrad and
- * adam).
+/* updaters (reference: -updater_type default|sgd|momentum_sgd|adagrad|dcasgd|dcasgda, plus rowwise_adagrad, adam
+ * and ftrl).
  * rowwise_adagrad is AdaGrad with one accumulator per (worker, table row): h += mean_j (g_j / lr)^2 over the
  * row's C columns, d_j -= rho * rsqrt(h + 1e-6) * g_j / lr. Its state slab is indexed by local row, not by
  * element, so the entry points that update whole rows take the row length (MvbDenseAdd.num_col,
@@ -32,7 +32,16 @@ enum { MVB_F32 = 0, MVB_F64 = 1, MVB_I32 = 2, MVB_I64 = 3, MVB_I8 = 4 };
  * state1, indexed by element (state_stride >= the shard's elements), and t of local row r is state1[state_stride
  * + r], after v's slab; a shard of R rows x C needs 2 round4(R C) + round4(R) elements. Like rowwise_adagrad it
  * needs the row length (mvb_push_dense_adam for the one-sided push) and mvb_updater_apply and
- * mvb_push_dense_stateful return -2 for it. Integer tables keep the plain add.
+ * mvb_push_dense_stateful return -2 for it.
+ * ftrl is FTRL-Proximal (McMahan et al. 2013) with per-element z and n, shared by every worker. With
+ * g = delta / lr, alpha = rho, lambda1 = lambda, lambda2 = momentum and beta = 1, one worker's delta is one step per
+ * element with g != 0: sigma = g^2 / (alpha (sqrt(n + g^2) + sqrt(n))), z += g - sigma d, n += g^2,
+ * d = |z| <= lambda1 ? 0 : (sign(z) lambda1 - z) / ((beta + sqrt(n)) / alpha + lambda2). An element with g == 0
+ * keeps d, z and n. Its state geometry is momentum_sgd's with two slabs: z is state0 and n state1, both indexed by
+ * element (state_stride >= the shard's elements; a shard of R rows x C needs 2 round4(R C) elements). It is an
+ * element-wise updater: mvb_add_dense_fused, mvb_updater_apply, mvb_push_dense_stateful, mvb_add_rows_owner and
+ * mvb_rowbox_apply serve it, and mvb_push_dense_rowwise and mvb_push_dense_adam return -2 for it.
+ * Integer tables keep the plain add.
  * Code 6 is left unassigned: it is the "unknown updater" of the dispatch tests. */
 enum {
   MVB_UPD_DEFAULT = 0,
@@ -42,7 +51,8 @@ enum {
   MVB_UPD_DCASGD = 4,
   MVB_UPD_DCASGDA = 5,
   MVB_UPD_ROWWISE_ADAGRAD = 7,
-  MVB_UPD_ADAM = 8
+  MVB_UPD_ADAM = 8,
+  MVB_UPD_FTRL = 9
 };
 
 /* Same 20-byte layout as the reference AddOption (updater.h:13-69):
@@ -148,7 +158,7 @@ typedef struct MvbDenseAdd {
 int mvb_add_dense_fused(const MvbDenseAdd* a, void* stream);
 
 /* Local (single-source) updater apply: the stand-alone K9 kernel used by the
- * NCCL comparator path and by row-wise / whole adds with one worker. Element-wise updaters only
+ * NCCL comparator path and by row-wise / whole adds with one worker. Element-wise updaters only, ftrl included
  * (-2 for rowwise_adagrad and adam, which need rows). */
 int mvb_updater_apply(int dtype, int updater, void* data, const void* delta, void* state0,
                       void* state1, int64_t n, const MvbAddOpt* opt, float scale, void* stream);
@@ -181,8 +191,9 @@ int mvb_push_dense_red(int dtype, const void* delta, int nservers, void* const* 
                        void* stream);
 
 /* One-sided async push for STATEFUL updaters: remote read-modify-write of the owners' shard +
- * state slabs (state must be peer-mapped). Per-worker state is exact; data is Hogwild.
- * f32 / f64 and the momentum, AdaGrad, DC-ASGD and DC-ASGD-A updaters only (-1 / -2 otherwise). */
+ * state slabs (state must be peer-mapped). Per-worker state is exact; data is Hogwild, and so is the shared state
+ * of momentum_sgd and ftrl (exact for one pusher). f32 / f64 and the momentum, AdaGrad, DC-ASGD, DC-ASGD-A and ftrl
+ * updaters only (-1 / -2 otherwise). */
 int mvb_push_dense_stateful(int dtype, int updater, const void* delta, int nservers,
                             void* const* shard_ptrs, void* const* state0_ptrs, void* const* state1_ptrs,
                             const int64_t* shard_offs, const int64_t* shard_lens,
@@ -237,7 +248,8 @@ int mvb_add_rows_delta(const MvbRowMap* m, const int64_t* row_ids, int64_t k, co
  * occurrences that are not adjacent race. rowwise_adagrad indexes its state slab by local row
  * (state_stride >= row_hi - row_lo). adam indexes m and v by element and keeps the step counts after v's slab
  * (state_stride >= (row_hi - row_lo) * num_col, else MVB_BAD_ROW_MAP before any CUDA call); a repeated row
- * counts one step per occurrence. */
+ * counts one step per occurrence. ftrl indexes z and n by element like momentum_sgd; a repeated row is one step
+ * per occurrence. */
 int mvb_add_rows_owner(int dtype, int updater, void* shard, void* state0, void* state1,
                        int64_t row_lo, int64_t row_hi, int64_t num_col, int64_t state_stride,
                        const int64_t* row_ids, int64_t k, const void* vals, int64_t vals_ld,
@@ -514,7 +526,8 @@ int mvb_rowbox_push_vals(const MvbRowBox* b, const int* ids, const int* n_ptr, i
                          int ctas_per_sm, void* stream);
 int mvb_rowbox_poll(const MvbRowBox* b, int src, int wait, void* stream);
 /* state_stride: elements per source slab; rowwise_adagrad indexes its slab by local row; adam's m and v are
- * element slabs, its step counts follow v's slab (st1 + state_stride + local row) */
+ * element slabs, its step counts follow v's slab (st1 + state_stride + local row); ftrl's z (st0) and n (st1) are
+ * element slabs */
 int mvb_rowbox_apply(const MvbRowBox* b, int updater, float* shard, float* st0, float* st1,
                      int64_t state_stride, int64_t row_lo, int src, int ctas_per_sm, void* stream);
 

@@ -199,6 +199,7 @@ MVB_DEVINL void red_add(int* p, int v) { red_add_s32(p, v); }
 //   dcasgda  : s0 = shadow copy, s1 = mean sq  (per worker)
 //   rowwise_adagrad : s0 = G^2 history of a ROW (per worker, one element per local row)
 //   adam     : s0 = m, s1 = v (shared), and a step count t per ROW after v's slab (see row_state_at)
+//   ftrl     : s0 = z, s1 = n                  (shared across workers)
 // Semantics follow the reference accessors (Q1/Q3); AdaGrad implements the
 // *intended* rule (Q2: the reference copies the history by value and subtracts
 // squares, so its history never persists).
@@ -336,6 +337,43 @@ struct Updater<MVB_UPD_ADAM, T> {
   }
   MVB_DEVINL static RowF Shfl(const RowF& f, int src) {
     return {__shfl_sync(0xffffffffu, f.step, src), __shfl_sync(0xffffffffu, f.bc2, src)};
+  }
+};
+
+// FTRL-Proximal's weight from its state (McMahan et al. 2013, Algorithm 1): 0 where |z| <= l1, else
+// (sign(z) l1 - z) / ((beta + sqrt(n)) / alpha + l2). Continuous at |z| = l1, where both branches give 0. Used by the
+// ftrl updater and by the LogisticRegression app's ftrl_weights_kernel. n_of() returns n; it is called only where
+// the weight is not 0, so a caller that loads n from memory loads it only there.
+template <typename T, class N>
+MVB_DEVINL T ftrl_weight(T z, N n_of, T alpha, T beta, T l1, T l2) {
+  const T sgn = z < (T)0 ? (T)-1 : (T)1;
+  T w = (T)0;
+  if (sgn * z > l1) w = (sgn * l1 - z) / ((beta + sqrt(n_of())) / alpha + l2);
+  return w;
+}
+
+// FTRL-Proximal: z (s0) and n (s1) per element, shared by every worker. With g = delta / lr, alpha = rho,
+// l1 = lambda, l2 = momentum and beta = 1 (fixed, as McMahan et al. recommend), one worker's delta is one step:
+//   sigma = g^2 / (alpha (sqrt(n + g^2) + sqrt(n))) ;  z += g - sigma d ;  n += g^2 ;  d = ftrl_weight(z, n, ...)
+// sigma is the cancellation-free form of the reference's (sqrt(n + g^2) - sqrt(n)) / alpha; where g^2 underflows on
+// the first step (n = 0) it takes its limit |g| / alpha instead of 0 / 0. An element with g == 0 is not stepped: d, z
+// and n keep their bits (as the LogReg app's ftrl_update_kernel), so an Add never replaces an untouched element by
+// the closed form of its state.
+template <typename T>
+struct Updater<MVB_UPD_FTRL, T> {
+  static constexpr int kStates = 2;
+  static constexpr bool kPerWorker = false;
+  static constexpr bool kRowState = false;
+  static constexpr bool kRowSum = false, kElemState = false;
+  MVB_DEVINL static void Apply(T& d, T g, T& z, T& n, const MvbAddOpt& o) {
+    const T gn = g / (T)o.lr;
+    if (gn == (T)0) return;
+    const T alpha = (T)o.rho, g2 = gn * gn;
+    const T den = alpha * (sqrt(n + g2) + sqrt(n));
+    const T sigma = den > (T)0 ? g2 / den : fabs(gn) / alpha;
+    z += gn - sigma * d;
+    n += g2;
+    d = ftrl_weight<T>(z, [&] { return n; }, alpha, (T)1, (T)o.lambda, (T)o.momentum);
   }
 };
 
@@ -586,6 +624,7 @@ static inline int with_updater(int upd, F&& f) {
       case MVB_UPD_DCASGDA: return f(integral_constant<int, MVB_UPD_DCASGDA>{});
       case MVB_UPD_ROWWISE_ADAGRAD: return f(integral_constant<int, MVB_UPD_ROWWISE_ADAGRAD>{});
       case MVB_UPD_ADAM: return f(integral_constant<int, MVB_UPD_ADAM>{});
+      case MVB_UPD_FTRL: return f(integral_constant<int, MVB_UPD_FTRL>{});
     }
     return -2;
   }

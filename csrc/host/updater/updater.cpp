@@ -6,6 +6,7 @@
 #include "multiverso/updater/adam_updater.h"
 #include "multiverso/updater/dcasgd_updater.h"
 #include "multiverso/updater/dcasgda_updater.h"
+#include "multiverso/updater/ftrl_updater.h"
 #include "multiverso/updater/momentum_updater.h"
 #include "multiverso/updater/rowwise_adagrad_updater.h"
 #include "multiverso/updater/sgd_updater.h"
@@ -50,6 +51,7 @@ Updater<T>* Updater<T>::GetUpdater(size_t size, size_t num_col) {
   if (type == "dcasgda") return new DCASGDAUpdater<T>(size);
   if (type == "rowwise_adagrad") return new RowwiseAdaGradUpdater<T>(size, num_col);
   if (type == "adam") return new AdamUpdater<T>(size, num_col);
+  if (type == "ftrl") return new FTRLUpdater<T>(size);
   if (type != "default") Log::Error("unknown updater_type '%s', using default", type.c_str());
   return new Updater<T>();
 }

@@ -77,8 +77,8 @@ class Updater {
   virtual size_t StateBytes() const { return 0; }
   virtual void StoreState(char*) const {}
   virtual void LoadState(const char*) {}
-  // Factory on -updater_type: default|sgd|adagrad|momentum_sgd|dcasgd|dcasgda|rowwise_adagrad|adam, for a shard of
-  // `size` elements in rows of `num_col` (the row length of a row-state updater; 1 for an array).
+  // Factory on -updater_type: default|sgd|adagrad|momentum_sgd|dcasgd|dcasgda|rowwise_adagrad|adam|ftrl, for a
+  // shard of `size` elements in rows of `num_col` (the row length of a row-state updater; 1 for an array).
   static Updater<T>* GetUpdater(size_t size = 0, size_t num_col = 1);
 };
 

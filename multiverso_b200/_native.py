@@ -23,10 +23,11 @@ F32, F64, I32, I64, I8 = 0, 1, 2, 3, 4
 UPD_DEFAULT, UPD_SGD, UPD_MOMENTUM, UPD_ADAGRAD, UPD_DCASGD, UPD_DCASGDA = range(6)
 UPD_ROWWISE_ADAGRAD = 7          # 6 is unassigned
 UPD_ADAM = 8
+UPD_FTRL = 9
 UPDATER_NAMES = {
     "default": UPD_DEFAULT, "sgd": UPD_SGD, "momentum_sgd": UPD_MOMENTUM,
     "adagrad": UPD_ADAGRAD, "dcasgd": UPD_DCASGD, "dcasgda": UPD_DCASGDA,
-    "rowwise_adagrad": UPD_ROWWISE_ADAGRAD, "adam": UPD_ADAM,
+    "rowwise_adagrad": UPD_ROWWISE_ADAGRAD, "adam": UPD_ADAM, "ftrl": UPD_FTRL,
 }
 
 _LIBDIR = Path(__file__).resolve().parent / "_lib"

@@ -127,7 +127,8 @@ class DenseDeviceTable(_AsyncOps):
             "default": (0, False, False, False), "sgd": (0, False, False, False),
             "momentum_sgd": (1, False, False, False), "adagrad": (1, True, False, False),
             "dcasgd": (1, True, False, False), "dcasgda": (2, True, False, False),
-            "rowwise_adagrad": (1, True, True, False), "adam": (2, False, False, True)}[name]
+            "rowwise_adagrad": (1, True, True, False), "adam": (2, False, False, True),
+            "ftrl": (2, False, False, False)}[name]
         self.n_states, self.state_per_worker, self.state_per_row = nst, per_worker, per_row
         # a slab holds one element per shard element, or per shard row; slabs start at multiples of 4 elements
         gran = self.num_col if per_row else 1

@@ -7,6 +7,7 @@ table/matrix_table.h:116-127, table/matrix.h:14-22, table/kv_table.h:120-124).
 """
 from __future__ import annotations
 
+import math
 import struct
 from dataclasses import dataclass
 from typing import Optional
@@ -52,7 +53,18 @@ def _f32(x: float) -> float:
 def check_add_option(updater: str, opt: AddOption) -> None:
     """Raises ValueError for an AddOption the updater cannot step with, as the fp32 values it travels as: adam needs
     beta1 (``momentum``) in [0, 1), ``learning_rate > 0`` (it recovers the gradient as delta / learning_rate) and
-    ``rho >= 0`` (the step size)."""
+    ``rho >= 0`` (the step size). ftrl needs finite ``learning_rate > 0``, ``rho > 0`` (alpha), ``lambda_ >= 0``
+    (lambda1) and ``momentum >= 0`` (lambda2)."""
+    if updater == "ftrl":
+        try:
+            lr, alpha, l1, l2 = (_f32(x) for x in (opt.learning_rate, opt.rho, opt.lambda_, opt.momentum))
+        except OverflowError:          # beyond the fp32 range
+            lr = alpha = l1 = l2 = float("inf")
+        if not (math.isfinite(lr + alpha + l1 + l2) and lr > 0.0 and alpha > 0.0 and l1 >= 0.0 and l2 >= 0.0):
+            raise ValueError(f"ftrl needs finite learning_rate > 0, rho (alpha) > 0, lambda_ (lambda1) >= 0 and "
+                             f"momentum (lambda2) >= 0 as fp32, got learning_rate={opt.learning_rate}, "
+                             f"rho={opt.rho}, lambda_={opt.lambda_}, momentum={opt.momentum}")
+        return
     if updater != "adam":
         return
     b1, lr, rho = _f32(opt.momentum), _f32(opt.learning_rate), _f32(opt.rho)
