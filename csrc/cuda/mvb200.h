@@ -836,6 +836,41 @@ int mvb_ss_sample(const MvbSampledSoftmax* a, void* stream);
 int mvb_ss_fwd_epilogue(const MvbSampledSoftmax* a, void* stream);
 int mvb_ss_bwd_epilogue(const MvbSampledSoftmax* a, void* stream);
 
+/* ---- hierarchical softmax over a row-sharded fp32 MatrixTable (hier_softmax.cu) ------------------------------- */
+/* Row p of the table is inner node p of a tree whose leaves are the n_classes labels. Example b with label y walks
+ * the path points[y, 0..L) (root first, L = lens[y]) with branch codes codes[y, 0..L):
+ *   z_i = hidden_b . w_{p_i},  loss_b = sum_i softplus(-(1 - 2 c_i) z_i),  g_i = sigmoid(z_i) - (1 - c_i),
+ *   u_b = sum_i g_i w_{p_i}   (so dloss_b / dhidden_b = u_b)
+ * One warp per example, rows read from their owners' shards as mvb_get_rows reads them. Every sum has a fixed order
+ * and no atomics: loss, g and u are bitwise reproducible and the same for every sharding. Widths above
+ * MVB_HSM_MAX_DIM are refused (-80). The caller validates labels (in [0, n_classes)) and that the tree's inner
+ * nodes are < wmap.num_row. Errors, all before any CUDA call: MVB_BAD_ROW_MAP; -80 dim (4 <= dim <= MVB_HSM_MAX_DIM,
+ * % 4 == 0, <= wmap.num_col) or a row pitch not % 4; -81 n_classes < 2, n_classes - 1 > wmap.num_row, or ldp outside
+ * [1, MVB_HSM_MAX_PATH]; -82 B < 0 or a pitch (ldh, ldu) below dim or not % 4; -83 a missing input, ids or g without
+ * offsets, or hidden, u or a shard not 16-byte aligned. B == 0 launches nothing. */
+#define MVB_HSM_MAX_DIM 1024
+#define MVB_HSM_MAX_PATH 64
+typedef struct MvbHsm {
+  MvbRowMap wmap;            /* fp32 shards, row pitch wmap.num_col (% 4 == 0); row p is inner node p          */
+  int64_t dim;               /* columns used                                                                 */
+  const float* hidden;       /* [B x ldh], 16-byte aligned                                                   */
+  int64_t B, ldh;
+  const int64_t* labels;     /* [B] in [0, n_classes)                                                        */
+  int64_t n_classes;         /* leaves; the tree has n_classes - 1 inner nodes                               */
+  const int* points;         /* [n_classes x ldp] inner-node ids of each label's path, root first            */
+  const signed char* codes;  /* [n_classes x ldp] branch codes, 0 or 1                                       */
+  const int* lens;           /* [n_classes] path lengths, 1 <= lens[y] <= ldp                                */
+  int64_t ldp;
+  const int64_t* offsets;    /* [B] exclusive scan of lens[labels]: example b's steps start at offsets[b];
+                                needed with ids or g                                                         */
+  float* loss;               /* [B] out, or NULL                                                             */
+  int64_t* ids;              /* [sum of lens[labels]] out: the path node of every step, or NULL              */
+  float* g;                  /* [sum of lens[labels]] out: dloss / dz of every step, or NULL                 */
+  float* u;                  /* [B x ldu] out, 16-byte aligned, columns >= dim untouched, or NULL            */
+  int64_t ldu;
+} MvbHsm;
+int mvb_hsm_fwd(const MvbHsm* a, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

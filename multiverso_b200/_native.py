@@ -218,6 +218,15 @@ class SampledSoftmax(C.Structure):
                 ("loss", vp), ("lse", vp), ("t_true", vp), ("g", vp), ("e_t", vp), ("e_true", vp)]
 
 
+HSM_MAX_DIM, HSM_MAX_PATH = 1024, 64
+
+
+class Hsm(C.Structure):
+    _fields_ = [("wmap", RowMap), ("dim", i64), ("hidden", vp), ("B", i64), ("ldh", i64), ("labels", vp),
+                ("n_classes", i64), ("points", vp), ("codes", vp), ("lens", vp), ("ldp", i64), ("offsets", vp),
+                ("loss", vp), ("ids", vp), ("g", vp), ("u", vp), ("ldu", i64)]
+
+
 class NativeError(RuntimeError):
     pass
 
@@ -359,6 +368,7 @@ _CUDA_FUNCS = {
     "mvb_ss_sample": _status(C.POINTER(SampledSoftmax), Ptr),
     "mvb_ss_fwd_epilogue": _status(C.POINTER(SampledSoftmax), Ptr),
     "mvb_ss_bwd_epilogue": _status(C.POINTER(SampledSoftmax), Ptr),
+    "mvb_hsm_fwd": _status(C.POINTER(Hsm), Ptr),
 }
 
 

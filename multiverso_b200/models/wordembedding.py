@@ -92,16 +92,23 @@ class HuffmanTables:
             c = c * (cls.FREQ_TOTAL_MAX / 4 / total)
         return np.ascontiguousarray(np.maximum(np.floor(c), 1.0).astype(np.int64))
 
-    def __init__(self, counts: np.ndarray, device):
+    @classmethod
+    def encode(cls, counts: np.ndarray):
+        """The encoder's tree over `int_frequencies(counts)`: (points [V, MAX_CODE] int32, codes [V, MAX_CODE]
+        int8, lens [V] int32, longest). `longest` is the longest code, or -1 when a code is longer than MAX_CODE."""
         from ..apps._applib import lib
         V = len(counts)
-        freq = self.int_frequencies(counts)
-        P = np.zeros((V, self.MAX_CODE), dtype=np.int32)
-        Cd = np.zeros((V, self.MAX_CODE), dtype=np.int8)
+        freq = cls.int_frequencies(counts)
+        P = np.zeros((V, cls.MAX_CODE), dtype=np.int32)
+        Cd = np.zeros((V, cls.MAX_CODE), dtype=np.int8)
         lens = np.zeros(V, dtype=np.int32)
-        longest = lib().MVA_HuffmanBuild(freq.ctypes.data_as(C.c_void_p), V, self.MAX_CODE,
+        longest = lib().MVA_HuffmanBuild(freq.ctypes.data_as(C.c_void_p), V, cls.MAX_CODE,
                                          P.ctypes.data_as(C.c_void_p), Cd.ctypes.data_as(C.c_void_p),
                                          lens.ctypes.data_as(C.c_void_p))
+        return P, Cd, lens, int(longest)
+
+    def __init__(self, counts: np.ndarray, device):
+        P, Cd, lens, longest = self.encode(counts)
         if longest < 0:
             Log.fatal("Huffman code longer than %d", self.MAX_CODE)
         self.max_code = max(int(longest), 1)

@@ -3,6 +3,7 @@ from .embedding_collection import EmbeddingBagConfig, PSEmbeddingCollection
 from .full_softmax import (FullSoftmaxResult, PSFullSoftmax, full_softmax, full_softmax_grad_reference,
                            full_softmax_reference, topk_dot)
 from .get_gemm import gemm_nt, get_gemm, get_gemm_supported
+from .hierarchical_softmax import PSHierarchicalSoftmax, hierarchical_softmax_reference
 from .ps_linear import PSLinear, ps_linear
 from .sampled_softmax import PSSampledSoftmax
 from .topk import TOPK_MAX, topk_cosine, topk_cosine_reference
@@ -11,4 +12,5 @@ __all__ = ["get_gemm", "get_gemm_supported", "ps_linear", "PSLinear", "topk_cosi
            "TOPK_MAX", "embedding_bag", "embedding_bag_reference", "PSEmbedding",
            "EmbeddingBagConfig", "PSEmbeddingCollection", "gemm_nt", "PSSampledSoftmax",
            "full_softmax", "full_softmax_reference", "topk_dot", "FullSoftmaxResult",
-           "PSFullSoftmax", "full_softmax_grad_reference"]
+           "PSFullSoftmax", "full_softmax_grad_reference", "PSHierarchicalSoftmax",
+           "hierarchical_softmax_reference"]
