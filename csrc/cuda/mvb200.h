@@ -871,6 +871,48 @@ typedef struct MvbHsm {
 } MvbHsm;
 int mvb_hsm_fwd(const MvbHsm* a, void* stream);
 
+/* ---- factorization machine over a row-sharded fp32 MatrixTable (fm.cu) ------------------------------------------ */
+/* Row r holds the k = dim - 1 factors v_r = W[r, 0:k] and the linear weight W[r, k]. Bag b holds the lookups
+ * [offsets[b], offsets[b + 1]) (the last bag ends at L) with ids i_j and values x_j:
+ *   S_b = sum_j x_j W[i_j, :dim],  q_b = sum_j x_j^2 |v_{i_j}|^2,  y_b = S_b[k] + (|S_b[0:k]|^2 - q_b) / 2
+ * (an empty bag gives 0). S_b is summed exactly as mvb_embedding_bag_fwd sums the bag with per-sample weights x.
+ * The backward pushes, once per unique row r, scale * sum over the lookups j of r of dy_b x_j (S'_b - x_j v'_r),
+ * S'_b being S_b with column k set to 1 and v'_r being v_r with 0 in column k, through the epilogues of
+ * MvbEmbBag. Results are bitwise reproducible and the same for every sharding; rows are read from their owners'
+ * shards as mvb_get_rows reads them. The caller validates ids (in [0, num_row)) and offsets. Errors, all before any
+ * CUDA call: MVB_BAD_ROW_MAP; -90 dim outside [2, MVB_FM_MAX_DIM] or above wmap.num_col, a row pitch not % 4, or a
+ * shard not 16-byte aligned; -91 B < 0, L < 0, or offsets / ids missing; -92 (fwd) y missing with B > 0, or sp set with a bad
+ * pitch or alignment; -93 (bwd, L > 0) dy, sp, perm or scratch missing, sp's pitch or alignment bad, or scratch too
+ * small; -94 (bwd) an unknown epilogue or a compact gradient without uniq, with a bad pitch or alignment. B == 0
+ * (fwd) and L == 0 (bwd) launch nothing. */
+#define MVB_FM_MAX_DIM 1024
+typedef struct MvbFm {
+  MvbRowMap wmap;            /* fp32 shards, row pitch wmap.num_col (% 4 == 0), 16-byte aligned             */
+  int64_t dim;               /* C = k + 1 columns used, 2 <= C <= min(MVB_FM_MAX_DIM, wmap.num_col)          */
+  const int64_t* ids;        /* [L]; backward: sorted ascending, equal ids in ascending position             */
+  int64_t L;
+  const int64_t* offsets;    /* [B]: offsets[0] == 0, non-decreasing, <= L                                   */
+  int64_t B;
+  const float* values;       /* [L] x by lookup position, or NULL (every x is 1)                             */
+  float* y;                  /* forward: [B] out                                                             */
+  float* sp;                 /* [B x lds] S': forward out (NULL: not written), backward in; 16-byte aligned   */
+  int64_t lds;               /* % 4 == 0, >= round4(dim); columns in [dim, round4(dim)) are written 0         */
+  const float* dy;           /* backward: [B] dL/dy                                                          */
+  const int64_t* perm;       /* backward: lookup position of each sorted id                                  */
+  int epilogue;              /* MVB_EMB_PUSH (red.add into the owner's row) or MVB_EMB_COMPACT               */
+  float scale;
+  float* grads;              /* compact: [U x ldg] (ldg % 4 == 0), 16-byte aligned; NULL: only write *n_unique */
+  int64_t ldg;
+  int64_t* uniq;             /* compact: [U] ascending                                                       */
+  int64_t* n_unique;         /* backward: device int64, the number of unique ids U, or NULL                  */
+  void* scratch;             /* backward: mvb_embedding_bag_scratch_bytes(L, dim) bytes of device memory      */
+  int64_t scratch_bytes;
+  int64_t push_rows;         /* backward: > 0: rows >= push_rows get no epilogue and are not counted (as in
+                                MvbEmbBag); <= 0: every row                                                  */
+} MvbFm;
+int mvb_fm_fwd(const MvbFm* a, void* stream);
+int mvb_fm_bwd(const MvbFm* a, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

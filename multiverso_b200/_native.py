@@ -227,6 +227,16 @@ class Hsm(C.Structure):
                 ("loss", vp), ("ids", vp), ("g", vp), ("u", vp), ("ldu", i64)]
 
 
+FM_MAX_DIM = 1024
+
+
+class Fm(C.Structure):
+    _fields_ = [("wmap", RowMap), ("dim", i64), ("ids", vp), ("L", i64), ("offsets", vp), ("B", i64),
+                ("values", vp), ("y", vp), ("sp", vp), ("lds", i64), ("dy", vp), ("perm", vp), ("epilogue", C.c_int),
+                ("scale", C.c_float), ("grads", vp), ("ldg", i64), ("uniq", vp), ("n_unique", vp), ("scratch", vp),
+                ("scratch_bytes", i64), ("push_rows", i64)]
+
+
 class NativeError(RuntimeError):
     pass
 
@@ -369,6 +379,8 @@ _CUDA_FUNCS = {
     "mvb_ss_fwd_epilogue": _status(C.POINTER(SampledSoftmax), Ptr),
     "mvb_ss_bwd_epilogue": _status(C.POINTER(SampledSoftmax), Ptr),
     "mvb_hsm_fwd": _status(C.POINTER(Hsm), Ptr),
+    "mvb_fm_fwd": _status(C.POINTER(Fm), Ptr),
+    "mvb_fm_bwd": _status(C.POINTER(Fm), Ptr),
 }
 
 
