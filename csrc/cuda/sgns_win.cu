@@ -850,230 +850,302 @@ __global__ void __launch_bounds__(kPlanThreads) sgns_det_plan_slots(const __grid
 
 // x + the fixed-point sum v: what the apply writes for an element whose sum is nonzero
 MVB_DEVINL float det_fix_add(float x, long long v) { return x + (float)((double)v * (1.0 / (double)kFixScale)); }
-template <int NJ>
-MVB_DEVINL void det_load(float (&v)[NJ], const float* row, int dim, int lane, bool on) {
-#pragma unroll
-  for (int u = 0; u < NJ; ++u) v[u] = (on && lane + 32 * u < dim) ? row[lane + 32 * u] : 0.f;
-}
-template <int NJ>
-MVB_DEVINL float det_dot(const float (&x)[NJ], const float (&y)[NJ]) {
-  float s = 0.f;
-#pragma unroll
-  for (int u = 0; u < NJ; ++u) s = __fmaf_rn(x[u], y[u], s);
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-  return s;
-}
 
-// Centres per CTA (one warp each) that the registers of a <NJ, KO> warp allow: its output rows stay in
-// registers, KO * NJ of them (60 at dim 300 with 5 negatives), so wide rows get fewer, fatter warps per SM.
-__host__ __device__ constexpr int det_max_s(int nj, int ko) { return nj * ko <= 64 ? 20 : nj * ko <= 96 ? 12 : 8; }
+// Warps of a wave CTA: 32 at 64 registers for rows up to 320 floats; wider rows keep their int64 and float sums in
+// registers with 16 warps at 128.
+__host__ __device__ constexpr int det_warps(int nj) { return nj <= 10 ? 32 : 16; }
+constexpr int kDetMaxS = 32;                      // centres per CTA: the scoring units are listed by one warp
 
-// Shared memory of a CTA of S centres: per staged position (S + 2W of them) an int64 accumulator row, the input
-// row and its id / scale / slot; per (centre, output row) its id and scale; per (centre, offset, output row) the
-// pair's error term.
+// Shared memory of a CTA of S centres: the 1+K output rows of every centre and the input row of every staged
+// position (S + 2W of them), rows padded to 16 bytes; per (centre, offset, output row) the pair's error term and
+// loss term; per staged position its id / scale / slot; per (centre, output row) its id / scale / slot; per centre
+// its window and the rows it uses; the slice's scoring units.
 __host__ __device__ inline size_t det_smem_bytes(int S, int W, int dim, int ko) {
-  return (size_t)(S + 2 * W) * ((size_t)dim * 12 + 12) + (size_t)S * ko * 8 + (size_t)S * (2 * W + 1) * ko * 4;
+  const size_t dimp = (size_t)(dim + 3) / 4 * 4;
+  return ((size_t)S * ko + S + 2 * W) * dimp * 4 + (size_t)S * (2 * W + 1) * ko * 8 + (size_t)S * 8 +
+         (size_t)(S + 2 * W) * 12 + (size_t)S * ko * 12 + (size_t)S * 4 + (size_t)S * W * 4 + 16;
 }
 
-// One CTA owns S consecutive centres [s0, s0 + S) of the wave, one warp per centre.  The slice's rows, scales,
-// windows and slots come from the plan; the input rows of the positions [s0 - W, s0 + S + W) that are a context
-// are staged once in shared memory, and each position's input delta is summed there over all its centres before
-// one row of REDs sends it to its accumulator slot.  The float arithmetic of every (centre, context) pair does not
-// depend on the tiling (element j on lane j % 32, register j / 32, fixed FMA chains and butterflies, one
-// conversion to fixed point per pair and per (centre, k)); only the grouping of the exact int64 sums does, so the
-// result is bitwise independent of S.
+MVB_DEVINL void det_cp16(float* dst, const float* src) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(dst)), "l"(src) : "memory");
+}
+MVB_DEVINL void det_cp4(float* dst, const float* src) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(smem_u32(dst)), "l"(src) : "memory");
+}
+
+// One CTA owns S consecutive centres [s0, s0 + S) of the wave.  It stages the 1+K output rows of every centre with a
+// context and the input rows of the positions [s0 - W, s0 + S + W) that are a context, all at once with cp.async,
+// then works from shared memory in two phases split by one barrier, each spread over all warps:
+//   scoring    a warp per two contexts of a centre: the 2 x (1+K) dots, in flight together and each output row
+//              read once for both, give the pairs' error terms (and the loss terms of loss-sampled centres) in
+//              shared memory;
+//   deltas     a warp per staged position sums, in int64 registers, the fixed-point input delta of every pair that
+//              writes it, then applies it in place (its only reader in the wave) or sends one row of REDs to its
+//              accumulator slot; a warp per (centre, pair of output rows) sums their output deltas over the centre's
+//              contexts and does the same, a row it alone reads taking the staged row as the wave found it.
+// The float arithmetic of every pair does not depend on the tiling (element j on lane j % 32, register j / 32; each
+// dot's FMA chain in element order, then the xor butterfly 16 .. 1; the input delta's chain over k, the output
+// delta's over the contexts in mask order; one conversion to fixed point per pair and per (centre, k); each
+// centre's loss summed in (offset, k) order); only the grouping of the exact int64 sums does, so the result is
+// bitwise independent of S and of the warp count.
 template <int NJ, int KO>
-__global__ void __launch_bounds__(32 * det_max_s(NJ, KO))
+__global__ void __launch_bounds__(32 * det_warps(NJ), 1)
 sgns_det_kernel(const __grid_constant__ DetDev a) {
+  static_assert(KO % 2 == 0, "output deltas are taken in pairs of rows");
+  constexpr int NW = det_warps(NJ);
   extern __shared__ __align__(16) unsigned char smem[];
-  const int S = blockDim.x >> 5, W = a.window, dim = a.dim;
-  const int c = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int S = a.S, W = a.window, dim = a.dim, dimp = (dim + 3) & ~3, span = S + 2 * W, nt = 2 * W + 1;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int64_t s0 = a.p0 + (int64_t)blockIdx.x * S;
   const int ns = (int)(a.p1 - s0 < S ? a.p1 - s0 : S);   // centres of this slice
   const int np = ns + 2 * W;                               // staged positions: i <-> token s0 - W + i
-  unsigned long long* hacc = reinterpret_cast<unsigned long long*>(smem);
-  float* hrow = reinterpret_cast<float*>(hacc + (size_t)(S + 2 * W) * dim);
-  int* crid = reinterpret_cast<int*>(hrow + (size_t)(S + 2 * W) * dim);
-  float* csc = reinterpret_cast<float*>(crid + S + 2 * W);
-  int* cslot = reinterpret_cast<int*>(csc + S + 2 * W);
-  int* orid = cslot + S + 2 * W;
+  float* orow = reinterpret_cast<float*>(smem);            // [S][KO][dimp] output rows
+  float* hrow = orow + (size_t)S * KO * dimp;              // [S + 2W][dimp] input rows
+  float* gsm = hrow + (size_t)span * dimp;                 // [S][2W + 1][KO] error terms, offset t = hw + d
+  float* lsm = gsm + S * nt * KO;                          // [S][2W + 1][KO] loss terms
+  int2* chw = reinterpret_cast<int2*>(lsm + S * nt * KO);  // [S] context mask and half window
+  int* crid = reinterpret_cast<int*>(chw + S);
+  float* csc = reinterpret_cast<float*>(crid + span);
+  int* cslot = reinterpret_cast<int*>(csc + span);
+  int* orid = cslot + span;
   float* osc = reinterpret_cast<float*>(orid + S * KO);
-  float* gsm = osc + S * KO;
+  int* oslot = reinterpret_cast<int*>(osc + S * KO);
+  int* cused = oslot + S * KO;                             // [S] output rows a centre with a context uses
+  int* plist = cused + S;                                  // [S * W] units: centre << 10 | offset tb << 5 | ta
+  int* nunits = plist + S * W;
 
-  // ---- the slice's plan: one thread per staged position, one per (centre, output row) ----------------------
+  // ---- the slice's plan: a thread per staged position, per (centre, output row), per centre ----------------
   const int base = __ldg(a.off + a.wi);                   // the wave's first entry in the list of shared rows
-  const int* pslot = a.slot + a.n_tokens * a.ko + ((int64_t)a.wi * a.spw + blockIdx.x) * (S + 2 * W);
-  for (int t = threadIdx.x; t < np + ns * KO; t += blockDim.x) {
-    if (t < np) {
-      const int64_t q = s0 - W + t;
+  const int* pslot = a.slot + a.n_tokens * a.ko + ((int64_t)a.wi * a.spw + blockIdx.x) * span;
+  for (int x = threadIdx.x; x < np + ns * KO + ns; x += blockDim.x) {
+    if (x < np) {
+      const int64_t q = s0 - W + x;
       const bool in = q >= 0 && q < a.n_tokens;
-      const int sl = __ldg(pslot + t);
-      crid[t] = in ? __ldg(a.in_rid + q) : -1;
-      csc[t] = in ? __ldg(a.in_sc + q) : 1.f;
-      cslot[t] = sl >= 0 ? sl - base : sl;
-    } else {
-      const int ck = t - np, k = ck % KO;
+      const int sl = __ldg(pslot + x);
+      crid[x] = in ? __ldg(a.in_rid + q) : -1;
+      csc[x] = in ? __ldg(a.in_sc + q) : 1.f;
+      cslot[x] = sl >= 0 ? sl - base : sl;
+    } else if (x < np + ns * KO) {
+      const int ck = x - np, k = ck % KO;
       const int64_t e = (s0 + ck / KO) * a.ko + k;
+      const int sl = k < a.ko ? __ldg(a.slot + e) : -2;
       orid[ck] = k < a.ko ? __ldg(a.out_rid + e) : -1;
       osc[ck] = k < a.ko ? __ldg(a.out_sc + e) : 1.f;
+      oslot[ck] = sl >= 0 ? sl - base : sl;
+    } else {
+      chw[x - np - ns * KO] = __ldg(a.chw + s0 + (x - np - ns * KO));
     }
   }
-  const int64_t p = s0 + c;
-  const int2 cx = c < ns ? __ldg(a.chw + p) : make_int2(0, 0);
-  const uint32_t ctx = (uint32_t)cx.x;                    // lane l <-> offset l - hw, staged position c + W + l - hw
-  const int hw = cx.y;
-  int oslot = -2;                                         // this lane's (centre, k = lane)
-  if (ctx && lane < a.ko) {
-    oslot = __ldg(a.slot + p * a.ko + lane);
-    if (oslot >= 0) oslot -= base;
-  }
-  for (int e = threadIdx.x; e < np * dim; e += blockDim.x) hacc[e] = 0ull;
   __syncthreads();
 
-  const int rid = ctx && lane < KO ? orid[c * KO + lane] : -1;
-  const uint32_t used = __ballot_sync(0xffffffffu, rid >= 0);
-  // output rows this (centre, k) alone reads in the wave: applied in place after phase 2
-  const uint32_t owned = __ballot_sync(0xffffffffu, rid >= 0 && oslot == -1);
-  float O[KO][NJ];
-#pragma unroll
-  for (int k = 0; k < KO; ++k) {
-    const int r = __shfl_sync(0xffffffffu, rid, k);
-    det_load(O[k], a.w_out + (int64_t)(r < 0 ? 0 : r) * a.ld, dim, lane, (used >> k) & 1u);
+  // ---- stage every row a pair reads, a warp per row, all copies in flight at once --------------------------
+  const bool vec = (dim & 3) == 0 && (a.ld & 3) == 0 &&
+                   ((reinterpret_cast<uintptr_t>(a.w_in) | reinterpret_cast<uintptr_t>(a.w_out)) & 15) == 0;
+  for (int r = warp; r < np + ns * KO; r += NW) {
+    const float* src;
+    float* dst;
+    if (r < np) {
+      if (cslot[r] < -1) continue;                        // not a context of any centre of the slice
+      src = a.w_in + (int64_t)crid[r] * a.ld;
+      dst = hrow + (size_t)r * dimp;
+    } else {
+      const int ck = r - np;
+      if (!chw[ck / KO].x || orid[ck] < 0) continue;
+      src = a.w_out + (int64_t)orid[ck] * a.ld;
+      dst = orow + (size_t)ck * dimp;
+    }
+    if (vec) {
+      for (int j = lane * 4; j < dim; j += 128) det_cp16(dst + j, src + j);
+    } else {
+      for (int j = lane; j < dim; j += 32) det_cp4(dst + j, src + j);
+    }
   }
-
-  // ---- stage the input rows that are a context of some centre of the slice ----------------------------------
-  for (int i = c; i < np; i += S) {
-    if (cslot[i] < -1) continue;
-    float h[NJ];
-    det_load(h, a.w_in + (int64_t)crid[i] * a.ld, dim, lane, true);
+  // the scoring units, two consecutive contexts of a centre each (offset 31: none), while the copies land
+  if (warp == 0) {
+    int2 cx = make_int2(0, 0);
+    int used = 0;
+    if (lane < ns) {
+      cx = chw[lane];
+      if (cx.x)
+        for (int k = 0; k < KO; ++k) used |= (orid[lane * KO + k] >= 0) << k;
+      cused[lane] = used;
+    }
+    const int pairs = __popc((uint32_t)cx.x), n = (pairs + 1) / 2;
+    int end = n;
 #pragma unroll
-    for (int u = 0; u < NJ; ++u)
-      if (lane + 32 * u < dim) hrow[(size_t)i * dim + lane + 32 * u] = h[u];
+    for (int o = 1; o < 32; o <<= 1) {
+      const int y = __shfl_up_sync(0xffffffffu, end, o);
+      if (lane >= o) end += y;
+    }
+    int at = end - n;
+    for (uint32_t m = (uint32_t)cx.x; m;) {
+      const int ta = __ffs(m) - 1;
+      m &= m - 1;
+      const int tb = m ? __ffs(m) - 1 : 31;
+      m &= m - 1;
+      plist[at++] = lane << 10 | tb << 5 | ta;
+    }
+    if (lane == 31) *nunits = end;
+    const int total = __reduce_add_sync(0xffffffffu, pairs);
+    if (lane == 0 && a.pair_count && total) atomicAdd(a.pair_count, (unsigned long long)total);
   }
+  asm volatile("cp.async.wait_all;" ::: "memory");
   __syncthreads();
 
-  // ---- phase 1 in offset rounds: 1+K dots per (centre, context) on the rows as the wave found them; the
-  // pair's input delta goes to position p + d's accumulator row.  Within a round the centres of the slice hit
-  // distinct positions, so a plain read-add-write is exact; rounds are ordered by the barrier.
-  float* gs = gsm + (size_t)c * (2 * W + 1) * KO;    // [offset + hw][k]: error terms of this centre's pairs
-  const bool want_loss = a.want_loss && (p & 7) == 0;
-  float loss = 0.f;
-  int pairs = 0;
-  for (int d = -W; d <= W; ++d) {
-    const int t = hw + d;
-    if (d != 0 && t >= 0 && ((ctx >> t) & 1u)) {
-      const int i = c + W + d;
-      const float isc = csc[i];
-      {
-        float h[NJ];
-        det_load(h, hrow + (size_t)i * dim, dim, lane, true);
+  // ---- scoring: the 1+K dots of two pairs of a centre on the rows as the wave found them, each output row read
+  // once for both ------------------------------------------------------------------------------------------
+  for (int q = warp; q < *static_cast<volatile int*>(nunits); q += NW) {   // re-read: no register held over the loop
+    const int c = plist[q] >> 10, ta = plist[q] & 31, tb = (plist[q] >> 5) & 31;
+    const int used = cused[c], hw = chw[c].y;
+    const float* ha = hrow + (size_t)(c + W + ta - hw) * dimp;
+    const float* hb = tb != 31 ? hrow + (size_t)(c + W + tb - hw) * dimp : ha;
+    const float* o = orow + (size_t)c * KO * dimp;
+    float s[2][KO];
 #pragma unroll
-        for (int k = 0; k < KO; ++k) {
-          float g = 0.f;
-          if ((used >> k) & 1u) {
-            const float f = det_dot(h, O[k]);
-            g = ((k == 0 ? 1.f : 0.f) - sigm_fast(f)) * a.lr;
-            if (want_loss && lane == 0) loss += 8.f * softplus_neg(k == 0 ? f : -f);
-          }
-          if (lane == k) gs[t * KO + k] = g;              // every lane holds the same butterfly sums
-        }
-      }
-      __syncwarp();
-      // h is dead before e is live: the registers hold the output rows plus one row
-      float e[NJ] = {};
+    for (int k = 0; k < KO; ++k) s[0][k] = s[1][k] = 0.f;
+#pragma unroll
+    for (int u = 0; u < NJ; ++u) {
+      const int j = lane + 32 * u;
+      const bool in = u < NJ - 1 || j < dim;              // NJ = ceil(dim / 32)
+      const float xa = in ? ha[j] : 0.f, xb = in ? hb[j] : 0.f;
 #pragma unroll
       for (int k = 0; k < KO; ++k) {
-        if (!((used >> k) & 1u)) continue;
-        const float g = gs[t * KO + k];
-#pragma unroll
-        for (int u = 0; u < NJ; ++u) e[u] = __fmaf_rn(g * isc, O[k][u], e[u]);
+        const float y = in && ((used >> k) & 1) ? o[k * dimp + j] : 0.f;
+        s[0][k] = __fmaf_rn(xa, y, s[0][k]);
+        s[1][k] = __fmaf_rn(xb, y, s[1][k]);
       }
-      unsigned long long* dst = hacc + (size_t)i * dim;
-#pragma unroll
-      for (int u = 0; u < NJ; ++u)
-        if (lane + 32 * u < dim) dst[lane + 32 * u] += (unsigned long long)__float2ll_rn(e[u] * kFixScale);
-      ++pairs;
     }
-    if (d != 0) __syncthreads();
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1)
+#pragma unroll
+      for (int k = 0; k < KO; ++k) {
+        s[0][k] += __shfl_xor_sync(0xffffffffu, s[0][k], off);
+        s[1][k] += __shfl_xor_sync(0xffffffffu, s[1][k], off);
+      }
+    // every lane holds every dot: lane k takes output row k of the first pair, lane 16 + k of the second
+    const int k = lane & 15, t = lane < 16 ? ta : tb;
+    float f = 0.f;
+#pragma unroll
+    for (int kk = 0; kk < KO; ++kk) {
+      if (lane == kk) f = s[0][kk];
+      if (lane == 16 + kk) f = s[1][kk];
+    }
+    if (k < KO && t != 31) {
+      const int e = (c * nt + t) * KO + k;
+      const bool u = (used >> k) & 1;
+      gsm[e] = u ? ((k == 0 ? 1.f : 0.f) - sigm_fast(f)) * a.lr : 0.f;
+      if (u && a.want_loss && ((s0 + c) & 7) == 0) lsm[e] = 8.f * softplus_neg(k == 0 ? f : -f);
+    }
   }
+  __syncthreads();
 
-  // ---- flush: one row per staged position that is a context (halo rows carry partial sums) ------------------
-  for (int i = c; i < np; i += S) {
-    const int sl = cslot[i];
-    if (sl < -1) continue;
-    if (sl == -1) {                                   // no other staged position reads the row: apply in place
-      float* row = a.w_in + (int64_t)crid[i] * a.ld;
-      for (int j = lane; j < dim; j += 32) {
-        const long long v = (long long)hacc[(size_t)i * dim + j];
-        if (v) row[j] = det_fix_add(hrow[(size_t)i * dim + j], v);
+  // ---- deltas: a unit per staged position, then per (centre, pair of output rows) -------------------------
+  constexpr int KP = KO / 2;
+  const bool tail = lane + 32 * (NJ - 1) < dim;            // this lane holds an element in the last register
+  for (int x = warp; x < np + ns * KP; x += NW) {
+    if (x < np) {
+      const int i = x, sl = cslot[i];
+      if (sl < -1) continue;
+      const float isc = csc[i];
+      unsigned long long v[NJ];
+#pragma unroll
+      for (int u = 0; u < NJ; ++u) v[u] = 0ull;
+      for (int c = (i - 2 * W > 0 ? i - 2 * W : 0); c < ns && c <= i; ++c) {
+        const int d = i - c - W;
+        const int2 cx = chw[c];
+        const int t = cx.y + d;
+        if (d == 0 || t < 0 || !((cx.x >> t) & 1)) continue;
+        const int used = cused[c];
+        const float* g = gsm + (c * nt + t) * KO;
+        const float* o = orow + (size_t)c * KO * dimp + lane;
+        float e[NJ];
+#pragma unroll
+        for (int u = 0; u < NJ; ++u) e[u] = 0.f;
+#pragma unroll
+        for (int k = 0; k < KO; ++k) {
+          if (!((used >> k) & 1)) continue;
+          const float gi = g[k] * isc;
+#pragma unroll
+          for (int u = 0; u < NJ; ++u) e[u] = __fmaf_rn(gi, u < NJ - 1 || tail ? o[k * dimp + 32 * u] : 0.f, e[u]);
+        }
+#pragma unroll
+        for (int u = 0; u < NJ; ++u) v[u] += (unsigned long long)__float2ll_rn(e[u] * kFixScale);
+      }
+      if (sl == -1) {                                     // no other staged position reads the row: in place
+        float* row = a.w_in + (int64_t)crid[i] * a.ld;
+#pragma unroll
+        for (int u = 0; u < NJ; ++u) {
+          const int j = lane + 32 * u;
+          if (j < dim && v[u]) row[j] = det_fix_add(hrow[(size_t)i * dimp + j], (long long)v[u]);
+        }
+      } else {
+        unsigned long long* dst = a.acc + (int64_t)sl * dim;
+#pragma unroll
+        for (int u = 0; u < NJ; ++u) {
+          const int j = lane + 32 * u;
+          if (j < dim && v[u]) atomicAdd(dst + j, v[u]);
+        }
       }
       continue;
     }
-    unsigned long long* dst = a.acc + (int64_t)sl * dim;
-    for (int j = lane; j < dim; j += 32) {
-      const unsigned long long v = hacc[(size_t)i * dim + j];
-      if (v) atomicAdd(dst + j, v);
+    const int c = (x - np) / KP, k0 = (x - np) % KP * 2;
+    const int2 cx = chw[c];
+    const int used = cused[c];
+    if (!((used >> k0) & 3)) continue;
+    float acc[2][NJ];
+#pragma unroll
+    for (int j = 0; j < 2; ++j)
+#pragma unroll
+      for (int u = 0; u < NJ; ++u) acc[j][u] = 0.f;
+    for (uint32_t m = (uint32_t)cx.x; m; m &= m - 1) {
+      const int t = __ffs(m) - 1;
+      const float* h = hrow + (size_t)(c + W + t - cx.y) * dimp;
+      const float g0 = gsm[(c * nt + t) * KO + k0] * osc[c * KO + k0];
+      const float g1 = gsm[(c * nt + t) * KO + k0 + 1] * osc[c * KO + k0 + 1];
+#pragma unroll
+      for (int u = 0; u < NJ; ++u) {
+        const int j = lane + 32 * u;
+        const float hv = u < NJ - 1 || j < dim ? h[j] : 0.f;
+        acc[0][u] = __fmaf_rn(g0, hv, acc[0][u]);
+        acc[1][u] = __fmaf_rn(g1, hv, acc[1][u]);
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      const int k = k0 + j;
+      if (!((used >> k) & 1)) continue;
+      const int sl = oslot[c * KO + k];
+      if (sl == -1) {                                     // this (centre, k) alone reads the row: in place
+        float* row = a.w_out + (int64_t)orid[c * KO + k] * a.ld;
+        const float* x0 = orow + (size_t)(c * KO + k) * dimp;
+#pragma unroll
+        for (int u = 0; u < NJ; ++u) {
+          const int e = lane + 32 * u;
+          const long long v = __float2ll_rn(acc[j][u] * kFixScale);
+          if (e < dim && v != 0) row[e] = det_fix_add(x0[e], v);
+        }
+      } else {
+        unsigned long long* dst = a.acc + (int64_t)sl * dim;
+#pragma unroll
+        for (int u = 0; u < NJ; ++u) {
+          const int e = lane + 32 * u;
+          const long long v = __float2ll_rn(acc[j][u] * kFixScale);
+          if (e < dim && v != 0) atomicAdd(dst + e, (unsigned long long)v);
+        }
+      }
     }
   }
 
-  // ---- phase 2: output-row deltas sum_c g_ck * in_c, two output rows at a time in registers (O is dead).  A row
-  // this (centre, k) alone reads is loaded before its sums start, so its loads are in flight during the sums, and
-  // is written in place: the row as the wave found it (nothing else reads or writes it in this wave) plus the one
-  // term its fixed-point sum would hold; zero terms leave the element untouched, as in the apply.  Every other row
-  // leaves as one row of REDs.  Each element's FMA chain runs over the contexts in mask order whatever the
-  // grouping of the rows, so the grouping changes no bit. ------------------------------------------------------
-  static_assert(KO % 2 == 0, "phase 2 takes the output rows in pairs");
-  if (ctx) {
-#pragma unroll 1
-    for (int k0 = 0; k0 < KO; k0 += 2) {
-      if (!((used >> k0) & 3u)) continue;
-      float x[2][NJ], acc[2][NJ];
-#pragma unroll
-      for (int j = 0; j < 2; ++j) {
-        if ((owned >> (k0 + j)) & 1u) {
-          const float* row = a.w_out + (int64_t)orid[c * KO + k0 + j] * a.ld;
-#pragma unroll
-          for (int u = 0; u < NJ - 1; ++u) x[j][u] = row[lane + 32 * u];   // NJ = ceil(dim / 32)
-          x[j][NJ - 1] = lane + 32 * (NJ - 1) < dim ? row[lane + 32 * (NJ - 1)] : 0.f;
-        }
-#pragma unroll
-        for (int u = 0; u < NJ; ++u) acc[j][u] = 0.f;
-      }
-      for (uint32_t m = ctx; m; m &= m - 1) {
-        const int t = __ffs(m) - 1;
-        float h[NJ];
-        det_load(h, hrow + (size_t)(c + W + t - hw) * dim, dim, lane, true);
-#pragma unroll
-        for (int j = 0; j < 2; ++j) {
-          const float gk = gs[t * KO + k0 + j] * osc[c * KO + k0 + j];
-#pragma unroll
-          for (int u = 0; u < NJ; ++u) acc[j][u] = __fmaf_rn(gk, h[u], acc[j][u]);
-        }
-      }
-#pragma unroll
-      for (int j = 0; j < 2; ++j) {
-        const int k = k0 + j;
-        if (!((used >> k) & 1u)) continue;
-        if ((owned >> k) & 1u) {
-          float* row = a.w_out + (int64_t)orid[c * KO + k] * a.ld;
-#pragma unroll
-          for (int u = 0; u < NJ; ++u) {
-            const long long v = __float2ll_rn(acc[j][u] * kFixScale);
-            if (lane + 32 * u < dim && v != 0) row[lane + 32 * u] = det_fix_add(x[j][u], v);
-          }
-          continue;
-        }
-        unsigned long long* dst = a.acc + (int64_t)__shfl_sync(0xffffffffu, oslot, k) * dim;
-#pragma unroll
-        for (int u = 0; u < NJ; ++u)
-          if (lane + 32 * u < dim) atomicAdd(dst + lane + 32 * u, (unsigned long long)__float2ll_rn(acc[j][u] * kFixScale));
-      }
+  // ---- each loss-sampled centre's loss, summed in (offset, k) order ---------------------------------------
+  if (a.want_loss && warp == NW - 1 && lane < ns && ((s0 + lane) & 7) == 0) {
+    const int used = cused[lane];
+    float loss = 0.f;
+    for (uint32_t m = (uint32_t)chw[lane].x; m; m &= m - 1) {
+      const float* l = lsm + (lane * nt + __ffs(m) - 1) * KO;
+      for (int k = 0; k < KO; ++k)
+        if ((used >> k) & 1) loss += l[k];
     }
-  }
-  if (lane == 0) {
-    if (a.want_loss && loss != 0.f) atomicAdd(a.loss_acc, (unsigned long long)__float2ll_rn(loss * kLossScale));
-    if (a.pair_count && pairs) atomicAdd(a.pair_count, (unsigned long long)pairs);
+    if (loss != 0.f) atomicAdd(a.loss_acc, (unsigned long long)__float2ll_rn(loss * kLossScale));
   }
 }
 
@@ -1241,14 +1313,15 @@ extern "C" int mvb_sgns_train_det(const MvbSgns* h, void* stream) {
   a.seed = h->seed; a.want_loss = h->loss_sum != nullptr; a.pair_count = h->pair_count; a.loss_sum = h->loss_sum;
   int wave = mvb_sgns_win_inflight(h->dim, h->negative, h->window);
   if (wave <= 0) wave = 2 * mvb_num_sms() * kNW;
-  // the <NJ, KO> instance, and as many centres per CTA as its registers and the opt-in shared memory allow
+  // the <NJ, KO> instance; a wave holds the same number of centres for every SM, so one CTA per SM takes
+  // wave / SMs of them, fewer where the opt-in shared memory does not hold their rows
   void (*kern)(DetDev) = nullptr;
-  int S = 0;
+  int threads = 0;
   const int ko = a.ko <= 6 ? 6 : 8;
 #define MVB_DET_KERNEL(NJ)                                              \
   case NJ:                                                              \
     kern = ko == 6 ? sgns_det_kernel<NJ, 6> : sgns_det_kernel<NJ, 8>;   \
-    S = det_max_s(NJ, ko);                                              \
+    threads = 32 * det_warps(NJ);                                       \
     break;
   switch ((h->dim + 31) / 32) {
     MVB_DET_KERNEL(1) MVB_DET_KERNEL(2) MVB_DET_KERNEL(3) MVB_DET_KERNEL(4)
@@ -1261,6 +1334,8 @@ extern "C" int mvb_sgns_train_det(const MvbSgns* h, void* stream) {
   int dev = 0, max_smem = 0;
   MVB_CUDA_CHECK(cudaGetDevice(&dev));
   MVB_CUDA_CHECK(cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+  int S = (wave + mvb_num_sms() - 1) / mvb_num_sms();
+  if (S > kDetMaxS) S = kDetMaxS;
   while (S > 1 && det_smem_bytes(S, h->window, h->dim, ko) > (size_t)max_smem) --S;
   const size_t smem = det_smem_bytes(S, h->window, h->dim, ko);
   if (smem > (size_t)max_smem) return -22;
@@ -1352,7 +1427,7 @@ extern "C" int mvb_sgns_train_det(const MvbSgns* h, void* stream) {
     a.p0 = p0;
     a.p1 = p0 + wave < N ? p0 + wave : N;
     a.wi = (int)w;
-    kern<<<(int)((a.p1 - p0 + S - 1) / S), 32 * S, smem, st>>>(a);
+    kern<<<(int)((a.p1 - p0 + S - 1) / S), threads, smem, st>>>(a);
     sgns_det_apply<<<apply_blocks, 256, 0, st>>>(a);
     mvb_sgns_launches += 2;
   }
