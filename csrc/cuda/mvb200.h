@@ -913,6 +913,40 @@ typedef struct MvbFm {
 int mvb_fm_fwd(const MvbFm* a, void* stream);
 int mvb_fm_bwd(const MvbFm* a, void* stream);
 
+/* ---- field-aware factorization machine over a row-sharded fp32 MatrixTable (ffm.cu) ---------------------------- */
+/* F fields of k factors, D = F k. Row r holds V_r[f] = W[r, f k : (f + 1) k] (f < F) and the linear weight
+ * w_r = W[r, D]; columns past D are never used. Bag b holds the lookups [offsets[b], offsets[b + 1]) (the last bag
+ * ends at L) with ids i_j, fields f_j and values x_j:
+ *   y_b = sum_j x_j w_{i_j} + sum_{j < l} x_j x_l <V_{i_j}[f_l], V_{i_l}[f_j]>   (an empty bag gives 0)
+ * With h set, the forward also writes, for every lookup j of bag b, H_j = dy_b / d(row values at j):
+ *   H_j[f k + c] = x_j sum_{l != j in the bag, f_l = f} x_l V_{i_l}[f_j][c] (l in position order),  H_j[D] = x_j,
+ * and 0 in the columns [D + 1, ldh). The row gradient of sum_b g_b y_b is then sum_{j: i_j = r} g_{b(j)} H_j: the
+ * embedding-bag backward (MvbEmbBag) over one bag per lookup with per-sample weights g_{b(j)} and dout = H.
+ * y_b = sum_j x_j w_{i_j} + (1/2) sum_j <H_j[0:D], W[i_j, 0:D]>, with each thread's terms in a fixed order and a
+ * fixed-tree reduction: y and H are bitwise reproducible, the same for every sharding and for any max_len, and y is
+ * the same with and without h. Rows are read from their owners' shards as mvb_get_rows reads them. The caller
+ * validates ids (in [0, num_row)), fields (in [0, F)) and offsets. Errors, all before any CUDA call:
+ * MVB_BAD_ROW_MAP; -95 k < 4, k not % 4, F < 1 or D + 1 > MVB_FFM_MAX_DIM; -96 wmap.num_col < D + 1 or not % 4,
+ * or a shard not 16-byte aligned; -97 B < 0 or L < 0; -98 offsets / y missing with B > 0, or ids / fields missing
+ * with L > 0; -99 h set with ldh not % 4, ldh < round4(D + 1), or h not 16-byte aligned. B == 0 launches nothing. */
+#define MVB_FFM_MAX_DIM 1024
+typedef struct MvbFfm {
+  MvbRowMap wmap;            /* fp32 shards, row pitch wmap.num_col (% 4 == 0, >= D + 1), 16-byte aligned     */
+  int64_t F;                 /* fields, >= 1                                                                 */
+  int64_t k;                 /* factors per field, % 4 == 0, >= 4; F k + 1 <= MVB_FFM_MAX_DIM                 */
+  const int64_t* ids;        /* [L] rows                                                                     */
+  const int* fields;         /* [L] field of every lookup, in [0, F)                                         */
+  const float* values;       /* [L] x by lookup position, or NULL (every x is 1)                             */
+  const int64_t* offsets;    /* [B]: offsets[0] == 0, non-decreasing, <= L                                   */
+  int64_t L;
+  int64_t B;
+  int64_t max_len;           /* the longest bag, or <= 0: unknown. Only sizes the shared-memory tile           */
+  float* y;                  /* [B] out                                                                      */
+  float* h;                  /* [L x ldh] out (16-byte aligned), or NULL: not written                         */
+  int64_t ldh;               /* % 4 == 0, >= round4(D + 1)                                                   */
+} MvbFfm;
+int mvb_ffm_fwd(const MvbFfm* a, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

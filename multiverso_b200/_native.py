@@ -237,6 +237,14 @@ class Fm(C.Structure):
                 ("scratch_bytes", i64), ("push_rows", i64)]
 
 
+FFM_MAX_DIM = 1024
+
+
+class Ffm(C.Structure):
+    _fields_ = [("wmap", RowMap), ("F", i64), ("k", i64), ("ids", vp), ("fields", vp), ("values", vp),
+                ("offsets", vp), ("L", i64), ("B", i64), ("max_len", i64), ("y", vp), ("h", vp), ("ldh", i64)]
+
+
 class NativeError(RuntimeError):
     pass
 
@@ -381,6 +389,7 @@ _CUDA_FUNCS = {
     "mvb_hsm_fwd": _status(C.POINTER(Hsm), Ptr),
     "mvb_fm_fwd": _status(C.POINTER(Fm), Ptr),
     "mvb_fm_bwd": _status(C.POINTER(Fm), Ptr),
+    "mvb_ffm_fwd": _status(C.POINTER(Ffm), Ptr),
 }
 
 

@@ -86,9 +86,11 @@ def _bags(ids, offsets, per_sample_weights, mode: str) -> Tuple[torch.Tensor, to
 
 
 def _check_values(ids: torch.Tensor, offsets: torch.Tensor, num_row: int, status: Optional[torch.Tensor] = None,
-                  hash_table=None) -> None:
+                  hash_table=None, extra=None) -> None:
     """ids in [0, num_row) and offsets that start at 0, never decrease and stay within the ids (one host read).
-    ``status``: the status word of the hash translation that produced ``ids``, read in the same copy."""
+    ``status``: the status word of the hash translation that produced ``ids``, read in the same copy. ``extra``: a
+    function of (ids, offsets) returning (int64 tensors to read in the same copy, a check called with their values
+    after the checks above), for a caller with more to check."""
     L, B = ids.numel(), offsets.numel()
     if B == 0:
         if L:
@@ -97,9 +99,11 @@ def _check_values(ids: torch.Tensor, offsets: torch.Tensor, num_row: int, status
     parts = [offsets[:1], (offsets[1:] < offsets[:-1]).any().view(1).to(torch.int64), offsets[-1:]]
     if L:
         parts += list(torch.aminmax(ids))
+    more, check = extra(ids, offsets) if extra is not None else ([], None)
+    parts += more
     if status is not None:
         parts.append(status)
-    v = torch.cat([p.view(-1) for p in parts]).tolist()
+    v = torch.cat([p.view(-1).to(torch.int64) for p in parts]).tolist()
     if status is not None:
         raise_hash_status(v.pop(), [hash_table])
     if v[0] != 0:
@@ -110,6 +114,8 @@ def _check_values(ids: torch.Tensor, offsets: torch.Tensor, num_row: int, status
         raise ValueError(f"embedding_bag: offsets exceed the number of ids ({v[2]} > {L})")
     if L and (v[3] < 0 or v[4] >= num_row):
         raise ValueError(f"embedding_bag: ids must be in [0, {num_row}), got min {v[3]} max {v[4]}")
+    if check is not None:
+        check(v[5 if L else 3:])
 
 
 def _bag_index(offsets: torch.Tensor, L: int) -> Tuple[torch.Tensor, torch.Tensor]:
@@ -170,10 +176,12 @@ def _fwd_device(rm, dim, ids, offsets, psw, mode) -> torch.Tensor:
 
 
 def _dout_padded(dout: torch.Tensor, dim: int) -> Tuple[torch.Tensor, int]:
-    """dout as rows of a multiple of 4 floats, 16-byte aligned (copied only when it is not already)."""
+    """dout as rows of a multiple of 4 floats, 16-byte aligned (copied only when it is not already). A contiguous
+    dout wider than dim whose pitch is a multiple of 4 is taken as it is: its first dim columns are the gradient."""
     dout = dout.to(torch.float32)
-    if dim % 4 == 0 and dout.is_contiguous() and dout.data_ptr() % 16 == 0:
-        return dout, dim
+    ld = dout.shape[1]
+    if ld >= dim and ld % 4 == 0 and dout.is_contiguous() and dout.data_ptr() % 16 == 0:
+        return dout, ld
     ldd = (dim + 3) // 4 * 4
     pad = torch.zeros(dout.shape[0], ldd, dtype=torch.float32, device=dout.device)
     pad[:, :dim] = dout
@@ -216,12 +224,13 @@ def _push_device(table, rm, dim, ids, offsets, psw, mode, dout, push_scale: floa
         a.n_unique = n_unique.data_ptr()
         lib.mvb_embedding_bag_bwd(a, st)     # count only
         U = int(n_unique.item())
-        alloc = torch.empty if dim == table.num_col else torch.zeros
-        grads = alloc(U, table.num_col, dtype=torch.float32, device=ids.device)
+        ldg = (table.num_col + 3) // 4 * 4             # the kernel writes whole 16-byte vectors
+        alloc = torch.empty if dim == ldg else torch.zeros
+        grads = alloc(U, ldg, dtype=torch.float32, device=ids.device)
         uniq = torch.empty(U, dtype=torch.int64, device=ids.device)
-        a.grads, a.ldg, a.uniq = grads.data_ptr(), table.num_col, uniq.data_ptr()
+        a.grads, a.ldg, a.uniq = grads.data_ptr(), ldg, uniq.data_ptr()
         lib.mvb_embedding_bag_bwd(a, st)
-    table.add_rows_async(uniq, grads, option)
+    table.add_rows_async(uniq, grads if ldg == table.num_col else grads[:, :table.num_col], option)
 
 
 # ------------------------------------------------------------------------------------------------ host
@@ -298,9 +307,9 @@ class _EmbeddingBagFn(torch.autograd.Function):
         return da, dpsw, None, None, None, None, None, None, None
 
 
-def _prepare(table, ids, offsets, per_sample_weights, mode, insert: bool = False):
+def _prepare(table, ids, offsets, per_sample_weights, mode, insert: bool = False, extra=None):
     """Checked (ids, offsets, weights) of a call; for a HashMatrixTable the ids are keys, translated to rows first
-    (``insert``: missing keys get rows; otherwise they read the zero row)."""
+    (``insert``: missing keys get rows; otherwise they read the zero row). ``extra``: as in ``_check_values``."""
     if _dtype_of(table) != torch.float32:
         raise TypeError(f"embedding_bag: the table must be float32, got {_dtype_of(table)}")
     ids, offsets, psw = _bags(ids, offsets, per_sample_weights, mode)
@@ -315,9 +324,9 @@ def _prepare(table, ids, offsets, per_sample_weights, mode, insert: bool = False
     if isinstance(table, HashMatrixTable):
         rows, status = torch.empty_like(ids), torch.empty(1, dtype=torch.int64, device=dev)
         table.lookup_call(ids, rows, status, insert)
-        _check_values(rows, offsets, num_row, status, table)
+        _check_values(rows, offsets, num_row, status, table, extra)
         return rows, offsets, psw
-    _check_values(ids, offsets, num_row)
+    _check_values(ids, offsets, num_row, extra=extra)
     return ids, offsets, psw
 
 
