@@ -855,15 +855,16 @@ MVB_DEVINL float det_fix_add(float x, long long v) { return x + (float)((double)
 // registers with 16 warps at 128.
 __host__ __device__ constexpr int det_warps(int nj) { return nj <= 10 ? 32 : 16; }
 constexpr int kDetMaxS = 32;                      // centres per CTA: the scoring units are listed by one warp
+constexpr int kDetGroups = 4;                     // staging groups of consecutive centres per CTA
 
 // Shared memory of a CTA of S centres: the 1+K output rows of every centre and the input row of every staged
 // position (S + 2W of them), rows padded to 16 bytes; per (centre, offset, output row) the pair's error term and
-// loss term; per staged position its id / scale / slot; per (centre, output row) its id / scale / slot; per centre
-// its window and the rows it uses; the slice's scoring units.
+// loss term; per centre its window; an mbarrier per staging group; per staged position its id / scale / slot; per
+// (centre, output row) its id / scale / slot; per centre the rows it uses; the slice's scoring units.
 __host__ __device__ inline size_t det_smem_bytes(int S, int W, int dim, int ko) {
   const size_t dimp = (size_t)(dim + 3) / 4 * 4;
   return ((size_t)S * ko + S + 2 * W) * dimp * 4 + (size_t)S * (2 * W + 1) * ko * 8 + (size_t)S * 8 +
-         (size_t)(S + 2 * W) * 12 + (size_t)S * ko * 12 + (size_t)S * 4 + (size_t)S * W * 4 + 16;
+         kDetGroups * 8 + (size_t)(S + 2 * W) * 12 + (size_t)S * ko * 12 + (size_t)S * 4 + (size_t)S * W * 4 + 16;
 }
 
 MVB_DEVINL void det_cp16(float* dst, const float* src) {
@@ -872,13 +873,23 @@ MVB_DEVINL void det_cp16(float* dst, const float* src) {
 MVB_DEVINL void det_cp4(float* dst, const float* src) {
   asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(smem_u32(dst)), "l"(src) : "memory");
 }
+// arrives on bar once every cp.async this thread issued so far has landed (the count was set for it at init)
+MVB_DEVINL void det_cp_arrive(uint64_t* bar) {
+  asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
+// Programmatic dependent launch: the next kernel of the stream may start; wait until the previous one has
+// finished and its writes are visible (returns at once when the kernel was not launched as a dependent).
+MVB_DEVINL void det_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+MVB_DEVINL void det_wait_previous() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
 // One CTA owns S consecutive centres [s0, s0 + S) of the wave.  It stages the 1+K output rows of every centre with a
-// context and the input rows of the positions [s0 - W, s0 + S + W) that are a context, all at once with cp.async,
-// then works from shared memory in two phases split by one barrier, each spread over all warps:
-//   scoring    a warp per two contexts of a centre: the 2 x (1+K) dots, in flight together and each output row
-//              read once for both, give the pairs' error terms (and the loss terms of loss-sampled centres) in
-//              shared memory;
+// context and the input rows of the positions [s0 - W, s0 + S + W) that are a context, all at once with cp.async in
+// kDetGroups groups of consecutive centres (a group: its centres' output rows and the input rows no earlier group
+// needs; each lands on the group's mbarrier), then works from shared memory in two phases split by one barrier, each
+// spread over all warps:
+//   scoring    a warp per two contexts of a centre, as soon as the centre's group has landed: the 2 x (1+K) dots,
+//              in flight together and each output row read once for both, give the pairs' error terms (and the
+//              loss terms of loss-sampled centres) in shared memory;
 //   deltas     a warp per staged position sums, in int64 registers, the fixed-point input delta of every pair that
 //              writes it, then applies it in place (its only reader in the wave) or sends one row of REDs to its
 //              accumulator slot; a warp per (centre, pair of output rows) sums their output deltas over the centre's
@@ -888,6 +899,12 @@ MVB_DEVINL void det_cp4(float* dst, const float* src) {
 // delta's over the contexts in mask order; one conversion to fixed point per pair and per (centre, k); each
 // centre's loss summed in (offset, k) order); only the grouping of the exact int64 sums does, so the result is
 // bitwise independent of S and of the warp count.
+//
+// The waves and their applies are chained by programmatic dependent launch: before griddepcontrol.wait a CTA reads
+// only the plan, which was complete before the first wave started, and adds its pairs to pair_count, which no kernel
+// of the chain reads; every table row, acc and loss_acc access comes after it.  Every CTA triggers its dependents
+// first thing, so a dependent grid is launched only once all CTAs of this one are resident: a dependent CTA waiting
+// for an SM never holds resources a CTA it waits on needs.
 template <int NJ, int KO>
 __global__ void __launch_bounds__(32 * det_warps(NJ), 1)
 sgns_det_kernel(const __grid_constant__ DetDev a) {
@@ -904,7 +921,8 @@ sgns_det_kernel(const __grid_constant__ DetDev a) {
   float* gsm = hrow + (size_t)span * dimp;                 // [S][2W + 1][KO] error terms, offset t = hw + d
   float* lsm = gsm + S * nt * KO;                          // [S][2W + 1][KO] loss terms
   int2* chw = reinterpret_cast<int2*>(lsm + S * nt * KO);  // [S] context mask and half window
-  int* crid = reinterpret_cast<int*>(chw + S);
+  uint64_t* mbar = reinterpret_cast<uint64_t*>(chw + S);   // [kDetGroups] staging groups landed
+  int* crid = reinterpret_cast<int*>(mbar + kDetGroups);
   float* csc = reinterpret_cast<float*>(crid + span);
   int* cslot = reinterpret_cast<int*>(csc + span);
   int* orid = cslot + span;
@@ -913,6 +931,9 @@ sgns_det_kernel(const __grid_constant__ DetDev a) {
   int* cused = oslot + S * KO;                             // [S] output rows a centre with a context uses
   int* plist = cused + S;                                  // [S * W] units: centre << 10 | offset tb << 5 | ta
   int* nunits = plist + S * W;
+
+  det_launch_dependents();
+  if (threadIdx.x < kDetGroups) mbar_init(mbar + threadIdx.x, blockDim.x);
 
   // ---- the slice's plan: a thread per staged position, per (centre, output row), per centre ----------------
   const int base = __ldg(a.off + a.wi);                   // the wave's first entry in the list of shared rows
@@ -938,29 +959,7 @@ sgns_det_kernel(const __grid_constant__ DetDev a) {
   }
   __syncthreads();
 
-  // ---- stage every row a pair reads, a warp per row, all copies in flight at once --------------------------
-  const bool vec = (dim & 3) == 0 && (a.ld & 3) == 0 &&
-                   ((reinterpret_cast<uintptr_t>(a.w_in) | reinterpret_cast<uintptr_t>(a.w_out)) & 15) == 0;
-  for (int r = warp; r < np + ns * KO; r += NW) {
-    const float* src;
-    float* dst;
-    if (r < np) {
-      if (cslot[r] < -1) continue;                        // not a context of any centre of the slice
-      src = a.w_in + (int64_t)crid[r] * a.ld;
-      dst = hrow + (size_t)r * dimp;
-    } else {
-      const int ck = r - np;
-      if (!chw[ck / KO].x || orid[ck] < 0) continue;
-      src = a.w_out + (int64_t)orid[ck] * a.ld;
-      dst = orow + (size_t)ck * dimp;
-    }
-    if (vec) {
-      for (int j = lane * 4; j < dim; j += 128) det_cp16(dst + j, src + j);
-    } else {
-      for (int j = lane; j < dim; j += 32) det_cp4(dst + j, src + j);
-    }
-  }
-  // the scoring units, two consecutive contexts of a centre each (offset 31: none), while the copies land
+  // ---- the scoring units, two consecutive contexts of a centre each (offset 31: none) ----------------------
   if (warp == 0) {
     int2 cx = make_int2(0, 0);
     int used = 0;
@@ -989,13 +988,47 @@ sgns_det_kernel(const __grid_constant__ DetDev a) {
     const int total = __reduce_add_sync(0xffffffffu, pairs);
     if (lane == 0 && a.pair_count && total) atomicAdd(a.pair_count, (unsigned long long)total);
   }
-  asm volatile("cp.async.wait_all;" ::: "memory");
   __syncthreads();
+  det_wait_previous();                                     // the rows as the previous wave and apply left them
+
+  // ---- stage every row a pair reads, all copies in flight at once, group by group; a warp per row ----------
+  // Group g is the centres [g * cg, (g + 1) * cg).  Centre c reads the staged positions [c, c + 2W], so a group's
+  // input rows are the positions up to its last centre's + 2W that no earlier group reads.
+  const int cg = (ns + kDetGroups - 1) / kDetGroups;
+  const bool vec = (dim & 3) == 0 && (a.ld & 3) == 0 &&
+                   ((reinterpret_cast<uintptr_t>(a.w_in) | reinterpret_cast<uintptr_t>(a.w_out)) & 15) == 0;
+  for (int g = 0, r0 = 0; g < kDetGroups; ++g) {
+    const int c0 = min(g * cg, ns), c1 = min(c0 + cg, ns);
+    const int i0 = g == 0 ? 0 : c0 + 2 * W, nin = c1 + 2 * W - i0, n = nin + (c1 - c0) * KO;
+    for (int r = r0 + (warp - r0 % NW + NW) % NW; r < r0 + n; r += NW) {   // warps take rows in turn across groups
+      const float* src;
+      float* dst;
+      if (r - r0 < nin) {
+        const int i = i0 + r - r0;
+        if (cslot[i] < -1) continue;                      // not a context of any centre of the slice
+        src = a.w_in + (int64_t)crid[i] * a.ld;
+        dst = hrow + (size_t)i * dimp;
+      } else {
+        const int ck = c0 * KO + r - r0 - nin;
+        if (!chw[ck / KO].x || orid[ck] < 0) continue;
+        src = a.w_out + (int64_t)orid[ck] * a.ld;
+        dst = orow + (size_t)ck * dimp;
+      }
+      if (vec) {
+        for (int j = lane * 4; j < dim; j += 128) det_cp16(dst + j, src + j);
+      } else {
+        for (int j = lane; j < dim; j += 32) det_cp4(dst + j, src + j);
+      }
+    }
+    det_cp_arrive(mbar + g);                               // completes once every thread's copies so far landed
+    r0 += n;
+  }
 
   // ---- scoring: the 1+K dots of two pairs of a centre on the rows as the wave found them, each output row read
   // once for both ------------------------------------------------------------------------------------------
   for (int q = warp; q < *static_cast<volatile int*>(nunits); q += NW) {   // re-read: no register held over the loop
     const int c = plist[q] >> 10, ta = plist[q] & 31, tb = (plist[q] >> 5) & 31;
+    mbar_wait(mbar + c / cg, 0);                           // the rows of c's group and every earlier one landed
     const int used = cused[c], hw = chw[c].y;
     const float* ha = hrow + (size_t)(c + W + ta - hw) * dimp;
     const float* hb = tb != 31 ? hrow + (size_t)(c + W + tb - hw) * dimp : ha;
@@ -1037,6 +1070,7 @@ sgns_det_kernel(const __grid_constant__ DetDev a) {
       if (u && a.want_loss && ((s0 + c) & 7) == 0) lsm[e] = 8.f * softplus_neg(k == 0 ? f : -f);
     }
   }
+  mbar_wait(mbar + kDetGroups - 1, 0);                    // every copy landed, whichever groups this warp scored
   __syncthreads();
 
   // ---- deltas: a unit per staged position, then per (centre, pair of output rows) -------------------------
@@ -1150,19 +1184,24 @@ sgns_det_kernel(const __grid_constant__ DetDev a) {
 }
 
 // Adds each shared row's sum to its table and clears its slot, a warp per entry of the wave's list; rolls the
-// wave's loss into loss_sum.
+// wave's loss into loss_sum.  Chained to its wave and the next one as the wave kernel is: only the plan is read
+// before griddepcontrol.wait.
 __global__ void __launch_bounds__(256)
 sgns_det_apply(const __grid_constant__ DetDev a) {
+  det_launch_dependents();
   const int tid = blockIdx.x * blockDim.x + threadIdx.x;
-  const int base = a.off[a.wi], n = a.off[a.wi + 1] - base;
+  const int base = __ldg(a.off + a.wi), n = __ldg(a.off + a.wi + 1) - base;
   float* __restrict__ w_in = a.w_in;
   float* __restrict__ w_out = a.w_out;
   const int dim = a.dim;
   const int64_t ld = a.ld;
   const int lane = threadIdx.x & 31;
   const int nwarps = (gridDim.x * blockDim.x) >> 5;
+  unsigned next = (tid >> 5) < n ? __ldg(a.list + base + (tid >> 5)) : 0u;
+  det_wait_previous();                            // the wave's sums and loss
   for (int w = tid >> 5; w < n; w += nwarps) {
-    const unsigned e = a.list[base + w];
+    const unsigned e = next;
+    if (w + nwarps < n) next = __ldg(a.list + base + w + nwarps);
     unsigned long long* q = a.acc + (int64_t)w * dim;
     float* row = ((e >> 31) ? w_out : w_in) + (int64_t)(e & 0x7fffffffu) * ld;
     for (int j0 = 0; j0 < dim; j0 += 128) {          // 4 elements per lane in flight
@@ -1422,13 +1461,30 @@ extern "C" int mvb_sgns_train_det(const MvbSgns* h, void* stream) {
   mvb_sgns_launches = 6;     // the plan's own kernels (the radix sort launches its own)
 
   // ---- the waves ------------------------------------------------------------------------------------------
+  // Each kernel may start while the one before it drains (programmatic dependent launch), except the first wave:
+  // its reads before griddepcontrol.wait are of the plan, which the kernel just before it is still writing.
   const int apply_blocks = mvb_num_sms() * 4;
+  cudaLaunchAttribute pdl{};
+  pdl.id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  pdl.val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchConfig_t wcfg{}, acfg{};
+  wcfg.blockDim = dim3(threads);
+  wcfg.dynamicSmemBytes = smem;
+  wcfg.stream = st;
+  acfg.gridDim = dim3(apply_blocks);
+  acfg.blockDim = dim3(256);
+  acfg.stream = st;
+  acfg.attrs = &pdl;
+  acfg.numAttrs = 1;
   for (int64_t p0 = 0, w = 0; p0 < N; p0 += wave, ++w) {
     a.p0 = p0;
     a.p1 = p0 + wave < N ? p0 + wave : N;
     a.wi = (int)w;
-    kern<<<(int)((a.p1 - p0 + S - 1) / S), threads, smem, st>>>(a);
-    sgns_det_apply<<<apply_blocks, 256, 0, st>>>(a);
+    wcfg.gridDim = dim3((unsigned)((a.p1 - p0 + S - 1) / S));
+    wcfg.attrs = w > 0 ? &pdl : nullptr;
+    wcfg.numAttrs = w > 0 ? 1 : 0;
+    MVB_CUDA_CHECK(cudaLaunchKernelEx(&wcfg, kern, a));
+    MVB_CUDA_CHECK(cudaLaunchKernelEx(&acfg, sgns_det_apply, a));
     mvb_sgns_launches += 2;
   }
   MVB_CUDA_CHECK(cudaGetLastError());
