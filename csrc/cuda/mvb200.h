@@ -947,6 +947,38 @@ typedef struct MvbFfm {
 } MvbFfm;
 int mvb_ffm_fwd(const MvbFfm* a, void* stream);
 
+/* ---- random walks on a CSR graph: DeepWalk and node2vec (walk.cu) ----------------------------------------------- */
+/* Node v's out-list is indices[indptr[v], indptr[v + 1]), sorted ascending (repeated entries are multi-edges); cum,
+ * when set, holds the weights' prefix sums within each list (mvb_csr_cumsum). Walk i is walk number g = first_walk + i:
+ * row i of out holds starts[i] and the nodes it visits, -1 in every slot after the walk ends (L nodes, or a node
+ * without out-arcs), up to the pitch. Every random number is a pure function of (seed, g, step, attempt)
+ * (multiverso_b200/ops/random_walk.py states the formula), so the walks do not depend on the launch or on how the
+ * starts are split between calls. With node_count set, the number of nodes written is added to it. The caller
+ * validates starts (in [0, num_nodes)). Errors, all before any CUDA call: -100 indptr / indices / starts / out
+ * missing, or a pointer not aligned to its element; -101 num_nodes < 0 or >= 2^31 - 1, or n < 0 or >= 2^31;
+ * -102 length < 1 or >= 2^31; -103 pitch < length; -104 p or q not finite and > 0, or 1/p or 1/q not finite and
+ * > 0 in fp32; -105 first_walk < 0 or first_walk + n > INT64_MAX. n == 0 launches nothing. */
+typedef struct MvbRandomWalk {
+  const int64_t* indptr;     /* [num_nodes + 1]                                                             */
+  const int* indices;        /* [E], each list sorted ascending                                             */
+  const double* cum;         /* [E] per-list prefix sums of positive weights, or NULL: unweighted            */
+  int64_t num_nodes;
+  const int* starts;         /* [n] first node of every walk                                                */
+  int64_t n;
+  int64_t length;            /* L >= 1 nodes per walk at most                                              */
+  int64_t pitch;             /* row pitch of out in ints, >= L                                              */
+  double p;                  /* return parameter                                                           */
+  double q;                  /* in-out parameter; p = q = 1: first-order (DeepWalk)                         */
+  uint64_t seed;
+  int64_t first_walk;        /* walk number of row 0                                                       */
+  int* out;                  /* [n x pitch]                                                                */
+  int64_t* node_count;       /* device int64 += nodes written, or NULL                                      */
+} MvbRandomWalk;
+int mvb_random_walk(const MvbRandomWalk* a, void* stream);
+/* cum[j] = w[indptr[v]] + ... + w[j] for j in v's list, summed in list order in fp64. Errors: -100 a pointer missing
+ * or not 8-byte aligned; -101 num_nodes < 0 or >= 2^31 - 1. */
+int mvb_csr_cumsum(const int64_t* indptr, const double* w, int64_t num_nodes, double* cum, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -37,7 +37,17 @@ void MVA_CorpusClose(void* corpus);
 int MVA_HuffmanBuild(const int64_t* freq, int n, int max_code, int32_t* points, int8_t* codes,
                      int32_t* lens);
 
-/* ---- LogisticRegression ------------------------------------------------------------------ */
+/* ---- GraphEmbedding ---------------------------------------------------------------------- */
+/* edge list: "src dst" lines ("src dst w" when weighted), labels integers in [0, 2^63 - 1], weights finite and
+ * > 0, blank lines and '#' comments skipped. Open parses the whole file: NULL when it cannot be opened; a
+ * malformed line stops the parse and Error returns "line <n>: <what>" (NULL when the file parsed). */
+void* MVA_EdgeListOpen(const char* path, int weighted);
+const char* MVA_EdgeListError(void* edges);
+int64_t MVA_EdgeListSize(void* edges);
+void MVA_EdgeListCopy(void* edges, int64_t* src, int64_t* dst, double* weights);
+void MVA_EdgeListClose(void* edges);
+
+/* ---- LogisticRegression------------------------------------------------------------------ */
 /* files: ';'-separated list; reader_type: "default" (libsvm "label k:v ..." when sparse, dense
  * "label v0 v1 ..." otherwise), "weight" ("label:weight ..."), "bsparse" (binary: count,label,
  * weight,keys...). A bias feature (key = input_size, value 1) is appended to every sample.

@@ -245,6 +245,12 @@ class Ffm(C.Structure):
                 ("offsets", vp), ("L", i64), ("B", i64), ("max_len", i64), ("y", vp), ("h", vp), ("ldh", i64)]
 
 
+class RandomWalk(C.Structure):
+    _fields_ = [("indptr", vp), ("indices", vp), ("cum", vp), ("num_nodes", i64), ("starts", vp), ("n", i64),
+                ("length", i64), ("pitch", i64), ("p", C.c_double), ("q", C.c_double), ("seed", C.c_uint64),
+                ("first_walk", i64), ("out", vp), ("node_count", vp)]
+
+
 class NativeError(RuntimeError):
     pass
 
@@ -390,6 +396,8 @@ _CUDA_FUNCS = {
     "mvb_fm_fwd": _status(C.POINTER(Fm), Ptr),
     "mvb_fm_bwd": _status(C.POINTER(Fm), Ptr),
     "mvb_ffm_fwd": _status(C.POINTER(Ffm), Ptr),
+    "mvb_random_walk": _status(C.POINTER(RandomWalk), Ptr),
+    "mvb_csr_cumsum": _status(Ptr, Ptr, i64, Ptr, Ptr),
 }
 
 

@@ -57,6 +57,14 @@ def lib():
         L.MVA_CorpusReset.argtypes = [vp]
         L.MVA_CorpusClose.argtypes = [vp]
         L.MVA_HuffmanBuild.argtypes = [vp, i32, i32, vp, vp, vp]
+        L.MVA_EdgeListOpen.restype = vp
+        L.MVA_EdgeListOpen.argtypes = [C.c_char_p, i32]
+        L.MVA_EdgeListError.restype = C.c_char_p
+        L.MVA_EdgeListError.argtypes = [vp]
+        L.MVA_EdgeListSize.restype = i64
+        L.MVA_EdgeListSize.argtypes = [vp]
+        L.MVA_EdgeListCopy.argtypes = [vp, vp, vp, vp]
+        L.MVA_EdgeListClose.argtypes = [vp]
         L.MVA_LRReaderOpen.restype = vp
         L.MVA_LRReaderOpen.argtypes = [C.c_char_p, C.c_char_p, i32, i64, i32]
         L.MVA_LRReaderNext.restype = i64
