@@ -282,21 +282,25 @@ lr_wide_epilogue_kernel(const float* __restrict__ logits, const float* __restric
   }
 }
 
-// out[c][r] = in[r][c] (in: [rows x cols] with pitch ld_in; out: [cols x ld_out], columns >= rows zeroed)
+// out[c][r] = in[r][c] (in: [rows x cols] with pitch ld_in; out: [cols x ld_out], columns >= rows zeroed).
+// The row tiles are grid-strided over blockIdx.y, so ld_out is not held to 32 * 65535 by the grid.y limit.
 __global__ void __launch_bounds__(256)
 transpose_pad_kernel(const float* __restrict__ in, int64_t rows, int64_t cols, int64_t ld_in,
                      float* __restrict__ out, int64_t ld_out) {
   __shared__ float tile[32][33];
-  const int64_t c0 = (int64_t)blockIdx.x * 32, r0 = (int64_t)blockIdx.y * 32;
+  const int64_t c0 = (int64_t)blockIdx.x * 32;
   const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;        // 32 x 8
-  for (int k = ty; k < 32; k += 8) {
-    const int64_t r = r0 + k, c = c0 + tx;
-    tile[k][tx] = (r < rows && c < cols) ? in[r * ld_in + c] : 0.f;
-  }
-  __syncthreads();
-  for (int k = ty; k < 32; k += 8) {
-    const int64_t c = c0 + k, r = r0 + tx;
-    if (c < cols && r < ld_out) out[c * ld_out + r] = tile[tx][k];
+  for (int64_t r0 = (int64_t)blockIdx.y * 32; r0 < ld_out; r0 += (int64_t)gridDim.y * 32) {
+    __syncthreads();                                             // the previous tile has been written out
+    for (int k = ty; k < 32; k += 8) {
+      const int64_t r = r0 + k, c = c0 + tx;
+      tile[k][tx] = (r < rows && c < cols) ? in[r * ld_in + c] : 0.f;
+    }
+    __syncthreads();
+    for (int k = ty; k < 32; k += 8) {
+      const int64_t c = c0 + k, r = r0 + tx;
+      if (c < cols && r < ld_out) out[c * ld_out + r] = tile[tx][k];
+    }
   }
 }
 
@@ -362,7 +366,8 @@ extern "C" int mvb_lr_wide_epilogue(const float* logits, const float* labels, in
 extern "C" int mvb_transpose_pad_f32(const float* in, int64_t rows, int64_t cols, int64_t ld_in, float* out,
                                      int64_t ld_out, void* stream) {
   if (rows <= 0 || cols <= 0) return 0;
-  dim3 grid((unsigned)((cols + 31) / 32), (unsigned)((ld_out + 31) / 32));
+  const int64_t row_tiles = (ld_out + 31) / 32;
+  dim3 grid((unsigned)((cols + 31) / 32), (unsigned)(row_tiles < 65535 ? row_tiles : 65535));
   transpose_pad_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(in, rows, cols, ld_in, out, ld_out);
   MVB_CUDA_CHECK(cudaGetLastError());
   return 0;

@@ -36,10 +36,10 @@ rows, ``logits = X W_S^T`` on the wgmma GEMM (TF32 operands, fp32 accumulation),
 (fp32 true logit, corrections, mask, logsumexp). The backward turns the logits into ``E = g softmax`` and ``E^T``,
 forms ``dX = E W_S + e_true w_y`` and ``dW_S = E^T X`` on the same GEMM, and pushes through the embedding-bag push
 (``mvb_embedding_bag_bwd``). It holds ``[B, S_pad]`` and ``[S_pad, B_pad]`` fp32 buffers (S and B rounded up to
-multiples of 4), about 512 MB at B = S = 8192. The forward reads the device once (the label checks); the backward
-does not synchronise with the host for the fused push and reads the unique-row count once for a compact push. The
-backward overwrites the saved logits, so a call's graph is backpropagated once: a second backward through a retained
-graph raises. An empty batch returns an empty loss and pushes nothing.
+multiples of 4), about 512 MB at B = S = 8192. A batch holds at most ``MAX_BATCH`` = 2,097,120 examples; S has no
+such limit. The forward reads the device once (the label checks); the backward does not synchronise with the host
+for the fused push and reads the unique-row count once for a compact push. The backward overwrites the saved logits,
+so a call's graph is backpropagated once: a second backward through a retained graph raises. An empty batch returns an empty loss and pushes nothing.
 
 On the host backend the same call draws the same ids, reads ``get_rows`` of the unique rows, evaluates the formula
 in torch fp32 with autograd for ``dL/dhidden`` and pushes the row gradients with one coalesced ``add_rows``.
@@ -69,6 +69,9 @@ from .topk import _rowmap_of
 SAMPLERS = ("log_uniform",)
 _WHAT = "PSSampledSoftmax"
 _M64 = (1 << 64) - 1
+# The backward epilogue tiles the batch in 32-example rows of a grid whose y extent is at most 65535
+# (mvb_ss_bwd_epilogue): larger batches are refused before the forward draws or runs anything.
+MAX_BATCH = 65535 * 32
 
 
 def _round4(n: int) -> int:
@@ -217,6 +220,9 @@ class PSSampledSoftmax(torch.nn.Module):
         dev = self._device
         if dev is not None and not hidden.is_cuda:
             raise ValueError(f"{_WHAT}: the table is on the GPU, hidden must be too")
+        if dev is not None and hidden.shape[0] > MAX_BATCH:
+            raise ValueError(f"{_WHAT}: a batch holds at most {MAX_BATCH} examples on the GPU (the backward's "
+                             f"epilogue grid), got {hidden.shape[0]}")
         y = labels.to(device=dev if dev is not None else "cpu", dtype=torch.int64).contiguous()
         if y.numel():                                     # one device read: range and zero-count labels
             lo, hi = torch.aminmax(y)
